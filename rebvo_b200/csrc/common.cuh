@@ -39,6 +39,7 @@ struct MapState {
     int fwd_match;
     int reg_num;
     unsigned int frame_count;  // global_tracker::FrameCount of this slot
+    int do_map;          // the per-frame pipeline's mapping gate of the frame that built this map (k_regularize_a_gate)
     double s_rho_q;
     double Kp, RKp;
 };

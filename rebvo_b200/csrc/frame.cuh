@@ -130,10 +130,13 @@ __device__ __forceinline__ void d_frame_pose(FrameState *fs) {
     fs->pose_done = 1;
 }
 
+// rescaled = false: the map's EstimateReScalingOpt has not run yet.  With DoReScaling=0 its Kp / RKp reach nothing but this
+// record (every frame sets Kp afresh: NaN guard, match-count restart or rescaling), so the pipeline runs it on a side
+// stream, which fills in the record's Kp / RKp when do_map is set; FrameState keeps the value of the last restart.
 __device__ __forceinline__ void d_frame_finish(FrameState *fs, const MapState *nst, const MapState *ost,
-                                               double lm_score, rb_nav *nav, const FrameArgs *fa) {
+                                               double lm_score, rb_nav *nav, const FrameArgs *fa, bool rescaled) {
     const double t = fa->t, dt_frame = fa->dt;
-    if (fs->do_map) {
+    if (rescaled && fs->do_map) {
         fs->Kp = nst->Kp;      // Kp=EstimateReScalingOpt(P_Kp,...)
         fs->P_Kp = nst->RKp;
     }

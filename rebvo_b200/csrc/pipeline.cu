@@ -57,6 +57,12 @@ struct rb_pipeline {
     int ss_sub;           // frames per scale-space sub-batch built on the detector stream (env REBVO_B200_SS_SUB, 0 = whole batch)
     bool fm_fused;        // FordwardMatch + rotate_keylines as one cluster kernel (env REBVO_B200_FM_FUSED)
     bool map_fused;       // gate + Regularize_1_iter + EKF inside the map-update cluster kernel (env REBVO_B200_MAP_FUSED)
+    // rescaling stream: with DoReScaling=0 a frame's EstimateReScalingOpt changes no keyline and only fills in its nav record,
+    // so it runs here (lowest priority) instead of at the end of the frame's tracker chain; the tracker stream joins it
+    // before the next frame's rotate_keylines, the first kernel after the fork that writes the map's rho / s_rho
+    cudaStream_t resc_stream;     // nullptr: the rescaling stays in the frame's map-update kernel on the tracker stream
+    cudaEvent_t ev_rfork, ev_rjoin;
+    bool resc_open;               // a rescaling was forked and not joined yet
     // host-input pushes are cut into a short head and the rest: the H2D copy of the rest (copy stream) runs beside the
     // kernels of the head.  The gray kernel reads its RGB source through rgb_src_dev, so one graph serves every region.
     cudaStream_t copy_stream;
@@ -141,7 +147,7 @@ __global__ void k_frame_post_match(FrameState *fs, const MapState *nst, int matc
 }
 __global__ void k_frame_finish(FrameState *fs, const MapState *nst, const MapState *ost, const TrackState *ts,
                                rb_nav *nav, const FrameArgs *fa) {
-    d_frame_finish(fs, nst, ost, ts->lm.score, nav, fa);
+    d_frame_finish(fs, nst, ost, ts->lm.score, nav, fa, true);
 }
 
 // record for the very first frame (it only initialises the ring, :109-121)
@@ -273,6 +279,15 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_det[i], cudaEventDisableTiming));
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
         }
+        // (the inline schedule where the rescaled keylines feed the next frame, the next quantile is folded into the
+        // map-update kernel, the map update is fused, or everything runs on one stream)
+        if (pl->overlap && !pl->q_fold && !pl->map_fused && p->DoReScaling <= 0) {
+            int lo = 0, hi = 0;
+            RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+            RB_CUDA(cudaStreamCreateWithPriority(&pl->resc_stream, cudaStreamNonBlocking, lo));   // minimiser blocks first
+            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_rfork, cudaEventDisableTiming));
+            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_rjoin, cudaEventDisableTiming));
+        }
     }
     for (int i = 0; i < 4; i++) RB_CUDA(cudaEventCreate(&pl->ev[i]));
     for (int i = 0; i < 8; i++) RB_CUDA(cudaEventCreate(&pl->user_ev[i]));
@@ -307,6 +322,7 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     if (pl->det_stream) cudaStreamSynchronize(pl->det_stream);
+    if (pl->resc_stream) cudaStreamSynchronize(pl->resc_stream);
     for (int i = 0; i < RB_NMAPS; i++)
         if (pl->maps[i]) rb_map_destroy(pl->maps[i]);
     if (pl->ev_dog) cudaEventDestroy(pl->ev_dog);
@@ -317,6 +333,9 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     delete[] pl->ev_det;
     delete[] pl->ev_trk;
     if (pl->det_stream) cudaStreamDestroy(pl->det_stream);
+    if (pl->resc_stream) cudaStreamDestroy(pl->resc_stream);
+    if (pl->ev_rfork) cudaEventDestroy(pl->ev_rfork);
+    if (pl->ev_rjoin) cudaEventDestroy(pl->ev_rjoin);
     if (pl->copy_stream) {
         cudaStreamSynchronize(pl->copy_stream);
         cudaStreamDestroy(pl->copy_stream);
@@ -379,6 +398,15 @@ extern "C" int rb_pipeline_reset(rb_pipeline *pl) {
     return pl_reset_state(pl);
 }
 
+// the tracker stream waits for the rescaling forked by the previous frame (or of the batch's last frame)
+static int resc_join(rb_pipeline *pl) {
+    rb_ctx *c = pl->c;
+    if (!pl->resc_open) return RB_OK;
+    RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_rjoin, 0));
+    pl->resc_open = false;
+    return RB_OK;
+}
+
 // one frame of the tracker/mapper stage: new = maps[f % RB_NMAPS] (already detected), old = the map of frame f-1
 static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, const FrameArgs *fa, rb_nav *nav_slot) {
     rb_ctx *c = pl->c;
@@ -423,11 +451,14 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
         k_frame_post_min<<<1, 1, 0, c->stream>>>(pl->fs, neu->ts);
         RB_LAUNCH_CHECK();
     }
-    // :354  FordwardMatch ; :369 rotate_keylines(R0)
+    // :354  FordwardMatch ; :369 rotate_keylines(R0).  Until the rotation, this frame only reads the old map's rho / s_rho
+    // (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may run until then.
     if (pl->fm_fused && pl->overlap) {   // (the arg-max scratch of the new map was cleared on the detector stream)
+        if ((r = resc_join(pl))) return r;
         if ((r = rb_forward_match_rotate_enqueue(c, old, neu, pl->fs->R0))) return r;
     } else {
         if ((r = rb_forward_match_enqueue(c, old, neu, pl->overlap, pl->fs))) return r;
+        if ((r = resc_join(pl))) return r;
         if ((r = rb_rotate_enqueue(c, old, pl->fs->R0))) return r;
     }
     RB_TRACE(c->stream, 11);
@@ -439,13 +470,31 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
     RB_TRACE(c->stream, 4);
     prof_mark(pl, ST_DMATCH);
     // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids, then
-    // :480-487 EstimateReScalingOpt and :545-585 pose integration + NavData in one cluster kernel (k_map_update)
+    // :480-487 EstimateReScalingOpt and :545-585 pose integration + NavData in one cluster kernel (k_map_update).
+    // With the rescaling stream, pose integration + NavData ride in the EKF kernel and the rescaling leaves the chain.
+    // (Not with the 168-byte keyline mirror: there the inline schedule measured 2-3 % faster on H100, while the 15-byte
+    // records gain from the side stream like the plain push; set_mirror drops the captured batches.)
+    const bool side = pl->resc_stream != nullptr && pl->mirror_on != 1;
     if (!pl->map_fused)
         if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
-                                           p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map)))
+                                           p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
+                                           side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
             return r;
     RB_TRACE(c->stream, 9);
     prof_mark(pl, ST_REG_EKF);
+    if (side) {   // gated by the map's own copy of do_map; writes the map's Kp / RKp and the record's, no FrameState
+        cudaStream_t main_stream = c->stream;
+        RB_CUDA(cudaEventRecord(pl->ev_rfork, main_stream));
+        RB_CUDA(cudaStreamWaitEvent(pl->resc_stream, pl->ev_rfork, 0));
+        c->stream = pl->resc_stream;
+        r = rb_rescale_enqueue(c, neu, RB_RHO_MAX, 1, 0, &neu->st->do_map, nav_slot);
+        c->stream = main_stream;
+        if (r) return r;
+        RB_CUDA(cudaEventRecord(pl->ev_rjoin, pl->resc_stream));
+        pl->resc_open = true;
+        RB_TRACE(c->stream, 5);
+        return RB_OK;
+    }
     rb_quantile_fold qf = {pl->q_fold ? p.QCutOffNumBins : 0, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, next->st};
     if ((r = rb_map_update_enqueue(c, neu, p.RegularizeThresh, pl->fs->V, p.ReshapeQAbsolute, p.LocationUncertainty,
                                    RB_RHO_MAX, 1, p.DoReScaling > 0 ? 1 : 0, pl->fs, p.MatchThreshold, old->st,
@@ -462,6 +511,7 @@ static int enqueue_batch(rb_pipeline *pl, int n, long long first_frame, bool wit
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
+    pl->resc_open = false;   // (a batch joins its last rescaling at its end; a failed enqueue must not leave a join behind)
     prof_mark(pl, ST_H2D);
     if (pl->und) r = rb_undistort_gray_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, n);   // rebvo_first_t.cpp:231 + RGB -> BW
     else r = rb_dog_gray(c, &pl->ws, n, pl->rgb_src_dev);
@@ -542,6 +592,7 @@ static int enqueue_batch(rb_pipeline *pl, int n, long long first_frame, bool wit
         }
         if (ov && i + 2 < n) RB_CUDA(cudaEventRecord(pl->ev_trk[i], main_stream));
     }
+    if ((r = resc_join(pl))) return r;   // the last frame's Kp / RKp are in its record before the nav copy
     if (pl->mirror_on) {   // the batch is complete when its last map has reached the host
         RB_CUDA(cudaEventRecord(pl->ev_mjoin, pl->mirror_stream));
         RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_mjoin, 0));

@@ -1752,7 +1752,10 @@ __global__ void __launch_bounds__(256) k_regularize_a_gate(KLSoA kl, MapState *s
     pdl_wait();
     pdl_launch();
     const bool en = fs->do_match && st->nmatch >= match_threshold;
-    if (blockIdx.x == 0 && threadIdx.x == 0) d_frame_post_match(fs, st, match_threshold);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        d_frame_post_match(fs, st, match_threshold);
+        st->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
+    }
     if (!en) return;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool did = i < st->kn ? d_reg_a(kl, i, r, s, set, thresh) : false;
@@ -1765,12 +1768,18 @@ __global__ void __launch_bounds__(256) k_regb_ekf(KLSoA kl, const MapState *st, 
                                                   const double *__restrict__ s,
                                                   const unsigned char *__restrict__ set,
                                                   const double *__restrict__ velp, double zf, double q_abs,
-                                                  double loc_unc, const int *enable, FrameState *pose_fs) {
+                                                  double loc_unc, const int *enable, FrameState *pose_fs,
+                                                  const MapState *ost, const LMState *lm, rb_nav *nav,
+                                                  const FrameArgs *fa) {
     pdl_wait();
     pdl_launch();
     // the frame's pose integration + matrix logarithms (one thread) beside the EKF instead of in the map-update
     // kernel's tail: V and R are final since the gate of the previous kernel.  The last block of the grid has no keylines.
-    if (pose_fs && blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) d_frame_pose(pose_fs);
+    // With nav, the whole nav record too (the rescaling runs on a side stream and only fills in its Kp / RKp).
+    if (pose_fs && blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+        if (nav) d_frame_finish(pose_fs, st, ost, lm->score, nav, fa, false);
+        else d_frame_pose(pose_fs);
+    }
     if (enable && !*enable) return;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= st->kn) return;
@@ -1788,12 +1797,14 @@ __global__ void __launch_bounds__(256) k_regb_ekf(KLSoA kl, const MapState *st, 
     d_ekf(kl, i, rho, s_rho, velp, zf, q_abs, loc_unc);
 }
 int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
-                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev) {
+                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
+                              const MapState *ost, rb_nav *nav, const FrameArgs *fa) {
     TrackState &t = m->ts_host;
     const int nb = rb_div_up(c->kcap, 256);
     RB_KLAUNCH(k_regularize_a_gate, nb, 256, 0, m->kl, m->st, t.reg_r, t.reg_s, t.reg_set, thresh, fs, match_threshold);
     RB_KLAUNCH(k_regb_ekf, nb, 256, 0, m->kl, (const MapState *)m->st, (const double *)t.reg_r, (const double *)t.reg_s,
-               (const unsigned char *)t.reg_set, vel_dev, c->zfm, q_abs, loc_unc, do_map_dev, fs);
+               (const unsigned char *)t.reg_set, vel_dev, c->zfm, q_abs, loc_unc, do_map_dev, fs, ost,
+               (const LMState *)&m->ts->lm, nav, fa);
     return RB_OK;
 }
 
@@ -1840,6 +1851,7 @@ struct MapUpdArgs {
     double q_min, q_max, q_perc;
     MapState *nst_next;
     int xchg;                // 1: st.async + mbarrier all-reduce inside the rescaling iterations, 0: barrier.cluster
+    rb_nav *kp_nav;          // pipeline, rescaling on the side stream: the record whose Kp / RKp it fills in (no fs)
 };
 
 __device__ __forceinline__ void mu_block_sum2(double &a, double &b, double (*sw)[2], int tid) {
@@ -2015,6 +2027,10 @@ __global__ void __cluster_dims__(MU_C, 1, 1) __launch_bounds__(MU_T) k_map_updat
             if (rank == 0 && tid == 0) {
                 st->Kp = Kp;
                 if (kn > 0) st->RKp = RKp;
+                if (a.kp_nav) {   // what d_frame_finish takes into the record after a rescaling
+                    a.kp_nav->Kp = st->Kp;
+                    a.kp_nav->RKp = st->RKp;
+                }
             }
         }
     }
@@ -2042,7 +2058,7 @@ __global__ void __cluster_dims__(MU_C, 1, 1) __launch_bounds__(MU_T) k_map_updat
         __syncthreads();
     }
     if (rank == 0 && tid == 0) {
-        if (a.fs && a.nav) d_frame_finish(a.fs, st, a.ost, a.lm->score, a.nav, a.fa);
+        if (a.fs && a.nav) d_frame_finish(a.fs, st, a.ost, a.lm->score, a.nav, a.fa, true);
         if (a.q_bins > 0) {
             const double range = a.q_max - a.q_min;
             double q = 1e3;
@@ -2059,7 +2075,7 @@ __global__ void __cluster_dims__(MU_C, 1, 1) __launch_bounds__(MU_T) k_map_updat
     }
 }
 
-static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a_in) {
+static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a_in, bool pdl) {
     MapUpdArgs a = a_in;
     a.xchg = c->mu_xchg ? 1 : 0;
     cudaLaunchConfig_t cfg = {};
@@ -2070,7 +2086,7 @@ static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a_in) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = c->pdl ? 1 : 0;
+    cfg.numAttrs = pdl ? 1 : 0;
     TrackState &t = m->ts_host;
     c->launches++;
     RB_CUDA(cudaLaunchKernelEx(&cfg, k_map_update, m->kl, m->st, t.reg_r, t.reg_s, t.reg_set, a));
@@ -2111,12 +2127,14 @@ int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double reg_thresh, const double 
         a.q_perc = qf->perc;
         a.nst_next = qf->nst_next;
     }
-    return launch_map_update(c, m, a);
+    return launch_map_update(c, m, a, c->pdl);
 }
 
-// EstimateReScalingOpt alone (stage-level API): the same kernel with only its last phase, hence the same bits
+// EstimateReScalingOpt alone (stage-level API, and the per-frame pipeline's side stream with kp_nav): the same kernel with
+// only its last phase, hence the same bits.  Launched without programmatic serialization: on the side stream it must not
+// become resident (16 SMs spinning in griddepcontrol.wait) while the tracker stream's kernels still run.
 int rb_rescale_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale,
-                       const int *enable_dev) {
+                       const int *enable_dev, rb_nav *kp_nav) {
     MapUpdArgs a;
     memset(&a, 0, sizeof(a));
     a.do_rescale = 1;
@@ -2124,7 +2142,8 @@ int rb_rescale_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int matc
     a.s_rho_min = s_rho_min;
     a.mnm = match_num_min;
     a.enable = enable_dev;
-    return launch_map_update(c, m, a);
+    a.kp_nav = kp_nav;
+    return launch_map_update(c, m, a, false);
 }
 
 // per-device opt-in of the mapper's 16-CTA cluster kernels (called from rb_minimizer_cluster_setup at context creation)

@@ -67,8 +67,10 @@ int rb_directed_matching_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMat
                                  double loc_uncertainty, const int *enable_dev);
 int rb_regularize_enqueue(rb_ctx *c, rb_map *m, double thresh, const int *enable_dev);
 struct rb_nav;
+// with nav: the frame's nav record is written beside the EKF (except Kp / RKp of a mapped frame: rb_rescale_enqueue)
 int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
-                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev);
+                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
+                              const MapState *ost = nullptr, rb_nav *nav = nullptr, const FrameArgs *fa = nullptr);
 int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double reg_thresh, const double *vel_dev, double q_abs,
                           double loc_unc, double s_rho_min, unsigned int match_num_min, int re_escale,
                           FrameState *fs, int match_threshold, const MapState *ost, rb_nav *nav,
@@ -76,5 +78,5 @@ int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double reg_thresh, const double 
 int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, double loc_unc,
                    const int *enable_dev);
 int rb_rescale_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale,
-                       const int *enable_dev);
+                       const int *enable_dev, rb_nav *kp_nav = nullptr);
 int rb_read_map_state(rb_map *m, MapState *host);
