@@ -158,8 +158,7 @@ struct TrackState {
     struct MinCtl *ctl;   // request slots / sequence base of the persistent minimiser kernel
     unsigned long long *ll;   // its inter-cluster slots
     // scratch for FordwardMatch / Regularize_1_iter
-    unsigned long long *fm_best;
-    int *fm_idx;
+    struct FmBest *fm_best;   // per new keyline: the old keyline that wins it (see d_fm_offer)
     double *reg_r, *reg_s;
     unsigned char *reg_set;
 };

@@ -534,7 +534,7 @@ template <int XCHG>   // 1: st.async + mbarrier complete_tx; 0: plain DSMEM stor
 __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
     k_minimizer_cluster(KLSoA old, const MapState *__restrict__ old_st, const unsigned long long *__restrict__ field,
                         const float4 *__restrict__ fpack, MapState *f_st, LMState *lm_out, int *abort_out, CamC cam,
-                        McPlan plan, MinSetup su, FrameState *post_fs, int kpc_cap, ResPtrs gres,
+                        McPlan plan, MinSetup su, FrameState *post_fs, FmBest *fm_best, int kpc_cap, ResPtrs gres,
                         unsigned long long *ll, MinCtl *ctl) {
     MC_STAMP(15, 0);
     // early_operands (set by the per-frame pipeline, whose previous kernel on this stream -- EstimateQuantile -- writes no
@@ -851,7 +851,15 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
                 }
                 MC_STAMP(e, 7);
             }
-        } else if (wid == 3 && !last) {
+        } else if (last) {
+            // FordwardMatch's arg-max over this CTA's keylines, whose m_id_f the pass above wrote: the CAS round trips
+            // run on the warps that are idle during the last exchange and LM step, not between the pass and the exchange
+            if (fm_best) {   // (two keylines per thread and step: loads and CAS round trips in flight together)
+                const int nkn = f_st->kn, st = MC_T - 96;
+                for (int li = tid - 96; li < v.cnt; li += 2 * st)
+                    d_fm_argmax_two(old, v.base + li, li + st < v.cnt ? v.base + li + st : -1, nkn, fm_best);
+            }
+        } else if (wid == 3) {
             asm volatile("bar.sync 1, 64;" ::: "memory");
             if (lane == 0) mc_req_RM(sm, 0, sm.lm);
         } else if (wid == 4 && next_two) {
@@ -862,19 +870,21 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         if (sm.abort) break;
     }
     // ---- epilogue ------------------------------------------------------------------------------------------------
-    if (!sm.abort) lm_finalize_cov(sm.lm, tid);   // the six columns of Cholesky<6>(JtJ).get_inverse() side by side
-    __syncthreads();
     if (sm.abort && tid == 0) {
         *abort_out = 1;
         for (int k = 0; k < 3; k++) sm.lm.Vel[k] = sm.lm.W0[k] = __longlong_as_double(0x7FF8000000000000ll);
     }
+    __syncthreads();
+    if (!sm.abort) lm_finalize_cov(sm.lm, tid);   // the six columns of Cholesky<6>(JtJ).get_inverse() side by side
+    // the per-frame pipeline's stage after the minimiser, folded in: what needs only V / W beside the covariance
+    if (first_cta && tid == 32 && post_fs) d_frame_post_min_pose(post_fs, sm.lm);
     __syncthreads();
     if (first_cta) {
         if (tid == 0 && G > 1) ctl->gen = seq0 + MIN_MAX_EVALS + 1u;   // the next minimisation gets fresh sequence numbers
         const double *src = reinterpret_cast<const double *>(&sm.lm);
         double *dst = reinterpret_cast<double *>(lm_out);
         for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += MC_T) dst[k] = src[k];
-        if (tid == 0 && post_fs) d_frame_post_min(post_fs, sm.lm);   // folded one-thread stage of the per-frame pipeline
+        if (tid == 0 && post_fs) d_frame_post_min_cov(post_fs, sm.lm);
     }
     MC_STAMP(15, 3);
     mc_cluster_sync();   // no CTA exits while a peer may still send to it

@@ -55,11 +55,11 @@ struct rb_pipeline {
     bool overlap;
     bool q_fold;          // EstimateQuantile + loop-body start of the next frame folded into this frame's map-update kernel
     int ss_sub;           // frames per scale-space sub-batch built on the detector stream (env REBVO_B200_SS_SUB, 0 = whole batch)
-    bool fm_fused;        // FordwardMatch + rotate_keylines as one cluster kernel (env REBVO_B200_FM_FUSED)
     bool map_fused;       // gate + Regularize_1_iter + EKF inside the map-update cluster kernel (env REBVO_B200_MAP_FUSED)
     // rescaling stream: with DoReScaling=0 a frame's EstimateReScalingOpt changes no keyline and only fills in its nav record,
     // so it runs here (lowest priority) instead of at the end of the frame's tracker chain; the tracker stream joins it
-    // before the next frame's rotate_keylines, the first kernel after the fork that writes the map's rho / s_rho
+    // before the next frame's FordwardMatch apply / rotate_keylines kernel, the first kernel after the fork that writes the
+    // map's rho / s_rho
     cudaStream_t resc_stream;     // nullptr: the rescaling stays in the frame's map-update kernel on the tracker stream
     cudaEvent_t ev_rfork, ev_rjoin;
     bool resc_open;               // a rescaling was forked and not joined yet
@@ -248,8 +248,6 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
     {
         const char *mf = getenv("REBVO_B200_MAP_FUSED");
         pl->map_fused = mf ? atoi(mf) != 0 : false;   // off by default: the wide kernels under PDL serve
-        const char *ff = getenv("REBVO_B200_FM_FUSED");
-        pl->fm_fused = ff ? atoi(ff) != 0 : false;
         const char *ov = getenv("REBVO_B200_OVERLAP");
         pl->overlap = !(ov && ov[0] == '0') && !pl->prof_on;
         // (off by default: the launch it saves is already hidden by programmatic dependent launch, and it costs the
@@ -419,9 +417,13 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
         if ((r = rb_quantile_enqueue(c, old, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, p.QCutOffNumBins, pl->fs,
                                      &fa->frame_count, neu->st)))
             return r;
-    // :177  new_buf.gt->build_field(...) only needs the new edge map: enqueue_batch runs it on the detector stream
-    if (!pl->overlap)
+    // :177  new_buf.gt->build_field(...) only needs the new edge map: enqueue_batch runs it on the detector stream, and
+    // clears the new map's FordwardMatch arg-max scratch there, which the minimiser's last evaluation already fills
+    // (the clear first: the minimiser stages its operands while the kernel before it runs, and build_field is the longer one)
+    if (!pl->overlap) {
+        if ((r = rb_forward_match_init_enqueue(c, neu))) return r;
         if ((r = rb_build_field_enqueue(c, neu, p.SearchRange, 0.f, true))) return r;
+    }
     prof_mark(pl, ST_FIELD);
     // :346  Minimizer_RV<double>(V,W,P_V,P_W,*old_buf.ef,...) ; :346-398 outputs / NaN guard folded into its last block
     rb_minimizer_args a;
@@ -438,29 +440,21 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
     // on this stream: the minimiser may stage the old map's operands while that kernel is still running)
     // (with q_fold the previous kernel is the old map's update itself: no early staging)
     c->min_early = !pl->q_fold && (getenv("REBVO_B200_MIN_EARLY") ? atoi(getenv("REBVO_B200_MIN_EARLY")) != 0 : true);
-    // the one-thread stage after the minimiser rides in a spare thread of the first FordwardMatch kernel (post_in_fm) rather
-    // than in the minimiser's tail; with the fused FordwardMatch + rotate kernel it stays in the minimiser
-    static const bool post_fm_env = getenv("REBVO_B200_POST_IN_FM") ? atoi(getenv("REBVO_B200_POST_IN_FM")) != 0 : true;
-    const bool post_in_fm = post_fm_env && !(pl->fm_fused && pl->overlap);
-    r = rb_minimizer_enqueue(c, neu, old, pl->fs->VW, &a, 0.0, true, 0, true, post_in_fm ? nullptr : pl->fs, &folded);
+    // (folded: the one-thread stage after the minimiser and FordwardMatch's arg-max ran in its epilogue / last evaluation)
+    r = rb_minimizer_enqueue(c, neu, old, pl->fs->VW, &a, 0.0, true, 0, true, pl->fs, &folded);
     c->min_early = false;
     if (r) return r;
     RB_TRACE(c->stream, 3);
     prof_mark(pl, ST_MINIM);
-    if (!folded && !post_in_fm) {
+    if (!folded) {
         k_frame_post_min<<<1, 1, 0, c->stream>>>(pl->fs, neu->ts);
         RB_LAUNCH_CHECK();
+        if ((r = rb_forward_match_argmax_enqueue(c, old, neu))) return r;
     }
-    // :354  FordwardMatch ; :369 rotate_keylines(R0).  Until the rotation, this frame only reads the old map's rho / s_rho
-    // (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may run until then.
-    if (pl->fm_fused && pl->overlap) {   // (the arg-max scratch of the new map was cleared on the detector stream)
-        if ((r = resc_join(pl))) return r;
-        if ((r = rb_forward_match_rotate_enqueue(c, old, neu, pl->fs->R0))) return r;
-    } else {
-        if ((r = rb_forward_match_enqueue(c, old, neu, pl->overlap, pl->fs))) return r;
-        if ((r = resc_join(pl))) return r;
-        if ((r = rb_rotate_enqueue(c, old, pl->fs->R0))) return r;
-    }
+    // :354  FordwardMatch ; :369 rotate_keylines(R0) in one kernel.  Until then, this frame only reads the old map's rho /
+    // s_rho (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may run until then.
+    if ((r = resc_join(pl))) return r;
+    if ((r = rb_forward_match_apply_enqueue(c, old, neu, pl->fs->R0))) return r;
     RB_TRACE(c->stream, 11);
     prof_mark(pl, ST_FWD_ROT);
     // :410  directed_matching(V,P_V,R,old_buf.ef,...)

@@ -21,6 +21,13 @@ struct MinCtl {
     int abort;                     // an exchange timed out (results are NaN); read and cleared by rb_minimizer_check_abort
 };
 
+// FordwardMatch's arg-max record of one new keyline: the lexicographic maximum of (dbl_key(rho), index) over the old
+// keylines that matched it; {0, -1} = none (written by rb_forward_match_init_enqueue)
+struct __align__(16) FmBest {
+    unsigned long long key;
+    long long idx;
+};
+
 int rb_minimizer_cluster_setup(rb_ctx *c);
 // reads (and clears) the abort flag of a map's minimiser; returns RB_ERR_CUDA with a message when it was set.  Synchronises.
 int rb_minimizer_check_abort(rb_ctx *c, rb_map *fmap);
@@ -38,6 +45,8 @@ struct rb_minimizer_args {
 // (V then W); max_s_rho is read from old->st->s_rho_q when s_rho_from_state, else from the argument.
 // The optional FrameState / FrameArgs / rb_nav arguments below belong to the per-frame pipeline (frame.cuh): when given,
 // the one-thread glue stage next to the kernel runs inside it instead of as its own launch.
+// rb_minimizer_enqueue with post_fs: when *post_folded comes back set, the stage after the minimiser (d_frame_post_min)
+// and FordwardMatch's arg-max of old into fmap (rb_forward_match_argmax_enqueue; scratch cleared before) ran inside it.
 struct FrameState;
 struct FrameArgs;
 int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_dev,
@@ -53,10 +62,13 @@ struct rb_quantile_fold {
     MapState *nst_next;
 };
 int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool min_mod_from_state);
+// FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu).
+// With R_dev the apply kernel then runs rotate_keylines(R) on the old map; rb_forward_match_enqueue is the whole stage.
 int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu);
-int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu, bool scratch_ready = false, FrameState *post_fs = nullptr);
+int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
+int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu, const double *R_dev);
+int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev);
-int rb_forward_match_rotate_enqueue(rb_ctx *c, rb_map *old, rb_map *neu, const double *R_dev);   // scratch cleared before
 struct DMatchArgs {       // device-resident arguments of directed_matching (after the back-rotation)
     double Vel[3];        // BackRot*Vel
     double RVel[9];       // BackRot*RVel*BackRot^T
