@@ -141,6 +141,9 @@ int rb_map_clone(const rb_map *src, rb_map **out);
 
 /* Image<float>::ConvertRGB2BW (image.h:197-203) after the H2D copy of the RGB24 frame */
 int rb_map_upload_rgb(rb_map *m, const uint8_t *rgb);
+/* the same for an 8-bit grayscale frame (w*h bytes): it stands for the RGB24 frame (m, m, m), so the gray plane
+ * (rb_map_get_plane 5) is float(3*v), bit-identical to rb_map_upload_rgb's on the replicated frame */
+int rb_map_upload_mono(rb_map *m, const uint8_t *mono);
 int rb_map_upload_gray(rb_map *m, const float *gray);
 /* sspace::build (sspace.cpp:52-60): bit-exact float32 integral-image DoG */
 int rb_map_dog_build(rb_map *m);
@@ -243,6 +246,14 @@ int rb_pipeline_push(rb_pipeline *pl, const uint8_t *rgb, const double *ts, int 
 /* same with frames already resident in device memory (device pointer) */
 int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *ts, int n,
                          rb_nav *nav_out);
+/* Mono input (8-bit grayscale cameras such as EuRoC cam0): n frames of w*h bytes, row-major, no stride.  A mono frame m is
+ * defined to be the RGB24 frame (m, m, m), which is what the reference's ROS nodelet (MONO8) and DataSetCam build from a gray
+ * image; the records, maps and mirror are bit-identical to rb_pipeline_push of the replicated frames, with and without
+ * undistortion, and in IMU mode.  The host copy and the device staging are a third of the RGB24 ones.  A pipeline may
+ * alternate formats from push to push.  Arguments are checked like rb_pipeline_push's; the device variant also returns
+ * RB_ERR_ARG for a pointer that is not 4-byte aligned (the kernels read 32-bit words), before anything is enqueued. */
+int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out);
+int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n, rb_nav *nav_out);
 /* REBVO::Reset (rebvo_second_t.cpp:609-620) */
 int rb_pipeline_reset(rb_pipeline *pl);
 /* newest / previous edge map of the ring (valid until the next push) */
@@ -278,7 +289,8 @@ int rb_pipeline_event_elapsed_between(rb_pipeline *pa, int a, rb_pipeline *pb, i
 int rb_pipeline_event_elapsed(rb_pipeline *pl, int a, int b, float *ms);
 /* Measurement hook: re-run ONE scale-space pass over the pipeline's batched workspace `iters` times and
  * return the mean CUDA-event duration per launch.  pass_id: 0 row pass (plain), 1 row pass with box
- * average (2*nimg images), 2 column pass (2*nimg images), 3 last box + DoG, 4 rgb->gray.
+ * average (2*nimg images), 2 column pass (2*nimg images), 3 last box + DoG, 4 rgb->gray, 5 undistortion + rgb->gray
+ * (needs rb_pipeline_set_undistort), 6 mono->gray, 7 undistortion + mono->gray (needs rb_pipeline_set_undistort).
  * bytes_per_launch receives the algorithmic bytes of one launch (DESIGN.md section 4). */
 int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, int iters, float *ms_per_launch,
                            double *bytes_per_launch);

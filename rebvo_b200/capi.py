@@ -76,13 +76,15 @@ KEYLINE = np.dtype({
 
 # every symbol include/rebvo_b200.h declares
 SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "rb_ctx_box_plan",
-           "rb_ctx_launch_count", "rb_map_create", "rb_map_destroy", "rb_map_clone", "rb_map_upload_rgb", "rb_map_upload_gray",
+           "rb_ctx_launch_count", "rb_map_create", "rb_map_destroy", "rb_map_clone", "rb_map_upload_rgb", "rb_map_upload_mono",
+           "rb_map_upload_gray",
            "rb_map_dog_build", "rb_map_get_plane", "rb_map_detect", "rb_map_detect_ss", "rb_map_reestimate_thresh", "rb_map_knum",
            "rb_map_sync_host_keylines", "rb_map_load_keylines", "rb_map_get_mask", "rb_map_quantile",
            "rb_map_build_field", "rb_map_get_field", "rb_try_vel_rot", "rb_minimizer_rv", "rb_forward_match",
            "rb_map_rotate_keylines", "rb_directed_matching", "rb_map_regularize", "rb_map_ekf_update",
            "rb_map_rescale_opt", "rb_map_set_frame_count", "rb_pipeline_create", "rb_pipeline_destroy",
-           "rb_pipeline_last_error", "rb_pipeline_push", "rb_pipeline_push_dev", "rb_pipeline_reset",
+           "rb_pipeline_last_error", "rb_pipeline_push", "rb_pipeline_push_dev", "rb_pipeline_push_mono",
+           "rb_pipeline_push_mono_dev", "rb_pipeline_reset",
            "rb_pipeline_map", "rb_pipeline_launch_count", "rb_pipeline_stage_ms", "rb_pipeline_stream",
            "rb_pipeline_event_record", "rb_pipeline_event_elapsed", "rb_pipeline_event_elapsed_between", "rb_pipeline_bench_pass",
            "rb_pipeline_set_imu", "rb_pipeline_set_mirror", "rb_pipeline_mirror", "rb_pipeline_set_undistort",
@@ -250,6 +252,13 @@ class Map:
         rgb = np.ascontiguousarray(rgb, np.uint8)
         assert rgb.size == self.w * self.h * 3
         self.ctx.check(self.L.rb_map_upload_rgb(self.h_, _p(rgb)))
+        self.ctx.check(self.L.rb_ctx_sync(self.ctx.h_))
+
+    def upload_mono(self, img):
+        """8-bit grayscale frame (h, w): the RGB24 frame (img, img, img) as far as the gray plane is concerned."""
+        img = np.ascontiguousarray(img, np.uint8)
+        assert img.size == self.w * self.h
+        self.ctx.check(self.L.rb_map_upload_mono(self.h_, _p(img)))
         self.ctx.check(self.L.rb_ctx_sync(self.ctx.h_))
 
     def upload_gray(self, g):
@@ -439,6 +448,27 @@ class Pipeline:
         else:
             ptr = C.c_void_p(int(rgb))
         self.check(self.L.rb_pipeline_push(self.h_, ptr, _p(ts), n, _p(nav)))
+        return nav
+
+    def push_mono(self, frames, ts):
+        """frames: (n,h,w) uint8 host array of 8-bit grayscale frames (or a raw host pointer int with n given by len(ts)).
+        Same records as push() of the frames replicated into three channels."""
+        ts = np.ascontiguousarray(ts, np.float64)
+        n = len(ts)
+        nav = np.zeros(n, NAV)
+        if isinstance(frames, np.ndarray):
+            frames = np.ascontiguousarray(frames, np.uint8)
+            ptr = _p(frames)
+        else:
+            ptr = C.c_void_p(int(frames))
+        self.check(self.L.rb_pipeline_push_mono(self.h_, ptr, _p(ts), n, _p(nav)))
+        return nav
+
+    def push_mono_dev(self, dev_ptr, ts):
+        """Mono frames already in device memory (4-byte aligned pointer), read in place."""
+        ts = np.ascontiguousarray(ts, np.float64)
+        nav = np.zeros(len(ts), NAV)
+        self.check(self.L.rb_pipeline_push_mono_dev(self.h_, C.c_void_p(int(dev_ptr)), _p(ts), len(ts), _p(nav)))
         return nav
 
     def set_imu(self, samples, imu_params=None):

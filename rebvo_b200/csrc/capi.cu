@@ -445,6 +445,15 @@ extern "C" int rb_map_upload_rgb(rb_map *m, const uint8_t *rgb) {
     return rb_dog_gray(c, &m->ws, 1);
 }
 
+extern "C" int rb_map_upload_mono(rb_map *m, const uint8_t *mono) {
+    if (!m || !mono) return RB_ERR_ARG;
+    RB_ENTER(m->c);
+    rb_ctx *c = m->c;
+    if (!m->owns_ws) return RB_ERR_STATE;
+    RB_CUDA(cudaMemcpyAsync(m->ws.rgb, mono, (size_t)c->N, cudaMemcpyHostToDevice, c->stream));
+    return rb_dog_gray_mono(c, &m->ws, 1);
+}
+
 extern "C" int rb_map_upload_gray(rb_map *m, const float *gray) {
     if (!m) return RB_ERR_ARG;
     RB_ENTER(m->c);

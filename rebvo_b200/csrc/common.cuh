@@ -58,7 +58,7 @@ struct BoxPlan {
 
 struct DogWS {           // batched scale-space workspace, B images of N floats per plane
     int B;
-    uint8_t *rgb;        // B * 3N
+    uint8_t *rgb;        // B * 3N    host-input staging: B RGB24 frames, or B mono frames in its first B * N bytes
     float *gray;         // B * N
     float *S;            // 2B * N   row-scanned plane (per filter)
     float *I0;           // B * N    integral of the input (shared by both filters)
@@ -252,6 +252,7 @@ static inline cudaError_t rb_klaunch(bool pdl, void (*kernel)(KArgs...), dim3 gr
 int rb_dogws_alloc(rb_ctx *c, DogWS *ws, int B);
 void rb_dogws_free(DogWS *ws);
 int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // rgb -> gray
+int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // mono -> gray
 int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg);          // gray -> img0, dog
 int rb_dog_build_range(rb_ctx *c, DogWS *ws, int f0, int m);     // the same for the images [f0, f0 + m)
 int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img);            // Img(1), dx, dy into ws->aux

@@ -70,6 +70,24 @@ __global__ void __launch_bounds__(256) k_rgb2gray(const uint32_t *__restrict__ r
     gray[i] = o;
 }
 
+// The same for 8-bit grayscale input (rb_pipeline_push_mono): a mono frame m stands for the RGB24 frame (m, m, m), so a
+// pixel's b+g+r is the integer 3v and the plane is bit-identical to k_rgb2gray's on the replicated frame.  4 pixels per
+// thread: one 32-bit load, one float4 store; the source is read through src_pp like k_rgb2gray's.
+__global__ void __launch_bounds__(256) k_mono2gray(const uint32_t *__restrict__ mono_fixed,
+                                                   const uint32_t *const *__restrict__ src_pp,
+                                                   float4 *__restrict__ gray, size_t n4) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const uint32_t *__restrict__ mono = src_pp ? *src_pp : mono_fixed;
+    const uint32_t a = mono[i];
+    float4 o;
+    o.x = (float)(3u * (a & 0xff));
+    o.y = (float)(3u * ((a >> 8) & 0xff));
+    o.z = (float)(3u * ((a >> 16) & 0xff));
+    o.w = (float)(3u * (a >> 24));
+    gray[i] = o;
+}
+
 // Row pass: warp per band of 32 rows of one image.  Tiles of 32x32 are produced coalesced (optionally
 // through box_avg of the previous integral image), transposed through shared memory so that each lane
 // owns one row, scanned sequentially (the reference's add order), and stored coalesced.
@@ -502,6 +520,16 @@ int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
     k_rgb2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
                                                                    (const uint32_t *const *)src_pp,
                                                                    (float4 *)ws->gray, n4);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
+// mono -> gray: nimg frames of N bytes (the source must be 4-byte aligned; N is a multiple of 4)
+int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
+    const size_t n4 = (size_t)nimg * c->N / 4;
+    k_mono2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
+                                                                    (const uint32_t *const *)src_pp,
+                                                                    (float4 *)ws->gray, n4);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
@@ -1060,6 +1088,9 @@ int rb_dog_single_pass(rb_ctx *c, DogWS *ws, int pass_id, int nimg, double *byte
         case 4:
             *bytes = 7.0 * N * nimg;       // read RGB 3N, write gray 4N
             return rb_dog_gray(c, ws, nimg);
+        case 6:
+            *bytes = 5.0 * N * nimg;       // read mono N, write gray 4N
+            return rb_dog_gray_mono(c, ws, nimg);
         default:
             return RB_ERR_ARG;
     }

@@ -266,19 +266,18 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
 }
 
 // a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking
-static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, bool on_device, const double *ts, int n, rb_nav *nav_out) {
+static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bool on_device, const double *ts, int n,
+                    rb_nav *nav_out) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
-    const size_t fbytes = (size_t)3 * c->N;
+    const size_t fbytes = frame_bytes(c, fmt);
     if (!on_device)
         RB_CUDA(cudaMemcpyAsync(pl->ws.rgb, rgb, (size_t)n * fbytes, cudaMemcpyHostToDevice, c->stream));
     const void *src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
     RB_CUDA(cudaMemcpyAsync(pl->rgb_src_dev, &src, sizeof(void *), cudaMemcpyHostToDevice, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));   // (&src is a stack variable)
-    if (pl->und) r = rb_undistort_gray_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, n);
-    else r = rb_dog_gray(c, &pl->ws, n, pl->rgb_src_dev);
-    if (r) return r;
+    if ((r = gray_pass(pl, fmt, n))) return r;
     if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
     for (int i = 0; i < n; i++) {
         const long long fr = pl->n_pushed + i;

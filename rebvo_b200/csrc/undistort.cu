@@ -139,6 +139,62 @@ int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float 
     return RB_OK;
 }
 
+// Mono twin of ug_pixel (rb_pipeline_push_mono): a mono frame m stands for the RGB24 frame (m, m, m), whose three channel
+// sums are all s = sum_k iw_k * m_k, so the RGB pass's (u8)(r>>16) + (u8)(g>>16) + (u8)(b>>16) is 3 * (u8)(s>>16), with the
+// same truncation.  One byte per tap.  The two taps of a row are adjacent bytes almost everywhere: one aligned word, plus
+// the next one only when the pair straddles a word boundary, and one funnel shift.  The source is 4-byte aligned (a frame
+// is N bytes with N % 4 == 0, and rb_pipeline_push_mono_dev refuses unaligned buffers).
+__device__ __forceinline__ float ug_pixel_mono(const uint8_t *__restrict__ src, const int4 ix, const int4 w) {
+    int s;
+    if (ix.y == ix.x + 1 && ix.w == ix.z + 1) {
+        const unsigned int *W = reinterpret_cast<const unsigned int *>(src);
+        s = 0;
+#pragma unroll
+        for (int row = 0; row < 2; row++) {
+            const int ofs = row ? ix.z : ix.x, wi = ofs >> 2;
+            // (ofs % 4 == 3: byte ofs + 1 <= N - 1 is in the next word, which therefore exists)
+            const unsigned int w0 = __ldg(W + wi), w1 = (ofs & 3) == 3 ? __ldg(W + wi + 1) : w0;
+            const unsigned int v = __funnelshift_r(w0, w1, (ofs & 3) * 8);   // bytes ofs, ofs + 1 in the low half
+            s += (row ? w.z : w.x) * (int)(v & 0xffu) + (row ? w.w : w.y) * (int)((v >> 8) & 0xffu);
+        }
+    } else {
+        s = w.x * (int)__ldg(src + ix.x) + w.y * (int)__ldg(src + ix.y) + w.z * (int)__ldg(src + ix.z) +
+            w.w * (int)__ldg(src + ix.w);
+    }
+    return (float)(3u * (unsigned int)(uint8_t)(s >> 16));
+}
+template <int IMGS>
+__global__ void __launch_bounds__(256) k_undistort_gray_mono(const uint8_t *const *__restrict__ src_pp,
+                                                             float *__restrict__ gray, const int4 *__restrict__ inx,
+                                                             const int4 *__restrict__ iw, int N, int nimg) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int img0 = blockIdx.y * IMGS;
+    if (i >= N) return;
+    const int4 ix = inx[i], w = iw[i];
+    const uint8_t *src = *src_pp + (size_t)img0 * N;
+    float v[IMGS];
+#pragma unroll
+    for (int k = 0; k < IMGS; k++) v[k] = img0 + k < nimg ? ug_pixel_mono(src + (size_t)k * N, ix, w) : 0.f;
+#pragma unroll
+    for (int k = 0; k < IMGS; k++)
+        if (img0 + k < nimg) gray[(size_t)(img0 + k) * N + i] = v[k];
+}
+int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg) {
+    rb_ctx *c = u->c;
+    static const int imgs_env = getenv("REBVO_B200_UG_IMGS") ? atoi(getenv("REBVO_B200_UG_IMGS")) : 4;
+    const int imgs = nimg >= 4 ? imgs_env : 1;
+#define UGM_LAUNCH(K)                                                                                              \
+    k_undistort_gray_mono<K><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(              \
+        (const uint8_t *const *)src_pp, gray, u->inx, u->iw, c->N, nimg)
+    if (imgs >= 8) UGM_LAUNCH(8);
+    else if (imgs >= 4) UGM_LAUNCH(4);
+    else if (imgs >= 2) UGM_LAUNCH(2);
+    else UGM_LAUNCH(1);
+#undef UGM_LAUNCH
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
 static inline bool inx_valid_f(float fx, float fy, int w, int h) {
     // Image::isInxValid takes `const uint&`: the float is converted to unsigned (x86-64: through a 64-bit
     // truncation, so negatives wrap to huge values and fail the upper bound)
