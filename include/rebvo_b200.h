@@ -159,6 +159,9 @@ int rb_map_detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p, double *t
 /* edge_finder::reEstimateThresh (edge_finder.cpp:373-405) */
 int rb_map_reestimate_thresh(rb_map *m, int knum, int nbins, float *out_thresh);
 int rb_map_knum(rb_map *m, int *kn);
+/* the matching counters of the frame that built this map: out = {fwd_match, nmatch, reg_num} (FordwardMatch winners,
+ * directed_matching hits, keylines Regularize_1_iter smoothed) */
+int rb_map_counters(rb_map *m, int out[3]);
 /* AoS mirror for host consumers (callback / net packer): kn records of 168 bytes */
 int rb_map_sync_host_keylines(rb_map *m, rb_keyline *dst, int capacity, int *kn);
 /* test / checkpoint path: load an edge map (keylines + mask) produced elsewhere */

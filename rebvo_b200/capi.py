@@ -79,6 +79,7 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_ctx_launch_count", "rb_map_create", "rb_map_destroy", "rb_map_clone", "rb_map_upload_rgb", "rb_map_upload_mono",
            "rb_map_upload_gray",
            "rb_map_dog_build", "rb_map_get_plane", "rb_map_detect", "rb_map_detect_ss", "rb_map_reestimate_thresh", "rb_map_knum",
+           "rb_map_counters",
            "rb_map_sync_host_keylines", "rb_map_load_keylines", "rb_map_get_mask", "rb_map_quantile",
            "rb_map_build_field", "rb_map_get_field", "rb_try_vel_rot", "rb_minimizer_rv", "rb_forward_match",
            "rb_map_rotate_keylines", "rb_directed_matching", "rb_map_regularize", "rb_map_ekf_update",
@@ -289,6 +290,12 @@ class Map:
         k = C.c_int(0)
         self.ctx.check(self.L.rb_map_knum(self.h_, C.byref(k)))
         return k.value
+
+    def counters(self):
+        """(fwd_match, nmatch, reg_num) of the frame that built this map"""
+        out = (C.c_int * 3)()
+        self.ctx.check(self.L.rb_map_counters(self.h_, out))
+        return tuple(out)
 
     def keylines(self):
         kn = self.knum()

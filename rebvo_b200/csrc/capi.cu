@@ -548,6 +548,18 @@ extern "C" int rb_map_knum(rb_map *m, int *kn) {
     return RB_OK;
 }
 
+extern "C" int rb_map_counters(rb_map *m, int out[3]) {
+    if (!m || !out) return RB_ERR_ARG;
+    RB_ENTER(m->c);
+    MapState s;
+    int r = read_state(m, &s);
+    if (r) return r;
+    out[0] = s.fwd_match;
+    out[1] = s.nmatch;
+    out[2] = s.reg_num;
+    return RB_OK;
+}
+
 /* which scale-space kernels this map's workspace dispatches to (after the first rb_map_dog_build): bit 0 = TMA row passes,
  * bit 1 = TMA last box + DoG; 0 before the workspace exists */
 extern "C" int rb_map_scale_space_path(const rb_map *m) {

@@ -540,10 +540,10 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
     // early_operands (set by the per-frame pipeline, whose previous kernel on this stream -- EstimateQuantile -- writes no
     // keyline array): the old map's operands are staged into shared memory BEFORE waiting for that kernel, i.e. while it runs
     const bool early = su.early_operands != 0 && su.a.match_num_thresh <= 255u;
-    if (!early) {
-        pdl_wait();
-        pdl_launch();
-    }
+    // (the dependents are released at the start of the last round, below: the grid after this kernel -- k_match of the
+    // per-frame pipeline -- then becomes resident a round before it may start, instead of occupying the SMs this kernel
+    // leaves free, where the detector stream runs the next frame, for the whole minimisation)
+    if (!early) pdl_wait();
     MC_STAMP(15, 1);
     extern __shared__ __align__(16) unsigned char mc_dyn[];
     __shared__ McSmem sm;
@@ -620,7 +620,6 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
     }
     if (early) {   // now the quantile and the frame counter of the previous kernel are needed
         pdl_wait();
-        pdl_launch();
         tc.s_rho_min = su.s_rho_from_state ? old_st->s_rho_q : su.max_s_rho;
         const unsigned int fc = su.fc_from_state ? f_st->frame_count : su.frame_count;
         tc.mnt = su.a.match_num_thresh < fc ? su.a.match_num_thresh : fc;   // (<= 255)
@@ -672,6 +671,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         const bool next_two = !last && plan.sa[e + 1] != STEP_NONE;
         const int res_out_p[2] = {sm.req_res[0][1], sm.req_res[1][1]};   // (warp 0 / 1 rewrite req_res for the next round)
         MC_STAMP(e, 0);
+        if (last) pdl_launch();
         // ---- keylines ---------------------------------------------------------------------------------------
         if (RW) mc_eval_pose<true, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
         else if (PJ) mc_eval_pose<false, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);

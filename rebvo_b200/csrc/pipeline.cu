@@ -56,10 +56,14 @@ struct rb_pipeline {
     bool q_fold;          // EstimateQuantile + loop-body start of the next frame folded into this frame's map-update kernel
     int ss_sub;           // frames per scale-space sub-batch built on the detector stream (env REBVO_B200_SS_SUB, 0 = whole batch)
     bool map_fused;       // gate + Regularize_1_iter + EKF inside the map-update cluster kernel (env REBVO_B200_MAP_FUSED)
+    // FordwardMatch's apply + directed_matching in k_match, then gate + Regularize_1_iter + EKF + rotate_keylines in
+    // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the four-kernel chain).  Not with map_fused, whose kernel reads the new map's
+    // rho after matching, which k_match leaves in the regularisation scratch.
+    bool map_chain;
     // rescaling stream: with DoReScaling=0 a frame's EstimateReScalingOpt changes no keyline and only fills in its nav record,
     // so it runs here (lowest priority) instead of at the end of the frame's tracker chain; the tracker stream joins it
-    // before the next frame's FordwardMatch apply / rotate_keylines kernel, the first kernel after the fork that writes the
-    // map's rho / s_rho
+    // before the next frame's first kernel after the minimiser (k_match, or k_fm_apply_rotate in the four-kernel chain,
+    // which writes the map's rho / s_rho)
     cudaStream_t resc_stream;     // nullptr: the rescaling stays in the frame's map-update kernel on the tracker stream
     cudaEvent_t ev_rfork, ev_rjoin;
     bool resc_open;               // a rescaling was forked and not joined yet
@@ -273,6 +277,8 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
     {
         const char *mf = getenv("REBVO_B200_MAP_FUSED");
         pl->map_fused = mf ? atoi(mf) != 0 : false;   // off by default: the wide kernels under PDL serve
+        const char *mc = getenv("REBVO_B200_MAP_CHAIN");
+        pl->map_chain = !(mc && atoi(mc) == 0) && !pl->map_fused;
         const char *ov = getenv("REBVO_B200_OVERLAP");
         pl->overlap = !(ov && ov[0] == '0') && !pl->prof_on;
         // (off by default: the launch it saves is already hidden by programmatic dependent launch, and it costs the
@@ -476,29 +482,51 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
         RB_LAUNCH_CHECK();
         if ((r = rb_forward_match_argmax_enqueue(c, old, neu))) return r;
     }
-    // :354  FordwardMatch ; :369 rotate_keylines(R0) in one kernel.  Until then, this frame only reads the old map's rho /
-    // s_rho (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may run until then.
-    if ((r = resc_join(pl))) return r;
-    if ((r = rb_forward_match_apply_enqueue(c, old, neu, pl->fs->R0))) return r;
-    RB_TRACE(c->stream, 11);
-    prof_mark(pl, ST_FWD_ROT);
-    // :410  directed_matching(V,P_V,R,old_buf.ef,...)
-    if ((r = rb_directed_matching_enqueue(c, neu, old, &pl->fs->dm, p.MatchThreshModule, p.MatchThreshAngle,
-                                          (double)p.SearchRange, p.LocationUncertaintyMatch, &pl->fs->do_match)))
-        return r;
-    RB_TRACE(c->stream, 4);
-    prof_mark(pl, ST_DMATCH);
-    // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids, then
-    // :480-487 EstimateReScalingOpt and :545-585 pose integration + NavData in one cluster kernel (k_map_update).
-    // With the rescaling stream, pose integration + NavData ride in the EKF kernel and the rescaling leaves the chain.
+    // :480-487 EstimateReScalingOpt and :545-585 pose integration + NavData: in one cluster kernel (k_map_update) after the
+    // EKF, or with the rescaling stream, pose integration + NavData ride in the EKF kernel and the rescaling leaves the chain.
     // (Not with the 168-byte keyline mirror: there the inline schedule measured 2-3 % faster on H100, while the 15-byte
     // records gain from the side stream like the plain push; set_mirror drops the captured batches.)
     const bool side = pl->resc_stream != nullptr && pl->mirror_on != 1;
-    if (!pl->map_fused)
-        if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
-                                           p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
-                                           side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
+    if (pl->map_chain) {
+        // (the old map's rescaling is joined here although k_match only reads that map: joining it before k_reg_ekf
+        // instead measured no faster on H100)
+        if ((r = resc_join(pl))) return r;
+        // (the eager stage profile reports k_match under "directed_match", nothing under "fwdmatch+rotate", and
+        // k_reg_ekf under "regularize+ekf")
+        prof_mark(pl, ST_FWD_ROT);
+        // :354  FordwardMatch + :410 directed_matching(V,P_V,R,old_buf.ef,...) against the old map before :369
+        // rotate_keylines(R0), which k_reg_ekf runs; this kernel rotates the old keylines it probes itself
+        if ((r = rb_match_enqueue(c, neu, old, &pl->fs->dm, pl->fs->R0, p.MatchThreshModule, p.MatchThreshAngle,
+                                  (double)p.SearchRange, p.LocationUncertaintyMatch, &pl->fs->do_match)))
             return r;
+        RB_TRACE(c->stream, 4);
+        prof_mark(pl, ST_DMATCH);
+        // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman + :369 rotate_keylines
+        if ((r = rb_reg_ekf_enqueue(c, neu, old, p.RegularizeThresh, pl->fs, p.MatchThreshold, p.ReshapeQAbsolute,
+                                    p.LocationUncertainty, pl->fs->R0, side ? nav_slot : nullptr, fa)))
+            return r;
+    } else {
+        // :354  FordwardMatch ; :369 rotate_keylines(R0) in one kernel.  Until then, this frame only reads the old map's
+        // rho / s_rho (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may
+        // run until then.
+        if ((r = resc_join(pl))) return r;
+        if ((r = rb_forward_match_apply_enqueue(c, old, neu, pl->fs->R0))) return r;
+        RB_TRACE(c->stream, 11);
+        prof_mark(pl, ST_FWD_ROT);
+        // :410  directed_matching(V,P_V,R,old_buf.ef,...)
+        if ((r = rb_directed_matching_enqueue(c, neu, old, &pl->fs->dm, p.MatchThreshModule, p.MatchThreshAngle,
+                                              (double)p.SearchRange, p.LocationUncertaintyMatch, &pl->fs->do_match)))
+            return r;
+        RB_TRACE(c->stream, 4);
+        prof_mark(pl, ST_DMATCH);
+        // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids (or in the
+        // map-update kernel with map_fused)
+        if (!pl->map_fused)
+            if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
+                                               p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
+                                               side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
+                return r;
+    }
     RB_TRACE(c->stream, 9);
     prof_mark(pl, ST_REG_EKF);
     if (side) {   // gated by the map's own copy of do_map; writes the map's Kp / RKp and the record's, no FrameState

@@ -1351,24 +1351,43 @@ int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *X
 // =====================================================================================================
 // rotate_keylines (edge_tracker.cpp:42-76)
 // =====================================================================================================
-// keyline i of kl rotated by R, from its p_m, rho, s_rho and m_m as loaded by the caller
-__device__ __forceinline__ void d_rotate_vals(const KLSoA &kl, int i, const double (&R)[9], double zf, float2 pm, double rho,
-                                              double s_rho, float2 m) {
+// The rotation of one keyline as values: the in-place rotation below and the matching kernel, which rotates the old
+// keylines it probes on the fly, share these two helpers, so both see the same bits.
+struct RotPt {
+    float2 pm;
+    double rho, s_rho;
+};
+// (p_m, rho, s_rho) rotated by R; unchanged when the rotated point has no finite depth
+__device__ __forceinline__ RotPt d_rot_pt(const double (&R)[9], double zf, float2 pm, double rho, double s_rho) {
     const double v0 = (double)pm.x / zf, v1 = (double)pm.y / zf, v2 = 1;
     double q0 = 0, q1 = 0, q2 = 0;   // TooN Matrix*Vector: dot accumulates from 0
     q0 = q0 + R[0] * v0; q0 = q0 + R[1] * v1; q0 = q0 + R[2] * v2;
     q1 = q1 + R[3] * v0; q1 = q1 + R[4] * v1; q1 = q1 + R[5] * v2;
     q2 = q2 + R[6] * v0; q2 = q2 + R[7] * v1; q2 = q2 + R[8] * v2;
+    RotPt o = {pm, rho, s_rho};
     if (fabs(q2) > 0) {
-        kl.p_m[i] = make_float2((float)(q0 / q2 * zf), (float)(q1 / q2 * zf));
-        kl.rho[i] = rho / q2;
-        kl.s_rho[i] = s_rho / q2;
+        o.pm = make_float2((float)(q0 / q2 * zf), (float)(q1 / q2 * zf));
+        o.rho = rho / q2;
+        o.s_rho = s_rho / q2;
     }
+    return o;
+}
+// m_m rotated by R
+__device__ __forceinline__ float2 d_rot_m(const double (&R)[9], float2 m) {
     const double m0 = (double)m.x, m1 = (double)m.y;
     double r0 = 0, r1 = 0;
     r0 = r0 + R[0] * m0; r0 = r0 + R[1] * m1; r0 = r0 + R[2] * 0.0;
     r1 = r1 + R[3] * m0; r1 = r1 + R[4] * m1; r1 = r1 + R[5] * 0.0;
-    const float2 mr = make_float2((float)r0, (float)r1);
+    return make_float2((float)r0, (float)r1);
+}
+// keyline i of kl rotated by R, from its p_m, rho, s_rho and m_m as loaded by the caller
+__device__ __forceinline__ void d_rotate_vals(const KLSoA &kl, int i, const double (&R)[9], double zf, float2 pm, double rho,
+                                              double s_rho, float2 m) {
+    const RotPt pt = d_rot_pt(R, zf, pm, rho, s_rho);
+    kl.p_m[i] = pt.pm;
+    kl.rho[i] = pt.rho;
+    kl.s_rho[i] = pt.s_rho;
+    const float2 mr = d_rot_m(R, m);
     kl.m_m[i] = mr;
     float4 p = kl.pack[2 * i];
     p.x = mr.x;
@@ -1484,32 +1503,27 @@ int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev) {
 // directed_matching + search_match (edge_tracker.cpp:158-374)
 // =====================================================================================================
 #define DM_G 4   // lanes per keyline of the directed search (must divide 32, even)
-__global__ void __launch_bounds__(128) k_directed_match(KLSoA neu, MapState *nst, KLSoA old,
-                                                        const int *__restrict__ omask, const DMatchArgs *__restrict__ ap,
-                                                        CamC cam, double min_thr_mod, double cang_min_edge,
-                                                        double max_radius, double loc_unc, const int *enable) {
-    pdl_wait();
-    pdl_launch();
-    if (enable && !*enable) return;
-    // DM_G lanes per keyline: the search along the epipolar segment probes up to 2 * t_steps pixels in a fixed order
-    // (t_i = 0, 1, ...; for each the near side, then the far side) and stops at the first accepted candidate.  Unmatched
-    // keylines walk the whole segment, a chain of ~80 dependent lookups; here probe number s = 2 t_i + dir belongs to lane
-    // s mod DM_G of the keyline's group, the lanes advance in lock step (DM_G probes per iteration) and the lowest lane with
-    // a hit in an iteration is the first hit of the sequential order.  tp / tn are still built by repeated +-1 (each lane
-    // takes DM_G / 2 steps per iteration), so every probe sees the same bits as the reference's.
-    const int gi = blockIdx.x * blockDim.x + threadIdx.x;
-    const int i = gi / DM_G, g = gi % DM_G, lane = threadIdx.x & 31;
-    bool got = false;
+// The search of new keyline (kpm, krho, ks_rho, km, kn_m) among the old keylines of omask; every lane of the warp calls
+// it.  Returns the matched old keyline (or -1) in every lane of the keyline's group.  ROT: the old map is not rotated yet,
+// so each candidate is rotated by R here, with the arithmetic of rotate_keylines.
+//
+// DM_G lanes per keyline: the search along the epipolar segment probes up to 2 * t_steps pixels in a fixed order
+// (t_i = 0, 1, ...; for each the near side, then the far side) and stops at the first accepted candidate.  Unmatched
+// keylines walk the whole segment, a chain of ~80 dependent lookups; here probe number s = 2 t_i + dir belongs to lane
+// s mod DM_G of the keyline's group, the lanes advance in lock step (DM_G probes per iteration) and the lowest lane with
+// a hit in an iteration is the first hit of the sequential order.  tp / tn are still built by repeated +-1 (each lane
+// takes DM_G / 2 steps per iteration), so every probe sees the same bits as the reference's.
+template <bool ROT>
+__device__ __forceinline__ int d_dm_search(const KLSoA &old, const int *__restrict__ omask,
+                                           const DMatchArgs *__restrict__ ap, const CamC &cam, double min_thr_mod,
+                                           double cang_min_edge, double max_radius, double loc_unc, bool valid, int g,
+                                           float2 kpm, double krho, double ks_rho, float2 km, float kn_m,
+                                           const double (&R)[9]) {
+    const int lane = threadIdx.x & 31;
     int jm = -1;
     {
-        const bool valid = i < nst->kn;
-        const int ic = valid ? i : 0;   // (lanes without a keyline run on keyline 0 and never probe)
         const double zf = cam.zfm;
         const double *BR = ap->BackRot, *Vel = ap->Vel, *RV = ap->RVel;
-        const float2 kpm = neu.p_m[ic];
-        const double krho = neu.rho[ic], ks_rho = neu.s_rho[ic];
-        const float2 km = neu.m_m[ic];
-        const float kn_m = neu.n_m[ic];
         // p_m3 = BackRot*(p_m.x, p_m.y, zfm)
         const double a0 = (double)kpm.x, a1 = (double)kpm.y, a2 = zf;
         double p30 = 0, p31 = 0, p32 = 0;
@@ -1576,10 +1590,15 @@ __global__ void __launch_bounds__(128) k_directed_match(KLSoA neu, MapState *nst
                         const int j = omask[(size_t)yi * cam.w + xi];
                         if (j >= 0) {
                             const double norm_m0 = (double)old.n_m[j];
-                            const float2 om = old.m_m[j];
+                            const float2 om = ROT ? d_rot_m(R, old.m_m[j]) : old.m_m[j];
                             const double cang = (double)(om.x * km.x + om.y * km.y) / (norm_m0 * norm_m);
                             if (!(cang < cang_min_edge || fabs(norm_m0 / norm_m - 1) > min_thr_mod)) {
-                                const double s_rho = old.s_rho[j], rho = old.rho[j];
+                                double s_rho = old.s_rho[j], rho = old.rho[j];
+                                if (ROT) {
+                                    const RotPt pt = d_rot_pt(R, zf, old.p_m[j], rho, s_rho);
+                                    rho = pt.rho;
+                                    s_rho = pt.s_rho;
+                                }
                                 const double v_rho_dr = (loc_unc * loc_unc + s_rho * s_rho * norm_t * norm_t + sigma2_t * rho * rho);
                                 const double e = t - norm_t * rho;
                                 if (!(e * e > v_rho_dr)) j_hit = j;
@@ -1604,20 +1623,106 @@ __global__ void __launch_bounds__(128) k_directed_match(KLSoA neu, MapState *nst
             t_i += DM_G / 2;
             if (!__any_sync(0xffffffffu, active && t_i < t_steps)) break;
         }
-        if (g != 0) jm = -1;   // one lane of the group writes
-        if (jm >= 0) {                                                     // :343-366
-            neu.rho[i] = old.rho[jm];
-            neu.s_rho[i] = old.s_rho[jm];
-            neu.m_id[i] = jm;
-            neu.m_num[i] = old.m_num[jm] + 1;
-            neu.p_m_0[i] = old.p_m[jm];
-            neu.m_m0[i] = old.m_m[jm];
-            neu.n_m0[i] = (double)old.n_m[jm];
-            got = true;
-        }
+    }
+    return jm;
+}
+__global__ void __launch_bounds__(128) k_directed_match(KLSoA neu, MapState *nst, KLSoA old,
+                                                        const int *__restrict__ omask, const DMatchArgs *__restrict__ ap,
+                                                        CamC cam, double min_thr_mod, double cang_min_edge,
+                                                        double max_radius, double loc_unc, const int *enable) {
+    pdl_wait();
+    pdl_launch();
+    if (enable && !*enable) return;
+    const int gi = blockIdx.x * blockDim.x + threadIdx.x;
+    const int i = gi / DM_G, g = gi % DM_G;
+    const bool valid = i < nst->kn;
+    const int ic = valid ? i : 0;   // (lanes without a keyline run on keyline 0 and never probe)
+    const double R[9] = {};
+    int jm = d_dm_search<false>(old, omask, ap, cam, min_thr_mod, cang_min_edge, max_radius, loc_unc, valid, g,
+                                neu.p_m[ic], neu.rho[ic], neu.s_rho[ic], neu.m_m[ic], neu.n_m[ic], R);
+    bool got = false;
+    if (g != 0) jm = -1;   // one lane of the group writes
+    if (jm >= 0) {                                                     // :343-366
+        neu.rho[i] = old.rho[jm];
+        neu.s_rho[i] = old.s_rho[jm];
+        neu.m_id[i] = jm;
+        neu.m_num[i] = old.m_num[jm] + 1;
+        neu.p_m_0[i] = old.p_m[jm];
+        neu.m_m0[i] = old.m_m[jm];
+        neu.n_m0[i] = (double)old.n_m[jm];
+        got = true;
     }
     const unsigned int bal = __ballot_sync(0xffffffffu, got);
     if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&nst->nmatch, __popc(bal));
+}
+
+// FordwardMatch's apply and directed_matching in one kernel, indexed by new keyline, with the old map still unrotated
+// (rb_match_enqueue): the forward winner of keyline i is final in best[i] once the minimiser has run, and the search
+// rotates the few old keylines it probes by R0 itself.  The result is the directed hit (rotated) if there is one, else
+// the forward winner (unrotated), else nothing.  The keyline's (rho, s_rho) after matching go to reg_r / reg_s for every
+// keyline, not to the map: the regularisation that follows reads its neighbours from there (k_reg_ekf).
+__global__ void __launch_bounds__(128) k_match(KLSoA neu, MapState *nst, KLSoA old, const int *__restrict__ omask,
+                                               const FmBest *best, const DMatchArgs *__restrict__ ap,
+                                               const double *__restrict__ Rp, double *__restrict__ reg_r,
+                                               double *__restrict__ reg_s, CamC cam, double min_thr_mod,
+                                               double cang_min_edge, double max_radius, double loc_unc,
+                                               const int *__restrict__ do_match) {
+    pdl_wait();
+    pdl_launch();
+    // (the grid covers the capacity: a block past the map's keylines has nothing to do, not even the search set-up)
+    if ((int)(blockIdx.x * (blockDim.x / DM_G)) >= nst->kn) return;
+    const int gi = blockIdx.x * blockDim.x + threadIdx.x;
+    const int i = gi / DM_G, g = gi % DM_G;
+    const bool valid = i < nst->kn;
+    const int ic = valid ? i : 0;   // (lanes without a keyline run on keyline 0 and never probe)
+    const longlong2 b = __ldcg(reinterpret_cast<const longlong2 *>(best + ic));   // FmBest {key, idx}, 16 bytes
+    const float2 kpm = neu.p_m[ic], km = neu.m_m[ic];
+    const float kn_m = neu.n_m[ic];
+    double R[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) R[k] = Rp[k];
+    const int fw = valid ? (int)b.y : -1;
+    double krho, ks_rho;   // what FordwardMatch leaves in the keyline: the search range depends on it
+    if (fw >= 0) {
+        krho = old.rho[fw];
+        ks_rho = old.s_rho[fw];
+    } else {
+        krho = neu.rho[ic];
+        ks_rho = neu.s_rho[ic];
+    }
+    int jm = -1;
+    if (*do_match)   // (uniform over the grid)
+        jm = d_dm_search<true>(old, omask, ap, cam, min_thr_mod, cang_min_edge, max_radius, loc_unc, valid, g, kpm, krho,
+                               ks_rho, km, kn_m, R);
+    bool got = false;
+    if (valid && g == 0) {   // one lane of the group writes
+        double rho = krho, s_rho = ks_rho;
+        if (jm >= 0) {                                                     // directed_matching :343-366
+            const RotPt pt = d_rot_pt(R, cam.zfm, old.p_m[jm], old.rho[jm], old.s_rho[jm]);
+            rho = pt.rho;
+            s_rho = pt.s_rho;
+            neu.m_id[i] = jm;
+            neu.m_num[i] = old.m_num[jm] + 1;
+            neu.p_m_0[i] = pt.pm;
+            neu.m_m0[i] = d_rot_m(R, old.m_m[jm]);
+            neu.n_m0[i] = (double)old.n_m[jm];
+            got = true;
+        } else if (fw >= 0) {                                              // FordwardMatch
+            neu.m_id[i] = fw;
+            neu.m_num[i] = old.m_num[fw] + 1;
+            neu.p_m_0[i] = old.p_m[fw];
+            neu.m_m0[i] = old.m_m[fw];
+            neu.n_m0[i] = (double)old.n_m[fw];
+        }
+        reg_r[i] = rho;
+        reg_s[i] = s_rho;
+    }
+    const unsigned int bal = __ballot_sync(0xffffffffu, got);
+    const unsigned int fbal = __ballot_sync(0xffffffffu, valid && g == 0 && fw >= 0);
+    if ((threadIdx.x & 31) == 0) {
+        if (bal) atomicAdd(&nst->nmatch, __popc(bal));
+        if (fbal) atomicAdd(&nst->fwd_match, __popc(fbal));
+    }
 }
 
 int rb_directed_matching_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, double min_thr_mod,
@@ -1631,20 +1736,30 @@ int rb_directed_matching_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMat
                make_cam(c), min_thr_mod, cang_min_edge, max_radius, loc_uncertainty, enable_dev);
     return RB_OK;
 }
+int rb_match_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, const double *R_dev,
+                     double min_thr_mod, double min_thr_ang, double max_radius, double loc_uncertainty,
+                     const int *do_match_dev) {
+    const double cang_min_edge = cos(min_thr_ang * M_PI / 180.0);
+    const TrackState &t = neu->ts_host;
+    RB_KLAUNCH(k_match, rb_div_up(c->kcap * DM_G, 128), 128, 0, neu->kl, neu->st, old->kl, (const int *)old->mask,
+               (const FmBest *)t.fm_best, args_dev, R_dev, t.reg_r, t.reg_s, make_cam(c), min_thr_mod, cang_min_edge,
+               max_radius, loc_uncertainty, do_match_dev);
+    return RB_OK;
+}
 
 // =====================================================================================================
 // Regularize_1_iter (edge_tracker.cpp:87-148), double buffered like the reference
 // =====================================================================================================
-// first half of Regularize_1_iter for keyline i: smoothed (rho, s_rho) into r / s, set[i] says whether it applies
-__device__ __forceinline__ bool d_reg_a(const KLSoA &kl, int i, double *__restrict__ r, double *__restrict__ s,
-                                        unsigned char *__restrict__ set, double thresh) {
+// first half of Regularize_1_iter for keyline i, with the (rho, s_rho) of i and its neighbours read from rho / s_rho:
+// whether it applies, and if so the smoothed pair in r_out / s_out
+__device__ __forceinline__ bool d_reg_vals(const KLSoA &kl, int i, const double *rho, const double *s_rho, double thresh,
+                                           double &r_out, double &s_out) {
     bool did = false;
-    unsigned char sv = 0;
     const int ni = kl.n_id[i], pi = kl.p_id[i];
     if (ni >= 0 && pi >= 0) {
-        const double krho = kl.rho[i], ks = kl.s_rho[i];
-        const double nrho = kl.rho[ni], ns = kl.s_rho[ni];
-        const double prho = kl.rho[pi], ps = kl.s_rho[pi];
+        const double krho = rho[i], ks = s_rho[i];
+        const double nrho = rho[ni], ns = s_rho[ni];
+        const double prho = rho[pi], ps = s_rho[pi];
         const double d = nrho - prho;
         if (!(d * d > ns * ns + ps * ps)) {
             const float2 nm = kl.m_m[ni], pmv = kl.m_m[pi];
@@ -1657,14 +1772,19 @@ __device__ __forceinline__ bool d_reg_a(const KLSoA &kl, int i, double *__restri
                 const double wr = 1 / (ks * ks);
                 const double wrn = alpha / (ns * ns);
                 const double wrp = alpha / (ps * ps);
-                r[i] = (krho * wr + nrho * wrn + prho * wrp) / (wr + wrn + wrp);
-                s[i] = (ks * wr + ns * wrn + ps * wrp) / (wr + wrn + wrp);
-                sv = 1;
+                r_out = (krho * wr + nrho * wrn + prho * wrp) / (wr + wrn + wrp);
+                s_out = (ks * wr + ns * wrn + ps * wrp) / (wr + wrn + wrp);
                 did = true;
             }
         }
     }
-    set[i] = sv;
+    return did;
+}
+// ... in place: smoothed (rho, s_rho) into r / s, set[i] says whether it applies
+__device__ __forceinline__ bool d_reg_a(const KLSoA &kl, int i, double *__restrict__ r, double *__restrict__ s,
+                                        unsigned char *__restrict__ set, double thresh) {
+    const bool did = d_reg_vals(kl, i, kl.rho, kl.s_rho, thresh, r[i], s[i]);
+    set[i] = did ? 1 : 0;
     return did;
 }
 __global__ void __launch_bounds__(256) k_regularize_a(KLSoA kl, MapState *st, double *__restrict__ r,
@@ -1815,6 +1935,52 @@ int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *f
     RB_KLAUNCH(k_regb_ekf, nb, 256, 0, m->kl, (const MapState *)m->st, (const double *)t.reg_r, (const double *)t.reg_s,
                (const unsigned char *)t.reg_set, vel_dev, c->zfm, q_abs, loc_unc, do_map_dev, fs, ost,
                (const LMState *)&m->ts->lm, nav, fa);
+    return RB_OK;
+}
+
+// The map update after k_match, in one pass: every thread evaluates the match-count gate itself (its inputs are final),
+// the regularisation reads (rho, s_rho) of a keyline and its neighbours from the scratch pair r / s that k_match filled,
+// and the EKF takes the smoothed pair from registers; every keyline's rho / s_rho is written back (the scratch values
+// when the gate is closed).  Thread i also runs rotate_keylines(R0) on old keyline i: nothing reads the old map after
+// k_match, and the map stays what a caller of the pipeline sees.  One spare thread runs the gate's frame part, then the
+// pose integration / nav record, as k_regularize_a_gate and k_regb_ekf do.
+__global__ void __launch_bounds__(256) k_reg_ekf(KLSoA kl, MapState *st, const double *__restrict__ r,
+                                                 const double *__restrict__ s, double thresh, FrameState *fs,
+                                                 int match_threshold, double zf, double q_abs, double loc_unc, KLSoA old,
+                                                 const MapState *ost, const double *__restrict__ Rp, const LMState *lm,
+                                                 rb_nav *nav, const FrameArgs *fa) {
+    pdl_wait();
+    pdl_launch();
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+        d_frame_post_match(fs, st, match_threshold);
+        st->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
+        if (nav) d_frame_finish(fs, st, ost, lm->score, nav, fa, false);
+        else d_frame_pose(fs);
+    }
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < ost->kn) d_rotate(old, i, Rp, zf);
+    // (the gate thread above only changes fs->V when the gate is closed, and then no thread reads it)
+    const bool en = fs->do_match && st->nmatch >= match_threshold;
+    bool did = false;
+    if (i < st->kn) {
+        double rho = r[i], s_rho = s[i];
+        if (en) did = d_reg_vals(kl, i, r, s, thresh, rho, s_rho);
+        if (en && kl.m_id[i] >= 0) {
+            d_ekf(kl, i, rho, s_rho, fs->V, zf, q_abs, loc_unc);
+        } else {
+            kl.rho[i] = rho;
+            kl.s_rho[i] = s_rho;
+        }
+    }
+    const unsigned int bal = __ballot_sync(0xffffffffu, did);
+    if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&st->reg_num, __popc(bal));
+}
+int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameState *fs, int match_threshold,
+                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa) {
+    const TrackState &t = m->ts_host;
+    RB_KLAUNCH(k_reg_ekf, rb_div_up(c->kcap, 256), 256, 0, m->kl, m->st, (const double *)t.reg_r,
+               (const double *)t.reg_s, thresh, fs, match_threshold, c->zfm, q_abs, loc_unc, old->kl,
+               (const MapState *)old->st, R_dev, (const LMState *)&m->ts->lm, nav, fa);
     return RB_OK;
 }
 

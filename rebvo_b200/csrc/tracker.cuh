@@ -79,6 +79,16 @@ int rb_directed_matching_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMat
                                  double loc_uncertainty, const int *enable_dev);
 int rb_regularize_enqueue(rb_ctx *c, rb_map *m, double thresh, const int *enable_dev);
 struct rb_nav;
+// The per-frame map chain of two kernels, with the old map rotated last.  rb_match_enqueue: FordwardMatch's apply (the
+// arg-max of neu is complete) and directed_matching against the unrotated old map, each probed keyline rotated by R_dev;
+// the matched (rho, s_rho) of every keyline go to neu's regularisation scratch.  rb_reg_ekf_enqueue: the match-count
+// gate, Regularize_1_iter from that scratch, the EKF, rotate_keylines(R_dev) of old, and (with nav) the frame's nav
+// record as rb_regularize_ekf_enqueue writes it.
+int rb_match_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, const double *R_dev,
+                     double min_thr_mod, double min_thr_ang, double max_radius, double loc_uncertainty,
+                     const int *do_match_dev);
+int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameState *fs, int match_threshold,
+                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa);
 // with nav: the frame's nav record is written beside the EKF (except Kp / RKp of a mapped frame: rb_rescale_enqueue)
 int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
                               const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
