@@ -58,7 +58,7 @@ typedef struct rb_camera {
 
 /* arguments of edge_finder::detect (edge_finder.cpp:342-365) */
 typedef struct rb_detect_params {
-    int32_t plane_fit_size; /* DetectorPlaneFitSize (only 2 is supported: 5x5 window) */
+    int32_t plane_fit_size; /* DetectorPlaneFitSize 1..4: a 3x3 to 9x9 plane-fit window (other values: RB_ERR_ARG) */
     double pos_neg_thresh;  /* DetectorPosNegThresh */
     double dog_thresh;      /* DetectorDoGThresh */
     int32_t kl_max;         /* MaxPoints */

@@ -226,6 +226,8 @@ static int pl_reset_state(rb_pipeline *pl) {
 extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params *p, int max_batch) {
     if (!out || !p || max_batch < 1) return RB_ERR_ARG;
     *out = nullptr;
+    // the detector's check, at creation: a bad DetectorPlaneFitSize must not surface at the first push
+    if (p->det.plane_fit_size < 1 || p->det.plane_fit_size > RB_PLANE_FIT_MAX) return RB_ERR_ARG;
     rb_ctx *c = nullptr;
     int kcap = p->kl_capacity > 0 ? p->kl_capacity : 50000;
     int r = rb_ctx_create(&c, device, &p->cam, p->Sigma0, p->KSigma, kcap);
