@@ -203,20 +203,10 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     c->ksigma = ksigma;
     c->kcap = kl_capacity;
     {
-        const char *ds = getenv("REBVO_B200_DOG_SUB");
-        c->dog_sub = ds ? atoi(ds) : 0;   // 0 = whole batch in one go (the passes are latency-bound)
-        if (c->dog_sub < 0) c->dog_sub = 0;
         const char *pd = getenv("REBVO_B200_PDL");
         c->pdl = !(pd && atoi(pd) == 0);
         const char *mp = getenv("REBVO_B200_MIN_PERSIST");
         c->min_persist = !(mp && atoi(mp) == 0);
-        const char *mc = getenv("REBVO_B200_MIN_CLUSTER");
-        c->min_cluster = !(mc && atoi(mc) == 0);
-        const char *rs = getenv("REBVO_B200_ROWSCAN");
-        c->rowscan_mode = rs ? atoi(rs) : 2;
-        c->mu_xchg = !(getenv("REBVO_B200_MU_XCHG") && atoi(getenv("REBVO_B200_MU_XCHG")) == 0);
-        c->row_ns = getenv("REBVO_B200_ROW_NS") ? atoi(getenv("REBVO_B200_ROW_NS")) : 0;
-        c->colscan_mode = getenv("REBVO_B200_COLSCAN") ? atoi(getenv("REBVO_B200_COLSCAN")) : 0;
     }
     // sspace::sspace (sspace.cpp:36-46): filter1 sigma = filter0.sigma_r * k_sigma
     box_plan_one(sigma0, 3, c->plan.d[0], &c->plan.sigma_r[0]);

@@ -78,7 +78,6 @@ struct DogWS {           // batched scale-space workspace, B images of N floats 
     float *aux;          // 3 * N    on-demand planes (Img(1), dx, dy) for the test/debug accessor
     void *tmaps;         // CUtensorMap[] (host, dog.cu TM_*): TMA-staged row passes, last box + DoG
     bool tma_ok;
-    int tma_row_mask;
     bool tma_row_ok;     // the row passes run on TMA tiles (k_rowscan_tma_*)
 };
 
@@ -107,22 +106,15 @@ struct rb_ctx {
     void *dev_small;     // small device buffer for scalar parameters / results (64 KiB, zero-initialised)
     float *boxtab;       // 6 x 64 reciprocal clipped-area tables (iimage::build_average), see dog.cu
     bool counters_preset; // set by rb_pipeline: match / regularise counters are zeroed by k_frame_pre
-    int dog_sub;         // frames per scale-space sub-batch, env REBVO_B200_DOG_SUB (0 = whole batch, the default)
     bool pdl;            // programmatic dependent launch of the per-frame chain (env REBVO_B200_PDL=0 disables)
     bool min_persist;    // whole Minimizer_RV in one launch (env REBVO_B200_MIN_PERSIST=0: one launch per evaluation)
-    bool min_cluster;    // Minimizer_RV in one 16-CTA cluster (min_cluster.cuh); env REBVO_B200_MIN_CLUSTER=0 disables
     int min_cluster_kpc; // keylines per CTA its shared memory is sized for (0: not available on this device / capacity)
     size_t min_cluster_dyn;
     int min_cluster_g;   // clusters per minimisation (env REBVO_B200_MIN_G, default 4; 1 = one cluster, co-residency guaranteed)
     int min_cluster_kpc_multi;
     size_t min_cluster_dyn_multi;
     int min_debug_abort;
-    bool mu_xchg;        // env REBVO_B200_MU_XCHG (default 1): st.async all-reduce in k_map_update's rescaling iterations
     bool min_early;      // set by rb_pipeline around its Minimizer_RV launch: operands may be staged before the PDL wait  // test hook (env REBVO_B200_MIN_FORCE_ABORT=1): the kernel raises its abort flag at once
-    int min_cluster_xchg; // 1: st.async + mbarrier exchange, 0: DSMEM stores + barrier.cluster (env REBVO_B200_MIN_XCHG)
-    int row_ns;          // env REBVO_B200_ROW_NS: depth of the TMA tile ring of the row passes (0 = default 4)
-    int colscan_mode;    // env REBVO_B200_COLSCAN: 1 = unpipelined column pass
-    int rowscan_mode;    // env REBVO_B200_ROWSCAN: 1 = register-prefetch kernel, 2 = cp.async shared-memory ring
 };
 // layout of rb_ctx::dev_small / pinned (byte offsets)
 #define RB_DS_REEST 0        // int[2 + nbins + 1]  reEstimateThresh min/max bits + histogram
@@ -264,7 +256,6 @@ void rb_dogws_free(DogWS *ws);
 int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // rgb -> gray
 int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // mono -> gray
 int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg);          // gray -> img0, dog
-int rb_dog_build_range(rb_ctx *c, DogWS *ws, int f0, int m);     // the same for the images [f0, f0 + m)
 int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img);            // Img(1), dx, dy into ws->aux
 int rb_dog_make_tables(rb_ctx *c);
 int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws);

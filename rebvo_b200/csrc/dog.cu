@@ -10,8 +10,8 @@
 // mul+add is ever contracted.
 //
 // Pass structure per box stage (B images x 2 filters in one launch):
-//   k_rowscan<AVG> : S(x,y)  = sum_{i<=x} avg(I_prev)(i,y)   warp per 32-row band, smem-transposed tiles
-//   k_colscan      : I(x,y)  = sum_{j<=y} S(x,j)              thread per 4 columns, float4 streams
+//   k_rowscan_tma_* / k_rowscan_ring : S(x,y) = sum_{i<=x} avg(I_prev)(i,y)   warp per 32-row band
+//   k_colscan_pipe                   : I(x,y) = sum_{j<=y} S(x,j)              thread per 4 columns, float4 streams
 // and a final k_blur_dog that evaluates the last box of both filters, Img(0) and the DoG.
 #include <stdlib.h>
 #include <new>
@@ -86,103 +86,6 @@ __global__ void __launch_bounds__(256) k_mono2gray(const uint32_t *__restrict__ 
     o.z = (float)(3u * ((a >> 16) & 0xff));
     o.w = (float)(3u * (a >> 24));
     gray[i] = o;
-}
-
-// Row pass: warp per band of 32 rows of one image.  Tiles of 32x32 are produced coalesced (optionally
-// through box_avg of the previous integral image), transposed through shared memory so that each lane
-// owns one row, scanned sequentially (the reference's add order), and stored coalesced.
-template <bool AVG>
-__global__ void __launch_bounds__(128) k_rowscan(const float *__restrict__ in, float *__restrict__ out,
-                                                 int w, int h, int nimg, int in_mod, int nper, int d_f0,
-                                                 int d_f1, const float *__restrict__ tab_f0,
-                                                 const float *__restrict__ tab_f1) {
-    __shared__ float tile[4][32][33];
-    __shared__ float stab[4][BOX_TAB_N];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int gw = blockIdx.x * 4 + warp;
-    const int bands = (h + 31) >> 5;
-    const int img = gw / bands, band = gw - img * bands;
-    if (img >= nimg) return;
-    const size_t N = (size_t)w * h;
-    const float *__restrict__ I = in + (size_t)(img % in_mod) * N;
-    float *__restrict__ O = out + (size_t)img * N;
-    const bool f1 = (img / nper) != 0;
-    const int d = f1 ? d_f1 : d_f0;
-    const int d2 = d / 2;
-    if (AVG) {
-        const float *__restrict__ tg = f1 ? tab_f1 : tab_f0;
-        stab[warp][lane] = tg[lane];
-        stab[warp][lane + 32] = tg[lane + 32];
-        __syncwarp();
-    }
-    const float *tab = stab[warp];
-    const int y0 = band * 32;
-    float v[32];
-    float carry = 0.f;
-
-    // branch-free tile production: clamped coordinates + select, so that all loads of a tile are in flight at once
-#define LOAD_TILE(X0)                                                           \
-    {                                                                           \
-        const int x = (X0) + lane;                                              \
-        const int xc = x < w ? x : w - 1;                                       \
-        _Pragma("unroll") for (int r = 0; r < 32; r++) {                        \
-            const int y = y0 + r;                                               \
-            const int yc = y < h ? y : h - 1;                                   \
-            const float t = AVG ? box_avg(I, xc, yc, w, h, d, d2, tab) : I[(size_t)yc * w + xc]; \
-            v[r] = (y < h && x < w) ? t : 0.f;                                  \
-        }                                                                       \
-    }
-    LOAD_TILE(0);
-    for (int x0 = 0; x0 < w; x0 += 32) {
-#pragma unroll
-        for (int r = 0; r < 32; r++) tile[warp][r][lane] = v[r];
-        __syncwarp();
-        if (x0 + 32 < w) LOAD_TILE(x0 + 32);  // next tile's loads overlap the dependent add chain
-        float *row = tile[warp][lane];
-#pragma unroll
-        for (int cidx = 0; cidx < 32; cidx++) {
-            carry = carry + row[cidx];  // I(x,y) = I(x-1,y) + in(x,y), iimage.cpp:56-60
-            row[cidx] = carry;
-        }
-        __syncwarp();
-        const int x = x0 + lane;
-        if (x < w) {
-#pragma unroll
-            for (int r = 0; r < 32; r++) {
-                const int y = y0 + r;
-                if (y < h) O[(size_t)y * w + x] = tile[warp][r][lane];
-            }
-        }
-        __syncwarp();
-    }
-#undef LOAD_TILE
-}
-
-// Column pass: thread per 4 adjacent columns; I(x,y) += I(x,y-1) top->bottom (iimage.cpp:62-66)
-__global__ void __launch_bounds__(64) k_colscan(const float4 *__restrict__ in, float4 *__restrict__ out,
-                                                int w4, int h, int nimg) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    const int img = idx / w4, cx = idx - img * w4;
-    if (img >= nimg) return;
-    const float4 *__restrict__ I = in + (size_t)img * w4 * h + cx;
-    float4 *__restrict__ O = out + (size_t)img * w4 * h + cx;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    constexpr int U = 16;
-    for (int y = 0; y < h; y += U) {
-        float4 v[U];
-#pragma unroll
-        for (int k = 0; k < U; k++)
-            if (y + k < h) v[k] = __ldcs(&I[(size_t)(y + k) * w4]);
-#pragma unroll
-        for (int k = 0; k < U; k++)
-            if (y + k < h) {
-                acc.x = v[k].x + acc.x;
-                acc.y = v[k].y + acc.y;
-                acc.z = v[k].z + acc.z;
-                acc.w = v[k].w + acc.w;
-                O[(size_t)(y + k) * w4] = acc;
-            }
-    }
 }
 
 // Column pass, software-pipelined: VW adjacent columns per thread, the next U rows are in flight while the current U are added
@@ -466,7 +369,6 @@ int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws) {
                   make_tmap3(&t[TM_I_F1], ws->I, c->w, c->h, 2 * ws->B, 32, 32 + d[1][1]);
         if (!ok) cudaGetLastError();
         ws->tma_row_ok = ok;
-        ws->tma_row_mask = er ? atoi(er) : 1;   // 1 = both row passes, 2 = plain only, 3 = box average only (diagnosis)
     }
     return RB_OK;
 }
@@ -540,7 +442,7 @@ int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) 
 // sequential scan never waits for a DRAM round trip.  Tile t of a box-averaged pass needs the columns
 // [32t-d2-1, 32t+31+d2], i.e. chunks t-1, t, t+1 of the rows [y0-d2-1, y0+31+d2]; every integral value is fetched
 // from memory once and the four taps of iimage::average come from shared memory.  Same arithmetic and add order as
-// k_rowscan (bit-identical output).
+// box_avg followed by one sequential add chain per row (bit-identical output).
 #define RING_NS 4          // ring slots: 3 live chunks + 1 in flight
 #define RING_WARPS 4
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc, int src_bytes) {
@@ -686,7 +588,7 @@ __global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *_
 //     and writes its row as eight conflict-free 16-byte accesses (unit k of row r sits at unit k ^ (r & 7));
 //   * the scanned tile leaves with one cp.async.bulk.tensor store; bounds are the tensor map's business (zero fill on the
 //     way in, clipping on the way out).
-// Same arithmetic and add order as k_rowscan (bit-identical output).
+// Same arithmetic and add order as k_rowscan_ring (bit-identical output).
 __device__ __forceinline__ unsigned int rt_s32(const void *p) { return (unsigned int)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void rt_load3(unsigned int dst, const CUtensorMap *tm, int x, int y, int z, unsigned int bar,
                                          unsigned int bytes) {
@@ -892,28 +794,16 @@ static int rowscan_tma(rb_ctx *c, DogWS *ws, int stage, const float *in, int nim
     const CUtensorMap *t = (const CUtensorMap *)ws->tmaps;
     const int bands = (c->h + 31) / 32;
     int *fail = (int *)((char *)c->dev_small + RB_DS_TMA_FAIL);
-    const int ns_env = c->row_ns;
     if (stage < 0) {
         const int zin0 = (int)((in - ws->gray) / (ptrdiff_t)c->N);
-        const int ns = ns_env ? ns_env : 4;
-#define RT_PLAIN(NS) k_rowscan_tma_plain<NS><<<nimg * bands, 32, NS * 4096 + 64 + 1024, c->stream>>>(t[TM_GRAY], t[TM_S], c->w, c->h, zin0, fail)
-        if (ns >= 8) RT_PLAIN(8);
-        else if (ns >= 6) RT_PLAIN(6);
-        else RT_PLAIN(4);
-#undef RT_PLAIN
+        k_rowscan_tma_plain<4><<<nimg * bands, 32, 4 * 4096 + 64 + 1024, c->stream>>>(t[TM_GRAY], t[TM_S], c->w, c->h, zin0, fail);
     } else {
+        // at most 2 * 4096 + 4 * 47 * 128 + 64 + 256 + 1024 = 33600 bytes (d <= 2 * BOX_TAB_W - 1 = 15): no opt-in above 48 KB
         const int d0 = c->plan.d[0][stage], d1 = c->plan.d[1][stage];
         const int rmax = 32 + (d0 > d1 ? d0 : d1);
-        const int ns = ns_env ? ns_env : 4;
-#define RT_AVG(NS)                                                                                                              \
-    k_rowscan_tma_avg<NS><<<nimg * bands, 32, 2 * 4096 + (size_t)NS * rmax * 128 + 64 + BOX_TAB_N * 4 + 1024, c->stream>>>(     \
-        t[stage == 0 ? TM_I0_F0 : TM_I_F0], t[stage == 0 ? TM_I0_F1 : TM_I_F1], t[TM_S], c->w, c->h, in_mod, nper, d0, d1,       \
-        c->boxtab + (0 * 3 + stage) * BOX_TAB_N, c->boxtab + (1 * 3 + stage) * BOX_TAB_N, rmax, fail)
-        if (ns >= 6) RT_AVG(6);
-        else if (ns >= 5) RT_AVG(5);
-        else if (ns == 3) RT_AVG(3);
-        else RT_AVG(4);
-#undef RT_AVG
+        k_rowscan_tma_avg<4><<<nimg * bands, 32, 2 * 4096 + (size_t)4 * rmax * 128 + 64 + BOX_TAB_N * 4 + 1024, c->stream>>>(
+            t[stage == 0 ? TM_I0_F0 : TM_I_F0], t[stage == 0 ? TM_I0_F1 : TM_I_F1], t[TM_S], c->w, c->h, in_mod, nper, d0, d1,
+            c->boxtab + (0 * 3 + stage) * BOX_TAB_N, c->boxtab + (1 * 3 + stage) * BOX_TAB_N, rmax, fail);
     }
     RB_LAUNCH_CHECK();
     return RB_OK;
@@ -922,7 +812,6 @@ static int rowscan_tma(rb_ctx *c, DogWS *ws, int stage, const float *in, int nim
 // per-device opt-ins of this file's kernels (function attributes are per device: called from rb_ctx_create after
 // cudaSetDevice, so that contexts on several GPUs of one process all get them)
 int rb_dog_device_setup(rb_ctx *c) {
-    RB_CUDA(cudaFuncSetAttribute(k_rowscan_tma_avg<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     RB_CUDA(cudaFuncSetAttribute(k_rowscan_ring<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     RB_CUDA(cudaFuncSetAttribute(k_rowscan_ring<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     return RB_OK;
@@ -948,36 +837,24 @@ static int rowscan_ring(rb_ctx *c, int stage, const float *in, float *out, int n
 
 // stage < 0: plain row scan of the input; stage 0..1: row scan of box `stage` of both filters
 static int rowscan(rb_ctx *c, DogWS *ws, int stage, const float *in, float *out, int nimg, int in_mod, int nper) {
-    if (ws->tma_row_ok && out == ws->S && stage <= 1 && (ws->tma_row_mask == 1 || ws->tma_row_mask == (stage < 0 ? 2 : 3)) &&
+    if (ws->tma_row_ok && out == ws->S && stage <= 1 &&
         (stage < 0 ? (in >= ws->gray && in < ws->gray + (size_t)ws->B * c->N) : in == (stage == 0 ? ws->I0 : ws->I)))
         return rowscan_tma(c, ws, stage, in, nimg, in_mod, nper);
-    if (c->rowscan_mode == 2) return rowscan_ring(c, stage, in, out, nimg, in_mod, nper);
-    const int bands = (c->h + 31) / 32;
-    const int warps = nimg * bands;
-    const int blocks = rb_div_up(warps, 4);
-    if (stage >= 0)
-        k_rowscan<true><<<blocks, 128, 0, c->stream>>>(in, out, c->w, c->h, nimg, in_mod, nper, c->plan.d[0][stage],
-                                                       c->plan.d[1][stage], c->boxtab + (0 * 3 + stage) * BOX_TAB_N,
-                                                       c->boxtab + (1 * 3 + stage) * BOX_TAB_N);
-    else
-        k_rowscan<false><<<blocks, 128, 0, c->stream>>>(in, out, c->w, c->h, nimg, in_mod, nper, 1, 1, nullptr, nullptr);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
+    return rowscan_ring(c, stage, in, out, nimg, in_mod, nper);
 }
 
-static int blur_dog(rb_ctx *c, DogWS *ws, int nimg, float *img1_opt, int out_slot = 0) {
+static int blur_dog(rb_ctx *c, DogWS *ws, int nimg, float *img1_opt) {
     if (ws->tma_ok && !img1_opt) {
         const CUtensorMap *t = (const CUtensorMap *)ws->tmaps;
         dim3 tg(rb_div_up(c->w, BT_W), rb_div_up(c->h, BT_H), nimg);
         k_blur_dog_tma<<<tg, BT_THREADS, sizeof(BlurTmaSmem) + 128, c->stream>>>(
-            t[TM_I_BLUR], t[TM_IMG0], t[TM_DOG], c->w, c->h, nimg, out_slot, c->plan.d[0][2], c->plan.d[1][2],
+            t[TM_I_BLUR], t[TM_IMG0], t[TM_DOG], c->w, c->h, nimg, 0, c->plan.d[0][2], c->plan.d[1][2],
             c->boxtab + (0 * 3 + 2) * BOX_TAB_N, c->boxtab + (1 * 3 + 2) * BOX_TAB_N, (int *)((char *)c->dev_small + RB_DS_TMA_FAIL));
         RB_LAUNCH_CHECK();
         return RB_OK;
     }
     dim3 grid(rb_div_up(c->w, 256), rb_div_up(c->h, BLUR_RY), nimg);
-    const size_t off = (size_t)out_slot * c->N;
-    k_blur_dog<<<grid, 256, 0, c->stream>>>(ws->I, ws->img0 + off, ws->dog + off, img1_opt, c->w, c->h, nimg,
+    k_blur_dog<<<grid, 256, 0, c->stream>>>(ws->I, ws->img0, ws->dog, img1_opt, c->w, c->h, nimg,
                                             c->plan.d[0][2],
                                             c->plan.d[1][2], c->boxtab + (0 * 3 + 2) * BOX_TAB_N,
                                             c->boxtab + (1 * 3 + 2) * BOX_TAB_N);
@@ -1008,31 +885,20 @@ int rb_dog_make_tables(rb_ctx *c) {
     return RB_OK;
 }
 
+// float4 x 16 rows pipelined
 static int colscan(rb_ctx *c, const float *in, float *out, int nimg) {
-    // default: float4 x 16 rows pipelined; REBVO_B200_COLSCAN=1: the unpipelined float4 x 16 loop
-    const int mode = c->colscan_mode;
-#define COL_PIPE(VW, U)                                                                                                \
-    k_colscan_pipe<VW, U><<<rb_div_up(nimg * (c->w / VW), 64), 64, 0, c->stream>>>(                                      \
-        (const ColVec<VW>::T *)in, (ColVec<VW>::T *)out, c->w / VW, c->h, nimg)
-    if (mode != 1) COL_PIPE(4, 16);
-    else {
-        const int w4 = c->w / 4;
-        const int threads = nimg * w4;
-        k_colscan<<<rb_div_up(threads, 64), 64, 0, c->stream>>>((const float4 *)in, (float4 *)out, w4, c->h, nimg);
-    }
-#undef COL_PIPE
+    k_colscan_pipe<4, 16><<<rb_div_up(nimg * (c->w / 4), 64), 64, 0, c->stream>>>((const float4 *)in, (float4 *)out, c->w / 4,
+                                                                                c->h, nimg);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
 
-// sspace::build for the m images [f0, f0 + m) of the workspace (gray already present): img0 / dog of those slots.  The
-// intermediate planes (S, I0, I) are scratch shared by all ranges: ranges must not run concurrently.
-int rb_dog_build_range(rb_ctx *c, DogWS *ws, int f0, int m) {
-    if (f0 < 0 || m < 1 || f0 + m > ws->B) return RB_ERR_ARG;
+// sspace::build for the m images of the workspace (gray already present)
+int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int m) {
+    if (m < 1 || m > ws->B) return RB_ERR_ARG;
     int r;
-    const size_t N = c->N;
     // iimage::load(in): identical for both filters -> computed once
-    if ((r = rowscan(c, ws, -1, ws->gray + f0 * N, ws->S, m, m, m))) return r;
+    if ((r = rowscan(c, ws, -1, ws->gray, ws->S, m, m, m))) return r;
     if ((r = colscan(c, ws->S, ws->I0, m))) return r;
     // box 0 of both filters reads the shared integral; image index = filter * m + b
     if ((r = rowscan(c, ws, 0, ws->I0, ws->S, 2 * m, m, m))) return r;
@@ -1041,19 +907,7 @@ int rb_dog_build_range(rb_ctx *c, DogWS *ws, int f0, int m) {
     if ((r = rowscan(c, ws, 1, ws->I, ws->S, 2 * m, 2 * m, m))) return r;
     if ((r = colscan(c, ws->S, ws->I, 2 * m))) return r;
     // box 2 + DoG.  Filter f of image b lives at I[(f*m + b)*N]
-    return blur_dog(c, ws, m, nullptr, f0);
-}
-
-// sspace::build for nimg images of the workspace (gray already present)
-int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg) {
-    if (nimg < 1 || nimg > ws->B) return RB_ERR_ARG;
-    int r;
-    // REBVO_B200_DOG_SUB: sub-batches whose intermediate planes (S, I0, I: 20 N bytes per frame) fit in L2 (50 MB on H100)
-    // (the passes are latency-, not capacity-bound); default: the whole batch in one go
-    const int sub = c->dog_sub > 0 ? c->dog_sub : nimg;
-    for (int s = 0; s < nimg; s += sub)
-        if ((r = rb_dog_build_range(c, ws, s, nimg - s < sub ? nimg - s : sub))) return r;
-    return RB_OK;
+    return blur_dog(c, ws, m, nullptr);
 }
 
 // Img(1), dx, dy of image `img` into ws->aux (debug accessor; needs ws->I from the last build with

@@ -31,8 +31,6 @@ __device__ __forceinline__ void d_eye(double *M, double v) {
 struct FrameArgs {
     double t, dt;
     unsigned int frame_count;   // global_tracker::FrameCount of the reference ring slot serving this frame
-    unsigned int next_frame_count;   // ... and of the slot serving the NEXT frame (its loop-body start may be folded into this
-                                     // frame's last kernel, before the next push's arguments exist)
 };
 
 // start of the SecondThread loop body (:167-169) + minimiser priors

@@ -87,9 +87,6 @@ __device__ __forceinline__ void mc_st_async_v2(unsigned int raddr, double a, dou
                  "d"(a), "d"(b), "r"(rmbar)
                  : "memory");
 }
-__device__ __forceinline__ void mc_st_remote_v2(unsigned int raddr, double a, double b) {
-    asm volatile("st.shared::cluster.v2.f64 [%0], {%1, %2};" ::"r"(raddr), "d"(a), "d"(b) : "memory");
-}
 __device__ __forceinline__ void mc_mbar_init(unsigned long long *bar, unsigned int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(mc_smem_u32(bar)), "r"(count) : "memory");
 }
@@ -530,7 +527,6 @@ __device__ __forceinline__ void mc_req_RM(McSmem &sm, int p, const LMState &s) {
     sm.req[p][15] = RMf[4];
 }
 
-template <int XCHG>   // 1: st.async + mbarrier complete_tx; 0: plain DSMEM stores + barrier.cluster
 __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
     k_minimizer_cluster(KLSoA old, const MapState *__restrict__ old_st, const unsigned long long *__restrict__ field,
                         const float4 *__restrict__ fpack, MapState *f_st, LMState *lm_out, int *abort_out, CamC cam,
@@ -638,11 +634,9 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
             }
             lm_request(sm.lm, sm.lm.X, -1, sm.lm.iRN);
         }
-        if (XCHG) {
-            mc_mbar_init(&sm.mbar[0], 1);
-            mc_mbar_init(&sm.mbar[1], 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
+        mc_mbar_init(&sm.mbar[0], 1);
+        mc_mbar_init(&sm.mbar[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         mc_req_R(sm, 0, sm.lm);
         mc_req_RM(sm, 0, sm.lm);
     } else if (tid == 32 && fused) {
@@ -686,7 +680,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         // right after the keyline pass, so that the store latency hides behind the slowest CTA) and add them in cluster
         // order; then every CTA sends its column sum to every CTA of its cluster through distributed shared memory.
         const unsigned int seq = seq0 + 1u + (unsigned int)e;
-        if (XCHG && tid == 0) mc_mbar_expect_tx(&sm.mbar[par], nval * MC_C * 8u);
+        if (tid == 0) mc_mbar_expect_tx(&sm.mbar[par], nval * MC_C * 8u);
         if (wid < 2 && (wid == 0 || two)) {
             const int p = wid;
             double t = lane < MC_PW ? sm.xout[p * MC_PW + lane] : 0.0;
@@ -725,21 +719,17 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
                 const unsigned int dst = idx / (MC_PW / 2), pair = idx - dst * (MC_PW / 2);
                 const unsigned int la = mc_smem_u32(&sm.gather[par][rank][p * MC_PW + 2 * pair]);
                 const double a = sm.xcol[p * MC_PW + 2 * pair], b = sm.xcol[p * MC_PW + 2 * pair + 1];
-                if (XCHG) mc_st_async_v2(mc_mapa(la, dst), a, b, mc_mapa(mc_smem_u32(&sm.mbar[par]), dst));
-                else mc_st_remote_v2(mc_mapa(la, dst), a, b);
+                mc_st_async_v2(mc_mapa(la, dst), a, b, mc_mapa(mc_smem_u32(&sm.mbar[par]), dst));
             }
         }
         MC_STAMP(e, 2);
-        if (!XCHG) mc_cluster_sync();
-        if (wid < 3) {
-            if (XCHG) {   // only the warps that consume the data wait for it
-                const unsigned int ph = (unsigned int)(e >> 1) & 1u;
-                const long long t0 = clock64();
-                while (!mc_mbar_try_wait(&sm.mbar[par], ph)) {
-                    if (clock64() - t0 > MC_SPIN_LIMIT) {
-                        sm.abort = 1;
-                        break;
-                    }
+        if (wid < 3) {   // only the warps that consume the data wait for it
+            const unsigned int ph = (unsigned int)(e >> 1) & 1u;
+            const long long t0 = clock64();
+            while (!mc_mbar_try_wait(&sm.mbar[par], ph)) {
+                if (clock64() - t0 > MC_SPIN_LIMIT) {
+                    sm.abort = 1;
+                    break;
                 }
             }
             MC_STAMP(e, 3);

@@ -53,12 +53,8 @@ struct rb_pipeline {
     cudaStream_t det_stream;
     cudaEvent_t ev_dog, *ev_det, *ev_trk;
     bool overlap;
-    bool q_fold;          // EstimateQuantile + loop-body start of the next frame folded into this frame's map-update kernel
-    int ss_sub;           // frames per scale-space sub-batch built on the detector stream (env REBVO_B200_SS_SUB, 0 = whole batch)
-    bool map_fused;       // gate + Regularize_1_iter + EKF inside the map-update cluster kernel (env REBVO_B200_MAP_FUSED)
     // FordwardMatch's apply + directed_matching in k_match, then gate + Regularize_1_iter + EKF + rotate_keylines in
-    // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the four-kernel chain).  Not with map_fused, whose kernel reads the new map's
-    // rho after matching, which k_match leaves in the regularisation scratch.
+    // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the four-kernel chain)
     bool map_chain;
     // rescaling stream: with DoReScaling=0 a frame's EstimateReScalingOpt changes no keyline and only fills in its nav record,
     // so it runs here (lowest priority) instead of at the end of the frame's tracker chain; the tracker stream joins it
@@ -277,18 +273,10 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
         for (int i = 0; i < pl->pcap; i++) RB_CUDA(cudaEventCreate(&pl->pev[i]));
     }
     {
-        const char *mf = getenv("REBVO_B200_MAP_FUSED");
-        pl->map_fused = mf ? atoi(mf) != 0 : false;   // off by default: the wide kernels under PDL serve
         const char *mc = getenv("REBVO_B200_MAP_CHAIN");
-        pl->map_chain = !(mc && atoi(mc) == 0) && !pl->map_fused;
+        pl->map_chain = !(mc && atoi(mc) == 0);
         const char *ov = getenv("REBVO_B200_OVERLAP");
         pl->overlap = !(ov && ov[0] == '0') && !pl->prof_on;
-        // (off by default: the launch it saves is already hidden by programmatic dependent launch, and it costs the
-        // minimiser its early operand staging)
-        pl->q_fold = getenv("REBVO_B200_Q_FOLD") && atoi(getenv("REBVO_B200_Q_FOLD")) != 0 && p->QCutOffNumBins >= 1 &&
-                     p->QCutOffNumBins <= 128;
-        pl->ss_sub = getenv("REBVO_B200_SS_SUB") ? atoi(getenv("REBVO_B200_SS_SUB")) : 0;
-        if (pl->ss_sub < 4) pl->ss_sub = 0;   // (a sub-batch must cover the frames the detector runs ahead)
         pl->ev_det = new (std::nothrow) cudaEvent_t[max_batch];
         pl->ev_trk = new (std::nothrow) cudaEvent_t[max_batch];
         if (!pl->ev_det || !pl->ev_trk) return RB_ERR_ARG;
@@ -310,9 +298,8 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_det[i], cudaEventDisableTiming));
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
         }
-        // (the inline schedule where the rescaled keylines feed the next frame, the next quantile is folded into the
-        // map-update kernel, the map update is fused, or everything runs on one stream)
-        if (pl->overlap && !pl->q_fold && !pl->map_fused && p->DoReScaling <= 0) {
+        // (the inline schedule where the rescaled keylines feed the next frame, or everything runs on one stream)
+        if (pl->overlap && p->DoReScaling <= 0) {
             int lo = 0, hi = 0;
             RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
             RB_CUDA(cudaStreamCreateWithPriority(&pl->resc_stream, cudaStreamNonBlocking, lo));   // minimiser blocks first
@@ -439,17 +426,15 @@ static int resc_join(rb_pipeline *pl) {
 }
 
 // one frame of the tracker/mapper stage: new = maps[f % RB_NMAPS] (already detected), old = the map of frame f-1
-static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, const FrameArgs *fa, rb_nav *nav_slot) {
+static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArgs *fa, rb_nav *nav_slot) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
     RB_TRACE(c->stream, 1);
     // :167-169 loop-body start (folded into the quantile kernel) ; :172  s_rho_q = old_buf.ef->EstimateQuantile(...)
-    // (q_fold: both were done by the previous frame's map-update kernel, or after k_frame_first for frame 1)
-    if (!pl->q_fold)
-        if ((r = rb_quantile_enqueue(c, old, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, p.QCutOffNumBins, pl->fs,
-                                     &fa->frame_count, neu->st)))
-            return r;
+    if ((r = rb_quantile_enqueue(c, old, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, p.QCutOffNumBins, pl->fs,
+                                 &fa->frame_count, neu->st)))
+        return r;
     // :177  new_buf.gt->build_field(...) only needs the new edge map: enqueue_batch runs it on the detector stream, and
     // clears the new map's FordwardMatch arg-max scratch there, which the minimiser's last evaluation already fills
     // (the clear first: the minimiser stages its operands while the kernel before it runs, and build_field is the longer one)
@@ -471,8 +456,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
     bool folded = false;
     // (since the old map's update only EstimateQuantile -- and build_field of the NEW map without the second stream -- ran
     // on this stream: the minimiser may stage the old map's operands while that kernel is still running)
-    // (with q_fold the previous kernel is the old map's update itself: no early staging)
-    c->min_early = !pl->q_fold && (getenv("REBVO_B200_MIN_EARLY") ? atoi(getenv("REBVO_B200_MIN_EARLY")) != 0 : true);
+    c->min_early = getenv("REBVO_B200_MIN_EARLY") ? atoi(getenv("REBVO_B200_MIN_EARLY")) != 0 : true;
     // (folded: the one-thread stage after the minimiser and FordwardMatch's arg-max ran in its epilogue / last evaluation)
     r = rb_minimizer_enqueue(c, neu, old, pl->fs->VW, &a, 0.0, true, 0, true, pl->fs, &folded);
     c->min_early = false;
@@ -521,13 +505,11 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
             return r;
         RB_TRACE(c->stream, 4);
         prof_mark(pl, ST_DMATCH);
-        // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids (or in the
-        // map-update kernel with map_fused)
-        if (!pl->map_fused)
-            if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
-                                               p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
-                                               side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
-                return r;
+        // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids
+        if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
+                                           p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
+                                           side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
+            return r;
     }
     RB_TRACE(c->stream, 9);
     prof_mark(pl, ST_REG_EKF);
@@ -544,10 +526,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, rb_map *next, 
         RB_TRACE(c->stream, 5);
         return RB_OK;
     }
-    rb_quantile_fold qf = {pl->q_fold ? p.QCutOffNumBins : 0, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, next->st};
-    if ((r = rb_map_update_enqueue(c, neu, p.RegularizeThresh, pl->fs->V, p.ReshapeQAbsolute, p.LocationUncertainty,
-                                   RB_RHO_MAX, 1, p.DoReScaling > 0 ? 1 : 0, pl->fs, p.MatchThreshold, old->st,
-                                   nav_slot, fa, pl->map_fused, &qf)))
+    if ((r = rb_map_update_enqueue(c, neu, RB_RHO_MAX, 1, p.DoReScaling > 0 ? 1 : 0, pl->fs, old->st, nav_slot, fa)))
         return r;
     prof_mark(pl, ST_RESCALE);   // rescaling + pose integration / nav record (folded)
     RB_TRACE(c->stream, 5);
@@ -565,13 +544,7 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     if ((r = gray_pass(pl, fmt, n))) return r;
     prof_mark(pl, ST_GRAY);
     if (with_events) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
-    // The scale space of a batch is a serial prefix of its first frame.  With two
-    // streams only the first ss_sub frames are built here; the detector stream builds the next sub-batch while the
-    // tracker works on this one (it runs up to two frames ahead, more than a sub-batch costs).
-    const int SB = (pl->overlap && pl->ss_sub > 0 && pl->ss_sub < n) ? pl->ss_sub : n;
-    if (SB == n) r = rb_dog_build_batch(c, &pl->ws, n);
-    else r = rb_dog_build_range(c, &pl->ws, 0, SB);
-    if (r) return r;
+    if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
     prof_mark(pl, ST_DOG);
     if (with_events) RB_CUDA(cudaEventRecord(pl->ev[2], c->stream));
     // Two streams, like the reference's first and second thread: the detector of frame f+1 only needs the scale space
@@ -593,13 +566,6 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
             c->stream = pl->det_stream;
         }
         RB_TRACE(c->stream, 6);
-        if (SB < n && i % SB == 2 && i - 2 + SB < n) {   // (after the detector has its two frames of lead)
-            const int f0 = i - 2 + SB;
-            if ((r = rb_dog_build_range(c, &pl->ws, f0, n - f0 < SB ? n - f0 : SB))) {
-                c->stream = main_stream;
-                return r;
-            }
-        }
         r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain);
         prof_mark(pl, ST_DETECT);
         if (!r) r = rb_reestimate_enqueue(c, neu, p.TrackPoints, p.QCutOffNumBins);
@@ -618,12 +584,8 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
         if (fr == 0) {
             k_frame_first<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, pl->nav_dev + i, pl->fa_dev + i);
             RB_LAUNCH_CHECK();
-            if (pl->q_fold)   // what frame 1 starts with: EstimateQuantile of this map + its loop-body start
-                if ((r = rb_quantile_enqueue(c, neu, RB_RHO_MIN, RB_RHO_MAX, p.QCutOffQuantile, p.QCutOffNumBins, pl->fs,
-                                             &(pl->fa_dev + i)->next_frame_count, pl->maps[(fr + 1) % RB_NMAPS]->st)))
-                    return r;
         } else {
-            if ((r = track_frame(pl, neu, old, pl->maps[(fr + 1) % RB_NMAPS], pl->fa_dev + i, pl->nav_dev + i))) return r;
+            if ((r = track_frame(pl, neu, old, pl->fa_dev + i, pl->nav_dev + i))) return r;
         }
         if (pl->mirror_on) {   // the frame's edge map as the reference's records, before the next frame touches it
             const size_t ofs = (size_t)i * pl->mirror_stride;
@@ -673,7 +635,6 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
         pl->fa_pin[i].t = ts[i];
         pl->fa_pin[i].dt = dt;
         pl->fa_pin[i].frame_count = fr > 0 ? (unsigned int)((fr - 1) / 8) : 0;
-        pl->fa_pin[i].next_frame_count = (unsigned int)(fr / 8);   // frame fr+1: ((fr+1)-1)/8
     }
     pl->pn = 0;
     prof_mark(pl, ST_NAV);   // origin of this push
@@ -682,22 +643,10 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     // frames) and the rest: only the head's H2D copy is exposed, the rest of the frames are copied on the copy stream into
     // their own staging region while the head computes (a frame costs ~8x more to track than to copy), and the scale
     // space of the rest still runs as one large batch.
-    // (REBVO_B200_SUB3=1: three stages -- sub/2, 3*sub/2, the rest -- expose half the copy, but add a launch and
-    // smaller scale-space batches)
-    static const bool three = getenv("REBVO_B200_SUB3") && atoi(getenv("REBVO_B200_SUB3")) != 0;
-    int soff[4] = {0, n, n, n}, nsub = 1;
+    int soff[3] = {0, n, n}, nsub = 1;
     if (!(on_device || pl->prof_on || n < 3 * pl->sub)) {
-        if (three && pl->sub >= 4) {
-            const int s0 = pl->sub / 2;
-            soff[1] = s0;
-            soff[2] = 4 * s0;
-            soff[3] = n;
-            nsub = 3;
-        } else {
-            soff[1] = pl->sub;
-            soff[2] = n;
-            nsub = 2;
-        }
+        soff[1] = pl->sub;
+        nsub = 2;
     }
     const size_t fbytes = frame_bytes(c, fmt);   // (ws.rgb holds max_batch frames of either format)
     for (int j = 0; j < nsub; j++) {

@@ -1156,8 +1156,6 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
     c->min_cluster_g = 1;
     const char *fa_ = getenv("REBVO_B200_MIN_FORCE_ABORT");
     c->min_debug_abort = fa_ ? atoi(fa_) : 0;
-    const char *xe = getenv("REBVO_B200_MIN_XCHG");
-    c->min_cluster_xchg = xe ? atoi(xe) : 1;
     int dev_max = 0;
     if (cudaDeviceGetAttribute(&dev_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device) != cudaSuccess) return RB_OK;
     int kfast = MC_KPC_FAST;                   // keylines per cluster rank kept in shared memory (the rest works from global memory)
@@ -1170,8 +1168,7 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
         if (kpc <= 512 * (3584 / 512)) {
             if (kpc > kfast) kpc = kfast;
             const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
-            if (mc_prepare(mc_one::k_minimizer_cluster<1>, 512, 1, dyn, dev_max) &&
-                mc_prepare(mc_one::k_minimizer_cluster<0>, 512, 1, dyn, dev_max)) {
+            if (mc_prepare(mc_one::k_minimizer_cluster, 512, 1, dyn, dev_max)) {
                 c->min_cluster_kpc = kpc;
                 c->min_cluster_dyn = dyn;
             }
@@ -1192,8 +1189,7 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
             int kf2 = (kfast / G + 31) & ~31;
             if (kpc > kf2) kpc = kf2;
             const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
-            if (mc_prepare(mc_multi::k_minimizer_cluster<1>, 256, G, dyn, dev_max) &&
-                mc_prepare(mc_multi::k_minimizer_cluster<0>, 256, G, dyn, dev_max)) {
+            if (mc_prepare(mc_multi::k_minimizer_cluster, 256, G, dyn, dev_max)) {
                 c->min_cluster_g = G;
                 c->min_cluster_kpc_multi = kpc;
                 c->min_cluster_dyn_multi = dyn;
@@ -1220,8 +1216,7 @@ static int launch_minimizer_cluster(rb_ctx *c, rb_map *fmap, rb_map *old, const 
     c->launches++;
     ResPtrs rp;
     for (int i = 0; i < 3; i++) rp.r[i] = fmap->res[i];
-    auto kern = G > 1 ? (c->min_cluster_xchg ? mc_multi::k_minimizer_cluster<1> : mc_multi::k_minimizer_cluster<0>)
-                      : (c->min_cluster_xchg ? mc_one::k_minimizer_cluster<1> : mc_one::k_minimizer_cluster<0>);
+    auto kern = G > 1 ? mc_multi::k_minimizer_cluster : mc_one::k_minimizer_cluster;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, old->kl, (const MapState *)old->st,
                                              (const unsigned long long *)fmap->field, (const float4 *)fmap->kl.pack,
                                              fmap->st, &fmap->ts->lm, &fmap->ts_host.ctl->abort, make_cam(c), plan, su,
@@ -1258,7 +1253,7 @@ int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_
     steps[ns++] = STEP_MAIN_FIRST;
     for (int j = 0; j < m; j++) steps[ns++] = j == m - 1 ? STEP_MAIN_LAST : STEP_MAIN_ITER;
     int r;
-    if (c->min_persist && c->min_cluster && c->min_cluster_kpc > 0 && ns <= MIN_MAX_EVALS) {
+    if (c->min_persist && c->min_cluster_kpc > 0 && ns <= MIN_MAX_EVALS) {
         // rounds of the cluster kernel: the two init tries of type 2 share their rounds
         McPlan plan;
         memset(&plan, 0, sizeof(plan));
@@ -1987,46 +1982,34 @@ int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameSt
 
 
 // =====================================================================================================
-// Map update of a frame in ONE thread-block cluster: Regularize_1_iter (edge_tracker.cpp:87-148),
-// UpdateInverseDepthKalman (:695-724, 954-1055), EstimateReScalingOpt (:1104-1140) and the rescaling itself.
+// EstimateReScalingOpt (edge_tracker.cpp:1104-1140) and the rescaling itself in ONE thread-block cluster.
 //
-// These stages are light per keyline but separated by grid-wide dependencies (the smoothing reads neighbours, each
-// of the five rescaling iterations needs sums over all keylines): as separate kernels, or as one kernel exchanging
-// through L2, a frame paid far more launch / hand-over latency than arithmetic.  A cluster of 16 CTAs holds
-// the whole edge map (thread t of CTA r owns keylines (j*16 + r)*MU_T + t), synchronises with barrier.cluster and
-// all-reduces the two sums of an iteration through distributed shared memory: every CTA stores its pair into every
-// CTA's slot table, one cluster barrier, every CTA adds the 16 pairs in rank order.  One launch, ~6 cluster barriers.
+// The stage is light per keyline, but each of its five iterations needs two sums over all keylines: as separate kernels,
+// or as one kernel exchanging through L2, a frame paid far more launch / hand-over latency than arithmetic.  A cluster of
+// 16 CTAs holds the whole edge map (thread t of CTA r owns keylines (j*16 + r)*MU_T + t) and all-reduces the two sums of
+// an iteration through distributed shared memory: every CTA sends its pair into every CTA's slot table with st.async,
+// completion counted on the receiver's mbarrier, and every CTA adds the 16 pairs in rank order.  One launch, two cluster
+// barriers.
 // Sums: per thread in keyline order, warp xor-tree, warps in order, ranks in order -- fixed, not the reference's
 // sequential order (parity to rounding, as for every other reduction here).
-// The optional head / tail are the per-frame pipeline's scalar glue (frame.cuh), folded in to save their launches.
+// The optional tail is the per-frame pipeline's pose integration and nav record (frame.cuh), folded in to save its launch.
 // =====================================================================================================
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
 #define MU_T 512
 #define MU_C 16   // (non-portable cluster size, like the minimiser's)
-#define MU_QBINS 128   // largest QCutOffNumBins the folded EstimateQuantile takes
 #define MU_KJ 2   // keylines per thread whose rescaling operands stay in registers (kn <= MU_KJ*MU_C*MU_T = 16384)
 
 struct MapUpdArgs {
-    int do_reg, do_ekf, do_rescale, re_escale, gate_post_match;
-    double reg_thresh;
-    const double *vel;       // EKF: translation of the frame (device)
-    double zf, q_abs, loc_unc;
-    double s_rho_min;        // rescaling
+    int re_escale;
+    double s_rho_min;
     unsigned int mnm;
-    const int *enable;       // stage-level API: run only if *enable (nullptr = run)
-    FrameState *fs;          // pipeline: gate = match count (post-match glue folded in), tail = pose integration
-    int match_threshold;
+    const int *enable;       // run only if *enable (nullptr = run)
+    FrameState *fs;          // pipeline: tail = pose integration + nav record
     const MapState *ost;
     const LMState *lm;
     rb_nav *nav;
     const FrameArgs *fa;
-    // EstimateQuantile of THIS map (what the next frame's loop body starts with, rebvo_second_t.cpp:172) and that loop-body
-    // start, folded into the tail: q_bins > 0 enables it
-    int q_bins;
-    double q_min, q_max, q_perc;
-    MapState *nst_next;
-    int xchg;                // 1: st.async + mbarrier all-reduce inside the rescaling iterations, 0: barrier.cluster
     rb_nav *kp_nav;          // pipeline, rescaling on the side stream: the record whose Kp / RKp it fills in (no fs)
 };
 
@@ -2053,207 +2036,112 @@ __device__ __forceinline__ void mu_block_sum2(double &a, double &b, double (*sw)
     __syncthreads();   // sw may be reused
 }
 
-__global__ void __cluster_dims__(MU_C, 1, 1) __launch_bounds__(MU_T) k_map_update(KLSoA kl, MapState *st,
-                                                                                  double *__restrict__ reg_r,
-                                                                                  double *__restrict__ reg_s,
-                                                                                  unsigned char *__restrict__ reg_set,
-                                                                                  MapUpdArgs a) {
+__global__ void __cluster_dims__(MU_C, 1, 1) __launch_bounds__(MU_T) k_map_update(KLSoA kl, MapState *st, MapUpdArgs a) {
     pdl_wait();
     pdl_launch();
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ double sw[MU_T / 32][2];
     __shared__ __align__(16) double slots[2][MU_C][2];   // [iteration parity][rank][sum]
-    __shared__ __align__(8) unsigned long long xbar[2];  // one mbarrier per iteration parity (st.async exchange)
+    __shared__ __align__(8) unsigned long long xbar[2];  // one mbarrier per iteration parity
     __shared__ int xfail;
-    __shared__ int qh[MU_QBINS];           // EstimateQuantile histogram of this CTA's keylines (rank 0, later: the cluster's)
-    __shared__ int qtab[MU_C][MU_QBINS];   // rank 0: every CTA's histogram (plain DSMEM stores: no initialisation to order)
     const int tid = threadIdx.x, rank = (int)cluster.block_rank();
     const int kn = st->kn;
-    if (a.q_bins > 0)
-        for (int b = tid; b < a.q_bins; b += MU_T) qh[b] = 0;   // (complete before anybody adds: cluster barriers below)
-    bool en;
-    if (a.fs && a.gate_post_match) {   // "after directed_matching" gate (rebvo_second_t.cpp:410-423) folded in
-        en = a.fs->do_match && st->nmatch >= a.match_threshold;
-        cluster.sync();   // every CTA has read the gate inputs before CTA 0 rewrites FrameState
-        if (rank == 0 && tid == 0) d_frame_post_match(a.fs, st, a.match_threshold);
-    } else {
-        en = !a.enable || *a.enable;
-    }
     const int i0 = rank * MU_T + tid, stride = MU_C * MU_T;
-    if (en) {
-        // ---- Regularize_1_iter, first half: needs every neighbour's (rho, s_rho) before anybody writes --------
-        if (a.do_reg) {
-            int cnt = 0;
-            for (int i = i0; i < kn; i += stride) cnt += d_reg_a(kl, i, reg_r, reg_s, reg_set, a.reg_thresh) ? 1 : 0;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-            if ((tid & 31) == 0 && cnt) atomicAdd(&st->reg_num, cnt);
-            cluster.sync();
-        }
-        // ---- write-back half + EKF: both only touch the thread's own keyline ------------------------------
-        if (a.do_reg || a.do_ekf) {
-            for (int i = i0; i < kn; i += stride) {
-                double rho, s_rho;
-                if (a.do_reg && reg_set[i]) {
-                    rho = reg_r[i];
-                    s_rho = reg_s[i];
-                    kl.rho[i] = rho;
-                    kl.s_rho[i] = s_rho;
-                } else {
-                    rho = kl.rho[i];
-                    s_rho = kl.s_rho[i];
-                }
-                if (a.do_ekf && kl.m_id[i] >= 0) d_ekf(kl, i, rho, s_rho, a.vel, a.zf, a.q_abs, a.loc_unc);
-            }
-        }
+    if (!a.enable || *a.enable) {
         // ---- EstimateReScalingOpt: 5 fixed-point iterations on Kp -----------------------------------------
-        if (a.do_rescale) {
-            bool valid[MU_KJ];
-            double r2[MU_KJ], r02[MU_KJ], s2[MU_KJ], s0v[MU_KJ];
+        bool valid[MU_KJ];
+        double r2[MU_KJ], r02[MU_KJ], s2[MU_KJ], s0v[MU_KJ];
 #pragma unroll
-            for (int j = 0; j < MU_KJ; j++) {
-                const int i = i0 + j * stride;
-                valid[j] = false;
-                r2[j] = r02[j] = s2[j] = s0v[j] = 0;
-                if (i < kn) {
-                    const double s0 = kl.s_rho0[i], s = kl.s_rho[i];
-                    if (!((unsigned int)kl.m_num[i] < a.mnm || s0 <= 0 || s > a.s_rho_min)) {
-                        const double r = kl.rho[i], r0 = kl.rho0[i];
-                        valid[j] = true;
-                        r2[j] = r * r;
-                        r02[j] = r0 * r0;
-                        s2[j] = s * s;
-                        s0v[j] = s0;
-                    }
-                }
-            }
-            // all-reduce of an iteration's two sums: every CTA sends its pair to every CTA with st.async, completion counted on the
-            // receiver's mbarrier (as in k_minimizer_cluster): no cluster barrier, no fence inside the five dependent iterations
-            // REBVO_B200_MU_XCHG=0: the barrier version (a barrier.cluster per iteration).
-            const bool xchg = a.xchg != 0;
-            if (xchg) {
-                if (tid == 0) {
-                    mc_mbar_init(&xbar[0], 1);
-                    mc_mbar_init(&xbar[1], 1);
-                    xfail = 0;
-                    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-                }
-                cluster.sync();   // every CTA's barriers exist before anybody sends
-            }
-            double Kp = 1.0, RKp = 0;
-            for (int iter = 0; iter < 5; iter++) {
-                if (xchg && tid == 0) mc_mbar_expect_tx(&xbar[iter & 1], MU_C * 16u);
-                double sa = 0, sb = 0;
-#pragma unroll
-                for (int j = 0; j < MU_KJ; j++)
-                    if (valid[j]) {   // r*r/den and r0*r0/den through one reciprocal (div_with_rcp == IEEE division)
-                        const double den = s2[j] + Kp * Kp * s0v[j] * s0v[j];
-                        const double iden = 1 / den;
-                        sa += div_with_rcp(r2[j], den, iden);
-                        sb += div_with_rcp(r02[j], den, iden);
-                    }
-                for (int i = i0 + MU_KJ * stride; i < kn; i += stride) {   // maps beyond the register window
-                    const double s0 = kl.s_rho0[i], s = kl.s_rho[i];
-                    if (!((unsigned int)kl.m_num[i] < a.mnm || s0 <= 0 || s > a.s_rho_min)) {
-                        const double r = kl.rho[i], r0 = kl.rho0[i];
-                        const double den = s * s + Kp * Kp * s0 * s0;
-                        sa += r * r / den;
-                        sb += r0 * r0 / den;
-                    }
-                }
-                mu_block_sum2(sa, sb, sw, tid);
-                if (xchg) {
-                    if (tid < MU_C)
-                        mc_st_async_v2(mc_mapa(mc_smem_u32(&slots[iter & 1][rank][0]), (unsigned int)tid), sa, sb,
-                                       mc_mapa(mc_smem_u32(&xbar[iter & 1]), (unsigned int)tid));
-                    if (tid < 32) {   // one warp waits for the 16 pairs, the block follows through the barrier below
-                        const long long t0 = clock64();
-                        while (!mc_mbar_try_wait(&xbar[iter & 1], (unsigned int)(iter >> 1) & 1u))
-                            if (clock64() - t0 > (1ll << 28)) {
-                                xfail = 1;
-                                break;
-                            }
-                    }
-                    __syncthreads();
-                } else {
-                    if (tid < MU_C) {   // this CTA's pair into every CTA's table
-                        double *dst = cluster.map_shared_rank(&slots[iter & 1][rank][0], tid);
-                        dst[0] = sa;
-                        dst[1] = sb;
-                    }
-                    cluster.sync();
-                }
-                double rTr = 0, rTr0 = 0;
-#pragma unroll
-                for (int k = 0; k < MU_C; k++) {
-                    rTr += slots[iter & 1][k][0];
-                    rTr0 += slots[iter & 1][k][1];
-                }
-                if (kn > 0) {   // "if(kn<=0) return 1;"
-                    Kp = rTr0 > 0 ? sqrt(rTr / rTr0) : 1;
-                    RKp = 1 / rTr0;
-                }
-            }
-            if (xchg && xfail) Kp = RKp = __longlong_as_double(0x7FF8000000000000ll);   // (an exchange timed out: poison, do not hang)
-            if (a.re_escale)
-                for (int i = i0; i < kn; i += stride) {
-                    kl.rho[i] = kl.rho[i] / Kp;
-                    kl.s_rho[i] = kl.s_rho[i] / Kp;
-                }
-            if (rank == 0 && tid == 0) {
-                st->Kp = Kp;
-                if (kn > 0) st->RKp = RKp;
-                if (a.kp_nav) {   // what d_frame_finish takes into the record after a rescaling
-                    a.kp_nav->Kp = st->Kp;
-                    a.kp_nav->RKp = st->RKp;
+        for (int j = 0; j < MU_KJ; j++) {
+            const int i = i0 + j * stride;
+            valid[j] = false;
+            r2[j] = r02[j] = s2[j] = s0v[j] = 0;
+            if (i < kn) {
+                const double s0 = kl.s_rho0[i], s = kl.s_rho[i];
+                if (!((unsigned int)kl.m_num[i] < a.mnm || s0 <= 0 || s > a.s_rho_min)) {
+                    const double r = kl.rho[i], r0 = kl.rho0[i];
+                    valid[j] = true;
+                    r2[j] = r * r;
+                    r02[j] = r0 * r0;
+                    s2[j] = s * s;
+                    s0v[j] = s0;
                 }
             }
         }
-    }
-    if (a.q_bins > 0) {   // EstimateQuantile (edge_finder.cpp: histogram of s_rho over all keylines) on the final s_rho of this map
-        __syncthreads();   // (qh zeroed; this thread's own s_rho writes are visible to it)
-        const double range = a.q_max - a.q_min;
-        for (int i = i0; i < kn; i += stride) {
-            int b = (int)((double)a.q_bins * (kl.s_rho[i] - a.q_min) / range);
-            b = b > a.q_bins - 1 ? a.q_bins - 1 : b;
-            b = b < 0 ? 0 : b;
-            atomicAdd(&qh[b], 1);
+        // all-reduce of an iteration's two sums: every CTA sends its pair to every CTA with st.async, completion counted on the
+        // receiver's mbarrier (as in k_minimizer_cluster): no cluster barrier, no fence inside the five dependent iterations
+        if (tid == 0) {
+            mc_mbar_init(&xbar[0], 1);
+            mc_mbar_init(&xbar[1], 1);
+            xfail = 0;
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
-        __syncthreads();
-        int *t0 = cluster.map_shared_rank(&qtab[rank][0], 0);
-        for (int b = tid; b < a.q_bins; b += MU_T) t0[b] = qh[b];
+        cluster.sync();   // every CTA's barriers exist before anybody sends
+        double Kp = 1.0, RKp = 0;
+        for (int iter = 0; iter < 5; iter++) {
+            if (tid == 0) mc_mbar_expect_tx(&xbar[iter & 1], MU_C * 16u);
+            double sa = 0, sb = 0;
+#pragma unroll
+            for (int j = 0; j < MU_KJ; j++)
+                if (valid[j]) {   // r*r/den and r0*r0/den through one reciprocal (div_with_rcp == IEEE division)
+                    const double den = s2[j] + Kp * Kp * s0v[j] * s0v[j];
+                    const double iden = 1 / den;
+                    sa += div_with_rcp(r2[j], den, iden);
+                    sb += div_with_rcp(r02[j], den, iden);
+                }
+            for (int i = i0 + MU_KJ * stride; i < kn; i += stride) {   // maps beyond the register window
+                const double s0 = kl.s_rho0[i], s = kl.s_rho[i];
+                if (!((unsigned int)kl.m_num[i] < a.mnm || s0 <= 0 || s > a.s_rho_min)) {
+                    const double r = kl.rho[i], r0 = kl.rho0[i];
+                    const double den = s * s + Kp * Kp * s0 * s0;
+                    sa += r * r / den;
+                    sb += r0 * r0 / den;
+                }
+            }
+            mu_block_sum2(sa, sb, sw, tid);
+            if (tid < MU_C)
+                mc_st_async_v2(mc_mapa(mc_smem_u32(&slots[iter & 1][rank][0]), (unsigned int)tid), sa, sb,
+                               mc_mapa(mc_smem_u32(&xbar[iter & 1]), (unsigned int)tid));
+            if (tid < 32) {   // one warp waits for the 16 pairs, the block follows through the barrier below
+                const long long t0 = clock64();
+                while (!mc_mbar_try_wait(&xbar[iter & 1], (unsigned int)(iter >> 1) & 1u))
+                    if (clock64() - t0 > (1ll << 28)) {
+                        xfail = 1;
+                        break;
+                    }
+            }
+            __syncthreads();
+            double rTr = 0, rTr0 = 0;
+#pragma unroll
+            for (int k = 0; k < MU_C; k++) {
+                rTr += slots[iter & 1][k][0];
+                rTr0 += slots[iter & 1][k][1];
+            }
+            if (kn > 0) {   // "if(kn<=0) return 1;"
+                Kp = rTr0 > 0 ? sqrt(rTr / rTr0) : 1;
+                RKp = 1 / rTr0;
+            }
+        }
+        if (xfail) Kp = RKp = __longlong_as_double(0x7FF8000000000000ll);   // (an exchange timed out: poison, do not hang)
+        if (a.re_escale)
+            for (int i = i0; i < kn; i += stride) {
+                kl.rho[i] = kl.rho[i] / Kp;
+                kl.s_rho[i] = kl.s_rho[i] / Kp;
+            }
+        if (rank == 0 && tid == 0) {
+            st->Kp = Kp;
+            if (kn > 0) st->RKp = RKp;
+            if (a.kp_nav) {   // what d_frame_finish takes into the record after a rescaling
+                a.kp_nav->Kp = st->Kp;
+                a.kp_nav->RKp = st->RKp;
+            }
+        }
     }
     cluster.sync();   // no CTA may exit while a peer can still store into its shared memory
-    if (rank == 0 && a.q_bins > 0) {
-        for (int b = tid; b < a.q_bins; b += MU_T) {
-            int t = 0;
-#pragma unroll
-            for (int r = 0; r < MU_C; r++) t += qtab[r][b];
-            qh[b] = t;
-        }
-        __syncthreads();
-    }
-    if (rank == 0 && tid == 0) {
-        if (a.fs && a.nav) d_frame_finish(a.fs, st, a.ost, a.lm->score, a.nav, a.fa, true);
-        if (a.q_bins > 0) {
-            const double range = a.q_max - a.q_min;
-            double q = 1e3;
-            for (int i = 0, acc = 0; i < a.q_bins; i++) {
-                if ((double)acc > a.q_perc * (double)kn) {
-                    q = (double)i * range / (double)a.q_bins + a.q_min;
-                    break;
-                }
-                acc += qh[i];
-            }
-            st->s_rho_q = q;
-            if (a.fs && a.nst_next) d_frame_pre(a.fs, a.fa->next_frame_count, a.nst_next);   // loop-body start of the next frame
-        }
-    }
+    if (rank == 0 && tid == 0 && a.fs && a.nav) d_frame_finish(a.fs, st, a.ost, a.lm->score, a.nav, a.fa, true);
 }
 
-static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a_in, bool pdl) {
-    MapUpdArgs a = a_in;
-    a.xchg = c->mu_xchg ? 1 : 0;
+static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a, bool pdl) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(MU_C);
     cfg.blockDim = dim3(MU_T);
@@ -2263,57 +2151,36 @@ static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a_in, bool 
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
-    TrackState &t = m->ts_host;
     c->launches++;
-    RB_CUDA(cudaLaunchKernelEx(&cfg, k_map_update, m->kl, m->st, t.reg_r, t.reg_s, t.reg_set, a));
+    RB_CUDA(cudaLaunchKernelEx(&cfg, k_map_update, m->kl, m->st, a));
     return RB_OK;
 }
 
-// the pipeline's whole map update (gate, smoothing, EKF, rescaling, pose integration / nav record)
-int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double reg_thresh, const double *vel_dev, double q_abs, double loc_unc,
-                          double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
-                          int match_threshold, const MapState *ost, rb_nav *nav, const FrameArgs *fa, bool fused,
-                          const rb_quantile_fold *qf) {
+// the pipeline's rescaling + pose integration / nav record, after the gate, smoothing and EKF have run on wide grids
+// (rb_regularize_ekf_enqueue or rb_reg_ekf_enqueue) and published fs->do_map
+int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
+                          const MapState *ost, rb_nav *nav, const FrameArgs *fa) {
     MapUpdArgs a;
     memset(&a, 0, sizeof(a));
-    // fused: the match-count gate, Regularize_1_iter and the EKF run inside this cluster kernel too (one launch instead of
-    // three); otherwise the pipeline has run them on wide grids (rb_regularize_ekf_enqueue) and published fs->do_map
-    a.do_reg = a.do_ekf = fused ? 1 : 0;
-    a.do_rescale = 1;
     a.re_escale = re_escale;
-    a.reg_thresh = reg_thresh;
-    a.vel = vel_dev;
-    a.zf = c->zfm;
-    a.q_abs = q_abs;
-    a.loc_unc = loc_unc;
     a.s_rho_min = s_rho_min;
     a.mnm = match_num_min;
     a.fs = fs;
-    a.enable = &fs->do_map;   // published by k_regularize_a_gate
-    a.gate_post_match = fused ? 1 : 0;
-    a.match_threshold = match_threshold;
+    a.enable = &fs->do_map;
     a.ost = ost;
     a.lm = &m->ts->lm;
     a.nav = nav;
     a.fa = fa;
-    if (qf && qf->nbins > 0 && qf->nbins <= MU_QBINS) {
-        a.q_bins = qf->nbins;
-        a.q_min = qf->smin;
-        a.q_max = qf->smax;
-        a.q_perc = qf->perc;
-        a.nst_next = qf->nst_next;
-    }
     return launch_map_update(c, m, a, c->pdl);
 }
 
-// EstimateReScalingOpt alone (stage-level API, and the per-frame pipeline's side stream with kp_nav): the same kernel with
-// only its last phase, hence the same bits.  Launched without programmatic serialization: on the side stream it must not
+// EstimateReScalingOpt alone (stage-level API, and the per-frame pipeline's side stream with kp_nav): the same kernel
+// without its tail, hence the same bits.  Launched without programmatic serialization: on the side stream it must not
 // become resident (16 SMs spinning in griddepcontrol.wait) while the tracker stream's kernels still run.
 int rb_rescale_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale,
                        const int *enable_dev, rb_nav *kp_nav) {
     MapUpdArgs a;
     memset(&a, 0, sizeof(a));
-    a.do_rescale = 1;
     a.re_escale = re_escale;
     a.s_rho_min = s_rho_min;
     a.mnm = match_num_min;

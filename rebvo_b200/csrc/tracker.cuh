@@ -55,12 +55,6 @@ int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_
                          bool *post_folded = nullptr);
 int rb_quantile_enqueue(rb_ctx *c, rb_map *m, double smin, double smax, double perc, int nbins,
                         FrameState *fs = nullptr, const unsigned int *frame_count_dev = nullptr, MapState *nst = nullptr);
-// EstimateQuantile of the map being updated + the next frame's loop-body start, folded into rb_map_update_enqueue's kernel
-struct rb_quantile_fold {
-    int nbins;
-    double smin, smax, perc;
-    MapState *nst_next;
-};
 int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool min_mod_from_state);
 // FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu).
 // With R_dev the apply kernel then runs rotate_keylines(R) on the old map; rb_forward_match_enqueue is the whole stage.
@@ -93,10 +87,8 @@ int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameSt
 int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
                               const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
                               const MapState *ost = nullptr, rb_nav *nav = nullptr, const FrameArgs *fa = nullptr);
-int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double reg_thresh, const double *vel_dev, double q_abs,
-                          double loc_unc, double s_rho_min, unsigned int match_num_min, int re_escale,
-                          FrameState *fs, int match_threshold, const MapState *ost, rb_nav *nav,
-                          const FrameArgs *fa, bool fused = false, const rb_quantile_fold *qf = nullptr);
+int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
+                          const MapState *ost, rb_nav *nav, const FrameArgs *fa);
 int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, double loc_unc,
                    const int *enable_dev);
 int rb_rescale_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale,

@@ -125,14 +125,10 @@ __global__ void __launch_bounds__(256) k_undistort_gray(const uint8_t *const *__
 }
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg) {
     rb_ctx *c = u->c;
-    static const int imgs_env = getenv("REBVO_B200_UG_IMGS") ? atoi(getenv("REBVO_B200_UG_IMGS")) : 4;
-    const int imgs = nimg >= 4 ? imgs_env : 1;
 #define UG_LAUNCH(K)                                                                                                       \
     k_undistort_gray<K><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>((const uint8_t *const *)src_pp, \
                                                                                            gray, u->inx, u->iw, c->N, nimg)
-    if (imgs >= 8) UG_LAUNCH(8);
-    else if (imgs >= 4) UG_LAUNCH(4);
-    else if (imgs >= 2) UG_LAUNCH(2);
+    if (nimg >= 4) UG_LAUNCH(4);
     else UG_LAUNCH(1);
 #undef UG_LAUNCH
     RB_LAUNCH_CHECK();
@@ -181,14 +177,10 @@ __global__ void __launch_bounds__(256) k_undistort_gray_mono(const uint8_t *cons
 }
 int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg) {
     rb_ctx *c = u->c;
-    static const int imgs_env = getenv("REBVO_B200_UG_IMGS") ? atoi(getenv("REBVO_B200_UG_IMGS")) : 4;
-    const int imgs = nimg >= 4 ? imgs_env : 1;
 #define UGM_LAUNCH(K)                                                                                              \
     k_undistort_gray_mono<K><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(              \
         (const uint8_t *const *)src_pp, gray, u->inx, u->iw, c->N, nimg)
-    if (imgs >= 8) UGM_LAUNCH(8);
-    else if (imgs >= 4) UGM_LAUNCH(4);
-    else if (imgs >= 2) UGM_LAUNCH(2);
+    if (nimg >= 4) UGM_LAUNCH(4);
     else UGM_LAUNCH(1);
 #undef UGM_LAUNCH
     RB_LAUNCH_CHECK();

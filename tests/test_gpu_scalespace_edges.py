@@ -43,10 +43,10 @@ def test_odd_geometries_bitwise(built, sigma0):
                 w, h, sigma0, k, int((ref.view(np.uint32) != got[k].view(np.uint32)).sum()))
 
 
-@pytest.mark.parametrize("env", [{"REBVO_B200_ROW_TMA": "0"}, {"REBVO_B200_ROW_TMA": "0", "REBVO_B200_ROWSCAN": "1"},
-                                 {"REBVO_B200_BLUR_TMA": "0"}, {"REBVO_B200_COLSCAN": "1"}, {"REBVO_B200_ROW_NS": "6"}])
+@pytest.mark.parametrize("env", [{"REBVO_B200_ROW_TMA": "0"}, {"REBVO_B200_BLUR_TMA": "0"}])
 def test_kernel_variants_agree(built, monkeypatch, env):
-    """The older kernels stay selectable for A/B measurements: same bits as the default path."""
+    """The non-TMA row and blur passes (which also serve widths the tensor maps cannot take): same bits as the default
+    path."""
     rng = np.random.default_rng(9)
     w, h = 200, 150
     rgb = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
