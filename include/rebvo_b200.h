@@ -50,7 +50,9 @@ typedef struct rb_keyline {
     double stereo_rho, stereo_s_rho;
 } rb_keyline;
 
-/* cam_model (include/UtilLib/cam_model.h:32-50): pinhole part used by the hot path */
+/* cam_model (include/UtilLib/cam_model.h:32-50): pinhole part used by the hot path.  Any w >= 32, h >= 32 (KITTI's
+ * 1241x376 and 1226x370 included): frames are always packed (3*w*h or w*h bytes, no row stride); the device keeps the
+ * scale-space planes in rows padded to a multiple of 4 floats, which no interface exposes. */
 typedef struct rb_camera {
     int32_t w, h;
     float ppx, ppy, zfx, zfy;
@@ -116,6 +118,7 @@ int rb_nav_format_log(const rb_nav *nav, int n, long long first_index, long long
                       size_t *written);
 
 /* ---- context ---------------------------------------------------------------------------------- */
+/* RB_ERR_ARG for cam->w < 32, cam->h < 32 or kl_capacity < 1; every other frame size is accepted */
 int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, double sigma0, double ksigma,
                   int kl_capacity);
 void rb_ctx_destroy(rb_ctx *c);
@@ -127,8 +130,8 @@ int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r);
 /* kernels launched on this context so far (bench.py's gpu_launches) */
 int64_t rb_ctx_launch_count(const rb_ctx *c);
 /* which scale-space kernels a map's own workspace dispatches to, valid after its first rb_map_dog_build: bit 0 = row passes on
- * TMA tiles, bit 1 = last box + DoG on TMA tiles (0 = the pre-TMA kernels: width not a multiple of 4, environment switch, or
- * tensor-map creation failed) */
+ * TMA tiles, bit 1 = last box + DoG on TMA tiles, for any width (0 = the pre-TMA kernels: environment switch, or tensor-map
+ * creation failed) */
 int rb_map_scale_space_path(const rb_map *m);
 
 /* ---- edge map (ring slot) ---------------------------------------------------------------------- */
@@ -254,7 +257,8 @@ int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *
  * image; the records, maps and mirror are bit-identical to rb_pipeline_push of the replicated frames, with and without
  * undistortion, and in IMU mode.  The host copy and the device staging are a third of the RGB24 ones.  A pipeline may
  * alternate formats from push to push.  Arguments are checked like rb_pipeline_push's; the device variant also returns
- * RB_ERR_ARG for a pointer that is not 4-byte aligned (the kernels read 32-bit words), before anything is enqueued. */
+ * RB_ERR_ARG for a pointer that is not 4-byte aligned (the kernels read 32-bit words), before anything is enqueued.  When
+ * w*h is not a multiple of 4 the frames after the first start at unaligned bytes of that buffer; they are read correctly. */
 int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out);
 int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n, rb_nav *nav_out);
 /* REBVO::Reset (rebvo_second_t.cpp:609-620) */

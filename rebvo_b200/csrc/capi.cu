@@ -182,7 +182,7 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     *out = nullptr;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device >= ndev) return RB_ERR_NO_DEVICE;
-    if (cam->w % 4 || cam->w < 32 || cam->h < 32 || kl_capacity < 1) return RB_ERR_ARG;
+    if (cam->w < 32 || cam->h < 32 || kl_capacity < 1) return RB_ERR_ARG;
     rb_ctx *c = new (std::nothrow) rb_ctx;
     if (!c) return RB_ERR_ARG;
     memset(c, 0, sizeof(*c));
@@ -196,6 +196,8 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     c->w = cam->w;
     c->h = cam->h;
     c->N = cam->w * cam->h;
+    c->pitch = (cam->w + 3) & ~3;
+    c->NP = c->pitch * cam->h;
     c->ppx = cam->ppx;
     c->ppy = cam->ppy;
     c->zfm = (double)((cam->zfx + cam->zfy) / 2);  // cam_model: zfm((focal_dist.x+focal_dist.y)/2) in float
@@ -460,7 +462,9 @@ extern "C" int rb_map_upload_gray(rb_map *m, const float *gray) {
     RB_ENTER(m->c);
     rb_ctx *c = m->c;
     if (!m->owns_ws) return RB_ERR_STATE;
-    RB_CUDA(cudaMemcpyAsync(m->ws.gray, gray, (size_t)4 * c->N, cudaMemcpyHostToDevice, c->stream));
+    // w * h floats in, rows of the pitched plane out (its padding columns keep their zeros)
+    RB_CUDA(cudaMemcpy2DAsync(m->ws.gray, (size_t)4 * c->pitch, gray, (size_t)4 * c->w, (size_t)4 * c->w, c->h,
+                              cudaMemcpyHostToDevice, c->stream));
     return RB_OK;
 }
 
@@ -483,9 +487,11 @@ extern "C" int rb_map_get_plane(rb_map *m, int which, float *out) {
     else {
         int r = rb_dog_aux_planes(c, &m->ws, 0);
         if (r) return r;
-        src = m->ws.aux + (size_t)(which == 1 ? 0 : which == 3 ? 1 : 2) * c->N;
+        src = m->ws.aux + (size_t)(which == 1 ? 0 : which == 3 ? 1 : 2) * c->NP;
     }
-    RB_CUDA(cudaMemcpyAsync(out, src, (size_t)4 * c->N, cudaMemcpyDeviceToHost, c->stream));
+    // the pitched plane without its padding columns: w * h floats
+    RB_CUDA(cudaMemcpy2DAsync(out, (size_t)4 * c->w, src, (size_t)4 * c->pitch, (size_t)4 * c->w, c->h,
+                              cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return RB_OK;
 }

@@ -66,16 +66,19 @@ struct BoxPlan {
     double sigma_r[2];
 };
 
-struct DogWS {           // batched scale-space workspace, B images of N floats per plane
+// Batched scale-space workspace, B images per plane.  The float planes are row-pitched: rows of rb_ctx::pitch floats
+// (w rounded up to 4, so every row starts on 16 bytes), NP = pitch * h floats per image; the columns w <= x < pitch are
+// zeroed at allocation and hold zeros throughout.  The byte staging `rgb` is unpitched (packed frames as pushed).
+struct DogWS {
     int B;
     uint8_t *rgb;        // B * 3N    host-input staging: B RGB24 frames, or B mono frames in its first B * N bytes
-    float *gray;         // B * N
-    float *S;            // 2B * N   row-scanned plane (per filter)
-    float *I0;           // B * N    integral of the input (shared by both filters)
-    float *I;            // 2B * N   integral image (per filter)
-    float *img0;         // B * N    blur 0
-    float *dog;          // B * N    blur1 - blur0
-    float *aux;          // 3 * N    on-demand planes (Img(1), dx, dy) for the test/debug accessor
+    float *gray;         // B * NP
+    float *S;            // 2B * NP  row-scanned plane (per filter)
+    float *I0;           // B * NP   integral of the input (shared by both filters)
+    float *I;            // 2B * NP  integral image (per filter)
+    float *img0;         // B * NP   blur 0
+    float *dog;          // B * NP   blur1 - blur0
+    float *aux;          // 3 * NP   on-demand planes (Img(1), dx, dy) for the test/debug accessor
     void *tmaps;         // CUtensorMap[] (host, dog.cu TM_*): TMA-staged row passes, last box + DoG
     bool tma_ok;
     bool tma_row_ok;     // the row passes run on TMA tiles (k_rowscan_tma_*)
@@ -87,6 +90,7 @@ struct rb_ctx {
     cudaStream_t stream;
     rb_camera cam;
     int w, h, N;
+    int pitch, NP;       // scale-space planes: row pitch (w rounded up to 4) and floats per image (pitch * h); see DogWS
     float ppx, ppy;
     double zfm;
     double sigma0, ksigma;

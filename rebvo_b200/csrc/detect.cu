@@ -35,14 +35,15 @@ __global__ void k_update_thresh(DetChain *ch, MapState *st, double gain, int kl_
 
 #define DET_BY 8
 // grid: (ceil(w/32), ceil(h/DET_BY)), block (32, DET_BY).  R = DetectorPlaneFitSize (build_mask's win_s): a (2R+1)^2
-// window, interior R <= x < w-R, R <= y < h-R (edge_finder.cpp:108-109)
+// window, interior R <= x < w-R, R <= y < h-R (edge_finder.cpp:108-109).  img0 / dog are scale-space planes with rows of
+// `pitch` floats; mask and cand are w-indexed.
 template <int R>
 __global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restrict__ img0,
                                                           const float *__restrict__ dog,
                                                           int *__restrict__ mask,
                                                           float4 *__restrict__ cand,
                                                           int *__restrict__ seg_cnt,
-                                                          const MapState *__restrict__ st, int w, int h,
+                                                          const MapState *__restrict__ st, int w, int h, int pitch,
                                                           int nchunk, float per_hist, float dog_thesh_f) {
     constexpr int NW = 2 * R + 1;                  // window width
     constexpr int TW = 32 + 2 * R, TH = DET_BY + 2 * R;
@@ -54,7 +55,7 @@ __global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restric
     for (int i = ty * 32 + lane; i < TH * TW; i += 32 * DET_BY) {
         const int r = i / TW, cc = i - r * TW;
         const int gx = x0 + cc - R, gy = y0 + r - R;
-        sd[r][cc] = (gx >= 0 && gx < w && gy >= 0 && gy < h) ? dog[(size_t)gy * w + gx] : 0.f;
+        sd[r][cc] = (gx >= 0 && gx < w && gy >= 0 && gy < h) ? dog[(size_t)gy * pitch + gx] : 0.f;
     }
     __syncthreads();
     const int x = x0 + lane, y = y0 + ty;
@@ -63,10 +64,10 @@ __global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restric
     float4 pay = make_float4(0.f, 0.f, 0.f, 0.f);
     const bool interior = (x >= R && x < w - R && y >= R && y < h - R);
     if (interior) {
-        const size_t idx = (size_t)y * w + x;
+        const size_t idx = (size_t)y * w + x, ip = (size_t)y * pitch + x;
         const float grad_thesh = st->thresh_used;
-        const float gx = img0[idx + 1] - img0[idx - 1];   // sspace::calc_gradient
-        const float gy = img0[idx + w] - img0[idx - w];
+        const float gx = img0[ip + 1] - img0[ip - 1];     // sspace::calc_gradient
+        const float gy = img0[ip + pitch] - img0[ip - pitch];
         const float n2gI = gx * gx + gy * gy;             // util::norm2
         const float t1 = grad_thesh * (float)RB_MAX_IMG_VALUE;
         bool ok = !(n2gI < t1 * t1);                      // edge_finder.cpp:117-120
@@ -354,9 +355,9 @@ int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
     dim3 ga(nchunk, rb_div_up(h, DET_BY)), ba(32, DET_BY);
     // one instance per radius (k_detect_a<R> is only instantiated for R = 1..RB_PLANE_FIT_MAX)
     void (*const detect_a[RB_PLANE_FIT_MAX])(const float *, const float *, int *, float4 *, int *, const MapState *, int,
-                                             int, int, float, float) = {k_detect_a<1>, k_detect_a<2>, k_detect_a<3>,
-                                                                         k_detect_a<4>};
-    detect_a[R - 1]<<<ga, ba, 0, c->stream>>>(img0, dog, m->mask, c->cand, c->seg_cnt, m->st, w, h, nchunk,
+                                             int, int, int, float, float) = {k_detect_a<1>, k_detect_a<2>, k_detect_a<3>,
+                                                                              k_detect_a<4>};
+    detect_a[R - 1]<<<ga, ba, 0, c->stream>>>(img0, dog, m->mask, c->cand, c->seg_cnt, m->st, w, h, c->pitch, nchunk,
                                               (float)p->pos_neg_thresh, (float)p->dog_thresh);
     RB_LAUNCH_CHECK();
     const int nseg = h * nchunk;

@@ -32,14 +32,15 @@
 // next pixels, and a 32x32 tile degenerates into 32 dependent L2 round trips.
 #define BOX_TAB_W 8
 #define BOX_TAB_N (BOX_TAB_W * BOX_TAB_W)
-__device__ __forceinline__ float box_avg(const float *__restrict__ I, int x, int y, int w, int h, int d,
+// (I has rows of `pitch` floats)
+__device__ __forceinline__ float box_avg(const float *__restrict__ I, int x, int y, int w, int h, int pitch, int d,
                                          int d2, const float *__restrict__ tab) {
     const bool left = x < d2 + 1, right = x >= w - d2;
     const bool top = y < d2 + 1, bottom = y >= h - d2;
     const int xr = right ? w - 1 : x + d2;
     const int yb = bottom ? h - 1 : y + d2;
     const int xl = left ? 0 : x - d2 - 1, yt = top ? 0 : y - d2 - 1;
-    const float A = I[yb * w + xr], B = I[yb * w + xl], C = I[yt * w + xr], D = I[yt * w + xl];
+    const float A = I[yb * pitch + xr], B = I[yb * pitch + xl], C = I[yt * pitch + xr], D = I[yt * pitch + xl];
     const float t1 = bottom ? C : B, t2 = bottom ? B : C;   // bottom band: A-C-B+D, elsewhere A-B-C+D
     const bool h1 = bottom ? !top : !left, h2 = bottom ? !left : !top;
     float r = A;
@@ -85,6 +86,67 @@ __global__ void __launch_bounds__(256) k_mono2gray(const uint32_t *__restrict__ 
     o.y = (float)(3u * ((a >> 8) & 0xff));
     o.z = (float)(3u * ((a >> 16) & 0xff));
     o.w = (float)(3u * (a >> 24));
+    gray[i] = o;
+}
+
+// The same two conversions for widths that are not a multiple of 4 (rows of the gray plane are then pitched, DogWS).  The
+// frames stay packed as pushed (3wh or wh bytes, no stride), so a row -- and, past the first, a frame -- starts at any byte
+// offset, in the staging buffer (the rest of a head / rest push starts mid-buffer) and in a caller's device buffer alike.
+// A thread makes the float4 of 4 pixels of one pitched row (zeros in the padding columns) from the aligned 32-bit words
+// that hold its 12 (RGB) / 4 (mono) source bytes and funnel shifts.  Word indices count from the source rounded down to 4
+// bytes; a word is loaded whole only when it lies inside the batch's bytes [lo, hi), so the (at most two) words that
+// straddle an end of the buffer are assembled from its bytes that do -- no load touches a byte outside the frames.
+__device__ __forceinline__ uint32_t in_word(const uint8_t *__restrict__ p0, long long wi, long long lo, long long hi) {
+    const long long b = 4 * wi;
+    if (b >= lo && b + 4 <= hi) return __ldg(reinterpret_cast<const uint32_t *>(p0) + wi);
+    uint32_t v = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (b + k >= lo && b + k < hi) v |= (uint32_t)__ldg(p0 + b + k) << (8 * k);
+    return v;
+}
+template <bool MONO>
+__global__ void __launch_bounds__(256) k_gray_pitched(const uint8_t *__restrict__ src_fixed,
+                                                      const uint8_t *const *__restrict__ src_pp,
+                                                      float4 *__restrict__ gray, int w, int h, int pitch, int nimg) {
+    const int pv = pitch >> 2;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the pitched batch
+    if (i >= (long long)nimg * h * pv) return;
+    const uint8_t *src = src_pp ? *src_pp : src_fixed;
+    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+    const int cb = MONO ? 1 : 3;   // bytes per pixel
+    const long long lo = (long long)(src - p0), hi = lo + (long long)nimg * cb * w * h;
+    const long long row = i / pv;  // frame * h + y: frames are packed, so the pixel index of the row's start is row * w
+    const int x = 4 * (int)(i - row * pv);
+    const int nv = w - x < 4 ? w - x : 4;   // valid pixels of this float4 (1..4)
+    const long long t = lo + (long long)cb * (row * w + x);   // byte of the first pixel
+    const long long wi = t >> 2, we = (t + cb * nv - 1) >> 2;   // first / last word holding a wanted byte
+    const int sh = (int)(t & 3) * 8;
+    float4 o;
+    if (MONO) {
+        const uint32_t w0 = in_word(p0, wi, lo, hi), w1 = we > wi ? in_word(p0, wi + 1, lo, hi) : 0u;
+        const uint32_t a = __funnelshift_r(w0, w1, sh);   // bytes t .. t+3
+        o.x = (float)(3u * (a & 0xff));
+        o.y = (float)(3u * ((a >> 8) & 0xff));
+        o.z = (float)(3u * ((a >> 16) & 0xff));
+        o.w = (float)(3u * (a >> 24));
+    } else {
+        uint32_t wd[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) wd[k] = wi + k <= we ? in_word(p0, wi + k, lo, hi) : 0u;
+        const uint32_t a = __funnelshift_r(wd[0], wd[1], sh), b = __funnelshift_r(wd[1], wd[2], sh),
+                       c = __funnelshift_r(wd[2], wd[3], sh);   // bytes t .. t+11, as k_rgb2gray's a, b, c
+        o.x = (float)((a & 0xff) + ((a >> 8) & 0xff) + ((a >> 16) & 0xff));
+        o.y = (float)((a >> 24) + (b & 0xff) + ((b >> 8) & 0xff));
+        o.z = (float)(((b >> 16) & 0xff) + (b >> 24) + (c & 0xff));
+        o.w = (float)(((c >> 8) & 0xff) + ((c >> 16) & 0xff) + (c >> 24));
+    }
+    // pixels past w came from the next row's bytes (or zeros): the padding columns get +0
+    if (nv < 4) {
+        o.w = 0.f;
+        if (nv < 3) o.z = 0.f;
+        if (nv < 2) o.y = 0.f;
+    }
     gray[i] = o;
 }
 
@@ -134,7 +196,7 @@ __global__ void __launch_bounds__(64) k_colscan_pipe(const typename ColVec<VW>::
 #define BLUR_RY 4
 __global__ void __launch_bounds__(256) k_blur_dog(const float *__restrict__ I, float *__restrict__ img0,
                                                   float *__restrict__ dog, float *__restrict__ img1_opt,
-                                                  int w, int h, int B, int d0, int d1,
+                                                  int w, int h, int pitch, int B, int d0, int d1,
                                                   const float *__restrict__ tab0, const float *__restrict__ tab1) {
     __shared__ float st0[BOX_TAB_N], st1[BOX_TAB_N];
     if (threadIdx.x < BOX_TAB_N) st0[threadIdx.x] = tab0[threadIdx.x];
@@ -144,7 +206,7 @@ __global__ void __launch_bounds__(256) k_blur_dog(const float *__restrict__ I, f
     const int y0 = blockIdx.y * BLUR_RY;
     const int b = blockIdx.z;
     if (x >= w) return;
-    const size_t N = (size_t)w * h;
+    const size_t N = (size_t)pitch * h;
     const float *I0 = I + (size_t)b * N, *I1 = I + (size_t)(B + b) * N;
     // BLUR_RY rows per thread, unrolled: 8 x BLUR_RY independent taps in flight per thread (one row per thread left
     // the pass latency-bound: 92k tiny blocks, each paying the table load and a barrier for 8 loads per thread)
@@ -152,17 +214,17 @@ __global__ void __launch_bounds__(256) k_blur_dog(const float *__restrict__ I, f
 #pragma unroll
     for (int r = 0; r < BLUR_RY; r++) {
         const int y = min(y0 + r, h - 1);
-        v0[r] = box_avg(I0, x, y, w, h, d0, d0 / 2, st0);
-        v1[r] = box_avg(I1, x, y, w, h, d1, d1 / 2, st1);
+        v0[r] = box_avg(I0, x, y, w, h, pitch, d0, d0 / 2, st0);
+        v1[r] = box_avg(I1, x, y, w, h, pitch, d1, d1 / 2, st1);
     }
 #pragma unroll
     for (int r = 0; r < BLUR_RY; r++) {
         const int y = y0 + r;
         if (y < h) {
-            const size_t o = (size_t)b * N + (size_t)y * w + x;
+            const size_t o = (size_t)b * N + (size_t)y * pitch + x;
             img0[o] = v0[r];
             dog[o] = v1[r] - v0[r];
-            if (img1_opt) img1_opt[(size_t)y * w + x] = v1[r];
+            if (img1_opt) img1_opt[(size_t)y * pitch + x] = v1[r];
         }
     }
 }
@@ -320,7 +382,9 @@ __global__ void __launch_bounds__(BT_THREADS) k_blur_dog_tma(const __grid_consta
 typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                         const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static bool make_tmap3(CUtensorMap *tm, float *base, int w, int h, int nimg, int bw, int bh, bool swizzle128 = false) {
+// dims {w, h, nimg} over rows of `pitch` floats: loads zero-fill and stores clip at column w, the padding is never touched
+static bool make_tmap3(CUtensorMap *tm, float *base, int w, int h, int pitch, int nimg, int bw, int bh,
+                       bool swizzle128 = false) {
     static PFN_tmapEncodeTiled enc = nullptr;
     if (!enc) {
         void *fn = nullptr;
@@ -329,7 +393,7 @@ static bool make_tmap3(CUtensorMap *tm, float *base, int w, int h, int nimg, int
         enc = (PFN_tmapEncodeTiled)fn;
     }
     const cuuint64_t dims[3] = {(cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)nimg};
-    const cuuint64_t strides[2] = {(cuuint64_t)w * 4, (cuuint64_t)w * h * 4};
+    const cuuint64_t strides[2] = {(cuuint64_t)pitch * 4, (cuuint64_t)pitch * h * 4};   // multiples of 16 bytes
     const cuuint32_t box[3] = {(cuuint32_t)bw, (cuuint32_t)bh, 1};
     const cuuint32_t es[3] = {1, 1, 1};
     return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -345,14 +409,14 @@ int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws) {
     const char *er = getenv("REBVO_B200_ROW_TMA");
     const bool want_blur = !(e && atoi(e) == 0), want_row = !(er && atoi(er) == 0);
     if (!want_blur && !want_row) return RB_OK;
-    if ((c->w * 4) % 16) return RB_OK;
     CUtensorMap *t = new (std::nothrow) CUtensorMap[TM_COUNT];
     if (!t) return RB_OK;
     ws->tmaps = t;
+    const int w = c->w, h = c->h, P = c->pitch;
     if (want_blur) {
-        bool ok = make_tmap3(&t[TM_I_BLUR], ws->I, c->w, c->h, 2 * ws->B, BT_BW, BT_BH) &&
-                  make_tmap3(&t[TM_IMG0], ws->img0, c->w, c->h, ws->B, BT_W, BT_H) &&
-                  make_tmap3(&t[TM_DOG], ws->dog, c->w, c->h, ws->B, BT_W, BT_H);
+        bool ok = make_tmap3(&t[TM_I_BLUR], ws->I, w, h, P, 2 * ws->B, BT_BW, BT_BH) &&
+                  make_tmap3(&t[TM_IMG0], ws->img0, w, h, P, ws->B, BT_W, BT_H) &&
+                  make_tmap3(&t[TM_DOG], ws->dog, w, h, P, ws->B, BT_W, BT_H);
         ok = ok && cudaFuncSetAttribute(k_blur_dog_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BlurTmaSmem) + 128) == cudaSuccess;
         if (!ok) cudaGetLastError();
         ws->tma_ok = ok;
@@ -361,12 +425,12 @@ int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws) {
         // row pass: 32 x 32 tiles, 128-byte swizzle on the tiles the sequential scan walks row-wise (gray in, S out); the
         // box-average inputs are (32 + d) x 32 windows read column-wise (no swizzle)
         const int (*d)[3] = c->plan.d;
-        bool ok = make_tmap3(&t[TM_GRAY], ws->gray, c->w, c->h, ws->B, 32, 32, true) &&
-                  make_tmap3(&t[TM_S], ws->S, c->w, c->h, 2 * ws->B, 32, 32, true) &&
-                  make_tmap3(&t[TM_I0_F0], ws->I0, c->w, c->h, ws->B, 32, 32 + d[0][0]) &&
-                  make_tmap3(&t[TM_I0_F1], ws->I0, c->w, c->h, ws->B, 32, 32 + d[1][0]) &&
-                  make_tmap3(&t[TM_I_F0], ws->I, c->w, c->h, 2 * ws->B, 32, 32 + d[0][1]) &&
-                  make_tmap3(&t[TM_I_F1], ws->I, c->w, c->h, 2 * ws->B, 32, 32 + d[1][1]);
+        bool ok = make_tmap3(&t[TM_GRAY], ws->gray, w, h, P, ws->B, 32, 32, true) &&
+                  make_tmap3(&t[TM_S], ws->S, w, h, P, 2 * ws->B, 32, 32, true) &&
+                  make_tmap3(&t[TM_I0_F0], ws->I0, w, h, P, ws->B, 32, 32 + d[0][0]) &&
+                  make_tmap3(&t[TM_I0_F1], ws->I0, w, h, P, ws->B, 32, 32 + d[1][0]) &&
+                  make_tmap3(&t[TM_I_F0], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[0][1]) &&
+                  make_tmap3(&t[TM_I_F1], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[1][1]);
         if (!ok) cudaGetLastError();
         ws->tma_row_ok = ok;
     }
@@ -375,32 +439,31 @@ int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws) {
 
 // sspace::calc_gradient (sspace.cpp:75-85), materialised only for the debug accessor; borders = 0
 __global__ void k_gradient(const float *__restrict__ img0, float *__restrict__ dx, float *__restrict__ dy,
-                           int w, int h) {
+                           int w, int h, int pitch) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= w) return;
     float gx = 0.f, gy = 0.f;
     if (x >= 1 && x < w - 1 && y >= 1 && y < h - 1) {
-        gx = img0[y * w + x + 1] - img0[y * w + x - 1];
-        gy = img0[(y + 1) * w + x] - img0[(y - 1) * w + x];
+        gx = img0[y * pitch + x + 1] - img0[y * pitch + x - 1];
+        gy = img0[(y + 1) * pitch + x] - img0[(y - 1) * pitch + x];
     }
-    dx[y * w + x] = gx;
-    dy[y * w + x] = gy;
+    dx[y * pitch + x] = gx;
+    dy[y * pitch + x] = gy;
 }
 
 // ---------------------------------------------------------------------------------------------------
 int rb_dogws_alloc(rb_ctx *c, DogWS *ws, int B) {
     memset(ws, 0, sizeof(*ws));
     ws->B = B;
-    const size_t N = c->N;
+    const size_t N = c->N, NP = c->NP;
     RB_CUDA(cudaMalloc(&ws->rgb, (size_t)B * 3 * N));
-    RB_CUDA(cudaMalloc(&ws->gray, (size_t)B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->S, (size_t)2 * B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->I0, (size_t)B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->I, (size_t)2 * B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->img0, (size_t)B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->dog, (size_t)B * N * 4));
-    RB_CUDA(cudaMalloc(&ws->aux, (size_t)3 * N * 4));
+    float **planes[] = {&ws->gray, &ws->S, &ws->I0, &ws->I, &ws->img0, &ws->dog, &ws->aux};
+    const size_t count[] = {(size_t)B, 2 * (size_t)B, (size_t)B, 2 * (size_t)B, (size_t)B, (size_t)B, 3};
+    for (int k = 0; k < 7; k++) {
+        RB_CUDA(cudaMalloc(planes[k], count[k] * NP * 4));
+        if (c->pitch != c->w) RB_CUDA(cudaMemset(*planes[k], 0, count[k] * NP * 4));   // the padding columns stay 0
+    }
     return rb_dog_make_tmaps(c, ws);
 }
 
@@ -417,7 +480,16 @@ void rb_dogws_free(DogWS *ws) {
     memset(ws, 0, sizeof(*ws));
 }
 
+static int gray_pitched(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp, bool mono) {
+    const size_t n4 = (size_t)nimg * c->NP / 4;
+    (mono ? k_gray_pitched<true> : k_gray_pitched<false>)<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>(
+        ws->rgb, (const uint8_t *const *)src_pp, (float4 *)ws->gray, c->w, c->h, c->pitch, nimg);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
 int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
+    if (c->pitch != c->w) return gray_pitched(c, ws, nimg, src_pp, false);
     const size_t n4 = (size_t)nimg * c->N / 4;
     k_rgb2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
                                                                    (const uint32_t *const *)src_pp,
@@ -426,8 +498,9 @@ int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
     return RB_OK;
 }
 
-// mono -> gray: nimg frames of N bytes (the source must be 4-byte aligned; N is a multiple of 4)
+// mono -> gray: nimg frames of N bytes (the source must be 4-byte aligned; k_mono2gray when N is a multiple of 4)
 int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
+    if (c->pitch != c->w) return gray_pitched(c, ws, nimg, src_pp, true);
     const size_t n4 = (size_t)nimg * c->N / 4;
     k_mono2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
                                                                     (const uint32_t *const *)src_pp,
@@ -457,8 +530,8 @@ __device__ __forceinline__ void cp_async_wait() {
 
 template <bool AVG>
 __global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *__restrict__ in, float *__restrict__ out,
-                                                                  int w, int h, int nimg, int in_mod, int nper, int d_f0,
-                                                                  int d_f1, const float *__restrict__ tab_f0,
+                                                                  int w, int h, int pitch, int nimg, int in_mod, int nper,
+                                                                  int d_f0, int d_f1, const float *__restrict__ tab_f0,
                                                                   const float *__restrict__ tab_f1, int rmax) {
     extern __shared__ __align__(16) float smem_ring[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -470,7 +543,7 @@ __global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *_
     float *ring = smem_ring + (size_t)warp * (RING_NS * rmax * 32 + 32 * 33 + BOX_TAB_N);
     float(*tile)[33] = reinterpret_cast<float(*)[33]>(ring + RING_NS * rmax * 32);
     float *tab = ring + RING_NS * rmax * 32 + 32 * 33;
-    const size_t N = (size_t)w * h;
+    const size_t N = (size_t)pitch * h;   // (rows of `pitch` floats: every row starts on 16 bytes)
     const float *__restrict__ I = in + (size_t)(img % in_mod) * N;
     float *__restrict__ O = out + (size_t)img * N;
     const bool f1 = (img / nper) != 0;
@@ -498,7 +571,7 @@ __global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *_
             for (int j = sub; j < R; j += 4) {
                 int gy = yb0 + j;
                 gy = gy < 0 ? 0 : (gy > h - 1 ? h - 1 : gy);
-                cp_async16(dst0 + j * 32 + piece * 4, I + (size_t)gy * w + gxc, bytes);
+                cp_async16(dst0 + j * 32 + piece * 4, I + (size_t)gy * pitch + gxc, bytes);
             }
         }
         cp_async_commit();
@@ -572,7 +645,7 @@ __global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *_
         if (x < w) {
 #pragma unroll 8
             for (int r = 0; r < 32; r++)
-                if (y0 + r < h) O[(size_t)(y0 + r) * w + x] = tile[r][lane];
+                if (y0 + r < h) O[(size_t)(y0 + r) * pitch + x] = tile[r][lane];
         }
         __syncwarp();
     }
@@ -795,7 +868,7 @@ static int rowscan_tma(rb_ctx *c, DogWS *ws, int stage, const float *in, int nim
     const int bands = (c->h + 31) / 32;
     int *fail = (int *)((char *)c->dev_small + RB_DS_TMA_FAIL);
     if (stage < 0) {
-        const int zin0 = (int)((in - ws->gray) / (ptrdiff_t)c->N);
+        const int zin0 = (int)((in - ws->gray) / (ptrdiff_t)c->NP);
         k_rowscan_tma_plain<4><<<nimg * bands, 32, 4 * 4096 + 64 + 1024, c->stream>>>(t[TM_GRAY], t[TM_S], c->w, c->h, zin0, fail);
     } else {
         // at most 2 * 4096 + 4 * 47 * 128 + 64 + 256 + 1024 = 33600 bytes (d <= 2 * BOX_TAB_W - 1 = 15): no opt-in above 48 KB
@@ -825,11 +898,11 @@ static int rowscan_ring(rb_ctx *c, int stage, const float *in, float *out, int n
     const size_t smem = (size_t)RING_WARPS * (RING_NS * rmax * 32 + 32 * 33 + BOX_TAB_N) * sizeof(float);
     if (stage >= 0) {
         k_rowscan_ring<true><<<blocks, 32 * RING_WARPS, smem, c->stream>>>(
-            in, out, c->w, c->h, nimg, in_mod, nper, c->plan.d[0][stage], c->plan.d[1][stage],
+            in, out, c->w, c->h, c->pitch, nimg, in_mod, nper, c->plan.d[0][stage], c->plan.d[1][stage],
             c->boxtab + (0 * 3 + stage) * BOX_TAB_N, c->boxtab + (1 * 3 + stage) * BOX_TAB_N, rmax);
     } else {
-        k_rowscan_ring<false><<<blocks, 32 * RING_WARPS, smem, c->stream>>>(in, out, c->w, c->h, nimg, in_mod, nper, 1, 1,
-                                                                          nullptr, nullptr, rmax);
+        k_rowscan_ring<false><<<blocks, 32 * RING_WARPS, smem, c->stream>>>(in, out, c->w, c->h, c->pitch, nimg, in_mod,
+                                                                          nper, 1, 1, nullptr, nullptr, rmax);
     }
     RB_LAUNCH_CHECK();
     return RB_OK;
@@ -838,7 +911,7 @@ static int rowscan_ring(rb_ctx *c, int stage, const float *in, float *out, int n
 // stage < 0: plain row scan of the input; stage 0..1: row scan of box `stage` of both filters
 static int rowscan(rb_ctx *c, DogWS *ws, int stage, const float *in, float *out, int nimg, int in_mod, int nper) {
     if (ws->tma_row_ok && out == ws->S && stage <= 1 &&
-        (stage < 0 ? (in >= ws->gray && in < ws->gray + (size_t)ws->B * c->N) : in == (stage == 0 ? ws->I0 : ws->I)))
+        (stage < 0 ? (in >= ws->gray && in < ws->gray + (size_t)ws->B * c->NP) : in == (stage == 0 ? ws->I0 : ws->I)))
         return rowscan_tma(c, ws, stage, in, nimg, in_mod, nper);
     return rowscan_ring(c, stage, in, out, nimg, in_mod, nper);
 }
@@ -854,7 +927,7 @@ static int blur_dog(rb_ctx *c, DogWS *ws, int nimg, float *img1_opt) {
         return RB_OK;
     }
     dim3 grid(rb_div_up(c->w, 256), rb_div_up(c->h, BLUR_RY), nimg);
-    k_blur_dog<<<grid, 256, 0, c->stream>>>(ws->I, ws->img0, ws->dog, img1_opt, c->w, c->h, nimg,
+    k_blur_dog<<<grid, 256, 0, c->stream>>>(ws->I, ws->img0, ws->dog, img1_opt, c->w, c->h, c->pitch, nimg,
                                             c->plan.d[0][2],
                                             c->plan.d[1][2], c->boxtab + (0 * 3 + 2) * BOX_TAB_N,
                                             c->boxtab + (1 * 3 + 2) * BOX_TAB_N);
@@ -885,10 +958,10 @@ int rb_dog_make_tables(rb_ctx *c) {
     return RB_OK;
 }
 
-// float4 x 16 rows pipelined
+// float4 x 16 rows pipelined, over whole pitched rows (the padding columns add up zeros)
 static int colscan(rb_ctx *c, const float *in, float *out, int nimg) {
-    k_colscan_pipe<4, 16><<<rb_div_up(nimg * (c->w / 4), 64), 64, 0, c->stream>>>((const float4 *)in, (float4 *)out, c->w / 4,
-                                                                                c->h, nimg);
+    const int wv = c->pitch / 4;
+    k_colscan_pipe<4, 16><<<rb_div_up(nimg * wv, 64), 64, 0, c->stream>>>((const float4 *)in, (float4 *)out, wv, c->h, nimg);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
@@ -917,8 +990,7 @@ int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img) {
     int r = blur_dog(c, ws, 1, ws->aux);
     if (r) return r;
     dim3 grid(rb_div_up(c->w, 256), c->h, 1);
-    k_gradient<<<grid, 256, 0, c->stream>>>(ws->img0, ws->aux + c->N, ws->aux + 2 * (size_t)c->N, c->w,
-                                            c->h);
+    k_gradient<<<grid, 256, 0, c->stream>>>(ws->img0, ws->aux + c->NP, ws->aux + 2 * (size_t)c->NP, c->w, c->h, c->pitch);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }

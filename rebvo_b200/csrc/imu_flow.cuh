@@ -282,7 +282,7 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bo
     for (int i = 0; i < n; i++) {
         const long long fr = pl->n_pushed + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
-        const float *img0 = pl->ws.img0 + (size_t)i * c->N, *dog = pl->ws.dog + (size_t)i * c->N;
+        const float *img0 = pl->ws.img0 + (size_t)i * c->NP, *dog = pl->ws.dog + (size_t)i * c->NP;
         if ((r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain))) return r;
         if ((r = rb_reestimate_enqueue(c, neu, p.TrackPoints, p.QCutOffNumBins))) return r;
         // FirstThr :296: the gyro / accelerometer samples between the previous frame and this one

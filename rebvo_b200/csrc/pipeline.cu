@@ -559,7 +559,7 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     for (int i = 0; i < n; i++) {
         const long long fr = first_frame + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
-        const float *img0 = pl->ws.img0 + (size_t)i * c->N, *dog = pl->ws.dog + (size_t)i * c->N;
+        const float *img0 = pl->ws.img0 + (size_t)i * c->NP, *dog = pl->ws.dog + (size_t)i * c->NP;
         // FirstThr: detect + reEstimateThresh (rebvo_first_t.cpp:266-272)
         if (ov) {
             if (i >= 2) RB_CUDA(cudaStreamWaitEvent(pl->det_stream, pl->ev_trk[i - 2], 0));

@@ -105,31 +105,88 @@ __device__ __forceinline__ float ug_pixel(const uint8_t *__restrict__ src, const
     const unsigned int s = (unsigned int)((uint8_t)(r >> 16)) + (unsigned int)((uint8_t)(g >> 16)) + (unsigned int)((uint8_t)(b >> 16));
     return (float)s;
 }
+// Widths that are not a multiple of 4 (ANYW below): the gray plane has rows of `pitch` floats, and a frame of 3N (RGB) or N
+// (mono) bytes may start at any byte offset -- the frames after the first one, the rest of a head / rest push, a caller's
+// device buffer.  Word indices then count from the batch's source rounded down to 4 bytes, and the frame starts at byte t0 of
+// that word array; a word is loaded whole when it lies inside the batch's bytes [lo, hi), the (at most two) words that
+// straddle an end of the buffer are assembled from its bytes that do.
+__device__ __forceinline__ unsigned int ug_word(const uint8_t *__restrict__ p0, long long wi, long long lo, long long hi) {
+    const long long b = 4 * wi;
+    if (b >= lo && b + 4 <= hi) return __ldg(reinterpret_cast<const unsigned int *>(p0) + wi);
+    unsigned int v = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (b + k >= lo && b + k < hi) v |= (unsigned int)__ldg(p0 + b + k) << (8 * k);
+    return v;
+}
+__device__ __forceinline__ float ug_pixel_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
+                                              const int4 ix, const int4 w) {
+    int r = 0, g = 0, b = 0;
+    if (ix.y == ix.x + 1 && ix.w == ix.z + 1) {   // two runs of two adjacent pixels, as ug_pixel
+#pragma unroll
+        for (int row = 0; row < 2; row++) {
+            const long long ofs = t0 + 3 * (row ? ix.z : ix.x), wi = ofs >> 2;
+            const int sh = (int)(ofs & 3) * 8;
+            const unsigned int w0 = ug_word(p0, wi, lo, hi), w1 = ug_word(p0, wi + 1, lo, hi), w2 = ug_word(p0, wi + 2, lo, hi);
+            const unsigned int l = __funnelshift_r(w0, w1, sh), m = __funnelshift_r(w1, w2, sh);
+            ug_acc(l, row ? w.z : w.x, r, g, b);
+            ug_acc(__funnelshift_r(l, m, 24), row ? w.w : w.y, r, g, b);
+        }
+    } else {
+        const int t[4] = {ix.x, ix.y, ix.z, ix.w}, ww[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const long long ofs = t0 + 3 * t[k], wi = ofs >> 2;
+            ug_acc(__funnelshift_r(ug_word(p0, wi, lo, hi), ug_word(p0, wi + 1, lo, hi), (int)(ofs & 3) * 8), ww[k], r, g, b);
+        }
+    }
+    const unsigned int s = (unsigned int)((uint8_t)(r >> 16)) + (unsigned int)((uint8_t)(g >> 16)) + (unsigned int)((uint8_t)(b >> 16));
+    return (float)s;
+}
 // IMGS frames per thread: the 32-byte map entry of a pixel (L2-resident, but 739 MB of L2 reads per 64-frame launch when every
-// frame fetches it again) is loaded once for IMGS frames
-template <int IMGS>
+// frame fetches it again) is loaded once for IMGS frames.  ANYW: any width (see ug_pixel_any); otherwise w % 4 == 0, the plane
+// is unpitched and the frames are word-aligned whenever the source is.
+template <int IMGS, bool ANYW>
 __global__ void __launch_bounds__(256) k_undistort_gray(const uint8_t *const *__restrict__ src_pp, float *__restrict__ gray,
                                                         const int4 *__restrict__ inx, const int4 *__restrict__ iw, int N,
-                                                        int nimg) {
+                                                        int nimg, int wd, int pitch) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int img0 = blockIdx.y * IMGS;
     if (i >= N) return;
     const int4 ix = inx[i], w = iw[i];
-    const uint8_t *src = *src_pp + (size_t)img0 * 3 * N;
     float v[IMGS];
+    if (ANYW) {
+        const uint8_t *src = *src_pp;
+        const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+        const long long lo = (long long)(src - p0), hi = lo + 3ll * N * nimg;
 #pragma unroll
-    for (int k = 0; k < IMGS; k++) v[k] = img0 + k < nimg ? ug_pixel(src + (size_t)k * 3 * N, ix, w, N) : 0.f;
+        for (int k = 0; k < IMGS; k++)
+            v[k] = img0 + k < nimg ? ug_pixel_any(p0, lo + 3ll * N * (img0 + k), lo, hi, ix, w) : 0.f;
+    } else {
+        const uint8_t *src = *src_pp + (size_t)img0 * 3 * N;
+#pragma unroll
+        for (int k = 0; k < IMGS; k++) v[k] = img0 + k < nimg ? ug_pixel(src + (size_t)k * 3 * N, ix, w, N) : 0.f;
+    }
+    const int y = ANYW ? i / wd : 0;
+    const size_t o = ANYW ? (size_t)y * pitch + (i - y * wd) : (size_t)i;   // gray[y * pitch + x]
+    const size_t plane = ANYW ? (size_t)pitch * (N / wd) : (size_t)N;
 #pragma unroll
     for (int k = 0; k < IMGS; k++)
-        if (img0 + k < nimg) gray[(size_t)(img0 + k) * N + i] = v[k];
+        if (img0 + k < nimg) gray[(size_t)(img0 + k) * plane + o] = v[k];
 }
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg) {
     rb_ctx *c = u->c;
-#define UG_LAUNCH(K)                                                                                                       \
-    k_undistort_gray<K><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>((const uint8_t *const *)src_pp, \
-                                                                                           gray, u->inx, u->iw, c->N, nimg)
-    if (nimg >= 4) UG_LAUNCH(4);
-    else UG_LAUNCH(1);
+#define UG_LAUNCH(K, A)                                                                                                    \
+    k_undistort_gray<K, A><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(                        \
+        (const uint8_t *const *)src_pp, gray, u->inx, u->iw, c->N, nimg, c->w, c->pitch)
+    const bool any = c->pitch != c->w;
+    if (nimg >= 4) {
+        if (any) UG_LAUNCH(4, true);
+        else UG_LAUNCH(4, false);
+    } else {
+        if (any) UG_LAUNCH(1, true);
+        else UG_LAUNCH(1, false);
+    }
 #undef UG_LAUNCH
     RB_LAUNCH_CHECK();
     return RB_OK;
@@ -159,29 +216,69 @@ __device__ __forceinline__ float ug_pixel_mono(const uint8_t *__restrict__ src, 
     }
     return (float)(3u * (unsigned int)(uint8_t)(s >> 16));
 }
-template <int IMGS>
+// Any width: frame f starts at byte t0 = lo + f * N of the word array from the aligned-down source (the device entry point
+// keeps its rule that the source is 4-byte aligned, so lo = 0 there; the frames after the first start at any byte when
+// N % 4 != 0).  The pair's second byte t0 + ix.x + 1 is inside the frame, so when the pair straddles a word boundary its
+// second word holds a byte of the batch and ug_word reads it whole or byte by byte.
+__device__ __forceinline__ float ug_pixel_mono_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
+                                                   const int4 ix, const int4 w) {
+    int s;
+    if (ix.y == ix.x + 1 && ix.w == ix.z + 1) {
+        s = 0;
+#pragma unroll
+        for (int row = 0; row < 2; row++) {
+            const long long ofs = t0 + (row ? ix.z : ix.x), wi = ofs >> 2;
+            const unsigned int w0 = ug_word(p0, wi, lo, hi), w1 = (ofs & 3) == 3 ? ug_word(p0, wi + 1, lo, hi) : w0;
+            const unsigned int v = __funnelshift_r(w0, w1, (int)(ofs & 3) * 8);   // bytes ofs, ofs + 1 in the low half
+            s += (row ? w.z : w.x) * (int)(v & 0xffu) + (row ? w.w : w.y) * (int)((v >> 8) & 0xffu);
+        }
+    } else {
+        s = w.x * (int)__ldg(p0 + t0 + ix.x) + w.y * (int)__ldg(p0 + t0 + ix.y) + w.z * (int)__ldg(p0 + t0 + ix.z) +
+            w.w * (int)__ldg(p0 + t0 + ix.w);
+    }
+    return (float)(3u * (unsigned int)(uint8_t)(s >> 16));
+}
+template <int IMGS, bool ANYW>
 __global__ void __launch_bounds__(256) k_undistort_gray_mono(const uint8_t *const *__restrict__ src_pp,
                                                              float *__restrict__ gray, const int4 *__restrict__ inx,
-                                                             const int4 *__restrict__ iw, int N, int nimg) {
+                                                             const int4 *__restrict__ iw, int N, int nimg, int wd, int pitch) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int img0 = blockIdx.y * IMGS;
     if (i >= N) return;
     const int4 ix = inx[i], w = iw[i];
-    const uint8_t *src = *src_pp + (size_t)img0 * N;
     float v[IMGS];
+    if (ANYW) {
+        const uint8_t *src = *src_pp;
+        const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+        const long long lo = (long long)(src - p0), hi = lo + (long long)N * nimg;
 #pragma unroll
-    for (int k = 0; k < IMGS; k++) v[k] = img0 + k < nimg ? ug_pixel_mono(src + (size_t)k * N, ix, w) : 0.f;
+        for (int k = 0; k < IMGS; k++)
+            v[k] = img0 + k < nimg ? ug_pixel_mono_any(p0, lo + (long long)N * (img0 + k), lo, hi, ix, w) : 0.f;
+    } else {
+        const uint8_t *src = *src_pp + (size_t)img0 * N;
+#pragma unroll
+        for (int k = 0; k < IMGS; k++) v[k] = img0 + k < nimg ? ug_pixel_mono(src + (size_t)k * N, ix, w) : 0.f;
+    }
+    const int y = ANYW ? i / wd : 0;
+    const size_t o = ANYW ? (size_t)y * pitch + (i - y * wd) : (size_t)i;   // gray[y * pitch + x]
+    const size_t plane = ANYW ? (size_t)pitch * (N / wd) : (size_t)N;
 #pragma unroll
     for (int k = 0; k < IMGS; k++)
-        if (img0 + k < nimg) gray[(size_t)(img0 + k) * N + i] = v[k];
+        if (img0 + k < nimg) gray[(size_t)(img0 + k) * plane + o] = v[k];
 }
 int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg) {
     rb_ctx *c = u->c;
-#define UGM_LAUNCH(K)                                                                                              \
-    k_undistort_gray_mono<K><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(              \
-        (const uint8_t *const *)src_pp, gray, u->inx, u->iw, c->N, nimg)
-    if (nimg >= 4) UGM_LAUNCH(4);
-    else UGM_LAUNCH(1);
+#define UGM_LAUNCH(K, A)                                                                                           \
+    k_undistort_gray_mono<K, A><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(           \
+        (const uint8_t *const *)src_pp, gray, u->inx, u->iw, c->N, nimg, c->w, c->pitch)
+    const bool any = c->pitch != c->w;
+    if (nimg >= 4) {
+        if (any) UGM_LAUNCH(4, true);
+        else UGM_LAUNCH(4, false);
+    } else {
+        if (any) UGM_LAUNCH(1, true);
+        else UGM_LAUNCH(1, false);
+    }
 #undef UGM_LAUNCH
     RB_LAUNCH_CHECK();
     return RB_OK;

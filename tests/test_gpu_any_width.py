@@ -1,0 +1,373 @@
+"""Frames of any width (w % 4 != 0): the scale-space planes are row-pitched (rows of w rounded up to 4 floats) and the input
+stage reads packed frames whose rows and frames start at any byte.  KITTI odometry's 1241x376 and 1226x370, and geometries
+with w = 1, 2, 3 (mod 4) and w * h odd or even, against the reference (compiled from its sources into oracle/_ref, which
+takes any size): scale-space planes and the detector bit for bit, the fused pipeline and the unmodified REBVO on the shim
+against the reference's three-thread run, and every way of feeding frames byte-identical to the host RGB push."""
+import os
+
+import numpy as np
+import pytest
+
+from parity_util import DOG_THRESH, KL_EXACT_DETECT, POS_NEG
+from plane_fit import ref_detect_child
+
+pytestmark = pytest.mark.gpu
+
+GEOMETRIES = [(1241, 376), (1226, 370), (750, 97), (37, 33), (331, 244)]
+KITTI = [(1241, 376), (1226, 370)]
+NF = 60
+KC = (-0.12, 0.03, 0.0, 1e-4, 2e-5)   # a mild rad-tan model for UseUndistort=1
+
+
+def _cam(w, h):
+    return dict(w=w, h=h, zfx=718.856, zfy=718.856, ppx=w / 2.0 - 13.3, ppy=h / 2.0 - 2.8)
+
+
+def _seq(w, h, seed=7):
+    from rebvo_b200 import synth
+    return synth.Sequence(w=w, h=h, seed=seed, zf=718.0)
+
+
+def _u32(a):
+    return np.ascontiguousarray(a).view(np.uint32)
+
+
+def _raw(nav):
+    return np.ascontiguousarray(nav).view(np.uint8)
+
+
+# ---- 1. scale space -------------------------------------------------------------------------------------------------
+def _inputs(w, h, seed):
+    rng = np.random.default_rng(seed)
+    rgb = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+    rgb[h // 3:, w // 4:] //= 3   # an edge, so that the planes are not just noise
+    mono = rng.integers(0, 256, (h, w), dtype=np.uint8)
+    mono[: h // 2, w // 3:] //= 4
+    gray = (rng.random((h, w)) * 765.0).astype(np.float32)
+    return rgb, mono, gray
+
+
+def _ref_planes(w, h, sigma0, how, img):
+    from oracle import refapi
+    r = refapi.RefMap(w, h, w / 2.0, h / 2.0, 300.0, 300.0, sigma0, 1.2599)
+    if how == "gray":
+        r.set_gray(img)
+    else:
+        r.rgb2bw(img if how == "rgb" else np.repeat(img[:, :, None], 3, axis=2))
+    r.build()
+    return {k: r.plane(k).copy() for k in ("gray", "img0", "img1", "dog")}
+
+
+def _gpu_planes(w, h, sigma0, how, img):
+    from rebvo_b200 import capi
+    cam = dict(w=w, h=h, zfx=300.0, zfy=300.0, ppx=w / 2.0, ppy=h / 2.0)
+    ctx = capi.Ctx(cam, sigma0, 1.2599, kl_capacity=20000)
+    m = ctx.new_map()
+    getattr(m, "upload_" + how)(img)
+    m.dog_build()
+    out = {k: m.plane(k).copy() for k in ("gray", "img0", "img1", "dog")}
+    path = m.scale_space_path()
+    m.close()
+    ctx.close()
+    return out, path
+
+
+@pytest.mark.parametrize("env", [{}, {"REBVO_B200_ROW_TMA": "0"}, {"REBVO_B200_BLUR_TMA": "0"}],
+                         ids=["tma", "ring_rows", "plain_blur"])
+@pytest.mark.parametrize("sigma0", [1.7818, 3.56359])
+def test_scale_space_bitwise(built, monkeypatch, sigma0, env):
+    """gray, Img(0), Img(1), DoG of RGB, mono and float uploads equal the reference's sspace::build bit for bit; the TMA
+    kernels serve these widths (path 3), and the non-TMA row / blur passes give the same bits."""
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    want_path = 3 & ~(1 if env.get("REBVO_B200_ROW_TMA") == "0" else 0) & ~(2 if env.get("REBVO_B200_BLUR_TMA") == "0" else 0)
+    for gi, (w, h) in enumerate(GEOMETRIES):
+        rgb, mono, gray = _inputs(w, h, 100 + gi)
+        for how, img in (("rgb", rgb), ("mono", mono), ("gray", gray)):
+            ref = _ref_planes(w, h, sigma0, how, img)
+            got, path = _gpu_planes(w, h, sigma0, how, img)
+            assert path == want_path, (w, h, how, path)
+            for k in ref:
+                assert ref[k].shape == got[k].shape == (h, w)
+                bad = int((_u32(ref[k]) != _u32(got[k])).sum())
+                assert bad == 0, "%dx%d sigma0 %.2f %s upload, plane %s: %d pixels differ" % (w, h, sigma0, how, k, bad)
+            if how == "mono":
+                assert np.array_equal(got["gray"], 3.0 * mono.astype(np.float32))
+
+
+def test_context_size_limits(built):
+    """Any width and height from 32 up is accepted, narrower or shorter frames are not."""
+    from rebvo_b200 import capi
+    for w, h in ((32, 32), (33, 32), (34, 35), (35, 32), (1241, 376)):
+        capi.Ctx(_cam(w, h), 1.7818, 1.2599, kl_capacity=1000).close()
+    for w, h in ((31, 64), (64, 31)):
+        with pytest.raises(capi.RbError):
+            capi.Ctx(_cam(w, h), 1.7818, 1.2599, kl_capacity=1000)
+
+
+# ---- 2. detector ----------------------------------------------------------------------------------------------------
+def _det_cfg(w, h):
+    return dict(name="kitti", cam=_cam(w, h), sigma0=3.56359, ksigma=1.2599, thresh=0.01, gain=5e-7, tmax=0.5,
+                tmin=0.005, kl_max=40000, kl_ref=15000, track_points=12000)
+
+
+def _frames3(w, h):
+    seq = _seq(w, h, seed=21)
+    return np.stack([seq.frame(i)[1] for i in (10, 11, 12)])
+
+
+def _det(capi, R, cfg):
+    return capi.DetectParams(R, POS_NEG, DOG_THRESH, cfg["kl_max"], cfg["kl_ref"], cfg["gain"], cfg["tmax"], cfg["tmin"])
+
+
+def _gpu_detect(cfg, frames, R):
+    """detect + reEstimateThresh on each frame, the threshold chained: [(kn, tresh, l_kl_num, keylines, mask, retuned)]"""
+    from rebvo_b200 import capi
+    ctx = capi.Ctx(cfg["cam"], cfg["sigma0"], cfg["ksigma"], kl_capacity=50000)
+    t, l, out = cfg["thresh"], 0, []
+    for fr in frames:
+        m = ctx.new_map()
+        m.upload_rgb(fr)
+        m.dog_build()
+        kn, t, l = m.detect(_det(capi, R, cfg), t, l)
+        out.append((kn, t, l, m.keylines(), m.mask(), m.reestimate(cfg["track_points"], 100)))
+        m.close()
+    ctx.close()
+    return out
+
+
+def _assert_detect(got, ref_kn_t_l, ref_kl, ref_mask, ref_retuned, what):
+    kn, t, l, kl, mask, retuned = got
+    assert [kn, t, l] == list(ref_kn_t_l), "%s: kn/tresh/l_kl_num gpu %s ref %s" % (what, [kn, t, l], list(ref_kn_t_l))
+    assert kn > 1000, what
+    assert len(kl) == len(ref_kl), what
+    for f in KL_EXACT_DETECT:
+        assert np.array_equal(np.ascontiguousarray(ref_kl[f]).view(np.uint8), np.ascontiguousarray(kl[f]).view(np.uint8)), \
+            "%s: keyline field %s" % (what, f)
+    assert np.array_equal(ref_mask, mask), "%s: mask" % what
+    assert np.float32(retuned) == np.float32(ref_retuned), "%s: reTunedThresh gpu %r ref %r" % (what, retuned, ref_retuned)
+
+
+@pytest.mark.parametrize("wh", KITTI, ids=["1241x376", "1226x370"])
+def test_detector_r2_vs_reference(built, wh):
+    """DetectorPlaneFitSize 2 against the in-process reference: keylines, mask, kn and the threshold feedback over three
+    chained frames, and reEstimateThresh."""
+    from oracle import refapi
+    cfg = _det_cfg(*wh)
+    cam = cfg["cam"]
+    frames = _frames3(*wh)
+    got = _gpu_detect(cfg, frames, 2)
+    t, l = cfg["thresh"], 0
+    for i, fr in enumerate(frames):
+        r = refapi.RefMap(cam["w"], cam["h"], cam["ppx"], cam["ppy"], cam["zfx"], cam["zfy"], cfg["sigma0"], cfg["ksigma"])
+        r.rgb2bw(fr)
+        r.build()
+        kn, t, l = r.detect(2, POS_NEG, DOG_THRESH, cfg["kl_max"], t, l, cfg["kl_ref"], cfg["gain"], cfg["tmax"], cfg["tmin"])
+        retuned = r.reestimate(cfg["track_points"], 100)[1]
+        _assert_detect(got[i], (kn, t, l), r.keylines(), r.mask(), retuned, "%dx%d R2 frame %d" % (wh + (i,)))
+
+
+@pytest.mark.parametrize("wh", KITTI, ids=["1241x376", "1226x370"])
+def test_detector_other_windows_vs_reference(built, wh, tmp_path):
+    """DetectorPlaneFitSize 1, 3 and 4, each against the reference in a process of its own (its pseudo inverse is cached
+    per process)."""
+    cfg = _det_cfg(*wh)
+    frames = _frames3(*wh)
+    for R in (1, 3, 4):
+        ref = ref_detect_child(tmp_path, frames, R, cfg["cam"], cfg["sigma0"], cfg["ksigma"], cfg["thresh"], cfg["kl_max"],
+                               cfg["kl_ref"], cfg["gain"], cfg["tmax"], cfg["tmin"], POS_NEG, DOG_THRESH,
+                               cfg["track_points"])
+        got = _gpu_detect(cfg, frames, R)
+        for i in range(len(frames)):
+            k = ref["f%d_kn_tresh" % i].tolist()
+            _assert_detect(got[i], (int(k[0]), k[1], int(k[2])), ref["f%d_kl" % i], ref["f%d_mask" % i],
+                           ref["f%d_retuned" % i][0], "%dx%d R%d frame %d" % (wh + (R, i)))
+
+
+# ---- 3. / 4. whole pipeline against the reference ----------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def kitti_stream():
+    w, h = KITTI[0]
+    ts, fr = _seq(w, h, seed=13).frames(NF)
+    return _cam(w, h), ts, fr
+
+
+def _pipeline(p, ts, fr, batch=20, kc=None):
+    from rebvo_b200 import capi
+    pl = capi.Pipeline(p, max_batch=batch)
+    if kc is not None:
+        pl.set_undistort(kc)
+    nav = np.concatenate([pl.push(fr[s:s + batch], ts[s:s + batch]) for s in range(0, len(ts), batch)])
+    pl.close()
+    return nav
+
+
+@pytest.mark.parametrize("kc", [None, KC], ids=["plain", "undistort"])
+def test_pipeline_vs_reference(built, kitti_stream, kc, tmp_path):
+    """The fused pipeline at 1241x376 against the reference's three-thread REBVO: identical keyline counts, match counts and
+    poses within the bars of the drop-in test (a frame whose LM decision sits on a knife edge may take the other branch),
+    equal estimation_ok."""
+    from oracle import refapi
+    from rebvo_b200 import capi, synth
+    if not os.path.exists(refapi.EXE):
+        pytest.skip("oracle/_ref/ref_rebvo not built")
+    cam, ts, fr = kitti_stream
+    p = capi.default_params(cam)
+    nav = _pipeline(p, ts, fr, kc=kc)
+    path = str(tmp_path / "frames.bin")
+    synth.write_frames_file(path, ts, fr)
+    extra = {} if kc is None else dict(UseUndistort=1, KcR2=kc[0], KcR4=kc[1], KcR6=kc[2], KcP1=kc[3], KcP2=kc[4])
+    _, ref = refapi.run_full_rebvo(path, path + ".ref", refapi.ref_params_from(p, **extra))
+    n = min(len(ref), len(nav))
+    assert n >= NF - 2
+    e = np.sqrt(((ref["Pos"][:n] - nav["Pos"][:n]) ** 2).sum(1))
+    ate = float(np.sqrt((e ** 2).mean()))
+    dm = np.abs(ref["matches"][1:n].astype(int) - nav["matches"][1:n].astype(int))
+    print("1241x376 %s: ATE %.3e m over %d frames, max |d matches| %d, kn %d..%d" % (
+        "undistorted" if kc else "plain", ate, n, dm.max(), nav["kn"][:n].min(), nav["kn"][:n].max()))
+    assert np.array_equal(ref["kn"][:n], nav["kn"][:n])
+    assert nav["kn"][:n].min() > 1000
+    assert np.array_equal(ref["est_ok"][1:n] != 0, nav["estimation_ok"][1:n] != 0)
+    assert dm.max() <= 0.005 * ref["matches"][1:n].max(), dm.max()
+    assert ate <= 1e-3 and e.max() <= 1e-3
+
+
+def test_unmodified_rebvo_on_the_gpu_library(built, kitti_stream, tmp_path):
+    """The reference's own REBVO class on include/rebvo_b200_shim.hpp at 1241x376: it initialises, is identical run after
+    run, and equals the fused pipeline."""
+    from oracle import refapi
+    from rebvo_b200 import capi, synth
+    shim_exe = os.path.join(os.path.dirname(refapi.EXE), "shim_rebvo")
+    if not os.path.exists(shim_exe):
+        pytest.skip("oracle/_ref/shim_rebvo not built")
+    cam, ts, fr = kitti_stream
+    p = capi.default_params(cam)
+    path = str(tmp_path / "frames.bin")
+    synth.write_frames_file(path, ts, fr)
+    runs = [refapi.run_full_rebvo(path, path + ".shim%d" % k, refapi.ref_params_from(p), exe=shim_exe)[1].copy()
+            for k in range(2)]
+    n = min(len(r) for r in runs)
+    assert n >= NF - 2
+    for f in ("kn", "matches", "Pos", "PoseLie", "Kp", "est_ok"):
+        assert np.array_equal(runs[0][f][:n], runs[1][f][:n]), f
+    rec = runs[0]
+    nav = _pipeline(p, ts, fr)[:n]
+    assert np.array_equal(nav["kn"], rec["kn"][:n])
+    assert np.array_equal(nav["matches"][1:], rec["matches"][1:n])
+    assert np.abs(nav["Pos"] - rec["Pos"][:n]).max() <= 1e-9
+
+
+# ---- 5. every way of feeding frames --------------------------------------------------------------------------------
+FEED_NF = 20
+# the two KITTI sizes (w * h % 4 == 0) and one with w = 3 (mod 4) and w * h odd, so that mono frames after the first start
+# at odd bytes of a device buffer
+FEED_GEOMETRIES = KITTI + [(1239, 375)]
+
+
+@pytest.fixture(scope="module", params=FEED_GEOMETRIES, ids=["%dx%d" % g for g in FEED_GEOMETRIES])
+def feed(request):
+    w, h = request.param
+    ts, rgb = _seq(w, h, seed=5).frames(FEED_NF)
+    assert np.array_equal(rgb[..., 0], rgb[..., 1]) and np.array_equal(rgb[..., 0], rgb[..., 2])
+    return _cam(w, h), ts, rgb, np.ascontiguousarray(rgb[..., 0])
+
+
+def _dev_frames(frames, offset):
+    """the frames in a device buffer, starting `offset` bytes past a 256-byte aligned allocation; (buffer, pointer)"""
+    import torch
+    flat = np.ascontiguousarray(frames).reshape(-1)
+    buf = torch.zeros(flat.size + offset + 8, dtype=torch.uint8, device="cuda")
+    buf[offset:offset + flat.size] = torch.from_numpy(flat).cuda()
+    return buf, buf.data_ptr() + offset
+
+
+def _feed_run(feed, fmt="rgb", how="host", batch=FEED_NF, offset=0, kc=None, mirror=0):
+    from rebvo_b200 import capi
+    cam, ts, rgb, mono = feed
+    frames = mono if fmt == "mono" else rgb
+    pl = capi.Pipeline(capi.default_params(cam), max_batch=batch)
+    if kc is not None:
+        pl.set_undistort(kc)
+    if mirror:
+        pl.set_mirror(mirror)
+    navs, mirrors = [], []
+    for s in range(0, len(ts), batch):
+        f, t = frames[s:s + batch], ts[s:s + batch]
+        if how == "host":
+            nav = pl.push_mono(f, t) if fmt == "mono" else pl.push(f, t)
+        else:
+            buf, ptr = _dev_frames(f, offset)
+            nav = pl.push_mono_dev(ptr, t) if fmt == "mono" else pl.push_dev(ptr, t)
+            del buf
+        navs.append(nav)
+        if mirror:   # batch 1: the records of the newest map, as the map itself gives them
+            m = pl.map(0)
+            want = m.keylines() if mirror == 1 else m.pack_net(float(nav[0]["K"]))
+            got = pl.mirror(0)
+            assert len(got) == len(want) == nav[0]["kn"]
+            assert got.tobytes() == np.ascontiguousarray(want).tobytes(), "mirror %d, frame %d" % (mirror, s)
+            mirrors.append(got.copy())
+    pl.close()
+    return np.concatenate(navs)
+
+
+def _same(a, b, what):
+    assert len(a) == len(b)
+    diff = np.nonzero((_raw(a) != _raw(b)).reshape(len(a), -1).any(1))[0]
+    assert len(diff) == 0, "%s: nav records differ from frame %d" % (what, diff[0])
+
+
+@pytest.mark.parametrize("kc", [None, KC], ids=["plain", "undistort"])
+def test_feeds_byte_identical(built, feed, monkeypatch, kc):
+    """Host / device, RGB / mono (mono = RGB of the replicated frames), batches 20, 7 and 1, the 5-frame head / rest cut of
+    host pushes, and device buffers whose frames start at odd bytes: one set of nav records."""
+    ref = _feed_run(feed, kc=kc)
+    assert np.isfinite(ref["Pos"]).all() and ref["kn"].min() > 500
+    _same(ref, _feed_run(feed, "rgb", "device", kc=kc), "device RGB")
+    _same(ref, _feed_run(feed, "mono", kc=kc), "host mono")
+    _same(ref, _feed_run(feed, "mono", "device", kc=kc), "device mono")
+    for batch in (7, 1):
+        _same(ref, _feed_run(feed, "rgb", batch=batch, kc=kc), "host RGB batch %d" % batch)
+        _same(ref, _feed_run(feed, "mono", "device", batch=batch, kc=kc), "device mono batch %d" % batch)
+    for off in (1, 3):
+        _same(ref, _feed_run(feed, "rgb", "device", offset=off, kc=kc), "device RGB at byte offset %d" % off)
+    monkeypatch.setenv("REBVO_B200_SUB", "5")
+    _same(ref, _feed_run(feed, "rgb", kc=kc), "host RGB, SUB=5")
+    _same(ref, _feed_run(feed, "mono", kc=kc), "host mono, SUB=5")
+
+
+def test_misaligned_mono_device_base_refused(built, feed):
+    """The device mono entry point keeps its rule: a base pointer that is not 4-byte aligned is refused."""
+    from rebvo_b200 import capi
+    cam, ts, _, mono = feed
+    pl = capi.Pipeline(capi.default_params(cam), max_batch=4)
+    buf, ptr = _dev_frames(mono[:4], 4)
+    for off in (1, 2, 3):
+        with pytest.raises(capi.RbError):
+            pl.push_mono_dev(ptr + off, ts[:4])
+    pl.close()
+    del buf
+
+
+@pytest.mark.parametrize("mode", [1, 2])
+def test_mirror(built, feed, mode):
+    """Mirror modes 1 and 2 with one-frame pushes: every frame's records equal rb_map_sync_host_keylines /
+    rb_map_pack_net_keylines of the same map, and the mirror leaves the nav records unchanged."""
+    ref = _feed_run(feed, batch=1)
+    _same(ref, _feed_run(feed, "rgb", batch=1, mirror=mode), "RGB, mirror %d" % mode)
+    _same(ref, _feed_run(feed, "mono", batch=1, mirror=mode), "mono, mirror %d" % mode)
+
+
+def test_imu_mode_mono_equals_rgb(built, feed):
+    from rebvo_b200 import capi, synth
+    cam, ts, rgb, mono = feed
+    n, B = 10, 5
+    seq = _seq(cam["w"], cam["h"], seed=5)
+    out = []
+    for frames, push in ((rgb, "push"), (mono, "push_mono")):
+        pl = capi.Pipeline(capi.default_params(cam), max_batch=B)
+        pl.set_imu(synth.imu_samples(seq, n), capi.default_imu_params(InitBias=1, InitBiasFrameNum=5))
+        out.append(np.concatenate([getattr(pl, push)(frames[s:s + B], ts[s:s + B]) for s in range(0, n, B)]))
+        pl.close()
+    _same(out[0], out[1], "IMU mode")
+    assert np.isfinite(out[0]["Pos"]).all()
