@@ -107,7 +107,11 @@ __global__ void __launch_bounds__(256) k_quantile(const double *__restrict__ s_r
     __syncthreads();
     const double range = smax - smin;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < kn; i += gridDim.x * blockDim.x) {
-        int b = (int)((double)n * (s_rho[i] - smin) / range);
+        // "int i=n*(s_rho-s_rho_min)/(s_rho_max-s_rho_min)" as x86-64 converts it (cvttsd2si): NaN or a value out of int
+        // range gives INT_MIN, which the clamp below puts in bin 0.  The device's conversion saturates instead, which
+        // would put s_rho >= 2^31 * range / n + smin (and +inf) in bin n-1.
+        const double x = (double)n * (s_rho[i] - smin) / range;
+        int b = x < 2147483648.0 ? (int)x : INT_MIN;
         b = b > n - 1 ? n - 1 : b;
         b = b < 0 ? 0 : b;
         atomicAdd(&sh[b], 1);

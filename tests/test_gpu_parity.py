@@ -194,8 +194,7 @@ def _run_stage_parity(cfg):
 @pytest.mark.parametrize("cfg", [TUM_CFG, EUROC_CFG, BIG_CFG], ids=["tum640", "euroc752", "synthetic1280x960"])
 def test_stage_parity(built, cfg):
     rep = _run_stage_parity(cfg)
-    # "EKF (bitwise)" is informative: float64 results may differ in the last ulp only through libm-free code
-    fails = [f for f in rep.failures() if "(bitwise)" not in f["what"]]
+    fails = rep.failures()
     assert not fails, "\n".join("%s: %s" % (f["what"], f["info"]) for f in fails)
 
 
