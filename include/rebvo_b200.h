@@ -129,10 +129,6 @@ int rb_ctx_sync(rb_ctx *c);
 int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r);
 /* kernels launched on this context so far (bench.py's gpu_launches) */
 int64_t rb_ctx_launch_count(const rb_ctx *c);
-/* which scale-space kernels a map's own workspace dispatches to, valid after its first rb_map_dog_build: bit 0 = row passes on
- * TMA tiles, bit 1 = last box + DoG on TMA tiles, for any width (0 = the pre-TMA kernels: environment switch, or tensor-map
- * creation failed) */
-int rb_map_scale_space_path(const rb_map *m);
 
 /* ---- edge map (ring slot) ---------------------------------------------------------------------- */
 int rb_map_create(rb_ctx *c, rb_map **out);

@@ -92,7 +92,7 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_stage_profile",
            "rb_undistort_create", "rb_undistort_destroy", "rb_undistort_rgb", "rb_undistort_rgb_dev",
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
-           "rb_nav_format_trajectory", "rb_nav_format_log", "rb_map_scale_space_path"]
+           "rb_nav_format_trajectory", "rb_nav_format_log"]
 
 _lib = None
 
@@ -303,10 +303,6 @@ class Map:
         k = C.c_int(0)
         self.ctx.check(self.L.rb_map_sync_host_keylines(self.h_, _p(out), len(out), C.byref(k)))
         return out[:kn]
-
-    def scale_space_path(self):
-        """bit 0: row passes on TMA tiles, bit 1: last box + DoG on TMA tiles (after dog_build)."""
-        return int(self.L.rb_map_scale_space_path(self.h_))
 
     def pack_net(self, k_prof=1.0, capacity=None):
         """15-byte net_keyline records (uint8 array [n, 15]) packed on the device."""

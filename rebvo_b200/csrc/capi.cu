@@ -232,7 +232,6 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     CK(cudaGetDeviceProperties(&prop, device));
     c->sm_count = prop.multiProcessorCount;
     rb_minimizer_cluster_setup(c);
-    if ((r = rb_dog_device_setup(c))) return fail(r);
     {   // the context's stream carries the latency-critical tracker chain: highest priority, so that its kernels get SM slots
         // before the queued blocks of the detector / mirror streams (env REBVO_B200_PRIO=0: default priority)
         int lo = 0, hi = 0;
@@ -565,13 +564,6 @@ extern "C" int rb_map_counters(rb_map *m, int out[3]) {
     out[1] = s.nmatch;
     out[2] = s.reg_num;
     return RB_OK;
-}
-
-/* which scale-space kernels this map's workspace dispatches to (after the first rb_map_dog_build): bit 0 = TMA row passes,
- * bit 1 = TMA last box + DoG; 0 before the workspace exists */
-extern "C" int rb_map_scale_space_path(const rb_map *m) {
-    if (!m || !m->ws.gray) return 0;
-    return (m->ws.tma_row_ok ? 1 : 0) | (m->ws.tma_ok ? 2 : 0);
 }
 
 extern "C" int rb_map_sync_host_keylines(rb_map *m, rb_keyline *dst, int capacity, int *kn) {

@@ -49,7 +49,7 @@ struct MapState {
     int fwd_match;
     int reg_num;
     unsigned int frame_count;  // global_tracker::FrameCount of this slot
-    int do_map;          // the per-frame pipeline's mapping gate of the frame that built this map (k_regularize_a_gate)
+    int do_map;          // the per-frame pipeline's mapping gate of the frame that built this map (d_frame_post_match)
     double s_rho_q;
     double Kp, RKp;
 };
@@ -80,8 +80,6 @@ struct DogWS {
     float *dog;          // B * NP   blur1 - blur0
     float *aux;          // 3 * NP   on-demand planes (Img(1), dx, dy) for the test/debug accessor
     void *tmaps;         // CUtensorMap[] (host, dog.cu TM_*): TMA-staged row passes, last box + DoG
-    bool tma_ok;
-    bool tma_row_ok;     // the row passes run on TMA tiles (k_rowscan_tma_*)
 };
 
 struct rb_ctx {
@@ -109,7 +107,7 @@ struct rb_ctx {
     void *pinned;        // small pinned host buffer for scalar read-back
     void *dev_small;     // small device buffer for scalar parameters / results (64 KiB, zero-initialised)
     float *boxtab;       // 6 x 64 reciprocal clipped-area tables (iimage::build_average), see dog.cu
-    bool counters_preset; // set by rb_pipeline: match / regularise counters are zeroed by k_frame_pre
+    bool counters_preset; // set by rb_pipeline: match / regularise counters are zeroed by its quantile kernel (d_frame_pre)
     bool pdl;            // programmatic dependent launch of the per-frame chain (env REBVO_B200_PDL=0 disables)
     bool min_persist;    // whole Minimizer_RV in one launch (env REBVO_B200_MIN_PERSIST=0: one launch per evaluation)
     int min_cluster_kpc; // keylines per CTA its shared memory is sized for (0: not available on this device / capacity)
@@ -263,7 +261,6 @@ int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg);          // gray -> img0
 int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img);            // Img(1), dx, dy into ws->aux
 int rb_dog_make_tables(rb_ctx *c);
 int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws);
-int rb_dog_device_setup(rb_ctx *c);
 // detect.cu
 int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
                       const rb_detect_params *p, DetChain *chain_dev);

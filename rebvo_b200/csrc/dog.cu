@@ -10,10 +10,10 @@
 // mul+add is ever contracted.
 //
 // Pass structure per box stage (B images x 2 filters in one launch):
-//   k_rowscan_tma_* / k_rowscan_ring : S(x,y) = sum_{i<=x} avg(I_prev)(i,y)   warp per 32-row band
-//   k_colscan_pipe                   : I(x,y) = sum_{j<=y} S(x,j)              thread per 4 columns, float4 streams
-// and a final k_blur_dog that evaluates the last box of both filters, Img(0) and the DoG.
-#include <stdlib.h>
+//   k_rowscan_tma_* : S(x,y) = sum_{i<=x} avg(I_prev)(i,y)   warp per 32-row band
+//   k_colscan_pipe  : I(x,y) = sum_{j<=y} S(x,j)              thread per 4 columns, float4 streams
+// and a final k_blur_dog_tma that evaluates the last box of both filters, Img(0) and the DoG (k_blur_dog when Img(1) is
+// wanted too: the debug accessor).
 #include <new>
 
 #include "common.cuh"
@@ -403,37 +403,32 @@ static bool make_tmap3(CUtensorMap *tm, float *base, int w, int h, int pitch, in
 // tensor map slots of a workspace
 enum { TM_I_BLUR = 0, TM_IMG0, TM_DOG, TM_GRAY, TM_S, TM_I0_F0, TM_I0_F1, TM_I_F0, TM_I_F1, TM_COUNT };
 int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws) {
-    ws->tma_ok = false;
-    ws->tma_row_ok = false;
-    const char *e = getenv("REBVO_B200_BLUR_TMA");
-    const char *er = getenv("REBVO_B200_ROW_TMA");
-    const bool want_blur = !(e && atoi(e) == 0), want_row = !(er && atoi(er) == 0);
-    if (!want_blur && !want_row) return RB_OK;
     CUtensorMap *t = new (std::nothrow) CUtensorMap[TM_COUNT];
-    if (!t) return RB_OK;
+    if (!t) {
+        snprintf(c->err, sizeof(c->err), "scale space: no host memory for the tensor maps");
+        return RB_ERR_ARG;
+    }
     ws->tmaps = t;
     const int w = c->w, h = c->h, P = c->pitch;
-    if (want_blur) {
-        bool ok = make_tmap3(&t[TM_I_BLUR], ws->I, w, h, P, 2 * ws->B, BT_BW, BT_BH) &&
-                  make_tmap3(&t[TM_IMG0], ws->img0, w, h, P, ws->B, BT_W, BT_H) &&
-                  make_tmap3(&t[TM_DOG], ws->dog, w, h, P, ws->B, BT_W, BT_H);
-        ok = ok && cudaFuncSetAttribute(k_blur_dog_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BlurTmaSmem) + 128) == cudaSuccess;
-        if (!ok) cudaGetLastError();
-        ws->tma_ok = ok;
+    const int (*d)[3] = c->plan.d;
+    // last box + DoG: (64 + d) x (32 + d) windows in, 64 x 32 tiles out.  Row passes: 32 x 32 tiles, 128-byte swizzle on
+    // the tiles the sequential scan walks row-wise (gray in, S out); the box-average inputs are (32 + d) x 32 windows read
+    // column-wise (no swizzle)
+    const bool ok = make_tmap3(&t[TM_I_BLUR], ws->I, w, h, P, 2 * ws->B, BT_BW, BT_BH) &&
+                    make_tmap3(&t[TM_IMG0], ws->img0, w, h, P, ws->B, BT_W, BT_H) &&
+                    make_tmap3(&t[TM_DOG], ws->dog, w, h, P, ws->B, BT_W, BT_H) &&
+                    make_tmap3(&t[TM_GRAY], ws->gray, w, h, P, ws->B, 32, 32, true) &&
+                    make_tmap3(&t[TM_S], ws->S, w, h, P, 2 * ws->B, 32, 32, true) &&
+                    make_tmap3(&t[TM_I0_F0], ws->I0, w, h, P, ws->B, 32, 32 + d[0][0]) &&
+                    make_tmap3(&t[TM_I0_F1], ws->I0, w, h, P, ws->B, 32, 32 + d[1][0]) &&
+                    make_tmap3(&t[TM_I_F0], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[0][1]) &&
+                    make_tmap3(&t[TM_I_F1], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[1][1]);
+    if (!ok) {
+        cudaGetLastError();   // (a failed driver entry-point query must not surface at the next launch check)
+        snprintf(c->err, sizeof(c->err), "scale space: cuTensorMapEncodeTiled failed for %dx%d planes, %d images", w, h, ws->B);
+        return RB_ERR_CUDA;
     }
-    if (want_row) {
-        // row pass: 32 x 32 tiles, 128-byte swizzle on the tiles the sequential scan walks row-wise (gray in, S out); the
-        // box-average inputs are (32 + d) x 32 windows read column-wise (no swizzle)
-        const int (*d)[3] = c->plan.d;
-        bool ok = make_tmap3(&t[TM_GRAY], ws->gray, w, h, P, ws->B, 32, 32, true) &&
-                  make_tmap3(&t[TM_S], ws->S, w, h, P, 2 * ws->B, 32, 32, true) &&
-                  make_tmap3(&t[TM_I0_F0], ws->I0, w, h, P, ws->B, 32, 32 + d[0][0]) &&
-                  make_tmap3(&t[TM_I0_F1], ws->I0, w, h, P, ws->B, 32, 32 + d[1][0]) &&
-                  make_tmap3(&t[TM_I_F0], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[0][1]) &&
-                  make_tmap3(&t[TM_I_F1], ws->I, w, h, P, 2 * ws->B, 32, 32 + d[1][1]);
-        if (!ok) cudaGetLastError();
-        ws->tma_row_ok = ok;
-    }
+    RB_CUDA(cudaFuncSetAttribute(k_blur_dog_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BlurTmaSmem) + 128));
     return RB_OK;
 }
 
@@ -510,158 +505,15 @@ int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) 
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Row pass, asynchronous version: the raw input of a band is streamed into a per-warp shared-memory ring of
-// 32-column chunks with cp.async (16 B per lane, no registers, NS-3 chunks in flight ahead of the consumer), so the
-// sequential scan never waits for a DRAM round trip.  Tile t of a box-averaged pass needs the columns
-// [32t-d2-1, 32t+31+d2], i.e. chunks t-1, t, t+1 of the rows [y0-d2-1, y0+31+d2]; every integral value is fetched
-// from memory once and the four taps of iimage::average come from shared memory.  Same arithmetic and add order as
-// box_avg followed by one sequential add chain per row (bit-identical output).
-#define RING_NS 4          // ring slots: 3 live chunks + 1 in flight
-#define RING_WARPS 4
-__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc, int src_bytes) {
-    const unsigned int s = (unsigned int)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gsrc), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
-}
-
-template <bool AVG>
-__global__ void __launch_bounds__(32 * RING_WARPS) k_rowscan_ring(const float *__restrict__ in, float *__restrict__ out,
-                                                                  int w, int h, int pitch, int nimg, int in_mod, int nper,
-                                                                  int d_f0, int d_f1, const float *__restrict__ tab_f0,
-                                                                  const float *__restrict__ tab_f1, int rmax) {
-    extern __shared__ __align__(16) float smem_ring[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int gw = blockIdx.x * RING_WARPS + warp;
-    const int bands = (h + 31) >> 5;
-    const int img = gw / bands, band = gw - img * bands;
-    if (img >= nimg) return;
-    // per-warp carve-up: ring [RING_NS][rmax][32], tile [32][33], table [64]
-    float *ring = smem_ring + (size_t)warp * (RING_NS * rmax * 32 + 32 * 33 + BOX_TAB_N);
-    float(*tile)[33] = reinterpret_cast<float(*)[33]>(ring + RING_NS * rmax * 32);
-    float *tab = ring + RING_NS * rmax * 32 + 32 * 33;
-    const size_t N = (size_t)pitch * h;   // (rows of `pitch` floats: every row starts on 16 bytes)
-    const float *__restrict__ I = in + (size_t)(img % in_mod) * N;
-    float *__restrict__ O = out + (size_t)img * N;
-    const bool f1 = (img / nper) != 0;
-    const int d = AVG ? (f1 ? d_f1 : d_f0) : 1;
-    const int d2 = AVG ? d / 2 : 0;
-    const int R = AVG ? 32 + d : 32;                 // rows staged per chunk
-    const int yb0 = AVG ? band * 32 - d2 - 1 : band * 32;   // image row of ring row 0
-    if (AVG) {
-        const float *__restrict__ tg = f1 ? tab_f1 : tab_f0;
-        tab[lane] = tg[lane];
-        tab[lane + 32] = tg[lane + 32];
-    }
-    const int y0 = band * 32;
-    const bool band_interior = AVG && (y0 >= d2 + 1) && (y0 + 31 < h - d2);
-    const int nchunk = (w + 31) >> 5;
-    const int sub = lane >> 3, piece = lane & 7;   // 8 lanes x 16 B cover one 32-float row; 4 rows per instruction
-
-    auto issue_chunk = [&](int ci) {
-        if (ci >= 0 && ci < nchunk) {
-            float *dst0 = ring + (size_t)(ci % RING_NS) * rmax * 32;
-            const int gx = ci * 32 + piece * 4;
-            int bytes = (w - gx) * 4;
-            bytes = bytes < 0 ? 0 : (bytes > 16 ? 16 : bytes);
-            const int gxc = gx < w ? gx : 0;
-            for (int j = sub; j < R; j += 4) {
-                int gy = yb0 + j;
-                gy = gy < 0 ? 0 : (gy > h - 1 ? h - 1 : gy);
-                cp_async16(dst0 + j * 32 + piece * 4, I + (size_t)gy * pitch + gxc, bytes);
-            }
-        }
-        cp_async_commit();
-    };
-    // prologue: chunks 0 .. RING_NS-2
-#pragma unroll
-    for (int ci = 0; ci < RING_NS - 1; ci++) issue_chunk(ci);
-
-    float carry = 0.f;
-    for (int t = 0; t < nchunk; t++) {
-        cp_async_wait<RING_NS - 3>();   // chunks <= t+1 have landed (this lane's copies)
-        __syncwarp();                   // ... and everybody else's
-        const int x = t * 32 + lane;
-        const int xc = x < w ? x : w - 1;
-        if (AVG && band_interior && t * 32 >= d2 + 1 && t * 32 + 31 < w - d2) {
-            // centre region of iimage::average for the whole tile (80 % of the tiles): constant tap offsets, no selects
-            const int xr = x + d2, xl = x - d2 - 1;
-            const float *colr = ring + (size_t)((xr >> 5) % RING_NS) * rmax * 32 + (xr & 31);
-            const float *coll = ring + (size_t)((xl >> 5) % RING_NS) * rmax * 32 + (xl & 31);
-            const float *colr_b = colr + d * 32, *coll_b = coll + d * 32;   // bottom taps: ring row r + d
-            const float a = tab[d2 * BOX_TAB_W + d2];
-#pragma unroll
-            for (int r = 0; r < 32; r++) {
-                float v = colr_b[r * 32] - coll_b[r * 32];   // A - B
-                v = v - colr[r * 32];                        //   - C
-                v = v + coll[r * 32];                        //   + D
-                tile[r][lane] = v * a;
-            }
-        } else if (AVG) {
-            const bool left = xc < d2 + 1, right = xc >= w - d2;
-            const int xr = right ? w - 1 : xc + d2, xl = left ? 0 : xc - d2 - 1;
-            const int cx = left ? xc + d2 + 1 : (right ? w - xc + d2 : d);
-            const float *colr = ring + (size_t)((xr >> 5) % RING_NS) * rmax * 32 + (xr & 31);
-            const float *coll = ring + (size_t)((xl >> 5) % RING_NS) * rmax * 32 + (xl & 31);
-            const float *tcol = tab + (cx - d2 - 1);
-#pragma unroll 8
-            for (int r = 0; r < 32; r++) {
-                const int y = y0 + r;
-                const int yc = y < h ? y : h - 1;
-                const bool top = yc < d2 + 1, bottom = yc >= h - d2;
-                const int jb = (bottom ? h - 1 : yc + d2) - yb0, jt = top ? 0 : yc - d2 - 1 - yb0;
-                const float A = colr[jb * 32], B = coll[jb * 32], C = colr[jt * 32], Dd = coll[jt * 32];
-                const float t1 = bottom ? C : B, t2 = bottom ? B : C;   // bottom band: A-C-B+D, elsewhere A-B-C+D
-                const bool h1 = bottom ? !top : !left, h2 = bottom ? !left : !top;
-                float v = A;
-                v = h1 ? v - t1 : v;
-                v = h2 ? v - t2 : v;
-                v = (!top && !left) ? v + Dd : v;
-                const int cy = top ? yc + d2 + 1 : (bottom ? h - yc + d2 : d);
-                v = v * tcol[(cy - d2 - 1) * BOX_TAB_W];
-                tile[r][lane] = (y < h && x < w) ? v : 0.f;
-            }
-        } else {
-            const float *col = ring + (size_t)(t % RING_NS) * rmax * 32 + lane;
-#pragma unroll 8
-            for (int r = 0; r < 32; r++) {
-                const float v = col[r * 32];
-                tile[r][lane] = (y0 + r < h && x < w) ? v : 0.f;
-            }
-        }
-        __syncwarp();
-        // the chunk t-1 (AVG) / t (plain) is no longer needed: refill its slot with the chunk RING_NS-1 ahead
-        issue_chunk(AVG ? t - 1 + RING_NS : t + RING_NS - 1);
-        float *row = tile[lane];
-#pragma unroll
-        for (int cidx = 0; cidx < 32; cidx++) {
-            carry = carry + row[cidx];  // I(x,y) = I(x-1,y) + in(x,y), iimage.cpp:56-60
-            row[cidx] = carry;
-        }
-        __syncwarp();
-        if (x < w) {
-#pragma unroll 8
-            for (int r = 0; r < 32; r++)
-                if (y0 + r < h) O[(size_t)(y0 + r) * pitch + x] = tile[r][lane];
-        }
-        __syncwarp();
-    }
-    cp_async_wait<0>();
-}
-
-// ---------------------------------------------------------------------------------------------------
 // Row pass on TMA tiles.  One warp = one 32-row band of one image (the sequential float add chain of iimage.cpp:56-60 runs
-// along x, one row per lane), one warp per CTA so that the CTAs spread evenly over the SMs.  The cp.async ring version is
-// warp-latency-bound (many instructions per 32 x 32 chunk, few warps active), not memory-bound; here a chunk costs ~80 (plain) / ~370 (box average) instructions:
+// along x, one row per lane), one warp per CTA so that the CTAs spread evenly over the SMs.  A chunk costs ~80 (plain) / ~370
+// (box average) instructions:
 //   * one lane issues one cp.async.bulk.tensor load per chunk on an mbarrier ring, RT_NS - 1 chunks ahead;
 //   * the tile the scan walks row-wise lives in shared memory in the 128-byte swizzle of the tensor map, so that a lane reads
 //     and writes its row as eight conflict-free 16-byte accesses (unit k of row r sits at unit k ^ (r & 7));
 //   * the scanned tile leaves with one cp.async.bulk.tensor store; bounds are the tensor map's business (zero fill on the
 //     way in, clipping on the way out).
-// Same arithmetic and add order as k_rowscan_ring (bit-identical output).
+// Same arithmetic and add order as box_avg followed by one sequential add chain per row (bit-identical output).
 __device__ __forceinline__ unsigned int rt_s32(const void *p) { return (unsigned int)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void rt_load3(unsigned int dst, const CUtensorMap *tm, int x, int y, int z, unsigned int bar,
                                          unsigned int bytes) {
@@ -863,7 +715,9 @@ __global__ void __launch_bounds__(32) k_rowscan_tma_avg(const __grid_constant__ 
     if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-static int rowscan_tma(rb_ctx *c, DogWS *ws, int stage, const float *in, int nimg, int in_mod, int nper) {
+// row pass into ws->S.  stage < 0: plain row scan of `in` (images of ws->gray); stage 0..1: row scan of box `stage` of both
+// filters (in = ws->I0, ws->I)
+static int rowscan(rb_ctx *c, DogWS *ws, int stage, const float *in, int nimg, int in_mod, int nper) {
     const CUtensorMap *t = (const CUtensorMap *)ws->tmaps;
     const int bands = (c->h + 31) / 32;
     int *fail = (int *)((char *)c->dev_small + RB_DS_TMA_FAIL);
@@ -882,42 +736,9 @@ static int rowscan_tma(rb_ctx *c, DogWS *ws, int stage, const float *in, int nim
     return RB_OK;
 }
 
-// per-device opt-ins of this file's kernels (function attributes are per device: called from rb_ctx_create after
-// cudaSetDevice, so that contexts on several GPUs of one process all get them)
-int rb_dog_device_setup(rb_ctx *c) {
-    RB_CUDA(cudaFuncSetAttribute(k_rowscan_ring<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    RB_CUDA(cudaFuncSetAttribute(k_rowscan_ring<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    return RB_OK;
-}
-
-static int rowscan_ring(rb_ctx *c, int stage, const float *in, float *out, int nimg, int in_mod, int nper) {
-    const int bands = (c->h + 31) / 32;
-    const int blocks = rb_div_up(nimg * bands, RING_WARPS);
-    const int dmax = stage >= 0 ? (c->plan.d[0][stage] > c->plan.d[1][stage] ? c->plan.d[0][stage] : c->plan.d[1][stage]) : 0;
-    const int rmax = 32 + dmax;
-    const size_t smem = (size_t)RING_WARPS * (RING_NS * rmax * 32 + 32 * 33 + BOX_TAB_N) * sizeof(float);
-    if (stage >= 0) {
-        k_rowscan_ring<true><<<blocks, 32 * RING_WARPS, smem, c->stream>>>(
-            in, out, c->w, c->h, c->pitch, nimg, in_mod, nper, c->plan.d[0][stage], c->plan.d[1][stage],
-            c->boxtab + (0 * 3 + stage) * BOX_TAB_N, c->boxtab + (1 * 3 + stage) * BOX_TAB_N, rmax);
-    } else {
-        k_rowscan_ring<false><<<blocks, 32 * RING_WARPS, smem, c->stream>>>(in, out, c->w, c->h, c->pitch, nimg, in_mod,
-                                                                          nper, 1, 1, nullptr, nullptr, rmax);
-    }
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
-// stage < 0: plain row scan of the input; stage 0..1: row scan of box `stage` of both filters
-static int rowscan(rb_ctx *c, DogWS *ws, int stage, const float *in, float *out, int nimg, int in_mod, int nper) {
-    if (ws->tma_row_ok && out == ws->S && stage <= 1 &&
-        (stage < 0 ? (in >= ws->gray && in < ws->gray + (size_t)ws->B * c->NP) : in == (stage == 0 ? ws->I0 : ws->I)))
-        return rowscan_tma(c, ws, stage, in, nimg, in_mod, nper);
-    return rowscan_ring(c, stage, in, out, nimg, in_mod, nper);
-}
-
+// k_blur_dog only when Img(1) is wanted too (img1_opt: the debug accessor's aux plane)
 static int blur_dog(rb_ctx *c, DogWS *ws, int nimg, float *img1_opt) {
-    if (ws->tma_ok && !img1_opt) {
+    if (!img1_opt) {
         const CUtensorMap *t = (const CUtensorMap *)ws->tmaps;
         dim3 tg(rb_div_up(c->w, BT_W), rb_div_up(c->h, BT_H), nimg);
         k_blur_dog_tma<<<tg, BT_THREADS, sizeof(BlurTmaSmem) + 128, c->stream>>>(
@@ -971,13 +792,13 @@ int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int m) {
     if (m < 1 || m > ws->B) return RB_ERR_ARG;
     int r;
     // iimage::load(in): identical for both filters -> computed once
-    if ((r = rowscan(c, ws, -1, ws->gray, ws->S, m, m, m))) return r;
+    if ((r = rowscan(c, ws, -1, ws->gray, m, m, m))) return r;
     if ((r = colscan(c, ws->S, ws->I0, m))) return r;
     // box 0 of both filters reads the shared integral; image index = filter * m + b
-    if ((r = rowscan(c, ws, 0, ws->I0, ws->S, 2 * m, m, m))) return r;
+    if ((r = rowscan(c, ws, 0, ws->I0, 2 * m, m, m))) return r;
     if ((r = colscan(c, ws->S, ws->I, 2 * m))) return r;
     // box 1
-    if ((r = rowscan(c, ws, 1, ws->I, ws->S, 2 * m, 2 * m, m))) return r;
+    if ((r = rowscan(c, ws, 1, ws->I, 2 * m, 2 * m, m))) return r;
     if ((r = colscan(c, ws->S, ws->I, 2 * m))) return r;
     // box 2 + DoG.  Filter f of image b lives at I[(f*m + b)*N]
     return blur_dog(c, ws, m, nullptr);
@@ -1001,10 +822,10 @@ int rb_dog_single_pass(rb_ctx *c, DogWS *ws, int pass_id, int nimg, double *byte
     switch (pass_id) {
         case 0:
             *bytes = 8.0 * N * nimg;   // read gray 4N, write S 4N
-            return rowscan(c, ws, -1, ws->gray, ws->S, nimg, nimg, nimg);
+            return rowscan(c, ws, -1, ws->gray, nimg, nimg, nimg);
         case 1:
             *bytes = 8.0 * N * 2 * nimg;   // read I 4N (each tap row is re-used from L1/L2), write S 4N
-            return rowscan(c, ws, 1, ws->I, ws->S, 2 * nimg, 2 * nimg, nimg);
+            return rowscan(c, ws, 1, ws->I, 2 * nimg, 2 * nimg, nimg);
         case 2:
             *bytes = 8.0 * N * 2 * nimg;   // read S 4N, write I 4N
             return colscan(c, ws->S, ws->I, 2 * nimg);

@@ -54,12 +54,12 @@ struct rb_pipeline {
     cudaEvent_t ev_dog, *ev_det, *ev_trk;
     bool overlap;
     // FordwardMatch's apply + directed_matching in k_match, then gate + Regularize_1_iter + EKF + rotate_keylines in
-    // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the four-kernel chain)
+    // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the stage kernels in the reference's order, the bitwise reference of the two)
     bool map_chain;
     // rescaling stream: with DoReScaling=0 a frame's EstimateReScalingOpt changes no keyline and only fills in its nav record,
     // so it runs here (lowest priority) instead of at the end of the frame's tracker chain; the tracker stream joins it
-    // before the next frame's first kernel after the minimiser (k_match, or k_fm_apply_rotate in the four-kernel chain,
-    // which writes the map's rho / s_rho)
+    // before the next frame's first kernel after the minimiser (k_match, or k_fm_apply before k_rotate, which writes the
+    // map's rho / s_rho, in the reference schedule)
     cudaStream_t resc_stream;     // nullptr: the rescaling stays in the frame's map-update kernel on the tracker stream
     cudaEvent_t ev_rfork, ev_rjoin;
     bool resc_open;               // a rescaling was forked and not joined yet
@@ -165,14 +165,15 @@ static void set_eye(double *M, double v) {
     M[0] = M[4] = M[8] = v;
 }
 
-__global__ void k_frame_pre(FrameState *fs, const FrameArgs *fa, MapState *nst) { d_frame_pre(fs, fa->frame_count, nst); }
 __global__ void k_frame_post_min(FrameState *fs, const TrackState *ts) { d_frame_post_min(fs, ts->lm); }
-__global__ void k_frame_post_match(FrameState *fs, const MapState *nst, int match_threshold) {
+__global__ void k_frame_post_match(FrameState *fs, MapState *nst, int match_threshold) {
     d_frame_post_match(fs, nst, match_threshold);
+    nst->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
 }
+// the nav record before the map's rescaling, which runs on the side stream and fills in its Kp / RKp
 __global__ void k_frame_finish(FrameState *fs, const MapState *nst, const MapState *ost, const TrackState *ts,
                                rb_nav *nav, const FrameArgs *fa) {
-    d_frame_finish(fs, nst, ost, ts->lm.score, nav, fa, true);
+    d_frame_finish(fs, nst, ost, ts->lm.score, nav, fa, false);
 }
 
 // record for the very first frame (it only initialises the ring, :109-121)
@@ -492,11 +493,14 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
                                     p.LocationUncertainty, pl->fs->R0, side ? nav_slot : nullptr, fa)))
             return r;
     } else {
-        // :354  FordwardMatch ; :369 rotate_keylines(R0) in one kernel.  Until then, this frame only reads the old map's
-        // rho / s_rho (the minimiser writes its m_id_f, which the rescaling does not read): the old map's rescaling may
-        // run until then.
+        // The reference's order (rebvo_second_t.cpp:354-470) on the stage kernels that tests/test_gpu_parity.py and
+        // tests/test_gpu_mapper_states.py pin to the reference: the bitwise reference of the two kernels above
+        // (tests/test_gpu_map_chain.py), not a schedule to tune.  k_rotate writes the old map's rho / s_rho, which its
+        // rescaling reads: joined before the first kernel.
         if ((r = resc_join(pl))) return r;
-        if ((r = rb_forward_match_apply_enqueue(c, old, neu, pl->fs->R0))) return r;
+        // :354  FordwardMatch (its arg-max ran with the minimiser) ; :369 rotate_keylines(R0)
+        if ((r = rb_forward_match_apply_enqueue(c, old, neu))) return r;
+        if ((r = rb_rotate_enqueue(c, old, pl->fs->R0))) return r;
         RB_TRACE(c->stream, 11);
         prof_mark(pl, ST_FWD_ROT);
         // :410  directed_matching(V,P_V,R,old_buf.ef,...)
@@ -505,11 +509,15 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
             return r;
         RB_TRACE(c->stream, 4);
         prof_mark(pl, ST_DMATCH);
-        // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman on wide grids
-        if ((r = rb_regularize_ekf_enqueue(c, neu, p.RegularizeThresh, pl->fs, p.MatchThreshold, pl->fs->V,
-                                           p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map,
-                                           side ? old->st : nullptr, side ? nav_slot : nullptr, fa)))
-            return r;
+        // :410-423 match-count gate ; :452-470 Regularize_1_iter, UpdateInverseDepthKalman
+        k_frame_post_match<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, p.MatchThreshold);
+        RB_LAUNCH_CHECK();
+        if ((r = rb_regularize_enqueue(c, neu, p.RegularizeThresh, &pl->fs->do_map))) return r;
+        if ((r = rb_ekf_enqueue(c, neu, pl->fs->V, p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map))) return r;
+        if (side) {   // :545-585 pose integration + NavData (else in k_map_update's tail)
+            k_frame_finish<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, old->st, neu->ts, nav_slot, fa);
+            RB_LAUNCH_CHECK();
+        }
     }
     RB_TRACE(c->stream, 9);
     prof_mark(pl, ST_REG_EKF);

@@ -1410,8 +1410,7 @@ __global__ void __launch_bounds__(256) k_rotate(KLSoA kl, const MapState *st, co
 
 // =====================================================================================================
 // FordwardMatch (edge_tracker.cpp:380-436), second part: the arg-max (d_fm_offer, above the minimiser) is complete.
-// Indexed by OLD keyline: the winner of new keyline f copies its own record into neu[f], then (ROT) rotates itself in
-// place -- no thread reads another thread's old keyline, so the two need no barrier between them.
+// Indexed by OLD keyline: the winner of new keyline f copies its own record into neu[f].
 // =====================================================================================================
 __global__ void __launch_bounds__(256) k_fm_init(FmBest *best, const MapState *nst) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1425,24 +1424,16 @@ __global__ void __launch_bounds__(256) k_fm_argmax(KLSoA old, const MapState *os
     if (i >= ost->kn) return;
     d_fm_argmax_one(old, i, nst->kn, best);
 }
-template <bool ROT>
-__global__ void __launch_bounds__(256) k_fm_apply_rotate(KLSoA old, KLSoA neu, const MapState *ost, MapState *nst,
-                                                         const FmBest *best, const double *__restrict__ Rp, double zf) {
+__global__ void __launch_bounds__(256) k_fm_apply(KLSoA old, KLSoA neu, const MapState *ost, MapState *nst,
+                                                  const FmBest *best) {
     pdl_wait();
     pdl_launch();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool in = i < ost->kn;
     bool hit = false;
-    double R[9], rho = 0, s_rho = 0;
-#pragma unroll
-    for (int k = 0; k < 9; k++) R[k] = ROT ? Rp[k] : 0.0;
-    float2 pm = make_float2(0.f, 0.f), m = pm;
-    if (in) {   // keyline i's record is loaded once, before any store, for the copy and for the rotation
+    if (i < ost->kn) {
         const int f = old.m_id_f[i];
-        rho = old.rho[i];
-        s_rho = old.s_rho[i];
-        pm = old.p_m[i];
-        m = old.m_m[i];
+        const double rho = old.rho[i], s_rho = old.s_rho[i];
+        const float2 pm = old.p_m[i], m = old.m_m[i];
         if (f >= 0 && f < nst->kn && __ldcg(&best[f].idx) == i) {
             neu.rho[f] = rho;
             neu.s_rho[f] = s_rho;
@@ -1456,7 +1447,6 @@ __global__ void __launch_bounds__(256) k_fm_apply_rotate(KLSoA old, KLSoA neu, c
     }
     const unsigned int bal = __ballot_sync(0xffffffffu, hit);
     if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&nst->fwd_match, __popc(bal));
-    if (ROT && in) d_rotate_vals(old, i, R, zf, pm, rho, s_rho, m);
 }
 __global__ void k_set_int(int *p, int v) { *p = v; }
 
@@ -1471,26 +1461,20 @@ int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
                (const MapState *)neu->st, neu->ts_host.fm_best);
     return RB_OK;
 }
-int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu, const double *R_dev) {
-    const int nb = rb_div_up(c->kcap, 256);
-    const FmBest *best = neu->ts_host.fm_best;
-    if (R_dev)
-        RB_KLAUNCH(k_fm_apply_rotate<true>, nb, 256, 0, old->kl, neu->kl, (const MapState *)old->st, neu->st, best, R_dev,
-                   c->zfm);
-    else
-        RB_KLAUNCH(k_fm_apply_rotate<false>, nb, 256, 0, old->kl, neu->kl, (const MapState *)old->st, neu->st, best, R_dev,
-                   c->zfm);
+int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
+    RB_KLAUNCH(k_fm_apply, rb_div_up(c->kcap, 256), 256, 0, old->kl, neu->kl, (const MapState *)old->st, neu->st,
+               (const FmBest *)neu->ts_host.fm_best);
     return RB_OK;
 }
 int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
-    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in k_frame_pre
+    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in its quantile kernel (d_frame_pre)
         k_set_int<<<1, 1, 0, c->stream>>>(&neu->st->fwd_match, 0);
         RB_LAUNCH_CHECK();
     }
     int r;
     if ((r = rb_forward_match_init_enqueue(c, neu))) return r;
     if ((r = rb_forward_match_argmax_enqueue(c, old, neu))) return r;
-    return rb_forward_match_apply_enqueue(c, old, neu, nullptr);
+    return rb_forward_match_apply_enqueue(c, old, neu);
 }
 
 int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev) {
@@ -1727,7 +1711,7 @@ __global__ void __launch_bounds__(128) k_match(KLSoA neu, MapState *nst, KLSoA o
 int rb_directed_matching_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, double min_thr_mod,
                                  double min_thr_ang, double max_radius, double loc_uncertainty, const int *enable_dev) {
     const double cang_min_edge = cos(min_thr_ang * M_PI / 180.0);
-    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in k_frame_pre
+    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in its quantile kernel (d_frame_pre)
         k_set_int<<<1, 1, 0, c->stream>>>(&neu->st->nmatch, 0);
         RB_LAUNCH_CHECK();
     }
@@ -1808,7 +1792,7 @@ __global__ void __launch_bounds__(256) k_regularize_b(KLSoA kl, const MapState *
 int rb_regularize_enqueue(rb_ctx *c, rb_map *m, double thresh, const int *enable_dev) {
     TrackState &t = m->ts_host;
     const int nb = rb_div_up(c->kcap, 256);
-    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in k_frame_pre
+    if (!c->counters_preset) {   // the per-frame pipeline zeroes the counters in its quantile kernel (d_frame_pre)
         k_set_int<<<1, 1, 0, c->stream>>>(&m->st->reg_num, 0);
         RB_LAUNCH_CHECK();
     }
@@ -1873,76 +1857,12 @@ int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, do
     return RB_OK;
 }
 
-// pipeline variants (wide grids: these two stages are FP64-heavy per keyline and want every SM):
-// first half of Regularize_1_iter with the "after directed_matching" gate folded in (block 0 publishes it) ...
-__global__ void __launch_bounds__(256) k_regularize_a_gate(KLSoA kl, MapState *st, double *__restrict__ r,
-                                                           double *__restrict__ s, unsigned char *__restrict__ set,
-                                                           double thresh, FrameState *fs, int match_threshold) {
-    pdl_wait();
-    pdl_launch();
-    const bool en = fs->do_match && st->nmatch >= match_threshold;
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        d_frame_post_match(fs, st, match_threshold);
-        st->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
-    }
-    if (!en) return;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool did = i < st->kn ? d_reg_a(kl, i, r, s, set, thresh) : false;
-    const unsigned int bal = __ballot_sync(0xffffffffu, did);
-    if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&st->reg_num, __popc(bal));
-}
-// ... and its write-back half + UpdateInverseDepthKalman in one pass: both only touch the thread's own keyline, so
-// the EKF takes the regularised (rho, s_rho) straight from registers
-__global__ void __launch_bounds__(256) k_regb_ekf(KLSoA kl, const MapState *st, const double *__restrict__ r,
-                                                  const double *__restrict__ s,
-                                                  const unsigned char *__restrict__ set,
-                                                  const double *__restrict__ velp, double zf, double q_abs,
-                                                  double loc_unc, const int *enable, FrameState *pose_fs,
-                                                  const MapState *ost, const LMState *lm, rb_nav *nav,
-                                                  const FrameArgs *fa) {
-    pdl_wait();
-    pdl_launch();
-    // the frame's pose integration + matrix logarithms (one thread) beside the EKF instead of in the map-update
-    // kernel's tail: V and R are final since the gate of the previous kernel.  The last block of the grid has no keylines.
-    // With nav, the whole nav record too (the rescaling runs on a side stream and only fills in its Kp / RKp).
-    if (pose_fs && blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
-        if (nav) d_frame_finish(pose_fs, st, ost, lm->score, nav, fa, false);
-        else d_frame_pose(pose_fs);
-    }
-    if (enable && !*enable) return;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= st->kn) return;
-    double rho, s_rho;
-    if (set[i]) {
-        rho = r[i];
-        s_rho = s[i];
-        kl.rho[i] = rho;
-        kl.s_rho[i] = s_rho;
-    } else {
-        rho = kl.rho[i];
-        s_rho = kl.s_rho[i];
-    }
-    if (kl.m_id[i] < 0) return;
-    d_ekf(kl, i, rho, s_rho, velp, zf, q_abs, loc_unc);
-}
-int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
-                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
-                              const MapState *ost, rb_nav *nav, const FrameArgs *fa) {
-    TrackState &t = m->ts_host;
-    const int nb = rb_div_up(c->kcap, 256);
-    RB_KLAUNCH(k_regularize_a_gate, nb, 256, 0, m->kl, m->st, t.reg_r, t.reg_s, t.reg_set, thresh, fs, match_threshold);
-    RB_KLAUNCH(k_regb_ekf, nb, 256, 0, m->kl, (const MapState *)m->st, (const double *)t.reg_r, (const double *)t.reg_s,
-               (const unsigned char *)t.reg_set, vel_dev, c->zfm, q_abs, loc_unc, do_map_dev, fs, ost,
-               (const LMState *)&m->ts->lm, nav, fa);
-    return RB_OK;
-}
-
 // The map update after k_match, in one pass: every thread evaluates the match-count gate itself (its inputs are final),
 // the regularisation reads (rho, s_rho) of a keyline and its neighbours from the scratch pair r / s that k_match filled,
 // and the EKF takes the smoothed pair from registers; every keyline's rho / s_rho is written back (the scratch values
 // when the gate is closed).  Thread i also runs rotate_keylines(R0) on old keyline i: nothing reads the old map after
 // k_match, and the map stays what a caller of the pipeline sees.  One spare thread runs the gate's frame part, then the
-// pose integration / nav record, as k_regularize_a_gate and k_regb_ekf do.
+// pose integration / nav record.
 __global__ void __launch_bounds__(256) k_reg_ekf(KLSoA kl, MapState *st, const double *__restrict__ r,
                                                  const double *__restrict__ s, double thresh, FrameState *fs,
                                                  int match_threshold, double zf, double q_abs, double loc_unc, KLSoA old,
@@ -2161,7 +2081,7 @@ static int launch_map_update(rb_ctx *c, rb_map *m, const MapUpdArgs &a, bool pdl
 }
 
 // the pipeline's rescaling + pose integration / nav record, after the gate, smoothing and EKF have run on wide grids
-// (rb_regularize_ekf_enqueue or rb_reg_ekf_enqueue) and published fs->do_map
+// (rb_reg_ekf_enqueue, or the stage kernels of the reference schedule) and published fs->do_map
 int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
                           const MapState *ost, rb_nav *nav, const FrameArgs *fa) {
     MapUpdArgs a;

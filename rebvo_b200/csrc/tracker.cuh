@@ -56,11 +56,11 @@ int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_
 int rb_quantile_enqueue(rb_ctx *c, rb_map *m, double smin, double smax, double perc, int nbins,
                         FrameState *fs = nullptr, const unsigned int *frame_count_dev = nullptr, MapState *nst = nullptr);
 int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool min_mod_from_state);
-// FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu).
-// With R_dev the apply kernel then runs rotate_keylines(R) on the old map; rb_forward_match_enqueue is the whole stage.
+// FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu);
+// rb_forward_match_enqueue is the whole stage.
 int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu);
 int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
-int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu, const double *R_dev);
+int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev);
 struct DMatchArgs {       // device-resident arguments of directed_matching (after the back-rotation)
@@ -76,17 +76,13 @@ struct rb_nav;
 // The per-frame map chain of two kernels, with the old map rotated last.  rb_match_enqueue: FordwardMatch's apply (the
 // arg-max of neu is complete) and directed_matching against the unrotated old map, each probed keyline rotated by R_dev;
 // the matched (rho, s_rho) of every keyline go to neu's regularisation scratch.  rb_reg_ekf_enqueue: the match-count
-// gate, Regularize_1_iter from that scratch, the EKF, rotate_keylines(R_dev) of old, and (with nav) the frame's nav
-// record as rb_regularize_ekf_enqueue writes it.
+// gate, Regularize_1_iter from that scratch, the EKF, rotate_keylines(R_dev) of old, and with nav the frame's nav record
+// (except Kp / RKp of a mapped frame, which rb_rescale_enqueue fills in).
 int rb_match_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, const double *R_dev,
                      double min_thr_mod, double min_thr_ang, double max_radius, double loc_uncertainty,
                      const int *do_match_dev);
 int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameState *fs, int match_threshold,
                        double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa);
-// with nav: the frame's nav record is written beside the EKF (except Kp / RKp of a mapped frame: rb_rescale_enqueue)
-int rb_regularize_ekf_enqueue(rb_ctx *c, rb_map *m, double thresh, FrameState *fs, int match_threshold,
-                              const double *vel_dev, double q_abs, double loc_unc, const int *do_map_dev,
-                              const MapState *ost = nullptr, rb_nav *nav = nullptr, const FrameArgs *fa = nullptr);
 int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
                           const MapState *ost, rb_nav *nav, const FrameArgs *fa);
 int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, double loc_unc,

@@ -66,27 +66,23 @@ def _gpu_planes(w, h, sigma0, how, img):
     getattr(m, "upload_" + how)(img)
     m.dog_build()
     out = {k: m.plane(k).copy() for k in ("gray", "img0", "img1", "dog")}
-    path = m.scale_space_path()
     m.close()
     ctx.close()
-    return out, path
+    return out
 
 
-@pytest.mark.parametrize("env", [{}, {"REBVO_B200_ROW_TMA": "0"}, {"REBVO_B200_BLUR_TMA": "0"}],
-                         ids=["tma", "ring_rows", "plain_blur"])
+@pytest.mark.parametrize("env", [{}], ids=["tma"])
 @pytest.mark.parametrize("sigma0", [1.7818, 3.56359])
 def test_scale_space_bitwise(built, monkeypatch, sigma0, env):
-    """gray, Img(0), Img(1), DoG of RGB, mono and float uploads equal the reference's sspace::build bit for bit; the TMA
-    kernels serve these widths (path 3), and the non-TMA row / blur passes give the same bits."""
+    """gray, Img(0), Img(1), DoG of RGB, mono and float uploads equal the reference's sspace::build bit for bit (the TMA
+    kernels, whose tensor maps serve every width)."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    want_path = 3 & ~(1 if env.get("REBVO_B200_ROW_TMA") == "0" else 0) & ~(2 if env.get("REBVO_B200_BLUR_TMA") == "0" else 0)
     for gi, (w, h) in enumerate(GEOMETRIES):
         rgb, mono, gray = _inputs(w, h, 100 + gi)
         for how, img in (("rgb", rgb), ("mono", mono), ("gray", gray)):
             ref = _ref_planes(w, h, sigma0, how, img)
-            got, path = _gpu_planes(w, h, sigma0, how, img)
-            assert path == want_path, (w, h, how, path)
+            got = _gpu_planes(w, h, sigma0, how, img)
             for k in ref:
                 assert ref[k].shape == got[k].shape == (h, w)
                 bad = int((_u32(ref[k]) != _u32(got[k])).sum())

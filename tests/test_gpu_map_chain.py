@@ -1,8 +1,9 @@
 """The per-frame map chain after the minimiser: k_match (FordwardMatch's apply + directed_matching against the unrotated
-old map) and k_reg_ekf (gate + Regularize_1_iter + EKF + rotate_keylines of the old map), against the four-kernel chain
-k_fm_apply_rotate -> k_directed_match -> k_regularize_a_gate -> k_regb_ekf (REBVO_B200_MAP_CHAIN=0).  Both must give the
-same bits: raw nav records, the keylines and masks of the two newest maps, and per frame the FordwardMatch winners,
-directed hits and regularised keylines."""
+old map) and k_reg_ekf (gate + Regularize_1_iter + EKF + rotate_keylines of the old map), against the reference schedule
+(REBVO_B200_MAP_CHAIN=0): the stage kernels in the reference's order, k_fm_apply -> k_rotate -> k_directed_match -> gate ->
+k_regularize_a / k_regularize_b -> k_ekf, the kernels that test_gpu_parity.py and test_gpu_mapper_states.py pin to the
+reference bit for bit.  Both must give the same bits: raw nav records, the keylines and masks of the two newest maps, and
+per frame the FordwardMatch winners, directed hits and regularised keylines."""
 import numpy as np
 import pytest
 
@@ -78,7 +79,7 @@ def _run(frames, batch, how="host", kc=None, mirror=0):
 
 
 def _both(monkeypatch, *args, **kw):
-    """the run with the two-kernel chain (the default) and with REBVO_B200_MAP_CHAIN=0"""
+    """the run with the two-kernel chain (the default) and with the reference schedule (REBVO_B200_MAP_CHAIN=0)"""
     a = _run(*args, **kw)
     with monkeypatch.context() as m:
         m.setenv("REBVO_B200_MAP_CHAIN", "0")
@@ -142,7 +143,7 @@ def test_chain_special_frames(built, special, monkeypatch):
 
 
 def test_stage_profile_keys(built, stream, monkeypatch):
-    """the eager stage profile runs the two-kernel chain and still reports every stage key as a number"""
+    """the eager stage profile runs both schedules and reports every stage key as a number"""
     monkeypatch.setenv("REBVO_B200_STAGE_PROF", "1")
     from rebvo_b200 import capi, synth
     ts, rgb = stream

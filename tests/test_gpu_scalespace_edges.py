@@ -1,16 +1,17 @@
 """Scale space on awkward geometries: widths / heights that are not multiples of the 32-column chunks, 32-row bands and 64x32
-tiles of the TMA kernels (partial tiles are clipped by the tensor maps, border tiles take the zero-fill path), both box plans
-(sigma0 = 1.78: boxes 3/3/5 + 3/5/5, sigma0 = 3.56: 7/7/7 + 9/9/9), and the non-TMA fallbacks behind the environment switches.
-Every plane must equal the reference's (sspace::build, compiled from /root/reference) bit for bit."""
+tiles of the TMA kernels (partial tiles are clipped by the tensor maps, border tiles take the zero-fill path), down to 32x32,
+where the (32 + d)-row windows of the box-average row pass are taller than the image, and both box plans (sigma0 = 1.78:
+boxes 3/3/5 + 3/5/5, sigma0 = 3.56: 7/7/7 + 9/9/9).  Every plane must equal the reference's (sspace::build, compiled from
+the reference's sources) bit for bit."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-GEOMETRIES = [(36, 33), (64, 48), (100, 76), (200, 150), (328, 244), (752, 97)]
+GEOMETRIES = [(36, 33), (64, 48), (100, 76), (200, 150), (328, 244), (752, 97), (32, 32)]
 
 
-def _planes(w, h, sigma0, rgb, want_path=None):
+def _planes(w, h, sigma0, rgb):
     from rebvo_b200 import capi
     cam = dict(w=w, h=h, zfx=300.0, zfy=300.0, ppx=w / 2.0, ppy=h / 2.0)
     ctx = capi.Ctx(cam, sigma0, 1.2599, kl_capacity=20000)
@@ -18,8 +19,6 @@ def _planes(w, h, sigma0, rgb, want_path=None):
     m.upload_rgb(rgb)
     m.dog_build()
     out = {k: m.plane(k).copy() for k in ("gray", "img0", "img1", "dog")}
-    if want_path is not None:
-        assert m.scale_space_path() == want_path, "scale-space kernels: path %d, expected %d" % (m.scale_space_path(), want_path)
     m.close()
     ctx.close()
     return out
@@ -35,25 +34,10 @@ def test_odd_geometries_bitwise(built, sigma0):
         r = refapi.RefMap(w, h, w / 2.0, h / 2.0, 300.0, 300.0, sigma0, 1.2599)
         r.rgb2bw(rgb)
         r.build()
-        got = _planes(w, h, sigma0, rgb, want_path=3)   # the TMA kernels, not a silent fallback
+        got = _planes(w, h, sigma0, rgb)
         for k in ("gray", "img0", "img1", "dog"):
             ref = r.plane(k)
             assert ref.shape == got[k].shape
             assert np.array_equal(ref.view(np.uint32), got[k].view(np.uint32)), "%dx%d sigma0 %.2f plane %s: %d pixels differ" % (
                 w, h, sigma0, k, int((ref.view(np.uint32) != got[k].view(np.uint32)).sum()))
 
-
-@pytest.mark.parametrize("env", [{"REBVO_B200_ROW_TMA": "0"}, {"REBVO_B200_BLUR_TMA": "0"}])
-def test_kernel_variants_agree(built, monkeypatch, env):
-    """The non-TMA row and blur passes (which also serve widths the tensor maps cannot take): same bits as the default
-    path."""
-    rng = np.random.default_rng(9)
-    w, h = 200, 150
-    rgb = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-    want = _planes(w, h, 3.56359, rgb, want_path=3)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    path = 3 & ~(1 if env.get("REBVO_B200_ROW_TMA") == "0" else 0) & ~(2 if env.get("REBVO_B200_BLUR_TMA") == "0" else 0)
-    got = _planes(w, h, 3.56359, rgb, want_path=path)
-    for k in want:
-        assert np.array_equal(want[k].view(np.uint32), got[k].view(np.uint32)), k
