@@ -129,6 +129,8 @@ int rb_ctx_sync(rb_ctx *c);
 int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r);
 /* kernels launched on this context so far (bench.py's gpu_launches) */
 int64_t rb_ctx_launch_count(const rb_ctx *c);
+/* thread-block clusters of one Minimizer_RV launch (REBVO_B200_MIN_G when all fit, else 1); 0: one launch per evaluation */
+int rb_ctx_minimizer_clusters(const rb_ctx *c);
 
 /* ---- edge map (ring slot) ---------------------------------------------------------------------- */
 int rb_map_create(rb_ctx *c, rb_map **out);

@@ -76,7 +76,7 @@ KEYLINE = np.dtype({
 
 # every symbol include/rebvo_b200.h declares
 SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "rb_ctx_box_plan",
-           "rb_ctx_launch_count", "rb_map_create", "rb_map_destroy", "rb_map_clone", "rb_map_upload_rgb", "rb_map_upload_mono",
+           "rb_ctx_launch_count", "rb_ctx_minimizer_clusters", "rb_map_create", "rb_map_destroy", "rb_map_clone", "rb_map_upload_rgb", "rb_map_upload_mono",
            "rb_map_upload_gray",
            "rb_map_dog_build", "rb_map_get_plane", "rb_map_detect", "rb_map_detect_ss", "rb_map_reestimate_thresh", "rb_map_knum",
            "rb_map_counters",
@@ -194,6 +194,9 @@ class Ctx:
 
     def launches(self):
         return self.L.rb_ctx_launch_count(self.h_)
+
+    def minimizer_clusters(self):
+        return self.L.rb_ctx_minimizer_clusters(self.h_)
 
     def new_map(self):
         return Map(self)

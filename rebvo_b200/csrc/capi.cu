@@ -296,6 +296,9 @@ extern "C" int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r)
 }
 
 extern "C" int64_t rb_ctx_launch_count(const rb_ctx *c) { return c->launches; }
+extern "C" int rb_ctx_minimizer_clusters(const rb_ctx *c) {
+    return c->min_persist && c->min_cluster_kpc > 0 ? c->min_cluster_g : 0;
+}
 
 // ---- map ------------------------------------------------------------------------------------------
 int rb_map_alloc(rb_ctx *c, rb_map **out, bool with_ws) {

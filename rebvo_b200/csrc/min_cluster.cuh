@@ -1,5 +1,5 @@
 // min_cluster.cuh -- global_tracker::Minimizer_RV (src/mtracklib/global_tracker.cpp:578-819) in ONE thread-block
-// cluster.  Included by tracker.cu after the per-keyline pieces (tvr_body, lm_*).
+// cluster.  Included by tracker.cu after the per-keyline body (tvr_keyline) and the LM pieces (lm_*).
 //
 // A minimisation is ~12 TryVelRot evaluations, each a sum over all old keylines followed by a 6x6 LM step whose result
 // is the next evaluation's pose: a chain of grid-wide reductions.  Exchanging through L2 between ~65 independent
@@ -17,20 +17,9 @@
 //     their LM steps run on two warps side by side, so 2*(init_iter+1) dependent rounds become init_iter+1.
 // Sums: per thread in keyline order, transposing warp butterfly, warps in order, ranks in order -- fixed, deterministic,
 // not the reference's pairwise tree (tests: rel 1e-10 on JtJ/JtF, V/W abs 1e-9).
-// This header is included once per CTA size (MC_T, namespace MC_NS): 512 threads for the one-cluster form, 256 for the
-// multi-cluster form (see k_minimizer_cluster).
-#ifndef MC_T
-#error "define MC_T and MC_NS before including min_cluster.cuh"
-#endif
-#undef MC_NW
-#undef MC_MAXJ
-#undef MC_NV
-#define MC_NW (MC_T / 32)
-#define MC_MAXJ (3584 / MC_T)         // keylines per thread of the one-cluster form: MC_C * MC_T * MC_MAXJ = 57344 >= KEYLINE_MAX
-#define MC_NV (MC_MAXJ * MC_NW)      // "virtual warps" of a CTA (32 consecutive keylines each)
+// The kernel is a template over the CTA size T: 512 threads for the one-cluster form, 256 for the multi-cluster form.
+#pragma once
 
-#ifndef MC_COMMON_PART
-#define MC_COMMON_PART
 #define MC_C 16                      // CTAs per cluster (non-portable size, one CTA per SM)
 #define MC_GMAX 8                    // clusters of one minimisation
 #define MC_PW 30                     // doubles per pose and CTA in the exchange: 28 sums, has-a-match, last matched fi
@@ -40,6 +29,8 @@
 #endif
 #define MC_SPIN_LIMIT (1ll << 29)    // ~0.27 s: a broken exchange aborts with NaN results instead of hanging the device
 #define MC_BYTES_PER_KL 57           // x0,y0,z0,s_rho, 3 residual buffers (double) + 1 flag byte
+#define MC_KPC_MAX 3584              // keylines per CTA at most: MC_C * MC_KPC_MAX = 57344 >= KEYLINE_MAX
+#define MC_NV (MC_KPC_MAX / 32)      // "virtual warps" of a CTA (32 consecutive keylines each)
 
 #ifdef RB_TVR_PROF   // stamps: [CTA][round (15 = kernel level)][16]
 #define MC_STAMP(e, k) do { if (threadIdx.x == 0 && blockIdx.x < 16) g_tvr_prof[(blockIdx.x * 16 + (e)) * 16 + (k)] = clock64(); } while (0)
@@ -47,19 +38,11 @@
 #define MC_STAMP(e, k) do { } while (0)
 #endif
 #ifdef RB_TVR_PROF   // %globaltimer of "sums published" / "column gathered" per CTA and round (inter-cluster skew vs mechanism)
-#ifndef MC_GT_DEFINED
-#define MC_GT_DEFINED
 __device__ long long g_mc_gt[128 * 16 * 2];
 extern "C" int rb_debug_fetch_gt(long long *out) { return (int)cudaMemcpyFromSymbol(out, g_mc_gt, sizeof(g_mc_gt)); }
-#endif
 #define MC_GT(e, k) do { if (threadIdx.x == 0 && blockIdx.x < 128) g_mc_gt[(blockIdx.x * 16 + (e)) * 2 + (k)] = tvr_gtime(); } while (0)
 #else
 #define MC_GT(e, k) do { } while (0)
-#endif
-#if defined(RB_TVR_PROF) && defined(MC_BODY_STAMPS)   // stage stamps of thread 0's first keyline of the last evaluation (CTA 0, round slot 14)
-#define MC_BSTAMP(k) do { if (threadIdx.x == 0 && blockIdx.x == 0) g_tvr_prof[(14) * 16 + (k)] = clock64(); } while (0)
-#else
-#define MC_BSTAMP(k) do { } while (0)
 #endif
 
 struct McPlan {
@@ -116,158 +99,6 @@ struct McView {
     int S;
     int base, cnt, J;     // first keyline, keylines of this CTA, iterations per thread (uniform over the cluster)
 };
-
-// Per-keyline part of TryVelRot (global_tracker.cpp:350-463) for U keylines of one thread at once.  Same operations
-// in the same order as tvr_body (tracker.cu), but written stage by stage over the U keylines with selects instead of
-// branches, so that their dependent chains (projection -> 1/z -> pixel -> field -> matched keyline -> residual ->
-// Jacobian -> 1/q_rho) interleave: one keyline alone is a ~1800-cycle latency chain, and a CTA here owns ~1000 of them.
-template <bool RW, bool PJ, int U>
-__device__ __forceinline__ void mc_body(const double (&x0)[U], const double (&y0)[U], const double (&z0)[U],
-                                        const double (&s_rho)[U], const float2 (&m)[U], const float (&n_m)[U],
-                                        const bool (&skip)[U], const bool (&act)[U], bool has_rin,
-                                        const double (&r_prev)[U], const double *sR, const double *sV, const double *sRM,
-                                        const TvrConst &tc, const CamC &cam, const unsigned long long *__restrict__ field,
-                                        const float4 *__restrict__ fpack, int *__restrict__ m_id_f, const int (&gi)[U],
-                                        double (&acc)[28], bool (&matched)[U], bool (&need)[U], double (&fi_own)[U],
-                                        bool (&wrote)[U]) {
-    MC_BSTAMP(0);
-    const double max_r = tc.max_r;
-    double px[U], py[U], pz[U], rho_p[U], qx[U], qy[U], pix[U], piy[U], weight[U];
-    bool inb[U], outside[U];
-    int pixel[U];
-    // SE3on3PMatrix (ne10wrapper.h:375-405) and ProyP3toI3PMatrix (:429-445)
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        double t = sR[0] * x0[u];
-        t = t + sR[1] * y0[u];
-        t = t + sR[2] * z0[u];
-        px[u] = sV[0] + t;
-        t = sR[3] * x0[u];
-        t = t + sR[4] * y0[u];
-        t = t + sR[5] * z0[u];
-        py[u] = sV[1] + t;
-        t = sR[6] * x0[u];
-        t = t + sR[7] * y0[u];
-        t = t + sR[8] * z0[u];
-        pz[u] = sV[2] + t;
-    }
-    MC_BSTAMP(1);
-#pragma unroll
-    for (int u = 0; u < U; u++) rho_p[u] = 1 / pz[u];
-    MC_BSTAMP(2);
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        const double pz_zf = cam.zfm * rho_p[u];
-        qx[u] = pz_zf * px[u];
-        qy[u] = pz_zf * py[u];
-        pix[u] = qx[u] + (double)cam.ppx;   // cam_mod.Hom2Img
-        piy[u] = qy[u] + (double)cam.ppy;
-        const int x = (int)(pix[u] + 0.5), y = (int)(piy[u] + 0.5);   // util::round2int_positive
-        weight[u] = 1;
-        if (RW && has_rin) {
-            const double r = fabs(r_prev[u]);
-            if (!skip[u] && r > tc.k_huber) weight[u] = tc.k_huber / r;   // :370-372
-        }
-        outside[u] = x < 1 || y < 1 || x >= cam.w - 1 || y >= cam.h - 1;   // :376
-        inb[u] = !skip[u] && !outside[u];
-        pixel[u] = inb[u] ? y * cam.w + x : 0;
-    }
-    MC_BSTAMP(3);
-    // field lookup, then the matched keyline's gather record
-    unsigned long long key[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) key[u] = inb[u] ? field[pixel[u]] : ~0ull;
-    float4 ga[U], gb[U];
-    int ikl[U];
-    bool cand[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        cand[u] = key[u] != ~0ull;
-        MC_BSTAMP(4);
-        ikl[u] = cand[u] ? (int)(0xFFFFFFFFu - (unsigned int)(key[u] & 0xFFFFFFFFull)) : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        ga[u] = cand[u] ? fpack[2 * ikl[u]] : make_float4(0.f, 0.f, 0.f, 0.f);
-        gb[u] = cand[u] ? fpack[2 * ikl[u] + 1] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    double f[U], dfx[U], dfy[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        if (ga[u].x != 12345.f) MC_BSTAMP(5);
-        const float mrx = (float)(sRM[0] * (double)m[u].x + sRM[1] * (double)m[u].y);   // :386-388
-        const float mry = (float)(sRM[2] * (double)m[u].x + sRM[3] * (double)m[u].y);
-        const double p_n2 = (double)(n_m[u] * n_m[u]);                                   // Test_f_k (global_tracker.h:89-104)
-        const double p_esc = (double)(mrx * ga[u].x + mry * ga[u].y);
-        const bool hit = cand[u] && !(fabs(p_esc - p_n2) > tc.match_thresh * p_n2);
-        const double dx = pix[u] - (double)ga[u].z, dy = piy[u] - (double)ga[u].w;      // Calc_f_J2 :254-262
-        const double fi = dx * (double)gb[u].x + dy * (double)gb[u].y;
-        matched[u] = hit;
-        need[u] = inb[u] && !hit;
-        wrote[u] = !skip[u] && outside[u];
-        fi_own[u] = hit ? fi : 0.0;
-        double fv = hit ? fi : max_r;
-        double gx = hit ? (double)gb[u].x : 0.0, gy = hit ? (double)gb[u].y : 0.0;
-        if (RW) {   // fm*=weigth; df_dPi*=weigth (:380,399-403); the weight of a skipped keyline is 1
-            fv = fv * weight[u];
-            gx = gx * weight[u];
-            gy = gy * weight[u];
-        }
-        f[u] = skip[u] ? 0.0 : fv;
-        dfx[u] = gx;
-        dfy[u] = gy;
-        if (m_id_f && act[u]) m_id_f[gi[u]] = hit ? ikl[u] : -1;
-    }
-    if (f[0] != 1e300) MC_BSTAMP(6);
-    // Jacobians (:419-449), the 1/q_rho scaling (:452-463), products
-    double q_rho[U], iq[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        const double qvel = (cam.zfm * dfx[u] * sV[0] + cam.zfm * dfy[u] * sV[1]) + (qx[u] * dfx[u] + qy[u] * dfy[u]) * sV[2];
-        q_rho[u] = RW ? sqrt(s_rho[u] * qvel * s_rho[u] * qvel + 1) : s_rho[u];
-    }
-    if (q_rho[0] != 1e300) MC_BSTAMP(7);
-    if (PJ) {
-#pragma unroll
-        for (int u = 0; u < U; u++) iq[u] = 1 / q_rho[u];
-        if (iq[0] != 1e300) MC_BSTAMP(8);
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-            double t0 = cam.zfm * rho_p[u];
-            const double J0 = t0 * dfx[u], J1 = t0 * dfy[u];
-            t0 = rho_p[u] * qx[u];
-            double J2 = t0 * dfx[u];
-            t0 = rho_p[u] * qy[u];
-            J2 = J2 + t0 * dfy[u];
-            double J3 = J1 * pz[u];
-            J3 = J3 + J2 * py[u];
-            double J4 = J0 * pz[u];
-            J4 = J4 + J2 * px[u];
-            t0 = J0 * py[u];
-            double J5 = -1.0 * t0;
-            J5 = J5 + J1 * px[u];
-            const double J[6] = {div_with_rcp(J0, q_rho[u], iq[u]), div_with_rcp(J1, q_rho[u], iq[u]),
-                                 div_with_rcp(J2, q_rho[u], iq[u]), div_with_rcp(J3, q_rho[u], iq[u]),
-                                 div_with_rcp(J4, q_rho[u], iq[u]), div_with_rcp(J5, q_rho[u], iq[u])};
-            const double fs = div_with_rcp(f[u], q_rho[u], iq[u]);
-            int k = 0;
-#pragma unroll
-            for (int a = 0; a < 6; a++)
-#pragma unroll
-                for (int b = a; b < 6; b++, k++) acc[k] = fma(J[a], J[b], acc[k]);   // (sums are order-toleranced anyway)
-#pragma unroll
-            for (int a = 0; a < 6; a++) acc[21 + a] = fma(J[a], fs, acc[21 + a]);
-            acc[27] = fma(fs, fs, acc[27]);
-        }
-        if (acc[27] != 1e300) MC_BSTAMP(9);
-    } else {
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-            const double fs = f[u] / q_rho[u];
-            acc[27] = fma(fs, fs, acc[27]);
-        }
-    }
-}
 
 // LM steps of the two init tries evaluated side by side (global_tracker.cpp:651-683 and :700-732)
 __device__ __forceinline__ void mc_lm_step_zero(LMState &z, int step) {
@@ -365,13 +196,10 @@ __device__ __forceinline__ bool mc_slot_gather(unsigned long long *ll, int G, in
         if (clock64() - t0 > MC_SPIN_LIMIT) return false;
     }
 }
-#endif   // MC_COMMON_PART
-
-namespace MC_NS {
-
+template <int T>
 struct __align__(16) McSmem {
     double gather[2][MC_C][MC_XW];   // [round parity][source rank][value]
-    double part[MC_NW][32];
+    double part[T / 32][32];
     double xout[64];
     double xcol[64];                 // column sums (this CTA's sums + those of the equal-rank CTAs of the other clusters)
     double req[2][16];               // per pose: R[9] V[3] RotM[4]
@@ -386,11 +214,8 @@ struct __align__(16) McSmem {
 
 // one TryVelRot evaluation of pose slot p over this CTA's keylines; leaves the CTA's 28 sums and stale-fi summary in
 // sm.xout[p * MC_PW ..]
-#ifndef MC_U
-#define MC_U 1                         // keylines of a thread evaluated side by side (2, 3 measured slower: register pressure)
-#endif
-template <bool RW, bool PJ>
-__device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p, const KLSoA &old, const TvrConst &tc,
+template <int T, bool RW, bool PJ>
+__device__ __forceinline__ void mc_eval_pose(McSmem<T> &sm, const McView &v, int p, const KLSoA &old, const TvrConst &tc,
                                              const CamC &cam, const unsigned long long *__restrict__ field,
                                              const float4 *__restrict__ fpack, bool write_mid, int tid, int lane,
                                              int wid) {
@@ -400,20 +225,21 @@ __device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p,
     const double *rin = v.res[has_rin ? res_in : 0], *grin = v.gres[has_rin ? res_in : 0];
     double *rout = v.res[res_out], *grout = v.gres[res_out];
     int *mid_out = write_mid ? old.m_id_f : nullptr;
+    constexpr int U = 1;   // keylines of a thread evaluated side by side (2, 3 measured slower: register pressure)
     double acc[28];
 #pragma unroll
     for (int k = 0; k < 28; k++) acc[k] = 0;
     MC_BSTAMP(10);
-    for (int j0 = 0; j0 < v.J; j0 += MC_U) {
-        if (j0 == MC_U) MC_BSTAMP(11);
-        double x0[MC_U], y0[MC_U], z0[MC_U], s_rho[MC_U], r_prev[MC_U], fi_own[MC_U];
-        float2 m[MC_U];
-        float n_m[MC_U];
-        bool skip[MC_U], act[MC_U], matched[MC_U], need[MC_U], wrote[MC_U];
-        int gi[MC_U], li[MC_U];
+    for (int j0 = 0; j0 < v.J; j0 += U) {
+        if (j0 == U) MC_BSTAMP(11);
+        double x0[U], y0[U], z0[U], s_rho[U], r_prev[U], fi_own[U];
+        float2 m[U];
+        float n_m[U];
+        bool skip[U], act[U], matched[U], need[U], outside[U];
+        int gi[U], li[U];
 #pragma unroll
-        for (int u = 0; u < MC_U; u++) {
-            li[u] = (j0 + u) * MC_T + tid;
+        for (int u = 0; u < U; u++) {
+            li[u] = (j0 + u) * T + tid;
             gi[u] = v.base + li[u];
             act[u] = li[u] < v.cnt;
             // lanes without a keyline run on harmless operands and contribute exact zeros
@@ -444,18 +270,18 @@ __device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p,
             double r = 0.0;
             if (has_rin && act[u]) {
                 r = li[u] < v.S ? rin[li[u]] : grin[gi[u]];
-                if ((unsigned long long)__double_as_longlong(r) == RES_SENTINEL) r = sm.wcarry[res_in][(j0 + u) * MC_NW + wid];
+                if ((unsigned long long)__double_as_longlong(r) == RES_SENTINEL) r = sm.wcarry[res_in][(j0 + u) * (T / 32) + wid];
             }
             r_prev[u] = r;
         }
-        mc_body<RW, PJ, MC_U>(x0, y0, z0, s_rho, m, n_m, skip, act, has_rin, r_prev, sR, sV, sRM, tc, cam, field, fpack,
-                              mid_out, gi, acc, matched, need, fi_own, wrote);
+        tvr_keyline<RW, PJ, U>(x0, y0, z0, s_rho, m, n_m, skip, act, has_rin, r_prev, sR, sV, sRM, tc, cam, field,
+                                  fpack, mid_out, gi, acc, matched, need, fi_own, outside);
         // "DResidualNew[ikl]=fi" keeps the fi of the last matched keyline before ikl (:341,399-408): in-warp scan here,
         // earlier warps / CTAs through wcarry once the round's exchange is complete
 #pragma unroll
-        for (int u = 0; u < MC_U; u++) {
+        for (int u = 0; u < U; u++) {
             if (j0 + u >= v.J) break;
-            const int vw = (j0 + u) * MC_NW + wid;
+            const int vw = (j0 + u) * (T / 32) + wid;
             const unsigned int bal = __ballot_sync(0xffffffffu, matched[u]);
             const unsigned int lower = bal & ((1u << lane) - 1u);
             const double prev_fi = __shfl_sync(0xffffffffu, fi_own[u], lower ? 31 - __clz(lower) : 0);
@@ -464,7 +290,7 @@ __device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p,
                 sm.vw_has[p][vw] = bal != 0;
                 sm.vw_last[p][vw] = wl;
             }
-            if (act[u] && (matched[u] || need[u] || wrote[u])) {
+            if (act[u] && (matched[u] || need[u] || outside[u])) {
                 const double rv = matched[u] ? fi_own[u]
                                   : need[u]  ? (lower ? prev_fi : __longlong_as_double((long long)RES_SENTINEL))
                                              : tc.max_r;
@@ -494,13 +320,13 @@ __device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p,
         if (PJ || tid == 27) {
             t = sm.part[0][tid];
 #pragma unroll
-            for (int ww = 1; ww < MC_NW; ww++) t += sm.part[ww][tid];
+            for (int ww = 1; ww < T / 32; ww++) t += sm.part[ww][tid];
         }
         sm.xout[p * MC_PW + tid] = t;
     } else if (tid == 32) {
         int has = 0;
         double lastv = 0;
-        for (int q = v.J * MC_NW - 1; q >= 0; q--)
+        for (int q = v.J * (T / 32) - 1; q >= 0; q--)
             if (sm.vw_has[p][q]) {
                 has = 1;
                 lastv = sm.vw_last[p][q];
@@ -512,13 +338,15 @@ __device__ __forceinline__ void mc_eval_pose(McSmem &sm, const McView &v, int p,
 }
 
 // next pose of a chain: R = exp(W), V, residual buffer ids (:309-311) / the z rotation RotM = exp((0,0,W.z)) (:313-314)
-__device__ __forceinline__ void mc_req_R(McSmem &sm, int p, const LMState &s) {
+template <int T>
+__device__ __forceinline__ void mc_req_R(McSmem<T> &sm, int p, const LMState &s) {
     so3_exp(s.Xeval + 3, sm.req[p]);
     for (int k = 0; k < 3; k++) sm.req[p][9 + k] = s.Xeval[k];
     sm.req_res[p][0] = s.res_in;
     sm.req_res[p][1] = s.res_out;
 }
-__device__ __forceinline__ void mc_req_RM(McSmem &sm, int p, const LMState &s) {
+template <int T>
+__device__ __forceinline__ void mc_req_RM(McSmem<T> &sm, int p, const LMState &s) {
     double wz[3] = {0, 0, s.Xeval[5]}, RMf[9];
     so3_exp(wz, RMf);
     sm.req[p][12] = RMf[0];
@@ -527,7 +355,8 @@ __device__ __forceinline__ void mc_req_RM(McSmem &sm, int p, const LMState &s) {
     sm.req[p][15] = RMf[4];
 }
 
-__global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
+template <int T>
+__global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
     k_minimizer_cluster(KLSoA old, const MapState *__restrict__ old_st, const unsigned long long *__restrict__ field,
                         const float4 *__restrict__ fpack, MapState *f_st, LMState *lm_out, int *abort_out, CamC cam,
                         McPlan plan, MinSetup su, FrameState *post_fs, FmBest *fm_best, int kpc_cap, ResPtrs gres,
@@ -542,7 +371,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
     if (!early) pdl_wait();
     MC_STAMP(15, 1);
     extern __shared__ __align__(16) unsigned char mc_dyn[];
-    __shared__ McSmem sm;
+    __shared__ McSmem<T> sm;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int rank = (int)mc_cluster_rank();
     const int G = (int)(gridDim.x / MC_C), cl = (int)(blockIdx.x / MC_C);   // clusters of this minimisation, mine
@@ -582,11 +411,11 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         v.gres[2] = gres.r[2];
         int kpc = (K0 + MC_C * G - 1) / (MC_C * G);
         kpc = (kpc + 31) & ~31;               // whole virtual warps
-        if (kpc > MC_T * MC_MAXJ) kpc = MC_T * MC_MAXJ;   // (the host only launches this kernel when the capacity fits)
+        if (kpc > MC_KPC_MAX) kpc = MC_KPC_MAX;   // (the host only launches this kernel when the capacity fits)
         v.base = (rank * G + cl) * kpc;        // slices in (rank, cluster) order: a column = the CTAs of equal rank
         v.cnt = K0 - v.base;
         v.cnt = v.cnt < 0 ? 0 : (v.cnt > kpc ? kpc : v.cnt);
-        v.J = (kpc + MC_T - 1) / MC_T;
+        v.J = (kpc + T - 1) / T;
     }
     TvrConst tc;
     tc.max_r = su.max_r;
@@ -600,7 +429,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         tc.mnt = su.a.match_num_thresh < fc ? su.a.match_num_thresh : fc;
     }
     // ---- prologue: operands -> shared memory, LM state, barriers -----------------------------------------------
-    for (int li = tid; li < v.cnt; li += MC_T) {
+    for (int li = tid; li < v.cnt; li += T) {
         if (li < v.S) {
             const KlOp o = load_klop(old, v.base + li, cam);
             v.x0[li] = o.x0;
@@ -620,7 +449,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         const unsigned int fc = su.fc_from_state ? f_st->frame_count : su.frame_count;
         tc.mnt = su.a.match_num_thresh < fc ? su.a.match_num_thresh : fc;   // (<= 255)
         const int ns = v.cnt < v.S ? v.cnt : v.S;
-        for (int li = tid; li < ns; li += MC_T) v.flag[li] = (unsigned int)v.flag[li] < tc.mnt ? 1 : 0;   // (own bytes)
+        for (int li = tid; li < ns; li += T) v.flag[li] = (unsigned int)v.flag[li] < tc.mnt ? 1 : 0;   // (own bytes)
     }
     const bool fused = plan.merge_round >= 0;
     if (tid == 0) {
@@ -667,12 +496,12 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         MC_STAMP(e, 0);
         if (last) pdl_launch();
         // ---- keylines ---------------------------------------------------------------------------------------
-        if (RW) mc_eval_pose<true, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
-        else if (PJ) mc_eval_pose<false, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
-        else mc_eval_pose<false, false>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
+        if (RW) mc_eval_pose<T, true, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
+        else if (PJ) mc_eval_pose<T, false, true>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
+        else mc_eval_pose<T, false, false>(sm, v, 0, old, tc, cam, field, fpack, last, tid, lane, wid);
         if (two) {
-            if (PJ) mc_eval_pose<false, true>(sm, v, 1, old, tc, cam, field, fpack, false, tid, lane, wid);
-            else mc_eval_pose<false, false>(sm, v, 1, old, tc, cam, field, fpack, false, tid, lane, wid);
+            if (PJ) mc_eval_pose<T, false, true>(sm, v, 1, old, tc, cam, field, fpack, false, tid, lane, wid);
+            else mc_eval_pose<T, false, false>(sm, v, 1, old, tc, cam, field, fpack, false, tid, lane, wid);
         }
         __syncthreads();
         MC_STAMP(e, 1);
@@ -767,7 +596,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
                         }
                     }
                 }
-                const int nvw = v.J * MC_NW;
+                const int nvw = v.J * (T / 32);
                 for (int q = lane; q < (two ? 2 : 1) * nvw; q += 32) {
                     const int p = q / nvw, vw = q - p * nvw;
                     double cy = 0;
@@ -845,7 +674,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
             // FordwardMatch's arg-max over this CTA's keylines, whose m_id_f the pass above wrote: the CAS round trips
             // run on the warps that are idle during the last exchange and LM step, not between the pass and the exchange
             if (fm_best) {   // (two keylines per thread and step: loads and CAS round trips in flight together)
-                const int nkn = f_st->kn, st = MC_T - 96;
+                const int nkn = f_st->kn, st = T - 96;
                 for (int li = tid - 96; li < v.cnt; li += 2 * st)
                     d_fm_argmax_two(old, v.base + li, li + st < v.cnt ? v.base + li + st : -1, nkn, fm_best);
             }
@@ -873,12 +702,10 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(MC_T, 1)
         if (tid == 0 && G > 1) ctl->gen = seq0 + MIN_MAX_EVALS + 1u;   // the next minimisation gets fresh sequence numbers
         const double *src = reinterpret_cast<const double *>(&sm.lm);
         double *dst = reinterpret_cast<double *>(lm_out);
-        for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += MC_T) dst[k] = src[k];
+        for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += T) dst[k] = src[k];
         if (tid == 0 && post_fs) d_frame_post_min_cov(post_fs, sm.lm);
     }
     MC_STAMP(15, 3);
     mc_cluster_sync();   // no CTA exits while a peer may still send to it
     MC_STAMP(15, 4);
 }
-
-}   // namespace MC_NS

@@ -31,6 +31,13 @@ extern "C" int rb_debug_fetch(long long *out) {
 #define TVR_STAMP(k) do { } while (0)
 #define TVR_GSTAMP(k) do { } while (0)
 #endif
+// Stage stamps of thread 0's first keyline of the cluster minimiser's last evaluation (CTA 0, round slot 14).  k_tvr_eval
+// runs the same body, so in such a build its block 0 stamps the same slots: read them after a cluster-kernel run only.
+#if defined(RB_TVR_PROF) && defined(MC_BODY_STAMPS)
+#define MC_BSTAMP(k) do { if (threadIdx.x == 0 && blockIdx.x == 0) g_tvr_prof[(14) * 16 + (k)] = clock64(); } while (0)
+#else
+#define MC_BSTAMP(k) do { } while (0)
+#endif
 
 struct CamC {
     double zfm, inv_zf;
@@ -599,7 +606,7 @@ __global__ void k_lm_begin(TrackState *ts, const MapState *old_st, const MapStat
 }
 
 // ---- pieces of one TryVelRot evaluation (global_tracker.cpp:285-543), shared by the one-launch-per-evaluation
-// kernel and by the persistent whole-minimisation kernel -------------------------------------------------------
+// kernel k_tvr_eval and by the whole-minimisation kernel k_minimizer_cluster ---------------------------------------
 struct TvrConst {          // constants of one minimisation
     double max_r, match_thresh, s_rho_min, k_huber;
     unsigned int mnt;      // min(match_num_thresh, FrameCount)
@@ -646,129 +653,173 @@ struct TrackPtrs {         // the pointers inside TrackState, passed by value (n
     unsigned long long *ll;
 };
 
-// per-keyline part: projection, field lookup, residual, Jacobian products
-template <bool RW, bool PJ>
-__device__ __forceinline__ void tvr_body(const KlOp &o, bool has_rin, double r_prev, const double *sR,
-                                         const double *sV, const double *sRM, const TvrConst &tc, const CamC &cam,
-                                         const unsigned long long *__restrict__ field,
-                                         const float4 *__restrict__ fpack, double *__restrict__ rout,
-                                         int *__restrict__ m_id_f, int i, double (&acc)[28], bool &matched,
-                                         bool &need, double &fi_own, bool &wrote, double &r_w) {
+// Per-keyline part of TryVelRot (global_tracker.cpp:350-463) for U keylines of one thread: projection, field lookup,
+// residual, Jacobian products added to acc.  k_tvr_eval runs one keyline per thread; the cluster kernel a thread's
+// keylines in turn, U = 1 at a time.  Written stage by stage over the U keylines with selects instead of branches: a
+// skipped keyline (or a lane without one, act false) runs the same path and adds zeros.  The stage-by-stage form is also
+// what keeps the cluster kernel's code as measured: the same body written for one scalar keyline compiles to different
+// instructions there (+2 % minimiser time in the one-cluster form).  Outputs per keyline: matched (its fi is fi_own),
+// need (a miss inside the image: the residual buffer gets the fi of the last matched keyline before it), outside
+// (evaluated, projected outside the image: the buffer gets max_r).
+template <bool RW, bool PJ, int U>
+__device__ __forceinline__ void tvr_keyline(const double (&x0)[U], const double (&y0)[U], const double (&z0)[U],
+                                            const double (&s_rho)[U], const float2 (&m)[U], const float (&n_m)[U],
+                                            const bool (&skip)[U], const bool (&act)[U], bool has_rin,
+                                            const double (&r_prev)[U], const double *sR, const double *sV,
+                                            const double *sRM, const TvrConst &tc, const CamC &cam,
+                                            const unsigned long long *__restrict__ field, const float4 *__restrict__ fpack,
+                                            int *__restrict__ m_id_f, const int (&gi)[U], double (&acc)[28],
+                                            bool (&matched)[U], bool (&need)[U], double (&fi_own)[U],
+                                            bool (&outside)[U]) {
+    MC_BSTAMP(0);
     const double max_r = tc.max_r;
-    const double x0 = o.x0, y0 = o.y0, z0 = o.z0;
-    // SE3on3PMatrix (ne10wrapper.h:375-405): MulC, MlAc, MlAc, then Vel + .
-    double px = sR[0] * x0;
-    px = px + sR[1] * y0;
-    px = px + sR[2] * z0;
-    px = sV[0] + px;
-    double py = sR[3] * x0;
-    py = py + sR[4] * y0;
-    py = py + sR[5] * z0;
-    py = sV[1] + py;
-    double pz = sR[6] * x0;
-    pz = pz + sR[7] * y0;
-    pz = pz + sR[8] * z0;
-    pz = sV[2] + pz;
-    // ProyP3toI3PMatrix (ne10wrapper.h:429-445)
-    const double rho_p = 1 / pz;
-    const double pz_zf = cam.zfm * rho_p;
-    const double qx = pz_zf * px, qy = pz_zf * py;
-    double f = 0, dfx = 0, dfy = 0;
-    int mid_f = -1;
-    const bool skip = (o.s_rho > tc.s_rho_min) || ((unsigned int)o.m_num < tc.mnt);   // :356
-    if (!skip) {
-        const double pix = qx + (double)cam.ppx, piy = qy + (double)cam.ppy;   // cam_mod.Hom2Img
-        const int x = (int)(pix + 0.5), y = (int)(piy + 0.5);                   // util::round2int_positive
-        double weight = 1;
+    double px[U], py[U], pz[U], rho_p[U], qx[U], qy[U], pix[U], piy[U], weight[U];
+    bool inb[U], off[U];
+    int pixel[U];
+    // SE3on3PMatrix (ne10wrapper.h:375-405) and ProyP3toI3PMatrix (:429-445)
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        double t = sR[0] * x0[u];
+        t = t + sR[1] * y0[u];
+        t = t + sR[2] * z0[u];
+        px[u] = sV[0] + t;
+        t = sR[3] * x0[u];
+        t = t + sR[4] * y0[u];
+        t = t + sR[5] * z0[u];
+        py[u] = sV[1] + t;
+        t = sR[6] * x0[u];
+        t = t + sR[7] * y0[u];
+        t = t + sR[8] * z0[u];
+        pz[u] = sV[2] + t;
+    }
+    MC_BSTAMP(1);
+#pragma unroll
+    for (int u = 0; u < U; u++) rho_p[u] = 1 / pz[u];
+    MC_BSTAMP(2);
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        const double pz_zf = cam.zfm * rho_p[u];
+        qx[u] = pz_zf * px[u];
+        qy[u] = pz_zf * py[u];
+        pix[u] = qx[u] + (double)cam.ppx;   // cam_mod.Hom2Img
+        piy[u] = qy[u] + (double)cam.ppy;
+        const int x = (int)(pix[u] + 0.5), y = (int)(piy[u] + 0.5);   // util::round2int_positive
+        weight[u] = 1;
         if (RW && has_rin) {
-            const double r = fabs(r_prev);
-            if (r > tc.k_huber) weight = tc.k_huber / r;                       // :370-372
+            const double r = fabs(r_prev[u]);
+            if (!skip[u] && r > tc.k_huber) weight[u] = tc.k_huber / r;   // :370-372
         }
-        if (x < 1 || y < 1 || x >= cam.w - 1 || y >= cam.h - 1) {               // :376
-            f = max_r;
-            if (RW) f *= weight;
-            if (rout) rout[i] = max_r;   // (the cluster kernel keeps the residual buffers in shared memory: rout == nullptr)
-            wrote = true;
-            r_w = max_r;
-        } else {
-            const float mrx = (float)(sRM[0] * (double)o.m.x + sRM[1] * (double)o.m.y);   // :386-388
-            const float mry = (float)(sRM[2] * (double)o.m.x + sRM[3] * (double)o.m.y);
-            const unsigned long long key = field[(size_t)y * cam.w + x];
-            bool hit = false;
-            if (key != ~0ull) {
-                const int ikl = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
-                const float4 a = fpack[2 * ikl], b = fpack[2 * ikl + 1];
-                const double p_n2 = (double)(o.n_m * o.n_m);                   // Test_f_k (global_tracker.h:89-104)
-                const double p_esc = (double)(mrx * a.x + mry * a.y);
-                if (!(fabs(p_esc - p_n2) > tc.match_thresh * p_n2)) {
-                    const double dx = pix - (double)a.z, dy = piy - (double)a.w;   // Calc_f_J2 :254-262
-                    const double fi = dx * (double)b.x + dy * (double)b.y;
-                    dfx = (double)b.x;
-                    dfy = (double)b.y;
-                    f = fi;
-                    matched = true;
-                    fi_own = fi;
-                    mid_f = ikl;
-                    hit = true;
-                }
-            }
-            if (!hit) {
-                f = max_r;
-                need = true;
-            }
-            if (RW) {
-                f *= weight;
-                dfx *= weight;
-                dfy *= weight;
-            }
-        }
+        off[u] = x < 1 || y < 1 || x >= cam.w - 1 || y >= cam.h - 1;   // :376
+        inb[u] = !skip[u] && !off[u];
+        pixel[u] = inb[u] ? y * cam.w + x : 0;
     }
-    if (m_id_f) m_id_f[i] = mid_f;   // only the last evaluation of a minimisation is visible afterwards
-    // Jacobians (:419-449) and the 1/q_rho scaling (:452-463)
-    const double qvel = (cam.zfm * dfx * sV[0] + cam.zfm * dfy * sV[1]) + (qx * dfx + qy * dfy) * sV[2];
-    double q_rho = sqrt(o.s_rho * qvel * o.s_rho * qvel + 1);
-    if (!RW) q_rho = o.s_rho;
+    MC_BSTAMP(3);
+    // field lookup, then the matched keyline's gather record
+    unsigned long long key[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) key[u] = inb[u] ? field[pixel[u]] : ~0ull;
+    float4 ga[U], gb[U];
+    int ikl[U];
+    bool cand[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        cand[u] = key[u] != ~0ull;
+        MC_BSTAMP(4);
+        ikl[u] = cand[u] ? (int)(0xFFFFFFFFu - (unsigned int)(key[u] & 0xFFFFFFFFull)) : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        ga[u] = cand[u] ? fpack[2 * ikl[u]] : make_float4(0.f, 0.f, 0.f, 0.f);
+        gb[u] = cand[u] ? fpack[2 * ikl[u] + 1] : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    double f[U], dfx[U], dfy[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        if (ga[u].x != 12345.f) MC_BSTAMP(5);
+        const float mrx = (float)(sRM[0] * (double)m[u].x + sRM[1] * (double)m[u].y);   // :386-388
+        const float mry = (float)(sRM[2] * (double)m[u].x + sRM[3] * (double)m[u].y);
+        const double p_n2 = (double)(n_m[u] * n_m[u]);                                   // Test_f_k (global_tracker.h:89-104)
+        const double p_esc = (double)(mrx * ga[u].x + mry * ga[u].y);
+        const bool hit = cand[u] && !(fabs(p_esc - p_n2) > tc.match_thresh * p_n2);
+        const double dx = pix[u] - (double)ga[u].z, dy = piy[u] - (double)ga[u].w;      // Calc_f_J2 :254-262
+        const double fi = dx * (double)gb[u].x + dy * (double)gb[u].y;
+        matched[u] = hit;
+        need[u] = inb[u] && !hit;
+        outside[u] = !skip[u] && off[u];
+        fi_own[u] = hit ? fi : 0.0;
+        double fv = hit ? fi : max_r;
+        double gx = hit ? (double)gb[u].x : 0.0, gy = hit ? (double)gb[u].y : 0.0;
+        if (RW) {   // fm*=weigth; df_dPi*=weigth (:380,399-403); the weight of a skipped keyline is 1
+            fv = fv * weight[u];
+            gx = gx * weight[u];
+            gy = gy * weight[u];
+        }
+        f[u] = skip[u] ? 0.0 : fv;
+        dfx[u] = gx;
+        dfy[u] = gy;
+        if (m_id_f && act[u]) m_id_f[gi[u]] = hit ? ikl[u] : -1;
+    }
+    if (f[0] != 1e300) MC_BSTAMP(6);
+    // Jacobians (:419-449), the 1/q_rho scaling (:452-463), products
+    double q_rho[U], iq[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        const double qvel = (cam.zfm * dfx[u] * sV[0] + cam.zfm * dfy[u] * sV[1]) + (qx[u] * dfx[u] + qy[u] * dfy[u]) * sV[2];
+        q_rho[u] = RW ? sqrt(s_rho[u] * qvel * s_rho[u] * qvel + 1) : s_rho[u];
+    }
+    if (q_rho[0] != 1e300) MC_BSTAMP(7);
     if (PJ) {
-        double t0 = cam.zfm * rho_p;
-        double J0 = t0 * dfx, J1 = t0 * dfy;
-        t0 = rho_p * qx;
-        double J2 = t0 * dfx;
-        t0 = rho_p * qy;
-        J2 = J2 + t0 * dfy;
-        double J3 = J1 * pz;
-        J3 = J3 + J2 * py;
-        double J4 = J0 * pz;
-        J4 = J4 + J2 * px;
-        t0 = J0 * py;
-        double J5 = -1.0 * t0;
-        J5 = J5 + J1 * px;
-        const double iq = 1 / q_rho;
-        double J[6] = {div_with_rcp(J0, q_rho, iq), div_with_rcp(J1, q_rho, iq), div_with_rcp(J2, q_rho, iq),
-                       div_with_rcp(J3, q_rho, iq), div_with_rcp(J4, q_rho, iq), div_with_rcp(J5, q_rho, iq)};
-        f = div_with_rcp(f, q_rho, iq);
-        int k = 0;
 #pragma unroll
-        for (int a = 0; a < 6; a++)
+        for (int u = 0; u < U; u++) iq[u] = 1 / q_rho[u];
+        if (iq[0] != 1e300) MC_BSTAMP(8);
 #pragma unroll
-            for (int b = a; b < 6; b++) acc[k++] = J[a] * J[b];
+        for (int u = 0; u < U; u++) {
+            double t0 = cam.zfm * rho_p[u];
+            const double J0 = t0 * dfx[u], J1 = t0 * dfy[u];
+            t0 = rho_p[u] * qx[u];
+            double J2 = t0 * dfx[u];
+            t0 = rho_p[u] * qy[u];
+            J2 = J2 + t0 * dfy[u];
+            double J3 = J1 * pz[u];
+            J3 = J3 + J2 * py[u];
+            double J4 = J0 * pz[u];
+            J4 = J4 + J2 * px[u];
+            t0 = J0 * py[u];
+            double J5 = -1.0 * t0;
+            J5 = J5 + J1 * px[u];
+            const double J[6] = {div_with_rcp(J0, q_rho[u], iq[u]), div_with_rcp(J1, q_rho[u], iq[u]),
+                                 div_with_rcp(J2, q_rho[u], iq[u]), div_with_rcp(J3, q_rho[u], iq[u]),
+                                 div_with_rcp(J4, q_rho[u], iq[u]), div_with_rcp(J5, q_rho[u], iq[u])};
+            const double fs = div_with_rcp(f[u], q_rho[u], iq[u]);
+            int k = 0;
 #pragma unroll
-        for (int a = 0; a < 6; a++) acc[21 + a] = J[a] * f;
+            for (int a = 0; a < 6; a++)
+#pragma unroll
+                for (int b = a; b < 6; b++, k++) acc[k] = fma(J[a], J[b], acc[k]);   // (sums are order-toleranced anyway)
+#pragma unroll
+            for (int a = 0; a < 6; a++) acc[21 + a] = fma(J[a], fs, acc[21 + a]);
+            acc[27] = fma(fs, fs, acc[27]);
+        }
+        if (acc[27] != 1e300) MC_BSTAMP(9);
     } else {
-        f = f / q_rho;
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const double fs = f[u] / q_rho[u];
+            acc[27] = fma(fs, fs, acc[27]);
+        }
     }
-    acc[27] = f * f;
 }
 
 // "DResidualNew[ikl]=fi" keeps the fi of the last matched keyline before ikl (fi is a function-level variable,
 // :341,399-408): in-block scan here; misses that precede the block's first match get RES_SENTINEL and are resolved
 // lazily by whoever reads the buffer, from the per-(buffer, block) carry table.  Then the block's 28 sums go to
 // partials[k][vb] in a fixed order, and its "has a match / last matched fi" summary to blk_has / blk_last_fi.
+// matched / need / outside / fi_own: tvr_keyline's outputs for keyline i.
 template <bool PJ>
-__device__ __forceinline__ void tvr_block_tail(bool active, bool matched, bool need, double fi_own,
+__device__ __forceinline__ void tvr_block_tail(bool matched, bool need, bool outside, double fi_own, double max_r,
                                                double *__restrict__ rout, int i, const double (&acc)[28],
                                                TvrSmem &sm, double *dst, int dst_stride, int *has_out,
-                                               double *last_out, int tid, int lane, int wid, bool &wrote,
-                                               double &r_w) {
+                                               double *last_out, int tid, int lane, int wid) {
     const unsigned int bal = __ballot_sync(0xffffffffu, matched);
     const unsigned int lower = bal & ((1u << lane) - 1u);
     const int src = lower ? 31 - __clz(lower) : 0;
@@ -781,27 +832,23 @@ __device__ __forceinline__ void tvr_block_tail(bool active, bool matched, bool n
         sm.wlast[wid] = wl;
     }
     __syncthreads();
-    if (active) {
-        if (matched) {
-            rout[i] = fi_own;
-            wrote = true;
-            r_w = fi_own;
-        } else if (need) {
-            double v = prev_fi;
-            bool found = lower != 0;
-            if (!found) {
-                for (int ww = wid - 1; ww >= 0; ww--)
-                    if (sm.whas[ww]) {
-                        v = sm.wlast[ww];
-                        found = true;
-                        break;
-                    }
-            }
-            if (!found) v = __longlong_as_double((long long)RES_SENTINEL);
-            reinterpret_cast<unsigned long long *>(rout)[i] = (unsigned long long)__double_as_longlong(v);
-            wrote = true;
-            r_w = v;
+    if (matched) {
+        rout[i] = fi_own;
+    } else if (need) {
+        double v = prev_fi;
+        bool found = lower != 0;
+        if (!found) {
+            for (int ww = wid - 1; ww >= 0; ww--)
+                if (sm.whas[ww]) {
+                    v = sm.wlast[ww];
+                    found = true;
+                    break;
+                }
         }
+        if (!found) v = __longlong_as_double((long long)RES_SENTINEL);
+        reinterpret_cast<unsigned long long *>(rout)[i] = (unsigned long long)__double_as_longlong(v);
+    } else if (outside) {
+        rout[i] = max_r;
     }
     if (tid == 0) {
         int has = 0;
@@ -910,7 +957,8 @@ __device__ __forceinline__ void lm_ingest(LMState &L, const double *s_tot) {
 }
 
 // One TryVelRot evaluation + the LM step that follows it, one launch per evaluation (stage-level API rb_try_vel_rot,
-// and minimisations whose keyline capacity exceeds what the persistent kernel below can keep co-resident).
+// every minimisation under REBVO_B200_MIN_PERSIST=0, and those whose keyline capacity exceeds what the cluster kernel
+// below can keep co-resident).
 template <bool RW, bool PJ>
 __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *__restrict__ old_st,
                                                     const unsigned long long *__restrict__ field,
@@ -948,22 +996,28 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
 
     const int K0 = old_st->kn;
     const int i = blockIdx.x * TVR_T + tid;
-    const bool active = i < K0;
+    const bool act = i < K0;
+    // a thread without a keyline runs on harmless operands and contributes zeros
+    KlOp o = {make_float2(0.f, 0.f), 0.0, 0.0, 1.0, 1.0, 0, 0.f};
+    double r_prev = 0.0;
+    if (act) {
+        o = load_klop(old, i, cam);
+        if (RW && rin) {
+            r_prev = rin[i];
+            if ((unsigned long long)__double_as_longlong(r_prev) == RES_SENTINEL)
+                r_prev = tp.carry[res_in * TVR_T + blockIdx.x];   // stale-fi carry of the evaluation that wrote rin
+        }
+    }
+    const bool skip = !act || o.s_rho > tc.s_rho_min || (unsigned int)o.m_num < tc.mnt;   // :356
     double acc[28];
 #pragma unroll
     for (int k = 0; k < 28; k++) acc[k] = 0;
-    bool matched = false, need = false, wrote = false;
-    double fi_own = 0, r_w = 0;
-    if (active) {
-        const KlOp o = load_klop(old, i, cam);
-        double r_prev = (RW && rin) ? rin[i] : 0.0;
-        if (RW && rin && (unsigned long long)__double_as_longlong(r_prev) == RES_SENTINEL)
-            r_prev = tp.carry[res_in * TVR_T + blockIdx.x];   // stale-fi carry of the evaluation that wrote rin
-        tvr_body<RW, PJ>(o, rin != nullptr, r_prev, sR, sV, sRM, tc, cam, field, fpack, rout, old.m_id_f, i, acc,
-                         matched, need, fi_own, wrote, r_w);
-    }
-    tvr_block_tail<PJ>(active, matched, need, fi_own, rout, i, acc, sm, tp.partials + blockIdx.x, TVR_T,
-                       tp.blk_has + blockIdx.x, tp.blk_last_fi + blockIdx.x, tid, lane, wid, wrote, r_w);
+    bool matched[1], need[1], outside[1];
+    double fi_own[1];
+    tvr_keyline<RW, PJ, 1>({o.x0}, {o.y0}, {o.z0}, {o.s_rho}, {o.m}, {o.n_m}, {skip}, {act}, rin != nullptr, {r_prev}, sR, sV,
+                           sRM, tc, cam, field, fpack, old.m_id_f, {i}, acc, matched, need, fi_own, outside);
+    tvr_block_tail<PJ>(matched[0], need[0], outside[0], fi_own[0], tc.max_r, rout, i, acc, sm, tp.partials + blockIdx.x, TVR_T,
+                       tp.blk_has + blockIdx.x, tp.blk_last_fi + blockIdx.x, tid, lane, wid);
     __threadfence();
     __syncthreads();
     if (tid == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
@@ -1012,7 +1066,7 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
 // =====================================================================================================
 // Whole Minimizer_RV in ONE launch (min_cluster.cuh).  The ~12 evaluations of a frame are strictly dependent (each pose
 // comes out of the LM step on the previous sums), so with one launch per evaluation a frame pays 12x (launch + operand
-// re-load + last-block hand-over through L2).  Shared declarations of the persistent forms:
+// re-load + last-block hand-over through L2).  Declarations of the cluster kernel k_minimizer_cluster<T>:
 // =====================================================================================================
 #define MIN_MAX_EVALS 32
 struct MinSetup {
@@ -1097,17 +1151,7 @@ __device__ __forceinline__ void d_fm_argmax_two(const KLSoA &old, int i0, int i1
     }
 }
 
-// one-cluster form (16 CTAs x 512 threads: co-residency guaranteed, 16 SMs) and multi-cluster form (G x 16 CTAs x 256 threads)
-#define MC_T 512
-#define MC_NS mc_one
 #include "min_cluster.cuh"
-#undef MC_T
-#undef MC_NS
-#define MC_T 256
-#define MC_NS mc_multi
-#include "min_cluster.cuh"
-#undef MC_T
-#undef MC_NS
 
 static TrackPtrs track_ptrs(const rb_map *fmap) {
     TrackPtrs tp;
@@ -1165,23 +1209,24 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
     int kfast = MC_KPC_FAST;                   // keylines per cluster rank kept in shared memory (the rest works from global memory)
     const char *kf = getenv("REBVO_B200_MIN_KPC");
     if (kf && atoi(kf) >= 32) kfast = atoi(kf) & ~31;
-    // one cluster: always possible when the capacity fits its virtual-warp tables
+    // one cluster of 512-thread CTAs: always possible when the capacity fits its virtual-warp tables
     {
         int kpc = (c->kcap + MC_C - 1) / MC_C;
         kpc = (kpc + 31) & ~31;
-        if (kpc <= 512 * (3584 / 512)) {
+        if (kpc <= MC_KPC_MAX) {
             if (kpc > kfast) kpc = kfast;
             const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
-            if (mc_prepare(mc_one::k_minimizer_cluster, 512, 1, dyn, dev_max)) {
+            if (mc_prepare(k_minimizer_cluster<512>, 512, 1, dyn, dev_max)) {
                 c->min_cluster_kpc = kpc;
                 c->min_cluster_dyn = dyn;
             }
         }
     }
     cudaGetLastError();
-    // several clusters (default 4 = 64 SMs): the per-evaluation keyline pass is the longest part of a round and scales with
-    // the SMs; the clusters exchange their sums through L2.  Needs all clusters co-resident: checked here for an idle
-    // device (spins are bounded and abort otherwise), so contexts that share a GPU should ask for REBVO_B200_MIN_G=1.
+    // several clusters of 256-thread CTAs (default 4 = 64 SMs): the per-evaluation keyline pass is the longest part of a
+    // round and scales with the SMs; the clusters exchange their sums through L2.  Needs all clusters co-resident: checked
+    // here for an idle device (spins are bounded and abort otherwise), so contexts that share a GPU should ask for
+    // REBVO_B200_MIN_G=1.
     int G = 4;
     const char *ge = getenv("REBVO_B200_MIN_G");
     if (ge) G = atoi(ge);
@@ -1189,11 +1234,11 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
     if (c->min_cluster_kpc > 0 && G > 1) {
         int kpc = (c->kcap + MC_C * G - 1) / (MC_C * G);
         kpc = (kpc + 31) & ~31;
-        if (kpc <= 256 * (3584 / 256)) {
+        if (kpc <= MC_KPC_MAX) {
             int kf2 = (kfast / G + 31) & ~31;
             if (kpc > kf2) kpc = kf2;
             const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
-            if (mc_prepare(mc_multi::k_minimizer_cluster, 256, G, dyn, dev_max)) {
+            if (mc_prepare(k_minimizer_cluster<256>, 256, G, dyn, dev_max)) {
                 c->min_cluster_g = G;
                 c->min_cluster_kpc_multi = kpc;
                 c->min_cluster_dyn_multi = dyn;
@@ -1220,7 +1265,7 @@ static int launch_minimizer_cluster(rb_ctx *c, rb_map *fmap, rb_map *old, const 
     c->launches++;
     ResPtrs rp;
     for (int i = 0; i < 3; i++) rp.r[i] = fmap->res[i];
-    auto kern = G > 1 ? mc_multi::k_minimizer_cluster : mc_one::k_minimizer_cluster;
+    auto kern = G > 1 ? k_minimizer_cluster<256> : k_minimizer_cluster<512>;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, old->kl, (const MapState *)old->st,
                                              (const unsigned long long *)fmap->field, (const float4 *)fmap->kl.pack,
                                              fmap->st, &fmap->ts->lm, &fmap->ts_host.ctl->abort, make_cam(c), plan, su,

@@ -84,7 +84,60 @@ def _run_stage_parity(cfg):
     _, rt = refs[1].reestimate(cfg["track_points"], 100)
     gm[1].reestimate(cfg["track_points"], 100)
 
-    # ---------------- tracker: old = frame 0 with seeded depth, new = frame 1 -----------------------------
+    m_r = _tracker_parity(rep, cfg, refs, gm, rt)
+    old_r, new_r, old_g, new_g = refs[0], refs[1], gm[0], gm[1]
+    # FordwardMatch
+    old_r.forward_match(new_r)
+    old_g.forward_match(new_g)
+    fm_fields = ["rho", "s_rho", "m_num", "m_id", "p_m_0"]
+    compare_keylines(rep, "FordwardMatch new", new_r.keylines(), new_g.keylines(), fm_fields)
+    mk = new_r.keylines()["m_id"] >= 0
+    rep.exact("FordwardMatch m_m0 (matched)", new_r.keylines()["m_m0"][mk], new_g.keylines()["m_m0"][mk])
+    rep.exact("FordwardMatch n_m0 (matched)", new_r.keylines()["n_m0"][mk], new_g.keylines()["n_m0"][mk])
+    # rotate_keylines with the reference's rotation
+    R0 = refapi.so3_exp(m_r["W"])
+    old_r.rotate(R0)
+    old_g.rotate(R0)
+    compare_keylines(rep, "rotate_keylines old", old_r.keylines(), old_g.keylines(), ["p_m", "m_m", "rho", "s_rho"])
+    # directed_matching from identical state
+    old_g.load_keylines(old_r.keylines(), old_r.mask())
+    new_g.load_keylines(new_r.keylines(), new_r.mask())
+    R = R0.T.copy()
+    n_r = new_r.directed_matching(old_r, m_r["V"], m_r["RVel"], R, cfg["thr_mod"], cfg["thr_ang"], cfg["radius"],
+                                  cfg["loc_unc_match"])
+    n_g = new_g.directed_matching(old_g, m_r["V"], m_r["RVel"], R, cfg["thr_mod"], cfg["thr_ang"], cfg["radius"],
+                                  cfg["loc_unc_match"])
+    rep.add("directed_matching count", n_r == n_g, "ref %d gpu %d" % (n_r, n_g))
+    compare_keylines(rep, "directed_matching new", new_r.keylines(), new_g.keylines(),
+                     ["rho", "s_rho", "m_num", "m_id", "p_m_0"])
+    mk = new_r.keylines()["m_id"] >= 0
+    rep.exact("directed_matching m_m0 (matched)", new_r.keylines()["m_m0"][mk], new_g.keylines()["m_m0"][mk])
+    # Regularize_1_iter
+    new_g.load_keylines(new_r.keylines(), new_r.mask())
+    r_r = new_r.regularize(cfg["reg_thresh"])
+    r_g = new_g.regularize(cfg["reg_thresh"])
+    rep.add("Regularize_1_iter count", r_r == r_g, "ref %d gpu %d" % (r_r, r_g))
+    compare_keylines(rep, "Regularize_1_iter", new_r.keylines(), new_g.keylines(), ["rho", "s_rho"])
+    # EKF
+    new_r.ekf(m_r["V"], m_r["RVel"], m_r["RW0"], cfg["q_abs"], 1.6968e-4, cfg["loc_unc"])
+    new_g.ekf(m_r["V"], cfg["q_abs"], cfg["loc_unc"])
+    compare_keylines(rep, "EKF", new_r.keylines(), new_g.keylines(), [], ["rho", "s_rho", "rho0", "s_rho0"], rtol=1e-13)
+    compare_keylines(rep, "EKF (bitwise)", new_r.keylines(), new_g.keylines(), ["rho", "s_rho", "rho0", "s_rho0"])
+    # EstimateReScalingOpt
+    kp_r, rkp_r = new_r.rescale(20.0, 1, False)
+    kp_g, rkp_g = new_g.rescale(20.0, 1, False)
+    rep.close("EstimateReScalingOpt Kp", kp_r, kp_g, 1e-12)
+    rep.close("EstimateReScalingOpt RKp", rkp_r, rkp_g, 1e-11)
+    rep.dump()
+    for g in gm:
+        g.close()
+    ctx.close()
+    return rep
+
+
+def _tracker_parity(rep, cfg, refs, gm, rt):
+    """TryVelRot at three poses x three (reweight, procjf) pairs, then Minimizer_RV; returns the reference's result."""
+    # old = frame 0 with seeded depth, new = frame 1
     old_r, new_r, old_g, new_g = refs[0], refs[1], gm[0], gm[1]
     old_r.set_keylines(_seed_depth(old_r.keylines()))
     old_g.load_keylines(old_r.keylines(), old_r.mask())
@@ -142,53 +195,7 @@ def _run_stage_parity(cfg):
     rep.close("Minimizer_RV W_X", m_r["W_X"], m_g["W_X"], 1e-8, atol=1e-9 * np.abs(m_r["W_X"]).max())
     rep.close("Minimizer_RV rel_err_score", m_r["rel_err_score"], m_g["rel_err_score"], 1e-8)
     rep.exact("Minimizer_RV m_id_f", old_r.keylines()["m_id_f"], old_g.keylines()["m_id_f"])
-    # FordwardMatch
-    old_r.forward_match(new_r)
-    old_g.forward_match(new_g)
-    fm_fields = ["rho", "s_rho", "m_num", "m_id", "p_m_0"]
-    compare_keylines(rep, "FordwardMatch new", new_r.keylines(), new_g.keylines(), fm_fields)
-    mk = new_r.keylines()["m_id"] >= 0
-    rep.exact("FordwardMatch m_m0 (matched)", new_r.keylines()["m_m0"][mk], new_g.keylines()["m_m0"][mk])
-    rep.exact("FordwardMatch n_m0 (matched)", new_r.keylines()["n_m0"][mk], new_g.keylines()["n_m0"][mk])
-    # rotate_keylines with the reference's rotation
-    R0 = refapi.so3_exp(m_r["W"])
-    old_r.rotate(R0)
-    old_g.rotate(R0)
-    compare_keylines(rep, "rotate_keylines old", old_r.keylines(), old_g.keylines(), ["p_m", "m_m", "rho", "s_rho"])
-    # directed_matching from identical state
-    old_g.load_keylines(old_r.keylines(), old_r.mask())
-    new_g.load_keylines(new_r.keylines(), new_r.mask())
-    R = R0.T.copy()
-    n_r = new_r.directed_matching(old_r, m_r["V"], m_r["RVel"], R, cfg["thr_mod"], cfg["thr_ang"], cfg["radius"],
-                                  cfg["loc_unc_match"])
-    n_g = new_g.directed_matching(old_g, m_r["V"], m_r["RVel"], R, cfg["thr_mod"], cfg["thr_ang"], cfg["radius"],
-                                  cfg["loc_unc_match"])
-    rep.add("directed_matching count", n_r == n_g, "ref %d gpu %d" % (n_r, n_g))
-    compare_keylines(rep, "directed_matching new", new_r.keylines(), new_g.keylines(),
-                     ["rho", "s_rho", "m_num", "m_id", "p_m_0"])
-    mk = new_r.keylines()["m_id"] >= 0
-    rep.exact("directed_matching m_m0 (matched)", new_r.keylines()["m_m0"][mk], new_g.keylines()["m_m0"][mk])
-    # Regularize_1_iter
-    new_g.load_keylines(new_r.keylines(), new_r.mask())
-    r_r = new_r.regularize(cfg["reg_thresh"])
-    r_g = new_g.regularize(cfg["reg_thresh"])
-    rep.add("Regularize_1_iter count", r_r == r_g, "ref %d gpu %d" % (r_r, r_g))
-    compare_keylines(rep, "Regularize_1_iter", new_r.keylines(), new_g.keylines(), ["rho", "s_rho"])
-    # EKF
-    new_r.ekf(m_r["V"], m_r["RVel"], m_r["RW0"], cfg["q_abs"], 1.6968e-4, cfg["loc_unc"])
-    new_g.ekf(m_r["V"], cfg["q_abs"], cfg["loc_unc"])
-    compare_keylines(rep, "EKF", new_r.keylines(), new_g.keylines(), [], ["rho", "s_rho", "rho0", "s_rho0"], rtol=1e-13)
-    compare_keylines(rep, "EKF (bitwise)", new_r.keylines(), new_g.keylines(), ["rho", "s_rho", "rho0", "s_rho0"])
-    # EstimateReScalingOpt
-    kp_r, rkp_r = new_r.rescale(20.0, 1, False)
-    kp_g, rkp_g = new_g.rescale(20.0, 1, False)
-    rep.close("EstimateReScalingOpt Kp", kp_r, kp_g, 1e-12)
-    rep.close("EstimateReScalingOpt RKp", rkp_r, rkp_g, 1e-11)
-    rep.dump()
-    for g in gm:
-        g.close()
-    ctx.close()
-    return rep
+    return m_r
 
 
 @pytest.mark.parametrize("cfg", [TUM_CFG, EUROC_CFG, BIG_CFG], ids=["tum640", "euroc752", "synthetic1280x960"])
