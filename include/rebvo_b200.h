@@ -117,6 +117,33 @@ int rb_nav_format_trajectory(const rb_nav *nav, int n, double time_scale, char *
 int rb_nav_format_log(const rb_nav *nav, int n, long long first_index, long long frame_id0, char *buf, size_t cap,
                       size_t *written);
 
+/* struct OdometryMeas (include/mtracklib/pose_graph.h:31-52): the relative motion of one tracked frame with its information
+ * matrix, as SecondThread appends it to REBVO::poses (rebvo_second_t.cpp:323-334 in IMU mode, :371-382 otherwise).  Fields in
+ * the order OdometryMeas::dumpToFile writes them.
+ *   relPosPose   [0:3] -R*V (translation), [3:6] SO3(R).ln(), with R the backward rotation and V the minimiser's
+ *                translation before the NaN guard (IMU mode: Rgva, Vgva)
+ *   WrelPosPose  J^T * W_X * J (row-major), J the inverse of J_rp_x = [[-R, [relPosPose[0:3]]x], [0, -I]] (the reference
+ *                takes TooN's SVD pseudo-inverse; the closed-form inverse used here agrees to rounding).  W_X: the minimiser's
+ *                JtJ (IMU mode: W_Xgv after BiasCorrect).  Deviation: after an empty old map the reference's W_X is an
+ *                uninitialised matrix (rebvo_second_t.cpp:345, Minimizer_RV returns at once); the pipeline writes zeros.
+ *   AcelMeas     the frame's mean accelerometer reading (zero without an IMU); IMU mode: As
+ *   VisualMeas, GMeas, Rs, Rv, Rg   zero without an IMU; IMU mode: Av, g_est, Rs, P_V / dt^4, P[1:4, 1:4]
+ *   K, WK, QK    1, 0 and P_Kp as the frame found it (the previous frame's RKp); IMU mode: K, 1 / P(0, 0), P_Kp
+ *   KF_ID        -1 (TrackKeyFrames is not supported) */
+typedef struct rb_odometry {
+    double relPosPose[6];
+    double WrelPosPose[36];
+    double AcelMeas[3], VisualMeas[3], GMeas[3];
+    double Rs[9], Rv[9], Rg[9];
+    double K, WK, QK;
+    int32_t KF_ID;   /* kf_list.size()-1 (rebvo_second_t.cpp:598): -1, keyframes are not tracked */
+    int32_t tracked; /* 0 for a frame SecondThread never tracked (the first frame of a sequence): not part of the pose graph */
+} rb_odometry;
+/* pose_graph::saveToFile (pose_graph.cpp:32-40, util::dumpElement / dumpVector / dumpMatrix of toon_util.h): a uint32 record
+ * count, then per record 6 + 36 + 3 * 3 + 3 * 9 + 3 raw doubles and one int32 (652 bytes); records with tracked == 0 are
+ * skipped.  Writes at most cap bytes and reports the size needed in *written; RB_ERR_ARG if it did not fit. */
+int rb_odometry_format_pose_graph(const rb_odometry *r, int n, void *buf, size_t cap, size_t *written);
+
 /* ---- context ---------------------------------------------------------------------------------- */
 /* RB_ERR_ARG for cam->w < 32, cam->h < 32 or kl_capacity < 1; every other frame size is accepted */
 int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, double sigma0, double ksigma,
@@ -276,6 +303,14 @@ int rb_pipeline_set_mirror(rb_pipeline *pl, int mode);
  * fixed-point bilinear map, fused into the RGB -> BW pass.  kc == NULL or all zero: off. */
 int rb_pipeline_set_undistort(rb_pipeline *pl, const double kc[5]);
 int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, int *n);
+/* Per-frame odometry measurements (rb_odometry, the reference's pose graph REBVO::poses).  on = 1: every push also produces one
+ * record per frame; the products run in a spare thread of a kernel that already follows the match-count gate (k_reg_ekf, or the
+ * gate kernel of the reference schedule) and the records reach the host with the nav records, so a push launches no more
+ * kernels than without them (the constant is 0).  In IMU mode the records are built by the host flow.  May be called between
+ * pushes; on = 0 restores the batches of a pipeline that never had it.  rb_pipeline_odometry: the n records of the last push,
+ * record i for frame i (like nav_out[i]), valid until the next push; RB_ERR_STATE when the last push ran without them. */
+int rb_pipeline_set_odometry(rb_pipeline *pl, int on);
+int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, int *n);
 int64_t rb_pipeline_launch_count(const rb_pipeline *pl);
 /* CUDA-event time (ms) of the last push split by stage: [0] h2d+gray, [1] DoG, [2] detect,
  * [3] tracker (field + minimiser), [4] mapper, [5] total */

@@ -62,6 +62,13 @@ NAV = np.dtype([("t", "f8"), ("dt", "f8"), ("Rot", "f8", 9), ("RotLie", "f8", 3)
                 ("matches", "i4"), ("fwd_matches", "i4"), ("estimation_ok", "i4"), ("thresh", "f4"),
                 ("retuned_thresh", "f4")])
 
+# rb_odometry: the reference's OdometryMeas (pose graph record) + whether the frame was tracked
+ODOM = np.dtype([("relPosPose", "f8", 6), ("WrelPosPose", "f8", (6, 6)), ("AcelMeas", "f8", 3), ("VisualMeas", "f8", 3),
+                 ("GMeas", "f8", 3), ("Rs", "f8", (3, 3)), ("Rv", "f8", (3, 3)), ("Rg", "f8", (3, 3)), ("K", "f8"),
+                 ("WK", "f8"), ("QK", "f8"), ("KF_ID", "i4"), ("tracked", "i4")])
+# one record of the pose graph file (pose_graph::saveToFile): ODOM without `tracked`, unpadded
+PS_REC = np.dtype([(n, ODOM.fields[n][0]) for n in ODOM.names if n != "tracked"])
+
 # struct KeyLine of the reference (168 bytes) == rb_keyline
 KEYLINE = np.dtype({
     "names": ["p_inx", "m_m", "u_m", "n_m", "score", "c_p", "rho", "s_rho", "rho_nr", "s_rho_nr",
@@ -92,7 +99,8 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_stage_profile",
            "rb_undistort_create", "rb_undistort_destroy", "rb_undistort_rgb", "rb_undistort_rgb_dev",
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
-           "rb_nav_format_trajectory", "rb_nav_format_log"]
+           "rb_nav_format_trajectory", "rb_nav_format_log", "rb_odometry_format_pose_graph", "rb_pipeline_set_odometry",
+           "rb_pipeline_odometry"]
 
 _lib = None
 
@@ -116,6 +124,34 @@ def format_trajectory(nav, time_scale=1.0):
 def format_log(nav, first_index=1, frame_id0=0):
     """Pose / map records of the reference's m-file log (LogFile, rebvo_third_t.cpp:265-281) for these NAV records."""
     return _format_nav("rb_nav_format_log", nav, C.c_longlong(first_index), C.c_longlong(frame_id0))
+
+
+def format_pose_graph(recs):
+    """Bytes of the reference's pose graph file (poses_list.ps, pose_graph::saveToFile) for these ODOM records; records with
+    tracked == 0 are left out."""
+    recs = np.ascontiguousarray(recs, ODOM)
+    need = C.c_size_t(0)
+    lib().rb_odometry_format_pose_graph(_p(recs), len(recs), None, C.c_size_t(0), C.byref(need))
+    buf = C.create_string_buffer(max(need.value, 1))
+    r = lib().rb_odometry_format_pose_graph(_p(recs), len(recs), buf, C.c_size_t(need.value), C.byref(need))
+    if r:
+        raise RbError("rb_odometry_format_pose_graph failed (%d)" % r)
+    return buf.raw[:need.value]
+
+
+def read_pose_graph(path):
+    """The records of a pose graph file (pose_graph::loadFromFile) as ODOM records with tracked = 1."""
+    with open(path, "rb") as f:
+        data = f.read()
+    n = int(np.frombuffer(data, np.uint32, count=1)[0])
+    if len(data) != 4 + n * PS_REC.itemsize:
+        raise ValueError("%s: %d bytes, not a pose graph of %d records" % (path, len(data), n))
+    ps = np.frombuffer(data, PS_REC, count=n, offset=4)
+    out = np.zeros(n, ODOM)
+    for k in PS_REC.names:
+        out[k] = ps[k]
+    out["tracked"] = 1
+    return out
 
 
 def lib():
@@ -544,6 +580,17 @@ class Pipeline:
         records, 2 = its 15-byte net_keyline wire records, 0 = off."""
         self.check(self.L.rb_pipeline_set_mirror(self.h_, int(mode)))
         self._mirror_mode = int(mode)
+
+    def set_odometry(self, on=True):
+        """Per-frame odometry records (the reference's pose graph measurements) with every push: on / off between pushes."""
+        self.check(self.L.rb_pipeline_set_odometry(self.h_, int(bool(on))))
+
+    def odometry(self):
+        """ODOM[n]: record i for frame i of the last push (a copy)."""
+        p, n = C.c_void_p(0), C.c_int(0)
+        self.check(self.L.rb_pipeline_odometry(self.h_, C.byref(p), C.byref(n)))
+        buf = (C.c_char * (n.value * ODOM.itemsize)).from_address(p.value)
+        return np.frombuffer(buf, dtype=ODOM, count=n.value).copy()
 
     def mirror(self, i):
         """View (no copy) of the records of frame `i` of the last push: KEYLINE[n] (mode 1) or uint8[n, 15] (mode 2); valid until

@@ -103,6 +103,20 @@ __device__ __forceinline__ void d_frame_post_min(FrameState *fs, const LMState &
     d_frame_post_min_cov(fs, lm);
 }
 
+// OdometryMeas of the vision-only branch (:371-382) from the values before the NaN guard: R (nothing writes fs->R after
+// d_frame_post_min_pose) and V as the minimiser returned it, which after an empty old map is the prior VW.  W_X of an empty
+// old map is not defined (the reference passes an uninitialised matrix): zeros.  QK, the P_Kp the frame found, is the previous
+// frame's nav RKp, which the host fills in (with DoReScaling=0 FrameState::P_Kp is not that value, see d_frame_finish).
+__device__ __forceinline__ void d_frame_odometry(const FrameState *fs, const LMState &lm, rb_odometry *out) {
+    double *d = reinterpret_cast<double *>(out);
+    for (int i = 0; i < (int)(sizeof(rb_odometry) / sizeof(double)); i++) d[i] = 0;
+    odom_rel_pose(fs->R, lm.no_keylines ? fs->VW : lm.Vel, fs->R, lm.no_keylines ? nullptr : lm.W_X, out->relPosPose,
+                  out->WrelPosPose);
+    out->K = 1;
+    out->KF_ID = -1;   // cf->kf_list.size()-1 without keyframes (:598)
+    out->tracked = 1;
+}
+
 // after directed_matching (:410-423)
 __device__ __forceinline__ void d_frame_post_match(FrameState *fs, const MapState *nst, int match_threshold) {
     if (!fs->do_match) {

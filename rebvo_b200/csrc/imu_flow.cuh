@@ -75,9 +75,10 @@ static void imu_flow_reset(ImuFlow &f) {
     if (!f.samples.empty()) f.buf.init(f.samples.data(), (int)f.samples.size(), p.use_se3 ? p.Rc2i : nullptr, p.use_se3 ? p.Tc2i : nullptr);
 }
 
-// one tracked frame: new = maps[fr % 3] (detected), old = maps[(fr-1) % 3]; returns the nav record
+// one tracked frame: new = maps[fr % 3] (detected), old = maps[(fr-1) % 3]; returns the nav record and, with odom, the
+// odometry record
 static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old, double t, double dt_frame,
-                           const rbimu::ImuIntegral &imu, rb_nav *nav) {
+                           const rbimu::ImuIntegral &imu, rb_nav *nav, rb_odometry *odom) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     const rb_imu_params &ip = f.ip;
@@ -170,6 +171,7 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
     const double dt4 = dt_frame * dt_frame * dt_frame * dt_frame;
     for (int i = 0; i < 9; i++) Rv[i] = f.P_V[i] / dt4;
     double Vgva[3], dWgva[3];
+    const double QKp = f.P_Kp;                               // istate.QKp=P_Kp
     if (f.n_frame > 4 + ip.InitBiasFrameNum) {
         f.K = rbimu::est_ka_gmek_bias(f.As, f.Av, 1, f.R, f.X, f.P, f.Qg, f.P_W, f.Qbias, f.P_Kp, f.Rg, f.Rs, Rv, f.g_est,
                                       f.b_est, W_Xgv, Xgva, ip.g_module);
@@ -186,6 +188,26 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
         memcpy(Vgva, Vgv, sizeof(Vgv));
     }
     if ((r = rb_map_rotate_keylines(old, R0))) return r;     // old_buf.ef->rotate_keylines(R0.get_matrix())
+    if (odom) {   // :320-334 cf->poses.addFrameMeas(...): relPose from Rgva / Vgva, J_rp_x from R, W_Xgv as BiasCorrect left it
+        rb_odometry &o = *odom;
+        memset(&o, 0, sizeof(o));
+        odom_rel_pose(f.Rgva, Vgva, f.R, W_Xgv, o.relPosPose, o.WrelPosPose);
+        for (int i = 0; i < 3; i++) {
+            o.AcelMeas[i] = f.As[i];
+            o.VisualMeas[i] = f.Av[i];
+            o.GMeas[i] = f.g_est[i];
+        }
+        for (int i = 0; i < 9; i++) {
+            o.Rs[i] = f.Rs[i];
+            o.Rv[i] = Rv[i];
+            o.Rg[i] = f.P[(1 + i / 3) * 7 + 1 + i % 3];   // istate.P.slice<1,1,3,3>()
+        }
+        o.K = f.K;
+        o.WK = 1 / f.P[0];
+        o.QK = QKp;
+        o.KF_ID = -1;   // cf->kf_list.size()-1 without keyframes (:598)
+        o.tracked = 1;
+    }
     // ---- common part (:387-487) ---------------------------------------------------------------------------------------------
     bool nan = false;
     for (int i = 0; i < 3; i++) nan = nan || isnan(f.V[i]) || isnan(f.W[i]);
@@ -267,7 +289,7 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
 
 // a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking
 static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bool on_device, const double *ts, int n,
-                    rb_nav *nav_out) {
+                    rb_nav *nav_out, rb_odometry *odom_out) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
@@ -305,10 +327,11 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bo
             no->kn = ns.kn;
             no->thresh = ns.thresh_used;
             no->retuned_thresh = ns.retuned;
+            if (odom_out) memset(odom_out + i, 0, sizeof(rb_odometry));   // tracked = 0
         } else {
             double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
             if (dt < 0.001) dt = 1 / p.config_fps;
-            if ((r = imu_track_frame(pl, f, neu, old, ts[i], dt, imu, no))) return r;
+            if ((r = imu_track_frame(pl, f, neu, old, ts[i], dt, imu, no, odom_out ? odom_out + i : nullptr))) return r;
         }
     }
     pl->t_prev = ts[n - 1];

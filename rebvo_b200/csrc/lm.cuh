@@ -150,6 +150,58 @@ RB_HD void mat3_vec(const double *A, const double *v, double *o) {
     for (int i = 0; i < 3; i++) o[i] = t[i];
 }
 
+// ---- pose-graph measurement (rebvo_second_t.cpp:323-334 and :371-382) ----------------------------------------
+// rel = [-Rrel*V ; SO3(Rrel).ln()] and, when W_X is given, Wrel = J^T*W_X*J with J the inverse of
+// J_rp_x = [[-Rj, [rel[0:3]]x], [0, -I]].  The reference inverts J_rp_x with TooN's SVD pseudo-inverse; the matrix is block
+// upper triangular with orthonormal diagonal blocks, so its inverse is [[-Rj^T, -Rj^T*[t]x], [0, -I]] in closed form, which
+// agrees with the pseudo-inverse to rounding.  W_X == nullptr: Wrel = 0.
+RB_HD void odom_rel_pose(const double Rrel[9], const double V[3], const double Rj[9], const double *W_X, double rel[6],
+                         double Wrel[36]) {
+    double t[3];
+    mat3_vec(Rrel, V, t);
+    for (int i = 0; i < 3; i++) rel[i] = -t[i];
+    so3_ln_of_matrix(Rrel, rel + 3);
+    if (!W_X) {
+        for (int i = 0; i < 36; i++) Wrel[i] = 0;
+        return;
+    }
+    const double cx[9] = {0, -rel[2], rel[1], rel[2], 0, -rel[0], -rel[1], rel[0], 0};   // util::crossMatrix
+    double RtC[9];
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) {
+            double s = 0;
+            for (int k = 0; k < 3; k++) s += Rj[k * 3 + r] * cx[k * 3 + c];
+            RtC[r * 3 + c] = s;
+        }
+    double J[36];
+    for (int i = 0; i < 36; i++) J[i] = 0;
+    for (int r = 0; r < 3; r++) {
+        for (int c = 0; c < 3; c++) {
+            J[r * 6 + c] = -Rj[c * 3 + r];
+            J[r * 6 + 3 + c] = -RtC[r * 3 + c];
+        }
+        J[(3 + r) * 6 + 3 + r] = -1;
+    }
+    // (one thread runs this beside a wide kernel: rolled loops keep J and T out of that kernel's register allocation)
+    double T[36];   // J^T * W_X (TooN evaluates the product left to right)
+#pragma unroll 1
+    for (int r = 0; r < 6; r++)
+#pragma unroll 1
+        for (int c = 0; c < 6; c++) {
+            double s = 0;
+            for (int k = 0; k < 6; k++) s += J[k * 6 + r] * W_X[k * 6 + c];
+            T[r * 6 + c] = s;
+        }
+#pragma unroll 1
+    for (int r = 0; r < 6; r++)
+#pragma unroll 1
+        for (int c = 0; c < 6; c++) {
+            double s = 0;
+            for (int k = 0; k < 6; k++) s += T[r * 6 + k] * J[k * 6 + c];
+            Wrel[r * 6 + c] = s;
+        }
+}
+
 // ---- Cholesky<6> (Cholesky.h do_compute / backsub / get_inverse): L D L^T, no square roots --------------
 struct Chol6 {
     double c[36];

@@ -6,9 +6,12 @@
 //                                                           (Kp, RKp, Rot, Vel, t, dt, i, Pose, Pos, K, KLN; std::scientific,
 //                                                           precision 16, :151); the IMU, stereo and wall-clock records of that
 //                                                           block (:283-305) are not part of the hot path's output
-// Text is produced from rb_nav records, so a consumer of the GPU pipeline writes the same files the reference writes.
+//   pose graph (poses_list.ps)   pose_graph.cpp:32-40       binary OdometryMeas records, written by rebvorun at exit
+// Text is produced from rb_nav records and the pose graph from rb_odometry records, so a consumer of the GPU pipeline writes the
+// same files the reference writes.
 #include "common.cuh"
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 
 namespace {
@@ -129,6 +132,25 @@ extern "C" int rb_nav_format_log(const rb_nav *nav, int n, long long first_index
         o.i(r.kn);
         o.s(";\n");
     }
+    if (written) *written = o.len;
+    return o.overflow ? RB_ERR_ARG : RB_OK;
+}
+
+// pose graph file (poses_list.ps, app/rebvorun/main.cpp:134): pose_graph::saveToFile writes a uint count, then
+// OdometryMeas::dumpToFile per record: every vector / matrix element as a raw double (matrices row by row), KF_ID as a raw int.
+// rb_odometry holds the 81 doubles in that order without padding, so a record is two contiguous pieces.
+static_assert(offsetof(rb_odometry, KF_ID) == 81 * sizeof(double), "rb_odometry: doubles of OdometryMeas, packed");
+extern "C" int rb_odometry_format_pose_graph(const rb_odometry *r, int n, void *buf, size_t cap, size_t *written) {
+    if (n < 0 || (!r && n > 0)) return RB_ERR_ARG;
+    Out o{static_cast<char *>(buf), cap, 0, false};
+    uint32_t count = 0;
+    for (int k = 0; k < n; k++) count += r[k].tracked != 0;
+    o.put(reinterpret_cast<const char *>(&count), sizeof(count));
+    for (int k = 0; k < n; k++)
+        if (r[k].tracked) {
+            o.put(reinterpret_cast<const char *>(r[k].relPosPose), (int)offsetof(rb_odometry, KF_ID));
+            o.put(reinterpret_cast<const char *>(&r[k].KF_ID), sizeof(int32_t));
+        }
     if (written) *written = o.len;
     return o.overflow ? RB_ERR_ARG : RB_OK;
 }

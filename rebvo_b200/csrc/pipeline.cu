@@ -106,6 +106,11 @@ struct rb_pipeline {
     cudaEvent_t *ev_mpack, ev_mjoin;
     int mirror_n;                                 // frames of the last push
     rb_undistort *und;                            // UseUndistort=1 (rb_pipeline_set_undistort): fused into the gray pass
+    // optional per-frame odometry records (rb_pipeline_set_odometry): written beside the nav records, copied with them
+    int odom_on;
+    rb_odometry *odom_dev, *odom_pin;             // [max_batch]
+    int odom_n;                                   // records of the last push
+    double rkp_last;                              // RKp of the last frame pushed: QK of the next push's first record
 };
 
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
@@ -166,9 +171,10 @@ static void set_eye(double *M, double v) {
 }
 
 __global__ void k_frame_post_min(FrameState *fs, const TrackState *ts) { d_frame_post_min(fs, ts->lm); }
-__global__ void k_frame_post_match(FrameState *fs, MapState *nst, int match_threshold) {
+__global__ void k_frame_post_match(FrameState *fs, MapState *nst, int match_threshold, const TrackState *ts, rb_odometry *odom) {
     d_frame_post_match(fs, nst, match_threshold);
     nst->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
+    if (odom) d_frame_odometry(fs, ts->lm, odom);
 }
 // the nav record before the map's rescaling, which runs on the side stream and fills in its Kp / RKp
 __global__ void k_frame_finish(FrameState *fs, const MapState *nst, const MapState *ost, const TrackState *ts,
@@ -385,6 +391,8 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     if (pl->abort_pin) cudaFreeHost(pl->abort_pin);
     cudaFree(pl->fa_dev);
     if (pl->fa_pin) cudaFreeHost(pl->fa_pin);
+    cudaFree(pl->odom_dev);
+    if (pl->odom_pin) cudaFreeHost(pl->odom_pin);
     if (pl->gexec) {
         for (int i = 0; i < graph_slots(pl); i++)
             if (pl->gexec[i]) cudaGraphExecDestroy(pl->gexec[i]);
@@ -427,7 +435,8 @@ static int resc_join(rb_pipeline *pl) {
 }
 
 // one frame of the tracker/mapper stage: new = maps[f % RB_NMAPS] (already detected), old = the map of frame f-1
-static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArgs *fa, rb_nav *nav_slot) {
+static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArgs *fa, rb_nav *nav_slot,
+                       rb_odometry *odom_slot) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
@@ -490,7 +499,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
         prof_mark(pl, ST_DMATCH);
         // :410-423 match-count gate + :452-470 Regularize_1_iter / UpdateInverseDepthKalman + :369 rotate_keylines
         if ((r = rb_reg_ekf_enqueue(c, neu, old, p.RegularizeThresh, pl->fs, p.MatchThreshold, p.ReshapeQAbsolute,
-                                    p.LocationUncertainty, pl->fs->R0, side ? nav_slot : nullptr, fa)))
+                                    p.LocationUncertainty, pl->fs->R0, side ? nav_slot : nullptr, fa, odom_slot)))
             return r;
     } else {
         // The reference's order (rebvo_second_t.cpp:354-470) on the stage kernels that tests/test_gpu_parity.py and
@@ -510,7 +519,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
         RB_TRACE(c->stream, 4);
         prof_mark(pl, ST_DMATCH);
         // :410-423 match-count gate ; :452-470 Regularize_1_iter, UpdateInverseDepthKalman
-        k_frame_post_match<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, p.MatchThreshold);
+        k_frame_post_match<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, p.MatchThreshold, neu->ts, odom_slot);
         RB_LAUNCH_CHECK();
         if ((r = rb_regularize_enqueue(c, neu, p.RegularizeThresh, &pl->fs->do_map))) return r;
         if ((r = rb_ekf_enqueue(c, neu, pl->fs->V, p.ReshapeQAbsolute, p.LocationUncertainty, &pl->fs->do_map))) return r;
@@ -593,7 +602,8 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
             k_frame_first<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, pl->nav_dev + i, pl->fa_dev + i);
             RB_LAUNCH_CHECK();
         } else {
-            if ((r = track_frame(pl, neu, old, pl->fa_dev + i, pl->nav_dev + i))) return r;
+            if ((r = track_frame(pl, neu, old, pl->fa_dev + i, pl->nav_dev + i, pl->odom_on ? pl->odom_dev + i : nullptr)))
+                return r;
         }
         if (pl->mirror_on) {   // the frame's edge map as the reference's records, before the next frame touches it
             const size_t ofs = (size_t)i * pl->mirror_stride;
@@ -627,10 +637,13 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
     RB_CUDA(cudaSetDevice(c->device));
     int r;
+    pl->odom_n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
-        if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin))) return r;
+        if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom_on ? pl->odom_pin : nullptr)))
+            return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
         if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
+        pl->odom_n = pl->odom_on ? n : 0;
         return RB_OK;
     }
     const long long first = pl->n_pushed;
@@ -722,6 +735,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
             c->launches += pl->glaunches[key];
         }
         RB_CUDA(cudaMemcpyAsync(pl->nav_pin + off, pl->nav_dev, sizeof(rb_nav) * nj, cudaMemcpyDeviceToHost, c->stream));
+        if (pl->odom_on)
+            RB_CUDA(cudaMemcpyAsync(pl->odom_pin + off, pl->odom_dev, sizeof(rb_odometry) * nj, cudaMemcpyDeviceToHost,
+                                    c->stream));
     }
     for (int k = 0; k < RB_NMAPS; k++)
         RB_CUDA(cudaMemcpyAsync(&pl->abort_pin[k], &pl->maps[k]->ts_host.ctl->abort, sizeof(int), cudaMemcpyDeviceToHost,
@@ -741,6 +757,17 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     }
     if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
     pl->mirror_n = pl->mirror_on ? n : 0;
+    // QK of a record: P_Kp as the frame found it = RKp of the previous frame's record, which holds the value after that frame's
+    // rescaling also when the rescaling ran on the side stream (:382, :480-487)
+    for (int i = 0; i < n && pl->odom_on; i++) {
+        if (first + i == 0) {   // the first frame of a sequence only initialises the ring (:109-121)
+            memset(&pl->odom_pin[i], 0, sizeof(rb_odometry));
+            continue;
+        }
+        pl->odom_pin[i].QK = i == 0 ? pl->rkp_last : pl->nav_pin[i - 1].RKp;
+    }
+    pl->odom_n = pl->odom_on ? n : 0;
+    pl->rkp_last = pl->nav_pin[n - 1].RKp;
     {   // did a minimiser of this push abort (an exchange between its CTAs timed out)?  Checked on every push.
         bool aborted = false;
         for (int k = 0; k < RB_NMAPS; k++) aborted = aborted || pl->abort_pin[k] != 0;
@@ -815,6 +842,28 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     pl->mirror_rec = on == 2 ? 15 : sizeof(rb_keyline);
     pl->mirror_stride = stride;
     pl->mirror_n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
+    if (!pl || on < 0 || on > 1) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    RB_CUDA(cudaSetDevice(c->device));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    if (on && !pl->odom_dev) {
+        RB_CUDA(cudaMalloc(&pl->odom_dev, sizeof(rb_odometry) * pl->max_batch));
+        RB_CUDA(cudaMallocHost(&pl->odom_pin, sizeof(rb_odometry) * pl->max_batch));
+    }
+    if (on != pl->odom_on) drop_graphs(pl);   // the captured batches pass (or not) the record slots to their kernels
+    pl->odom_on = on;
+    pl->odom_n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, int *n) {
+    if (!pl || !recs || !n) return RB_ERR_ARG;
+    if (!pl->odom_n) return RB_ERR_STATE;
+    *recs = pl->odom_pin;
+    *n = pl->odom_n;
     return RB_OK;
 }
 extern "C" int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, int *n) {

@@ -1907,12 +1907,12 @@ int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, do
 // and the EKF takes the smoothed pair from registers; every keyline's rho / s_rho is written back (the scratch values
 // when the gate is closed).  Thread i also runs rotate_keylines(R0) on old keyline i: nothing reads the old map after
 // k_match, and the map stays what a caller of the pipeline sees.  One spare thread runs the gate's frame part, then the
-// pose integration / nav record.
+// pose integration / nav record; another one (next warp) the odometry record, which reads nothing the first one writes.
 __global__ void __launch_bounds__(256) k_reg_ekf(KLSoA kl, MapState *st, const double *__restrict__ r,
                                                  const double *__restrict__ s, double thresh, FrameState *fs,
                                                  int match_threshold, double zf, double q_abs, double loc_unc, KLSoA old,
                                                  const MapState *ost, const double *__restrict__ Rp, const LMState *lm,
-                                                 rb_nav *nav, const FrameArgs *fa) {
+                                                 rb_nav *nav, const FrameArgs *fa, rb_odometry *odom) {
     pdl_wait();
     pdl_launch();
     if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
@@ -1921,6 +1921,7 @@ __global__ void __launch_bounds__(256) k_reg_ekf(KLSoA kl, MapState *st, const d
         if (nav) d_frame_finish(fs, st, ost, lm->score, nav, fa, false);
         else d_frame_pose(fs);
     }
+    if (odom && blockIdx.x == gridDim.x - 1 && threadIdx.x == 32) d_frame_odometry(fs, *lm, odom);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < ost->kn) d_rotate(old, i, Rp, zf);
     // (the gate thread above only changes fs->V when the gate is closed, and then no thread reads it)
@@ -1940,11 +1941,12 @@ __global__ void __launch_bounds__(256) k_reg_ekf(KLSoA kl, MapState *st, const d
     if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&st->reg_num, __popc(bal));
 }
 int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameState *fs, int match_threshold,
-                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa) {
+                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa,
+                       rb_odometry *odom) {
     const TrackState &t = m->ts_host;
     RB_KLAUNCH(k_reg_ekf, rb_div_up(c->kcap, 256), 256, 0, m->kl, m->st, (const double *)t.reg_r,
                (const double *)t.reg_s, thresh, fs, match_threshold, c->zfm, q_abs, loc_unc, old->kl,
-               (const MapState *)old->st, R_dev, (const LMState *)&m->ts->lm, nav, fa);
+               (const MapState *)old->st, R_dev, (const LMState *)&m->ts->lm, nav, fa, odom);
     return RB_OK;
 }
 

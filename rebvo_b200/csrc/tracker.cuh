@@ -77,12 +77,13 @@ struct rb_nav;
 // arg-max of neu is complete) and directed_matching against the unrotated old map, each probed keyline rotated by R_dev;
 // the matched (rho, s_rho) of every keyline go to neu's regularisation scratch.  rb_reg_ekf_enqueue: the match-count
 // gate, Regularize_1_iter from that scratch, the EKF, rotate_keylines(R_dev) of old, and with nav the frame's nav record
-// (except Kp / RKp of a mapped frame, which rb_rescale_enqueue fills in).
+// (except Kp / RKp of a mapped frame, which rb_rescale_enqueue fills in); with odom the frame's odometry record (d_frame_odometry).
 int rb_match_enqueue(rb_ctx *c, rb_map *neu, rb_map *old, const DMatchArgs *args_dev, const double *R_dev,
                      double min_thr_mod, double min_thr_ang, double max_radius, double loc_uncertainty,
                      const int *do_match_dev);
 int rb_reg_ekf_enqueue(rb_ctx *c, rb_map *m, rb_map *old, double thresh, FrameState *fs, int match_threshold,
-                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa);
+                       double q_abs, double loc_unc, const double *R_dev, rb_nav *nav, const FrameArgs *fa,
+                       rb_odometry *odom);
 int rb_map_update_enqueue(rb_ctx *c, rb_map *m, double s_rho_min, unsigned int match_num_min, int re_escale, FrameState *fs,
                           const MapState *ost, rb_nav *nav, const FrameArgs *fa);
 int rb_ekf_enqueue(rb_ctx *c, rb_map *m, const double *vel_dev, double q_abs, double loc_unc,
