@@ -2,27 +2,19 @@
 byte for byte, the TrayFile and the pose / map records of the LogFile the unmodified reference writes (SaveLog=1,
 rebvo_third_t.cpp:259-311, 373-397) when they are fed the values of the reference's own output callbacks.  Host code: runs
 without a GPU."""
-import os
-
 import numpy as np
-import pytest
+
+from pipeline_util import euroc_stream, run_reference
 
 
 LOG_KEYS = ("Kp_cv", "RKp_cv", "Rot_cv", "Vel_cv", "t_cv", "dt_cv", "i_cv", "Pose_cv", "Pos_cv", "K_cv", "KLN_cv")
 
 
 def test_trajectory_and_log_files_match_reference(built, tmp_path):
-    from oracle import refapi
-    from rebvo_b200 import capi, synth
-    if not os.path.exists(refapi.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo not built")
-    cam = synth.EUROC
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"])
-    ts, fr = seq.frames(14)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
+    from rebvo_b200 import capi
+    ts, fr = euroc_stream(14)
     tray, log = str(tmp_path / "tray.txt"), str(tmp_path / "log.m")
-    info, rec = refapi.run_full_rebvo(path, str(tmp_path / "out.bin"), dict(SaveLog=1, TrayFile=tray, LogFile=log))
+    info, rec = run_reference(tmp_path, ts, fr, SaveLog=1, TrayFile=tray, LogFile=log)
     assert len(rec) >= 10
     nav = np.zeros(len(rec), capi.NAV)
     for k in ("t", "dt", "Pos", "PoseLie", "Pose", "Rot", "Vel", "K", "Kp", "RKp", "kn"):

@@ -2,23 +2,18 @@
 reproduce, byte for byte, the file the unmodified reference writes (oracle/_ref/ref_rebvo_pg with PoseGraphFile=) when it is fed
 the reference's own records.  Host code: runs without a GPU."""
 import ctypes as C
-import os
 
 import numpy as np
-import pytest
+
+from pipeline_util import euroc_stream, run_reference
 
 
 def test_pose_graph_file_matches_reference(built, tmp_path):
-    from oracle import build_pose_graph, refapi
-    from rebvo_b200 import capi, synth
-    if not os.path.exists(build_pose_graph.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo_pg not built")
-    cam = synth.EUROC
-    ts, fr = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"]).frames(14)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
+    from oracle import build_pose_graph
+    from rebvo_b200 import capi
+    ts, fr = euroc_stream(14)
     ps = str(tmp_path / "poses_list.ps")
-    refapi.run_full_rebvo(path, str(tmp_path / "out.bin"), dict(PoseGraphFile=ps), exe=build_pose_graph.EXE)
+    run_reference(tmp_path, ts, fr, exe=build_pose_graph.EXE, PoseGraphFile=ps)
     want = open(ps, "rb").read()
     recs = capi.read_pose_graph(ps)
     assert len(recs) >= 10 and len(want) == 4 + 652 * len(recs)

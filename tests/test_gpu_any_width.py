@@ -3,12 +3,12 @@ stage reads packed frames whose rows and frames start at any byte.  KITTI odomet
 with w = 1, 2, 3 (mod 4) and w * h odd or even, against the reference (compiled from its sources into oracle/_ref, which
 takes any size): scale-space planes and the detector bit for bit, the fused pipeline and the unmodified REBVO on the shim
 against the reference's three-thread run, and every way of feeding frames byte-identical to the host RGB push."""
-import os
-
 import numpy as np
 import pytest
 
 from parity_util import DOG_THRESH, KL_EXACT_DETECT, POS_NEG
+from pipeline_util import (assert_knife_edge, assert_runs_identical, assert_shim_equals, push, run_pipeline,
+                           run_reference, shim_exe)
 from plane_fit import ref_detect_child
 
 pytestmark = pytest.mark.gpu
@@ -30,10 +30,6 @@ def _seq(w, h, seed=7):
 
 def _u32(a):
     return np.ascontiguousarray(a).view(np.uint32)
-
-
-def _raw(nav):
-    return np.ascontiguousarray(nav).view(np.uint8)
 
 
 # ---- 1. scale space -------------------------------------------------------------------------------------------------
@@ -188,69 +184,32 @@ def kitti_stream():
     return _cam(w, h), ts, fr
 
 
-def _pipeline(p, ts, fr, batch=20, kc=None):
-    from rebvo_b200 import capi
-    pl = capi.Pipeline(p, max_batch=batch)
-    if kc is not None:
-        pl.set_undistort(kc)
-    nav = np.concatenate([pl.push(fr[s:s + batch], ts[s:s + batch]) for s in range(0, len(ts), batch)])
-    pl.close()
-    return nav
-
-
 @pytest.mark.parametrize("kc", [None, KC], ids=["plain", "undistort"])
 def test_pipeline_vs_reference(built, kitti_stream, kc, tmp_path):
     """The fused pipeline at 1241x376 against the reference's three-thread REBVO: identical keyline counts, match counts and
     poses within the bars of the drop-in test (a frame whose LM decision sits on a knife edge may take the other branch),
     equal estimation_ok."""
-    from oracle import refapi
-    from rebvo_b200 import capi, synth
-    if not os.path.exists(refapi.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo not built")
+    from rebvo_b200 import capi
     cam, ts, fr = kitti_stream
     p = capi.default_params(cam)
-    nav = _pipeline(p, ts, fr, kc=kc)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
-    extra = {} if kc is None else dict(UseUndistort=1, KcR2=kc[0], KcR4=kc[1], KcR6=kc[2], KcP1=kc[3], KcP2=kc[4])
-    _, ref = refapi.run_full_rebvo(path, path + ".ref", refapi.ref_params_from(p, **extra))
-    n = min(len(ref), len(nav))
-    assert n >= NF - 2
-    e = np.sqrt(((ref["Pos"][:n] - nav["Pos"][:n]) ** 2).sum(1))
-    ate = float(np.sqrt((e ** 2).mean()))
-    dm = np.abs(ref["matches"][1:n].astype(int) - nav["matches"][1:n].astype(int))
-    print("1241x376 %s: ATE %.3e m over %d frames, max |d matches| %d, kn %d..%d" % (
-        "undistorted" if kc else "plain", ate, n, dm.max(), nav["kn"][:n].min(), nav["kn"][:n].max()))
-    assert np.array_equal(ref["kn"][:n], nav["kn"][:n])
-    assert nav["kn"][:n].min() > 1000
-    assert np.array_equal(ref["est_ok"][1:n] != 0, nav["estimation_ok"][1:n] != 0)
-    assert dm.max() <= 0.005 * ref["matches"][1:n].max(), dm.max()
-    assert ate <= 1e-3 and e.max() <= 1e-3
+    _, ref = run_reference(tmp_path, ts, fr, p, kc=kc)
+    nav = run_pipeline(p, ts, fr, 20, kc=kc).nav
+    assert_knife_edge(ref, nav, NF - 2, "1241x376 " + ("undistorted" if kc else "plain"))
+    assert nav["kn"][:len(ref)].min() > 1000
 
 
 def test_unmodified_rebvo_on_the_gpu_library(built, kitti_stream, tmp_path):
     """The reference's own REBVO class on include/rebvo_b200_shim.hpp at 1241x376: it initialises, is identical run after
     run, and equals the fused pipeline."""
-    from oracle import refapi
-    from rebvo_b200 import capi, synth
-    shim_exe = os.path.join(os.path.dirname(refapi.EXE), "shim_rebvo")
-    if not os.path.exists(shim_exe):
-        pytest.skip("oracle/_ref/shim_rebvo not built")
+    from rebvo_b200 import capi
     cam, ts, fr = kitti_stream
     p = capi.default_params(cam)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
-    runs = [refapi.run_full_rebvo(path, path + ".shim%d" % k, refapi.ref_params_from(p), exe=shim_exe)[1].copy()
-            for k in range(2)]
+    runs = [run_reference(tmp_path, ts, fr, p, exe=shim_exe())[1].copy() for _ in range(2)]
     n = min(len(r) for r in runs)
     assert n >= NF - 2
     for f in ("kn", "matches", "Pos", "PoseLie", "Kp", "est_ok"):
         assert np.array_equal(runs[0][f][:n], runs[1][f][:n]), f
-    rec = runs[0]
-    nav = _pipeline(p, ts, fr)[:n]
-    assert np.array_equal(nav["kn"], rec["kn"][:n])
-    assert np.array_equal(nav["matches"][1:], rec["matches"][1:n])
-    assert np.abs(nav["Pos"] - rec["Pos"][:n]).max() <= 1e-9
+    assert_shim_equals(run_pipeline(p, ts, fr, 20).nav[:n], runs[0][:n])
 
 
 # ---- 5. every way of feeding frames --------------------------------------------------------------------------------
@@ -265,105 +224,62 @@ def feed(request):
     w, h = request.param
     ts, rgb = _seq(w, h, seed=5).frames(FEED_NF)
     assert np.array_equal(rgb[..., 0], rgb[..., 1]) and np.array_equal(rgb[..., 0], rgb[..., 2])
-    return _cam(w, h), ts, rgb, np.ascontiguousarray(rgb[..., 0])
+    return _cam(w, h), ts, rgb
 
 
-def _dev_frames(frames, offset):
-    """the frames in a device buffer, starting `offset` bytes past a 256-byte aligned allocation; (buffer, pointer)"""
-    import torch
-    flat = np.ascontiguousarray(frames).reshape(-1)
-    buf = torch.zeros(flat.size + offset + 8, dtype=torch.uint8, device="cuda")
-    buf[offset:offset + flat.size] = torch.from_numpy(flat).cuda()
-    return buf, buf.data_ptr() + offset
-
-
-def _feed_run(feed, fmt="rgb", how="host", batch=FEED_NF, offset=0, kc=None, mirror=0):
+def _feed(feed, fmt="rgb", how="host", batch=FEED_NF, offset=0, kc=None, mirror=0):
     from rebvo_b200 import capi
-    cam, ts, rgb, mono = feed
-    frames = mono if fmt == "mono" else rgb
-    pl = capi.Pipeline(capi.default_params(cam), max_batch=batch)
-    if kc is not None:
-        pl.set_undistort(kc)
-    if mirror:
-        pl.set_mirror(mirror)
-    navs, mirrors = [], []
-    for s in range(0, len(ts), batch):
-        f, t = frames[s:s + batch], ts[s:s + batch]
-        if how == "host":
-            nav = pl.push_mono(f, t) if fmt == "mono" else pl.push(f, t)
-        else:
-            buf, ptr = _dev_frames(f, offset)
-            nav = pl.push_mono_dev(ptr, t) if fmt == "mono" else pl.push_dev(ptr, t)
-            del buf
-        navs.append(nav)
-        if mirror:   # batch 1: the records of the newest map, as the map itself gives them
-            m = pl.map(0)
-            want = m.keylines() if mirror == 1 else m.pack_net(float(nav[0]["K"]))
-            got = pl.mirror(0)
-            assert len(got) == len(want) == nav[0]["kn"]
-            assert got.tobytes() == np.ascontiguousarray(want).tobytes(), "mirror %d, frame %d" % (mirror, s)
-            mirrors.append(got.copy())
-    pl.close()
-    return np.concatenate(navs)
-
-
-def _same(a, b, what):
-    assert len(a) == len(b)
-    diff = np.nonzero((_raw(a) != _raw(b)).reshape(len(a), -1).any(1))[0]
-    assert len(diff) == 0, "%s: nav records differ from frame %d" % (what, diff[0])
+    cam, ts, rgb = feed
+    return run_pipeline(capi.default_params(cam), ts, rgb, batch, how, fmt, offset, kc, mirror,
+                        check_mirror=bool(mirror))
 
 
 @pytest.mark.parametrize("kc", [None, KC], ids=["plain", "undistort"])
 def test_feeds_byte_identical(built, feed, monkeypatch, kc):
     """Host / device, RGB / mono (mono = RGB of the replicated frames), batches 20, 7 and 1, the 5-frame head / rest cut of
     host pushes, and device buffers whose frames start at odd bytes: one set of nav records."""
-    ref = _feed_run(feed, kc=kc)
-    assert np.isfinite(ref["Pos"]).all() and ref["kn"].min() > 500
-    _same(ref, _feed_run(feed, "rgb", "device", kc=kc), "device RGB")
-    _same(ref, _feed_run(feed, "mono", kc=kc), "host mono")
-    _same(ref, _feed_run(feed, "mono", "device", kc=kc), "device mono")
+    ref = _feed(feed, kc=kc)
+    assert np.isfinite(ref.nav["Pos"]).all() and ref.nav["kn"].min() > 500
+    assert_runs_identical(ref, _feed(feed, "rgb", "device", kc=kc), "device RGB")
+    assert_runs_identical(ref, _feed(feed, "mono", kc=kc), "host mono")
+    assert_runs_identical(ref, _feed(feed, "mono", "device", kc=kc), "device mono")
     for batch in (7, 1):
-        _same(ref, _feed_run(feed, "rgb", batch=batch, kc=kc), "host RGB batch %d" % batch)
-        _same(ref, _feed_run(feed, "mono", "device", batch=batch, kc=kc), "device mono batch %d" % batch)
+        assert_runs_identical(ref, _feed(feed, "rgb", batch=batch, kc=kc), "host RGB batch %d" % batch)
+        assert_runs_identical(ref, _feed(feed, "mono", "device", batch=batch, kc=kc), "device mono batch %d" % batch)
     for off in (1, 3):
-        _same(ref, _feed_run(feed, "rgb", "device", offset=off, kc=kc), "device RGB at byte offset %d" % off)
+        assert_runs_identical(ref, _feed(feed, "rgb", "device", offset=off, kc=kc),
+                              "device RGB at byte offset %d" % off)
     monkeypatch.setenv("REBVO_B200_SUB", "5")
-    _same(ref, _feed_run(feed, "rgb", kc=kc), "host RGB, SUB=5")
-    _same(ref, _feed_run(feed, "mono", kc=kc), "host mono, SUB=5")
+    assert_runs_identical(ref, _feed(feed, "rgb", kc=kc), "host RGB, SUB=5")
+    assert_runs_identical(ref, _feed(feed, "mono", kc=kc), "host mono, SUB=5")
 
 
 def test_misaligned_mono_device_base_refused(built, feed):
     """The device mono entry point keeps its rule: a base pointer that is not 4-byte aligned is refused."""
     from rebvo_b200 import capi
-    cam, ts, _, mono = feed
+    cam, ts, rgb = feed
+    mono = rgb[:4, ..., 0]
     pl = capi.Pipeline(capi.default_params(cam), max_batch=4)
-    buf, ptr = _dev_frames(mono[:4], 4)
     for off in (1, 2, 3):
         with pytest.raises(capi.RbError):
-            pl.push_mono_dev(ptr + off, ts[:4])
+            push(pl, mono, ts[:4], "device", offset=4 + off)
     pl.close()
-    del buf
 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_mirror(built, feed, mode):
     """Mirror modes 1 and 2 with one-frame pushes: every frame's records equal rb_map_sync_host_keylines /
     rb_map_pack_net_keylines of the same map, and the mirror leaves the nav records unchanged."""
-    ref = _feed_run(feed, batch=1)
-    _same(ref, _feed_run(feed, "rgb", batch=1, mirror=mode), "RGB, mirror %d" % mode)
-    _same(ref, _feed_run(feed, "mono", batch=1, mirror=mode), "mono, mirror %d" % mode)
+    ref = _feed(feed, batch=1)
+    assert_runs_identical(ref, _feed(feed, "rgb", batch=1, mirror=mode), "RGB, mirror %d" % mode)
+    assert_runs_identical(ref, _feed(feed, "mono", batch=1, mirror=mode), "mono, mirror %d" % mode)
 
 
 def test_imu_mode_mono_equals_rgb(built, feed):
     from rebvo_b200 import capi, synth
-    cam, ts, rgb, mono = feed
+    cam, ts, rgb = feed
     n, B = 10, 5
-    seq = _seq(cam["w"], cam["h"], seed=5)
-    out = []
-    for frames, push in ((rgb, "push"), (mono, "push_mono")):
-        pl = capi.Pipeline(capi.default_params(cam), max_batch=B)
-        pl.set_imu(synth.imu_samples(seq, n), capi.default_imu_params(InitBias=1, InitBiasFrameNum=5))
-        out.append(np.concatenate([getattr(pl, push)(frames[s:s + B], ts[s:s + B]) for s in range(0, n, B)]))
-        pl.close()
-    _same(out[0], out[1], "IMU mode")
-    assert np.isfinite(out[0]["Pos"]).all()
+    imu = synth.imu_samples(_seq(cam["w"], cam["h"], seed=5), n)
+    out = [run_pipeline(capi.default_params(cam), ts[:n], rgb[:n], B, fmt=fmt, imu=imu) for fmt in ("rgb", "mono")]
+    assert_runs_identical(out[0], out[1], "IMU mode")
+    assert np.isfinite(out[0].nav["Pos"]).all()

@@ -17,12 +17,11 @@ map are outside it: there FordwardMatch's arg-max over a monotonic integer key o
 
 The second half runs the whole per-frame pipeline against the reference's own three-thread REBVO on streams that take
 the rescaling, the serial quantile, a static stretch and a fast camera, with the bars of test_long_run_752x480."""
-import os
-
 import numpy as np
 import pytest
 
 from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG
+from pipeline_util import assert_tight, euroc_stream, run_both, run_pipeline
 
 pytestmark = pytest.mark.gpu
 
@@ -562,50 +561,6 @@ def test_rescale_degenerate(bench):
 
 
 # ---- B. the per-frame pipeline against the reference's three-thread REBVO -------------------------------------------
-def _both(tmp_path, ts, fr, params, batch=20):
-    from oracle import refapi
-    from rebvo_b200 import synth
-    if not os.path.exists(refapi.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo not built")
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
-    _, rec = refapi.run_full_rebvo(path, str(tmp_path / "out.bin"), refapi.ref_params_from(params), timeout=1500)
-    os.remove(path)
-    nav = _gpu(ts, fr, params, batch)
-    n = min(len(rec), len(nav))
-    return rec[:n], nav[:n]
-
-
-def _gpu(ts, fr, params, batch):
-    from rebvo_b200 import capi
-    pl = capi.Pipeline(params, max_batch=batch)
-    nav = np.concatenate([pl.push(fr[s:s + batch], ts[s:s + batch]) for s in range(0, len(ts), batch)])
-    pl.close()
-    return nav
-
-
-def _bars(rec, nav, min_frames):
-    """test_long_run_752x480's bars: equal kn / matches / est_ok, ATE <= 1e-7 m, Kp within rtol 1e-8."""
-    from oracle import refapi
-    par = refapi.trajectory_parity(rec, nav)
-    print(par)
-    assert par["frames"] >= min_frames
-    assert np.array_equal(rec["kn"], nav["kn"]), np.nonzero(rec["kn"] != nav["kn"])[0][:10]
-    bad = np.nonzero(rec["matches"][1:] != nav["matches"][1:])[0] + 1
-    assert not len(bad), "match counts differ at frames %s: ref %s gpu %s" % (bad[:5], rec["matches"][bad[:5]],
-                                                                             nav["matches"][bad[:5]])
-    assert np.array_equal(rec["est_ok"][1:] != 0, nav["estimation_ok"][1:] != 0)
-    assert par["ate_m"] <= 1e-7, par
-    assert np.allclose(rec["Kp"][1:], nav["Kp"][1:], rtol=1e-8, atol=0)
-    return par
-
-
-def _stream(n, seed=7, **kw):
-    from rebvo_b200 import synth
-    cam = synth.EUROC
-    return synth.Sequence(w=cam["w"], h=cam["h"], seed=seed, zf=cam["zfx"], **kw).frames(n)
-
-
 NAV_FIELDS = ("Pos", "Pose", "kn", "matches", "Kp", "RKp", "score", "s_rho_p")
 
 
@@ -613,14 +568,14 @@ def test_pipeline_rescaling(built, tmp_path, monkeypatch):
     """DoReScaling = 1: the rescaled map goes into the next frame (the inline map update); batch 7 == batch 20 and graph
     replay == eager launches, bit for bit."""
     from rebvo_b200 import capi, synth
-    ts, fr = _stream(60)
+    ts, fr = euroc_stream(60)
     p = capi.default_params(synth.EUROC, DoReScaling=1.0)
-    rec, nav = _both(tmp_path, ts, fr, p, batch=20)
-    _bars(rec, nav, 58)
+    rec, nav = run_both(tmp_path, ts, fr, p, batch=20)
+    assert_tight(rec, nav, 58)
     assert np.abs(nav["Kp"][2:] - 1.0).max() > 1e-6, "no rescaling happened"
-    b7 = _gpu(ts, fr, p, 7)
+    b7 = run_pipeline(p, ts, fr, 7).nav
     monkeypatch.setenv("REBVO_B200_NO_GRAPH", "1")
-    eager = _gpu(ts, fr, p, 20)
+    eager = run_pipeline(p, ts, fr, 20).nav
     monkeypatch.delenv("REBVO_B200_NO_GRAPH")
     for f in NAV_FIELDS:
         assert not _diff(f, nav[f], b7[f][:len(nav)]), ("batch 7", f)
@@ -631,11 +586,11 @@ def test_pipeline_static_stretch(built, tmp_path):
     """12 identical frames inside a walk, as at the start of a EuRoC sequence: V shrinks towards 0 and directed matching
     searches along shorter and shorter epipolar segments."""
     from rebvo_b200 import capi, synth
-    ts, fr = _stream(40)
+    ts, fr = euroc_stream(40)
     fr = np.concatenate([fr[:20], np.repeat(fr[20:21], 12, axis=0), fr[21:]])
     ts = np.arange(len(fr)) / 20.0
-    rec, nav = _both(tmp_path, ts, fr, capi.default_params(synth.EUROC), batch=10)
-    _bars(rec, nav, len(fr) - 2)
+    rec, nav = run_both(tmp_path, ts, fr, capi.default_params(synth.EUROC), batch=10)
+    assert_tight(rec, nav, len(fr) - 2)
     vz = np.linalg.norm(nav["V"][21:32], axis=1) * synth.EUROC["zfx"]
     print("smallest |V| * zf in the static stretch: %.3e px" % vz.min())
     assert vz.min() < 0.5
@@ -644,19 +599,20 @@ def test_pipeline_static_stretch(built, tmp_path):
 def test_pipeline_serial_quantile(built, tmp_path):
     """QCutOffNumBins = 200: EstimateQuantile's serial bin loop in every frame."""
     from rebvo_b200 import capi, synth
-    ts, fr = _stream(60)
-    rec, nav = _both(tmp_path, ts, fr, capi.default_params(synth.EUROC, QCutOffNumBins=200), batch=20)
-    _bars(rec, nav, 58)
-    assert not np.array_equal(nav["s_rho_p"][2:], _gpu(ts, fr, capi.default_params(synth.EUROC), 20)["s_rho_p"][2:])
+    ts, fr = euroc_stream(60)
+    rec, nav = run_both(tmp_path, ts, fr, capi.default_params(synth.EUROC, QCutOffNumBins=200), batch=20)
+    assert_tight(rec, nav, 58)
+    plain = run_pipeline(capi.default_params(synth.EUROC), ts, fr, 20).nav
+    assert not np.array_equal(nav["s_rho_p"][2:], plain["s_rho_p"][2:])
 
 
 def test_pipeline_fast_stream(built, tmp_path):
     """Four times the default camera speed: the directed search window is clamped at SearchRange."""
     from rebvo_b200 import capi, synth
-    ts, fr = _stream(40, speed=0.024)
+    ts, fr = euroc_stream(40, speed=0.024)
     p = capi.default_params(synth.EUROC)
-    rec, nav = _both(tmp_path, ts, fr, p, batch=20)
-    _bars(rec, nav, 38)
+    rec, nav = run_both(tmp_path, ts, fr, p, batch=20)
+    assert_tight(rec, nav, 38)
     px = np.linalg.norm(nav["V"][2:, :2], axis=1) * synth.EUROC["zfx"] * RHO_MAX
     print("largest |V_xy| * zf * RHO_MAX: %.1f px (SearchRange %d)" % (px.max(), p.SearchRange))
     assert px.max() > p.SearchRange

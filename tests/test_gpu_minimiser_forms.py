@@ -4,8 +4,7 @@ per-keyline body and the LM steps.  Each form runs test_gpu_parity.py's tracker 
 bars: the stage-level TryVelRot at three poses x three (reweight, procjf) pairs, then Minimizer_RV, m_id_f exact."""
 import pytest
 
-from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG, Report
-from test_gpu_parity import _frames, _tracker_parity
+from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG, Report, parity_frames, tracker_parity
 
 pytestmark = pytest.mark.gpu
 
@@ -34,7 +33,7 @@ def test_minimiser_form(built, monkeypatch, form):
                             cfg["tmin"])
     t_ref, l_ref = cfg["thresh"], 0
     t_gpu, l_gpu = cfg["thresh"], 0
-    for r, g, fr in zip(refs, gm, _frames(cfg)):
+    for r, g, fr in zip(refs, gm, parity_frames(cfg)):
         r.rgb2bw(fr)
         r.build()
         g.upload_rgb(fr)
@@ -48,7 +47,7 @@ def test_minimiser_form(built, monkeypatch, form):
     _, rt = refs[1].reestimate(cfg["track_points"], 100)
     gm[1].reestimate(cfg["track_points"], 100)
 
-    m_r = _tracker_parity(rep, cfg, refs, gm, rt)
+    m_r = tracker_parity(rep, cfg, refs, gm, rt)
     # the switches took effect: the cluster forms run a minimisation in one launch, the other in one per evaluation
     n0 = ctx.launches()
     gm[1].minimizer_rv(gm[0], m_r["V"], m_r["W"], cfg["match_thresh"], cfg["iter_max"], cfg["init_type"],

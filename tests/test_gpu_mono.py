@@ -2,91 +2,33 @@
 (m, m, m), so every result must equal the RGB path's on the replicated frames bit for bit: the gray plane, the keylines
 and masks, the nav records (compared as raw bytes), the host mirror, and the IMU-mode records.  The synthetic streams
 are gray replicated into three channels, so the mono frames are their first channel."""
-import os
-
 import numpy as np
 import pytest
+
+from pipeline_util import EUROC_KC, assert_runs_identical, euroc_sequence, keylines_equal, push, raw, run_pipeline, \
+    run_reference
 
 pytestmark = pytest.mark.gpu
 
 NF = 40
-EUROC_KC = (-0.28340811, 0.07395907, 0.0, 0.00019359, 1.76187114e-05)   # GlobalConfig_EuRoC_2.txt, UseUndistort=1
 
 
 @pytest.fixture(scope="module")
 def stream():
-    from rebvo_b200 import synth
-    cam = synth.EUROC
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"])
+    seq = euroc_sequence()
     ts, rgb = seq.frames(NF)
     assert np.array_equal(rgb[..., 0], rgb[..., 1]) and np.array_equal(rgb[..., 0], rgb[..., 2])
     return seq, ts, rgb, np.ascontiguousarray(rgb[..., 0])
 
 
-def _raw(nav):
-    return np.ascontiguousarray(nav).view(np.uint8)
-
-
-def _keylines_equal(a, b):
-    from rebvo_b200 import capi
-    if len(a) != len(b):
-        return False
-    return all(np.array_equal(a[f], b[f], equal_nan=True) for f in capi.KEYLINE.names)
-
-
-def _push(pl, how, frames, ts):
-    """one push of `frames` (RGB24 [n,h,w,3] or mono [n,h,w]) from host or device memory"""
-    mono = frames.ndim == 3
-    if how == "host":
-        return pl.push_mono(frames, ts) if mono else pl.push(frames, ts)
-    import torch
-    dev = torch.from_numpy(np.ascontiguousarray(frames)).cuda()
-    nav = pl.push_mono_dev(dev.data_ptr(), ts) if mono else pl.push_dev(dev.data_ptr(), ts)
-    del dev
-    return nav
-
-
-def _run(stream, fmt, batch, how="host", kc=None, mirror=0, imu=False, n=NF):
-    """nav records of the stream pushed in `batch`-frame pushes; fmt 'rgb', 'mono' or a list with one format per push.
-    Also returns the keylines + masks of the two newest maps after the last push, and the mirror records per frame."""
+def _stream_run(stream, fmt, batch, how="host", kc=None, mirror=0, imu=False, n=NF):
+    """the first n frames of the stream in `batch`-frame pushes (fmt: 'rgb', 'mono' or one of them per push), with the
+    two newest maps after the last push and every frame's mirror records"""
     from rebvo_b200 import capi, synth
-    seq, ts, rgb, mono = stream
-    pl = capi.Pipeline(capi.default_params(synth.EUROC), max_batch=batch)
-    if kc is not None:
-        pl.set_undistort(kc)
-    if mirror:
-        pl.set_mirror(mirror)
-    if imu:
-        pl.set_imu(synth.imu_samples(seq, n), capi.default_imu_params(InitBias=1, InitBiasFrameNum=5))
-    navs, mirrors = [], []
-    for k, s in enumerate(range(0, n, batch)):
-        f = fmt if isinstance(fmt, str) else fmt[k % len(fmt)]
-        src = mono if f == "mono" else rgb
-        nav = _push(pl, how, src[s:s + batch], ts[s:s + batch])
-        navs.append(nav)
-        for i in range(len(nav) if mirror else 0):
-            mirrors.append(pl.mirror(i).copy())
-    maps = []
-    for age in (0, 1):
-        m = pl.map(age)
-        maps.append((m.keylines(), m.mask()))
-    pl.close()
-    return np.concatenate(navs), maps, mirrors
-
-
-def _assert_same(a, b, what):
-    nav_a, maps_a, mir_a = a
-    nav_b, maps_b, mir_b = b
-    assert len(nav_a) == len(nav_b)
-    diff = np.nonzero((_raw(nav_a) != _raw(nav_b)).reshape(len(nav_a), -1).any(1))[0]
-    assert len(diff) == 0, "%s: nav records differ from frame %d" % (what, diff[0])
-    for age in (0, 1):
-        assert _keylines_equal(maps_a[age][0], maps_b[age][0]), "%s: keylines of map %d" % (what, age)
-        assert np.array_equal(maps_a[age][1], maps_b[age][1]), "%s: mask of map %d" % (what, age)
-    assert len(mir_a) == len(mir_b)
-    for i, (x, y) in enumerate(zip(mir_a, mir_b)):
-        ok = np.array_equal(x, y) if x.dtype == np.uint8 else _keylines_equal(x, y)
-        assert ok, "%s: mirror records of frame %d" % (what, i)
+    seq, ts, rgb, _ = stream
+    return run_pipeline(capi.default_params(synth.EUROC), ts[:n], rgb[:n], batch, how, fmt, kc=kc, mirror=mirror,
+                        imu=synth.imu_samples(seq, n) if imu else None,
+                        collect=("maps", "mirrors") if mirror else ("maps",))
 
 
 def _ramp_frame(w, h):
@@ -127,7 +69,7 @@ def test_stage_gray_and_detect(built, stream, which):
     assert np.array_equal(g1, 3.0 * mono.astype(np.float32))
     assert np.array_equal(d0.view(np.uint32), d1.view(np.uint32))
     assert kn0 == kn1 and kn1 > 100 and (t0, l0) == (t1, l1)
-    assert _keylines_equal(kl0, kl1)
+    assert keylines_equal(kl0, kl1)
     assert np.array_equal(mk0, mk1)
 
 
@@ -137,55 +79,50 @@ def test_pipeline_mono_equals_rgb(built, stream, monkeypatch, kc, how):
     """Byte-identical nav records and equal newest maps for batch sizes 20, 7 and 1, and with host pushes cut into a
     5-frame head and the rest (REBVO_B200_SUB=5)."""
     for batch in (20, 7, 1):
-        _assert_same(_run(stream, "rgb", batch, how, kc), _run(stream, "mono", batch, how, kc), "batch %d" % batch)
+        assert_runs_identical(_stream_run(stream, "rgb", batch, how, kc), _stream_run(stream, "mono", batch, how, kc),
+                              "batch %d" % batch)
     monkeypatch.setenv("REBVO_B200_SUB", "5")
-    _assert_same(_run(stream, "rgb", 20, how, kc), _run(stream, "mono", 20, how, kc), "SUB=5")
+    assert_runs_identical(_stream_run(stream, "rgb", 20, how, kc), _stream_run(stream, "mono", 20, how, kc), "SUB=5")
 
 
 def test_graph_replay_equals_eager_mono(built, stream, monkeypatch):
-    a = _run(stream, "mono", 10, kc=EUROC_KC)
+    a = _stream_run(stream, "mono", 10, kc=EUROC_KC)
     monkeypatch.setenv("REBVO_B200_NO_GRAPH", "1")
-    b = _run(stream, "mono", 10, kc=EUROC_KC)
-    _assert_same(a, b, "eager")
-    _assert_same(_run(stream, "rgb", 10, kc=EUROC_KC), b, "eager vs RGB")
+    b = _stream_run(stream, "mono", 10, kc=EUROC_KC)
+    assert_runs_identical(a, b, "eager")
+    assert_runs_identical(_stream_run(stream, "rgb", 10, kc=EUROC_KC), b, "eager vs RGB")
 
 
 @pytest.mark.parametrize("kc", [None, EUROC_KC], ids=["plain", "undistort"])
 def test_alternating_formats(built, stream, kc):
     """One pipeline fed mono, RGB, mono, ... (the captured batches are kept per input format): the records of an all-RGB
     run, from host and from device memory."""
-    ref = _run(stream, "rgb", 5, kc=kc)
-    _assert_same(ref, _run(stream, ["mono", "rgb"], 5, kc=kc), "mono/rgb")
-    _assert_same(ref, _run(stream, ["rgb", "mono", "mono"], 5, "device", kc=kc), "rgb/mono/mono, device")
+    ref = _stream_run(stream, "rgb", 5, kc=kc)
+    assert_runs_identical(ref, _stream_run(stream, ["mono", "rgb"], 5, kc=kc), "mono/rgb")
+    assert_runs_identical(ref, _stream_run(stream, ["rgb", "mono", "mono"], 5, "device", kc=kc),
+                          "rgb/mono/mono, device")
 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_mirror_mono(built, stream, mode):
-    _assert_same(_run(stream, "rgb", 20, kc=EUROC_KC, mirror=mode), _run(stream, "mono", 20, kc=EUROC_KC, mirror=mode),
-                 "mirror %d" % mode)
+    assert_runs_identical(_stream_run(stream, "rgb", 20, kc=EUROC_KC, mirror=mode),
+                          _stream_run(stream, "mono", 20, kc=EUROC_KC, mirror=mode), "mirror %d" % mode)
 
 
 @pytest.mark.parametrize("how", ["host", "device"])
 def test_imu_mode_mono(built, stream, how):
     """IMU mode (the EuRoC mono + IMU configuration, with undistortion)."""
-    a = _run(stream, "rgb", 10, how, kc=EUROC_KC, imu=True)
-    b = _run(stream, "mono", 10, how, kc=EUROC_KC, imu=True)
-    _assert_same(a, b, "IMU mode")
-    assert np.isfinite(a[0]["Pos"]).all()
+    a = _stream_run(stream, "rgb", 10, how, kc=EUROC_KC, imu=True)
+    b = _stream_run(stream, "mono", 10, how, kc=EUROC_KC, imu=True)
+    assert_runs_identical(a, b, "IMU mode")
+    assert np.isfinite(a.nav["Pos"]).all()
 
 
 def test_mono_vs_reference(built, stream, tmp_path):
     """The mono push against the unmodified reference run on the RGB frames, with the bars of the RGB trajectory test."""
-    from oracle import refapi
-    from rebvo_b200 import synth
-    if not os.path.exists(refapi.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo not built")
     _, ts, rgb, _ = stream
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, rgb)
-    _, rec = refapi.run_full_rebvo(path, str(tmp_path / "out.bin"))
-    os.remove(path)
-    nav = _run(stream, "mono", 20)[0]
+    _, rec = run_reference(tmp_path, ts, rgb)
+    nav = _stream_run(stream, "mono", 20).nav
     n = min(len(rec), NF - 1)
     assert n >= NF - 2
     assert np.array_equal(rec["kn"][:n], nav["kn"][:n])
@@ -228,7 +165,7 @@ def test_bad_arguments(built, stream):
     from rebvo_b200 import capi, synth
     _, ts, _, mono = stream
     B, n = 5, 15
-    ref = _run(stream, "mono", B, n=n)[0]
+    ref = _stream_run(stream, "mono", B, n=n).nav
     pl = capi.Pipeline(capi.default_params(synth.EUROC), max_batch=B)
     dev = torch.from_numpy(np.ascontiguousarray(mono[:n])).cuda()
     navs = []
@@ -236,10 +173,10 @@ def test_bad_arguments(built, stream):
         for call in _bad_calls(pl, dev, mono, ts, B):
             with pytest.raises(capi.RbError):
                 call()
-        navs.append(pl.push_mono(mono[s:s + B], ts[s:s + B]))
+        navs.append(push(pl, mono[s:s + B], ts[s:s + B]))
     pl.close()
     del dev
-    assert np.array_equal(_raw(np.concatenate(navs)), _raw(ref))
+    assert np.array_equal(raw(np.concatenate(navs)), raw(ref))
 
 
 def test_bench_pass_mono(built, stream):
@@ -247,7 +184,7 @@ def test_bench_pass_mono(built, stream):
     from rebvo_b200 import capi, synth
     _, ts, _, mono = stream
     pl = capi.Pipeline(capi.default_params(synth.EUROC), max_batch=8)
-    pl.push_mono(mono[:8], ts[:8])
+    push(pl, mono[:8], ts[:8])
     N = synth.EUROC["w"] * synth.EUROC["h"]
     ms, by = pl.bench_pass(6, 8, 3)
     assert ms > 0 and by == 5.0 * N * 8

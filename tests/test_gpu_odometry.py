@@ -3,65 +3,29 @@ SecondThread appends to REBVO::poses (rebvo_second_t.cpp:323-334 IMU mode, :371-
 the reference's own 3-thread REBVO writes on the same frames (oracle/_ref/ref_rebvo_pg with PoseGraphFile=).  Also: the
 match-count restart that sets QK, the empty old map, the records across schedules and resets, and that the records leave the
 nav records and the launches of a push unchanged."""
-import os
-
 import numpy as np
 import pytest
+
+from pipeline_util import euroc_sequence, euroc_stream, push, raw, run_pipeline, run_reference
 
 pytestmark = pytest.mark.gpu
 
 ZERO_FIELDS = ("AcelMeas", "VisualMeas", "GMeas", "Rs", "Rv", "Rg")
 
 
-def _pushes(pl, fr, ts, batch, push="push"):
-    navs, recs, launches = [], [], []
-    for s in range(0, len(ts), batch):
-        l0 = pl.launches()
-        navs.append(getattr(pl, push)(fr[s:s + batch], ts[s:s + batch]))
-        launches.append(pl.launches() - l0)
-        recs.append(pl.odometry() if pl._odom else None)
-    return np.concatenate(navs), (np.concatenate(recs) if pl._odom else None), launches
+def _records(params, ts, fr, batch, **kw):
+    """nav and odometry records of the frames pushed with the records on, in `batch`-frame pushes"""
+    r = run_pipeline(params, ts, fr, batch, odometry=True, collect=("odometry",), **kw)
+    return r.nav, r.odometry
 
 
-def _pipeline(params, batch, odom=True, env=None, monkeypatch=None):
+def _pose_graph(tmp_path, params, fr, ts, **kw):
+    """the records of the pose graph file the reference writes on the frames"""
+    from oracle import build_pose_graph
     from rebvo_b200 import capi
-    for k, v in (env or {}).items():
-        monkeypatch.setenv(k, v)
-    pl = capi.Pipeline(params, max_batch=batch)
-    for k in (env or {}):
-        monkeypatch.delenv(k)
-    pl._odom = odom
-    if odom:
-        pl.set_odometry(True)
-    return pl
-
-
-def _run(params, fr, ts, batch, odom=True, env=None, monkeypatch=None):
-    pl = _pipeline(params, batch, odom, env, monkeypatch)
-    try:
-        return _pushes(pl, fr, ts, batch)
-    finally:
-        pl.close()
-
-
-def _reference(tmp_path, params, fr, ts, **kv):
-    from oracle import build_pose_graph, refapi
-    from rebvo_b200 import capi, synth
-    if not os.path.exists(build_pose_graph.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo_pg not built")
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
     ps = str(tmp_path / "poses_list.ps")
-    _, nav = refapi.run_full_rebvo(path, str(tmp_path / "out.bin"), refapi.ref_params_from(params, PoseGraphFile=ps, **kv),
-                                   timeout=1500, exe=build_pose_graph.EXE)
-    os.remove(path)
-    return capi.read_pose_graph(ps), nav
-
-
-def _euroc(n, seed=7):
-    from rebvo_b200 import synth
-    cam = synth.EUROC
-    return synth.Sequence(w=cam["w"], h=cam["h"], seed=seed, zf=cam["zfx"]).frames(n)
+    run_reference(tmp_path, ts, fr, params, exe=build_pose_graph.EXE, timeout=1500, PoseGraphFile=ps, **kw)
+    return capi.read_pose_graph(ps)
 
 
 def _w_err(ref, got):
@@ -70,16 +34,12 @@ def _w_err(ref, got):
     return np.abs(got["WrelPosPose"] - ref["WrelPosPose"]).reshape(len(ref), -1).max(1) / scale
 
 
-def _raw(a):
-    return np.ascontiguousarray(a).view(np.uint8)
-
-
 def test_vision_records_match_reference(built, tmp_path):
     from rebvo_b200 import capi, synth
-    ts, fr = _euroc(60)
+    ts, fr = euroc_stream(60)
     p = capi.default_params(synth.EUROC)
-    ref, _ = _reference(tmp_path, p, fr, ts)
-    _, odo, _ = _run(p, fr, ts, 7)
+    ref = _pose_graph(tmp_path, p, fr, ts)
+    _, odo = _records(p, ts, fr, 7)
     assert len(odo) == 60 and odo["tracked"][0] == 0 and np.all(odo["tracked"][1:] == 1)
     got = odo[1:]
     assert len(ref) == len(got)
@@ -97,16 +57,16 @@ def test_vision_records_match_reference(built, tmp_path):
     with open(path, "wb") as f:
         f.write(capi.format_pose_graph(odo))
     back = capi.read_pose_graph(path)
-    assert np.array_equal(_raw(back), _raw(got))
+    assert np.array_equal(raw(back), raw(got))
 
 
 def test_restart_branch_qk(built, tmp_path):
     """GlobalMatchThreshold above every frame's match count: every frame restarts, P_Kp = 10 from the second tracked frame on."""
     from rebvo_b200 import capi, synth
-    ts, fr = _euroc(24)
+    ts, fr = euroc_stream(24)
     p = capi.default_params(synth.EUROC, MatchThreshold=10 ** 6)
-    ref, _ = _reference(tmp_path, p, fr, ts)
-    _, odo, _ = _run(p, fr, ts, 8)
+    ref = _pose_graph(tmp_path, p, fr, ts)
+    _, odo = _records(p, ts, fr, 8)
     got = odo[1:]
     assert len(ref) == len(got)
     assert got["QK"][0] == 5e-6 and np.all(got["QK"][1:] == 10)
@@ -120,12 +80,11 @@ def test_black_frame_and_empty_old_map(built, tmp_path):
     P_Kp = 10, in the reference as here), and frame 7 tracks against the empty old map, for which the pipeline writes a
     zero information matrix (the reference's W_X is uninitialised there) and V is the prior; frame 8 restarts again."""
     from rebvo_b200 import capi, synth
-    ts, fr = _euroc(14)
-    fr = fr.copy()
+    ts, fr = euroc_stream(14)
     fr[6] = 0
     p = capi.default_params(synth.EUROC)
-    ref, _ = _reference(tmp_path, p, fr, ts)
-    nav, odo, _ = _run(p, fr, ts, 7)
+    ref = _pose_graph(tmp_path, p, fr, ts)
+    nav, odo = _records(p, ts, fr, 7)
     got = odo[1:]
     assert len(ref) == len(got)
     assert nav["kn"][6] == 0 and nav["estimation_ok"][6] == 0 and nav["estimation_ok"][7] == 0
@@ -145,20 +104,12 @@ def test_black_frame_and_empty_old_map(built, tmp_path):
 def test_imu_mode_records_match_reference(built, tmp_path):
     from rebvo_b200 import capi, synth
     nf = 50
-    cam = synth.EUROC
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"])
+    seq = euroc_sequence()
     ts, fr = seq.frames(nf)
     smp = synth.imu_samples(seq, nf)
-    csv = str(tmp_path / "imu.csv")
-    synth.write_imu_csv(csv, smp)
-    p = capi.default_params(cam)
-    ref, _ = _reference(tmp_path, p, fr, ts, ImuMode=2, ImuFile=csv, ImuTimeScale=1, InitBias=1, InitBiasFrameNum=5)
-    pl = capi.Pipeline(p, max_batch=10)
-    pl.set_imu(smp, capi.default_imu_params(InitBias=1, InitBiasFrameNum=5))
-    pl._odom = True
-    pl.set_odometry(True)
-    _, odo, _ = _pushes(pl, fr, ts, 10)
-    pl.close()
+    p = capi.default_params(synth.EUROC)
+    ref = _pose_graph(tmp_path, p, fr, ts, imu=smp)
+    _, odo = _records(p, ts, fr, 10, imu=smp)
     assert odo["tracked"][0] == 0 and np.all(odo["tracked"][1:] == 1)
     got = odo[1:]
     # the reference's last record is not comparable: its first thread waits for that frame's inertial samples in a loop that
@@ -190,62 +141,68 @@ def test_records_leave_nav_and_launches_unchanged(built, monkeypatch):
     """With the records on, the nav records are bit-identical and a push launches exactly the kernels it launches without
     them (the constant of rb_pipeline_set_odometry is 0), in both map schedules; switching them off restores the launches."""
     from rebvo_b200 import capi, synth
-    ts, fr = _euroc(40)
+    ts, fr = euroc_stream(40)
     p = capi.default_params(synth.EUROC)
     for env in ({}, {"REBVO_B200_MAP_CHAIN": "0"}):
-        nav0, _, l0 = _run(p, fr, ts, 7, odom=False, env=env, monkeypatch=monkeypatch)
-        nav1, _, l1 = _run(p, fr, ts, 7, odom=True, env=env, monkeypatch=monkeypatch)
-        assert np.array_equal(_raw(nav0), _raw(nav1)), env
-        assert l1 == l0, (env, l0, l1)
-        pl = _pipeline(p, 7, True, env, monkeypatch)   # on for the first pushes, then off
+        with monkeypatch.context() as m:   # the map schedule is chosen at creation
+            for k, v in env.items():
+                m.setenv(k, v)
+            off = run_pipeline(p, ts, fr, 7, collect=("launches",))
+            on = run_pipeline(p, ts, fr, 7, odometry=True, collect=("launches",))
+            pl = capi.Pipeline(p, max_batch=7)   # on for the first pushes, then off
+        assert np.array_equal(raw(off.nav), raw(on.nav)), env
+        assert on.launches == off.launches, (env, off.launches, on.launches)
+        pl.set_odometry(True)
         navs, lc = [], []
         for k, s in enumerate(range(0, len(ts), 7)):
             if k == 3:
                 pl.set_odometry(False)
-                pl._odom = False
                 with pytest.raises(capi.RbError):
                     pl.odometry()
             n0 = pl.launches()
-            navs.append(pl.push(fr[s:s + 7], ts[s:s + 7]))
+            navs.append(push(pl, fr[s:s + 7], ts[s:s + 7]))
             lc.append(pl.launches() - n0)
         pl.close()
-        assert lc == l0, (env, l0, lc)
-        assert np.array_equal(_raw(np.concatenate(navs)), _raw(nav0))
+        assert lc == off.launches, (env, off.launches, lc)
+        assert np.array_equal(raw(np.concatenate(navs)), raw(off.nav))
 
 
 def test_records_same_across_schedules_and_resets(built, monkeypatch):
     """Bit-identical records from the default schedule, the reference map schedule (REBVO_B200_MAP_CHAIN=0) and the
     one-cluster minimiser (REBVO_B200_MIN_G=1), with host and device input; after rb_pipeline_reset the records are those of
     a fresh pipeline (first frame untracked, QK from 5e-6 again)."""
-    import torch
     from rebvo_b200 import capi, synth
-    ts, fr = _euroc(30)
+    ts, fr = euroc_stream(30)
     p = capi.default_params(synth.EUROC)
-    nav_b, base, _ = _run(p, fr, ts, 7)
-    _, odo, _ = _run(p, fr, ts, 7, env={"REBVO_B200_MAP_CHAIN": "0"}, monkeypatch=monkeypatch)
-    assert np.array_equal(_raw(odo), _raw(base))
+    nav_b, base = _records(p, ts, fr, 7)
+    with monkeypatch.context() as m:
+        m.setenv("REBVO_B200_MAP_CHAIN", "0")
+        _, odo = _records(p, ts, fr, 7)
+    assert np.array_equal(raw(odo), raw(base))
     # the one-cluster minimiser sums its reductions over one cluster instead of four: its nav records already differ from
     # the default's in the last bits, and so do the records (measured on H100: 2e-17 in relPosPose, 4e-14 of max |W|)
-    nav_g, odo, _ = _run(p, fr, ts, 7, env={"REBVO_B200_MIN_G": "1"}, monkeypatch=monkeypatch)
+    with monkeypatch.context() as m:
+        m.setenv("REBVO_B200_MIN_G", "1")
+        nav_g, odo = _records(p, ts, fr, 7)
     print("MIN_G=1: nav identical %s, max |d relPosPose| %.3e, W rel %.3e" %
-          (np.array_equal(_raw(nav_g), _raw(nav_b)), np.abs(odo["relPosPose"] - base["relPosPose"]).max(),
+          (np.array_equal(raw(nav_g), raw(nav_b)), np.abs(odo["relPosPose"] - base["relPosPose"]).max(),
            _w_err(base[1:], odo[1:]).max()))
     for k in ("K", "WK", "KF_ID", "tracked") + ZERO_FIELDS:
         assert np.array_equal(odo[k], base[k]), k
     assert np.abs(odo["relPosPose"] - base["relPosPose"]).max() <= 1e-15
     assert np.allclose(odo["QK"], base["QK"], rtol=1e-12, atol=0)
     assert _w_err(base[1:], odo[1:]).max() <= 1e-12
-    pl = _pipeline(p, 10)
-    dev = torch.from_numpy(np.ascontiguousarray(fr)).cuda()
+    pl = capi.Pipeline(p, max_batch=10)
+    pl.set_odometry(True)
     for s in range(0, 30, 10):   # device input, other batch size
-        pl.push_dev(dev[s:s + 10].data_ptr(), ts[s:s + 10])
-        assert np.array_equal(_raw(pl.odometry()), _raw(base[s:s + 10]))
+        push(pl, fr[s:s + 10], ts[s:s + 10], "device")
+        assert np.array_equal(raw(pl.odometry()), raw(base[s:s + 10]))
     pl.reset()
     again = []
     for s in range(0, 30, 10):
-        pl.push(fr[s:s + 10], ts[s:s + 10])
+        push(pl, fr[s:s + 10], ts[s:s + 10])
         again.append(pl.odometry())
     pl.close()
     again = np.concatenate(again)
     assert again["tracked"][0] == 0 and again["QK"][1] == 5e-6
-    assert np.array_equal(_raw(again), _raw(base))
+    assert np.array_equal(raw(again), raw(base))

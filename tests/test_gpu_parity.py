@@ -8,29 +8,9 @@ import numpy as np
 import pytest
 
 from parity_util import (BIG_CFG, DOG_THRESH, EUROC_CFG, KL_EXACT_DETECT, PLANE_FIT, POS_NEG, TUM_CFG, Report,
-                         compare_keylines)
+                         compare_keylines, parity_frames, tracker_parity)
 
 pytestmark = pytest.mark.gpu
-
-
-def _frames(cfg):
-    from rebvo_b200 import synth
-    cam = cfg["cam"]
-    if cfg["name"] == "tum":
-        return synth.frame_pair(seed=42, w=cam["w"], h=cam["h"], nrect=220, shift=(1.5, 0.7))
-    if cfg["name"] == "big":
-        seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=100, zf=cam["zfx"], nrect_bg=1500, nrect_fg=200)
-        return seq.frame(10)[1], seq.frame(11)[1]
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"])
-    return seq.frame(10)[1], seq.frame(11)[1]
-
-
-def _seed_depth(kl):
-    kl = kl.copy()
-    kl["rho"] = 1.0
-    kl["s_rho"] = 0.2
-    kl["m_num"] = 5
-    return kl
 
 
 def _run_stage_parity(cfg):
@@ -38,7 +18,7 @@ def _run_stage_parity(cfg):
     from rebvo_b200 import capi
     cam = cfg["cam"]
     rep = Report(cfg["name"])
-    f0, f1 = _frames(cfg)
+    f0, f1 = parity_frames(cfg)
     refs = [refapi.RefMap(cam["w"], cam["h"], cam["ppx"], cam["ppy"], cam["zfx"], cam["zfy"], cfg["sigma0"],
                           cfg["ksigma"]) for _ in range(2)]
     ctx = capi.Ctx(cam, cfg["sigma0"], cfg["ksigma"], kl_capacity=50000)
@@ -84,7 +64,7 @@ def _run_stage_parity(cfg):
     _, rt = refs[1].reestimate(cfg["track_points"], 100)
     gm[1].reestimate(cfg["track_points"], 100)
 
-    m_r = _tracker_parity(rep, cfg, refs, gm, rt)
+    m_r = tracker_parity(rep, cfg, refs, gm, rt)
     old_r, new_r, old_g, new_g = refs[0], refs[1], gm[0], gm[1]
     # FordwardMatch
     old_r.forward_match(new_r)
@@ -133,69 +113,6 @@ def _run_stage_parity(cfg):
         g.close()
     ctx.close()
     return rep
-
-
-def _tracker_parity(rep, cfg, refs, gm, rt):
-    """TryVelRot at three poses x three (reweight, procjf) pairs, then Minimizer_RV; returns the reference's result."""
-    # old = frame 0 with seeded depth, new = frame 1
-    old_r, new_r, old_g, new_g = refs[0], refs[1], gm[0], gm[1]
-    old_r.set_keylines(_seed_depth(old_r.keylines()))
-    old_g.load_keylines(old_r.keylines(), old_r.mask())
-    new_g.load_keylines(new_r.keylines(), new_r.mask())
-    q_r = old_r.quantile(1e-3, 20.0, 0.9, 100)
-    q_g = old_g.quantile(1e-3, 20.0, 0.9, 100)
-    rep.add("EstimateQuantile", q_r == q_g, "ref %.17g gpu %.17g" % (q_r, q_g))
-    new_r.build_field(cfg["radius"], rt)
-    new_g.build_field(cfg["radius"], rt)
-    fr_, fg_ = new_r.field(), new_g.field()
-    rep.exact("field ikl", fr_[:, :, 1], fg_[:, :, 1])
-    has = fr_[:, :, 1] >= 0
-    rep.exact("field dist (where set)", fr_[:, :, 0][has], fg_[:, :, 0][has])
-    # single evaluations of TryVelRot
-    k0 = old_r.knum()
-    pnum = (k0 + 3) & ~3
-    rng = np.random.default_rng(3)
-    res_prev = np.zeros(pnum)
-    Xs = [np.zeros(6), np.array([0.002, -0.001, 0.0005, 0.001, -0.002, 0.003]),
-          np.array([-0.004, 0.003, -0.001, -0.003, 0.001, -0.004])]
-    for xi, X in enumerate(Xs):
-        for (rw, pj) in ((False, True), (True, True), (False, False)):
-            s_r, J_r, F_r, res_r = new_r.try_vel_rot(old_r, X, rw, pj, cfg["match_thresh"], q_r,
-                                                     cfg["match_num_thresh"], cfg["reweight"], res_prev)
-            mf_r = old_r.keylines()["m_id_f"].copy()
-            s_g, J_g, F_g, res_g = new_g.try_vel_rot(old_g, X, rw, pj, cfg["match_thresh"], q_r,
-                                                     cfg["match_num_thresh"], cfg["reweight"], res_prev)
-            mf_g = old_g.keylines()["m_id_f"]
-            tag = "TryVelRot X%d rw=%d pj=%d" % (xi, rw, pj)
-            rep.close(tag + " score", s_r, s_g, 1e-10)
-            if pj:
-                rep.close(tag + " JtJ", J_r, J_g, 1e-9, atol=1e-9 * np.abs(J_r).max())
-                rep.close(tag + " JtF", F_r, F_g, 1e-9, atol=1e-9 * np.abs(F_r).max())
-            rep.exact(tag + " m_id_f", mf_r, mf_g)
-            kl0 = old_r.keylines()
-            used = (kl0["s_rho"] <= q_r)
-            rep.close(tag + " DResidualNew", res_r[:k0][used], res_g[used], 1e-12, atol=1e-12)
-            if pj and not rw:
-                res_prev = res_r.copy()
-                res_prev[~np.isfinite(res_prev)] = 0
-    # full minimisation
-    V0, W0 = np.zeros(3), np.zeros(3)
-    old_r.set_keylines(_seed_depth(old_r.keylines()))
-    m_r = new_r.minimizer_rv(old_r, V0, W0, cfg["match_thresh"], cfg["iter_max"], cfg["init_type"], cfg["reweight"],
-                             q_r, cfg["match_num_thresh"], cfg["init_iter"])
-    new_g.set_frame_count(0)
-    m_g = new_g.minimizer_rv(old_g, V0, W0, cfg["match_thresh"], cfg["iter_max"], cfg["init_type"], cfg["reweight"],
-                             q_r, cfg["match_num_thresh"], cfg["init_iter"])
-    rep.add("Minimizer_RV values", True, "ref V=%s W=%s F=%.6g" % (m_r["V"], m_r["W"], m_r["F"]))
-    rep.close("Minimizer_RV V", m_r["V"], m_g["V"], 0.0, atol=1e-9)     # SURVEY 8(c): abs 1e-9
-    rep.close("Minimizer_RV W", m_r["W"], m_g["W"], 0.0, atol=1e-9)
-    rep.close("Minimizer_RV F", m_r["F"], m_g["F"], 1e-8)
-    rep.close("Minimizer_RV RVel", m_r["RVel"], m_g["RVel"], 1e-8, atol=1e-9 * np.abs(m_r["RVel"]).max())
-    rep.close("Minimizer_RV RW0", m_r["RW0"], m_g["RW0"], 1e-8, atol=1e-9 * np.abs(m_r["RW0"]).max())
-    rep.close("Minimizer_RV W_X", m_r["W_X"], m_g["W_X"], 1e-8, atol=1e-9 * np.abs(m_r["W_X"]).max())
-    rep.close("Minimizer_RV rel_err_score", m_r["rel_err_score"], m_g["rel_err_score"], 1e-8)
-    rep.exact("Minimizer_RV m_id_f", old_r.keylines()["m_id_f"], old_g.keylines()["m_id_f"])
-    return m_r
 
 
 @pytest.mark.parametrize("cfg", [TUM_CFG, EUROC_CFG, BIG_CFG], ids=["tum640", "euroc752", "synthetic1280x960"])

@@ -4,12 +4,12 @@ fused pipeline, the unmodified REBVO on the shim and IMU mode, against the unmod
 The reference caches its plane-fit pseudo inverse per process (edge_finder.cpp:83-84), so every reference result for a
 window other than 5x5 comes from a child process (tests/plane_fit.py) or from a whole reference run (ref_rebvo), one
 window size per process."""
-import os
-
 import numpy as np
 import pytest
 
 from parity_util import BIG_CFG, DOG_THRESH, EUROC_CFG, KL_EXACT_DETECT, POS_NEG, TUM_CFG, Report, compare_keylines
+from pipeline_util import (assert_knife_edge, assert_shim_equals, euroc_sequence, euroc_stream, run_pipeline,
+                           run_reference, shim_exe)
 from plane_fit import ref_detect_child
 
 pytestmark = pytest.mark.gpu
@@ -207,71 +207,30 @@ def test_rejected_sizes(built):
             capi.Pipeline(capi.default_params(synth.EUROC, plane_fit_size=R), max_batch=4)
 
 
-def _stream(nf=NF):
-    from rebvo_b200 import synth
-    cam = synth.EUROC
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=7, zf=cam["zfx"])
-    ts, fr = seq.frames(nf)
-    return cam, seq, ts, fr
-
-
-def _run(p, ts, fr, batch):
-    from rebvo_b200 import capi
-    pl = capi.Pipeline(p, max_batch=batch)
-    nav = np.concatenate([pl.push(fr[s:s + batch], ts[s:s + batch]) for s in range(0, len(ts), batch)])
-    pl.close()
-    return nav
-
-
 @pytest.mark.parametrize("R", [1, 3])
 def test_pipeline_vs_reference(built, R, tmp_path):
     """The fused pipeline at R against the reference's whole REBVO run with the same DetectorPlaneFitSize."""
-    from oracle import refapi
     from rebvo_b200 import capi, synth
-    if not os.path.exists(refapi.EXE):
-        pytest.skip("oracle/_ref/ref_rebvo not built")
-    cam, _, ts, fr = _stream()
-    p = capi.default_params(cam, plane_fit_size=R)
-    nav = _run(p, ts, fr, 20)
-    nav7 = _run(p, ts, fr, 7)
+    ts, fr = euroc_stream(NF)
+    p = capi.default_params(synth.EUROC, plane_fit_size=R)
+    _, ref = run_reference(tmp_path, ts, fr, p)
+    nav = run_pipeline(p, ts, fr, 20).nav
+    nav7 = run_pipeline(p, ts, fr, 7).nav
     assert nav.tobytes() == nav7.tobytes()
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
-    _, ref = refapi.run_full_rebvo(path, path + ".ref", refapi.ref_params_from(p))
-    n = min(len(ref), len(nav))
-    assert n >= NF - 2
-    e = np.sqrt(((ref["Pos"][:n] - nav["Pos"][:n]) ** 2).sum(1))
-    ate = float(np.sqrt((e ** 2).mean()))
-    first = int(np.nonzero(e > 1e-9)[0][0]) if (e > 1e-9).any() else -1
-    dm = np.abs(ref["matches"][1:n].astype(int) - nav["matches"][1:n].astype(int))
-    print("R=%d pipeline vs reference: ATE %.3e m over %d frames, first frame above 1e-9 m: %d, max |d matches| %d, "
-          "kn %d..%d" % (R, ate, n, first, dm.max(), nav["kn"][:n].min(), nav["kn"][:n].max()))
-    assert np.array_equal(ref["kn"][:n], nav["kn"][:n])
-    assert np.array_equal(ref["est_ok"][1:n] != 0, nav["estimation_ok"][1:n] != 0)
     # the detector is bit-exact; the tracker's sums run in another order, so a frame whose LM decision sits on a knife
     # edge may take the other branch (as in test_gpu_dropin.py): matches within 0.5 %, poses within north_star's bar
-    assert dm.max() <= 0.005 * ref["matches"][1:n].max(), dm.max()
-    assert ate <= 1e-3 and e.max() <= 1e-3
+    assert_knife_edge(ref, nav, NF - 2, "R=%d pipeline vs reference" % R)
 
 
 def test_dropin_shim_at_r3(built, tmp_path):
     """The unmodified REBVO on include/rebvo_b200_shim.hpp with DetectorPlaneFitSize=3 equals the fused pipeline at R = 3."""
-    from oracle import refapi
     from rebvo_b200 import capi, synth
-    shim_exe = os.path.join(os.path.dirname(refapi.EXE), "shim_rebvo")
-    if not os.path.exists(shim_exe):
-        pytest.skip("oracle/_ref/shim_rebvo not built")
-    cam, _, ts, fr = _stream()
-    p = capi.default_params(cam, plane_fit_size=3)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
-    _, rec = refapi.run_full_rebvo(path, path + ".shim", refapi.ref_params_from(p), exe=shim_exe)
-    nav = _run(p, ts, fr, 20)
-    n = min(len(rec), len(nav))
-    assert n >= NF - 2
-    assert np.array_equal(nav["kn"][:n], rec["kn"][:n])
-    assert np.array_equal(nav["matches"][1:n], rec["matches"][1:n])
-    assert np.abs(nav["Pos"][:n] - rec["Pos"][:n]).max() <= 1e-9
+    ts, fr = euroc_stream(NF)
+    p = capi.default_params(synth.EUROC, plane_fit_size=3)
+    _, rec = run_reference(tmp_path, ts, fr, p, exe=shim_exe())
+    nav = run_pipeline(p, ts, fr, 20).nav
+    assert min(len(rec), len(nav)) >= NF - 2
+    assert_shim_equals(nav, rec)
 
 
 def test_imu_mode_kn_at_r3(built):
@@ -279,12 +238,10 @@ def test_imu_mode_kn_at_r3(built):
     threshold feedback alone."""
     from rebvo_b200 import capi, synth
     nf = 50
-    cam, seq, ts, fr = _stream(nf)
-    p = capi.default_params(cam, plane_fit_size=3)
-    vis = _run(p, ts, fr, 10)
-    pl = capi.Pipeline(p, max_batch=10)
-    pl.set_imu(synth.imu_samples(seq, nf), capi.default_imu_params(InitBias=1, InitBiasFrameNum=5))
-    nav = np.concatenate([pl.push(fr[s:s + 10], ts[s:s + 10]) for s in range(0, nf, 10)])
-    pl.close()
+    seq = euroc_sequence()
+    ts, fr = seq.frames(nf)
+    p = capi.default_params(synth.EUROC, plane_fit_size=3)
+    vis = run_pipeline(p, ts, fr, 10).nav
+    nav = run_pipeline(p, ts, fr, 10, imu=synth.imu_samples(seq, nf)).nav
     assert np.array_equal(vis["kn"], nav["kn"])
     assert np.isfinite(nav["Pos"]).all()

@@ -7,6 +7,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from pipeline_util import assert_shim_equals, euroc_stream, frames_file, run_pipeline, run_reference
+
 pytestmark = pytest.mark.gpu
 NF = 30
 
@@ -17,11 +19,8 @@ def test_shim_classes_reproduce_reference_flow(built, tmp_path):
     exe = os.path.join(os.path.dirname(refapi.EXE), "shim_driver")
     if not os.path.exists(exe):
         pytest.skip("oracle/_ref/shim_driver not built (needs the reference headers)")
-    cam = synth.EUROC
-    seq = synth.Sequence(w=cam["w"], h=cam["h"], seed=9, zf=cam["zfx"])
-    ts, fr = seq.frames(NF)
-    path = str(tmp_path / "frames.bin")
-    synth.write_frames_file(path, ts, fr)
+    ts, fr = euroc_stream(NF, seed=9)
+    path = frames_file(tmp_path, ts, fr)
     r = subprocess.run([refapi.runnable(exe, str(tmp_path)), path, path + ".shim"], capture_output=True, text=True,
                        timeout=600, env=refapi.lib_env())
     assert r.returncode == 0, r.stderr[-2000:]
@@ -29,18 +28,13 @@ def test_shim_classes_reproduce_reference_flow(built, tmp_path):
         n, sz = np.frombuffer(f.read(8), np.int32)
         assert sz == refapi.OUTREC.itemsize
         shim = np.frombuffer(f.read(), refapi.OUTREC, count=n)
-    pl = capi.Pipeline(capi.default_params(cam), max_batch=10)
-    nav = np.concatenate([pl.push(fr[s:s + 10], ts[s:s + 10]) for s in range(0, NF, 10)])
-    pl.close()
+    nav = run_pipeline(capi.default_params(synth.EUROC), ts, fr, 10).nav
     assert len(shim) == NF
-    assert np.array_equal(shim["kn"], nav["kn"])
-    assert np.array_equal(shim["matches"][1:], nav["matches"][1:])
-    d = np.abs(shim["Pos"] - nav["Pos"]).max()
-    print("shim vs pipeline max |dPos| %.3e" % d)
-    assert d <= 1e-9
+    assert_shim_equals(nav, shim)
     assert np.abs(shim["PoseLie"] - nav["PoseLie"]).max() <= 1e-9
-    if os.path.exists(refapi.EXE):
-        info, rec = refapi.run_full_rebvo(path, path + ".ref")
+    ref = run_reference(tmp_path, ts, fr, required=False)
+    if ref is not None:
+        rec = ref[1]
         m = min(len(rec), NF - 1)
         assert np.array_equal(rec["kn"][:m], shim["kn"][:m])
         ate = float(np.sqrt(((rec["Pos"][:m] - shim["Pos"][:m]) ** 2).sum(1).mean()))

@@ -3,10 +3,9 @@ the reference's bit for bit, including the frame border where taps fall outside 
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from pipeline_util import EUROC_KC
 
-# EuRoC cam0 radial-tangential coefficients (Kc2, Kc4, Kc6, P1, P2), app/rebvorun/GlobalConfig_EuRoC_2.txt
-EUROC_KC = [-0.28340811, 0.07395907, 0.0, 0.00019359, 1.76187114e-05]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("kc", [EUROC_KC, [0.12, -0.05, 0.01, -0.002, 0.003], [0, 0, 0, 0, 0]])
