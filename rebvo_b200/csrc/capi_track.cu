@@ -131,7 +131,12 @@ extern "C" int rb_minimizer_rv(rb_map *fmap, rb_map *old, double V[3], double W[
     a.init_iter = init_iter;
     a.reweight_distance = reweight_distance;
     a.match_num_thresh = match_num_thresh;
-    if ((r = rb_minimizer_enqueue(c, fmap, old, args_dev(c), &a, max_s_rho, false, 0, true))) return r;
+    // operands staged as the per-frame pipeline stages them (REBVO_B200_MIN_EARLY, default on): the copy of V / W above is
+    // the stream's last operation, so no kernel that writes the old map can still be running when they are read
+    c->min_early = getenv("REBVO_B200_MIN_EARLY") ? atoi(getenv("REBVO_B200_MIN_EARLY")) != 0 : true;
+    r = rb_minimizer_enqueue(c, fmap, old, args_dev(c), &a, max_s_rho, false, 0, true);
+    c->min_early = false;
+    if (r) return r;
     LMState *lmh = (LMState *)((char *)c->pinned + 4096);
     RB_CUDA(cudaMemcpyAsync(lmh, &fmap->ts->lm, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
     if ((r = rb_minimizer_check_abort(c, fmap))) return r;   // (synchronises)

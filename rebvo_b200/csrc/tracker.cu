@@ -602,7 +602,16 @@ __device__ void lm_begin(LMState &s, const MapState *old_st, const MapState *f_s
 __global__ void k_lm_begin(TrackState *ts, const MapState *old_st, const MapState *f_st, const double *VW,
                            rb_minimizer_args a, double max_r, double max_s_rho, int s_rho_from_state,
                            unsigned int frame_count, int fc_from_state) {
-    lm_begin(ts->lm, old_st, f_st, VW, a, max_r, max_s_rho, s_rho_from_state, frame_count, fc_from_state);
+    LMState &s = ts->lm;
+    lm_begin(s, old_st, f_st, VW, a, max_r, max_s_rho, s_rho_from_state, frame_count, fc_from_state);
+    if (old_st->kn <= 0) {   // "if(klist.KNum()<=0) return 0;" (:598): the evaluations launched after this do nothing,
+        s.no_keylines = 1;   // Vel / W0 stay what the caller passed, no FrameCount++
+        s.score = 0;
+        for (int i = 0; i < 3; i++) {
+            s.Vel[i] = VW[i];
+            s.W0[i] = VW[3 + i];
+        }
+    }
 }
 
 // ---- pieces of one TryVelRot evaluation (global_tracker.cpp:285-543), shared by the one-launch-per-evaluation
@@ -969,6 +978,7 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
     __shared__ double s_tot[28];
     __shared__ bool s_last;
     LMState &lm = *tp.lm;
+    if (lm.no_keylines) return;   // (the minimisation of an empty old map ended in k_lm_begin)
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) {   // the two exponentials run on two warps side by side (each is a serial sin/cos chain)
         double X[6];
@@ -1377,6 +1387,7 @@ __global__ void k_lm_single(TrackState *ts, const double *X, int res_in, int res
     s.match_num_thresh = mnt;
     s.frame_count = fc;
     s.k_huber = k_huber;
+    s.no_keylines = 0;
 }
 
 int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *X_dev, int reweight, int procjf,

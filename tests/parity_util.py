@@ -112,6 +112,93 @@ def parity_frames(cfg):
     return seq.frame(10)[1], seq.frame(11)[1]
 
 
+# ---- seeded edge-map states (tests/test_gpu_mapper_states.py, tests/test_gpu_minimiser_forms.py) --------------------
+RHO_MIN, RHO_MAX = 1e-3, 20.0
+
+
+def _bits(a):
+    a = np.ascontiguousarray(a)
+    if a.dtype.kind == "f":
+        return a.view(np.uint32 if a.dtype.itemsize == 4 else np.uint64)
+    return a
+
+
+def _diff(tag, ref, got):
+    """'' if ref and got are equal bit for bit (NaN == NaN), else a short description of the first mismatches."""
+    ref, got = np.asarray(ref), np.asarray(got)
+    if ref.shape != got.shape:
+        return "%s: shape %s vs %s" % (tag, ref.shape, got.shape)
+    same = _bits(ref) == _bits(got)
+    if ref.dtype.kind == "f":
+        same |= np.isnan(ref) & np.isnan(got)
+    if same.ndim > 1:
+        same = same.reshape(len(same), -1).all(1)
+    bad = np.nonzero(~same)[0]
+    if not len(bad):
+        return ""
+    i = bad[:3]
+    return "%s: %d/%d differ, first %s ref %s gpu %s" % (tag, len(bad), len(same), i.tolist(), ref[i].tolist(),
+                                                           got[i].tolist())
+
+
+class Bench:
+    """Two detected frames on the reference (two RefMap ring slots) and two GPU maps of one context.  The detector is the
+    reference's (its parity with the GPU detector is test_gpu_parity's business); every mapper stage starts from a
+    state loaded identically on both sides."""
+
+    def __init__(self, cam, frames, kl_capacity=50000, cfg=EUROC_CFG):
+        from oracle import refapi
+        from rebvo_b200 import capi
+        self.cam = cam
+        self.zfm = float(np.float32((np.float32(cam["zfx"]) + np.float32(cam["zfy"])) / np.float32(2)))
+        self.ref = [refapi.RefMap(cam["w"], cam["h"], cam["ppx"], cam["ppy"], cam["zfx"], cam["zfy"], cfg["sigma0"],
+                                  cfg["ksigma"]) for _ in range(2)]
+        t, l = cfg["thresh"], 0
+        self.kl, self.mask = [], []
+        for r, fr in zip(self.ref, frames):
+            r.rgb2bw(fr)
+            r.build()
+            _, t, l = r.detect(PLANE_FIT, POS_NEG, DOG_THRESH, cfg["kl_max"], t, l, cfg["kl_ref"], cfg["gain"],
+                               cfg["tmax"], cfg["tmin"])
+            self.kl.append(r.keylines())
+            self.mask.append(r.mask())
+        self.ctx = capi.Ctx(cam, cfg["sigma0"], cfg["ksigma"], kl_capacity=kl_capacity)
+        self.gpu = [self.ctx.new_map(), self.ctx.new_map()]
+
+    def load(self, i, kl, mask=None):
+        mask = self.mask[i] if mask is None else mask
+        kl = np.ascontiguousarray(kl)
+        self.ref[i].set_keylines(kl)
+        self.ref[i].set_mask(mask, len(kl))
+        self.gpu[i].load_keylines(kl, mask)
+
+    def close(self):
+        for g in self.gpu:
+            g.close()
+        self.ctx.close()
+
+
+def _depth_state(kl, rng, new=False):
+    """Seeded depth state inside the per-frame flow's domain: rho in [RHO_MIN, RHO_MAX] (log-uniform, plus exact 1e-3,
+    1.0 and 20.0, plus runs of equal values), s_rho in [1e-6, 20], m_num in 0..10; new keylines with m_id = -1."""
+    kl = kl.copy()
+    k = len(kl)
+    rho = np.exp(rng.uniform(np.log(RHO_MIN), np.log(RHO_MAX), k))
+    u = rng.random(k)
+    rho[u < 0.03] = RHO_MIN
+    rho[(u >= 0.03) & (u < 0.06)] = 1.0
+    rho[(u >= 0.06) & (u < 0.09)] = RHO_MAX
+    for s in rng.choice(k, max(1, k // 64), replace=False):   # runs of equal values
+        rho[s:s + 8] = rho[s]
+    s_rho = np.exp(rng.uniform(np.log(1e-6), np.log(20.0), k))
+    kl["rho"] = rho
+    kl["s_rho"] = s_rho
+    kl["m_num"] = rng.integers(0, 11, k)
+    if new:
+        kl["m_id"] = -1
+    return kl
+
+
 def _seed_depth(kl):
     kl = kl.copy()
     kl["rho"] = 1.0

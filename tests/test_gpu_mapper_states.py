@@ -20,41 +20,14 @@ the rescaling, the serial quantile, a static stretch and a fast camera, with the
 import numpy as np
 import pytest
 
-from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG
+from parity_util import EUROC_CFG, RHO_MAX, RHO_MIN, Bench, _bits, _depth_state, _diff
 from pipeline_util import assert_tight, euroc_stream, run_both, run_pipeline
 
 pytestmark = pytest.mark.gpu
 
-RHO_MIN, RHO_MAX = 1e-3, 20.0
 MIN_HITS = 50          # keylines (or tie groups, bins ...) a case must put on its target branch
 CFG = EUROC_CFG
 KITTI_CAM = dict(w=1241, h=376, zfx=718.856, zfy=718.856, ppx=1241 / 2.0 - 13.3, ppy=376 / 2.0 - 2.8)
-
-
-# ---- bit comparison -------------------------------------------------------------------------------------------------
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    if a.dtype.kind == "f":
-        return a.view(np.uint32 if a.dtype.itemsize == 4 else np.uint64)
-    return a
-
-
-def _diff(tag, ref, got):
-    """'' if ref and got are equal bit for bit (NaN == NaN), else a short description of the first mismatches."""
-    ref, got = np.asarray(ref), np.asarray(got)
-    if ref.shape != got.shape:
-        return "%s: shape %s vs %s" % (tag, ref.shape, got.shape)
-    same = _bits(ref) == _bits(got)
-    if ref.dtype.kind == "f":
-        same |= np.isnan(ref) & np.isnan(got)
-    if same.ndim > 1:
-        same = same.reshape(len(same), -1).all(1)
-    bad = np.nonzero(~same)[0]
-    if not len(bad):
-        return ""
-    i = bad[:3]
-    return "%s: %d/%d differ, first %s ref %s gpu %s" % (tag, len(bad), len(same), i.tolist(), ref[i].tolist(),
-                                                           got[i].tolist())
 
 
 def _compare(kl_r, kl_g, fields, matched_fields=()):
@@ -68,44 +41,6 @@ def _compare(kl_r, kl_g, fields, matched_fields=()):
     for f in matched_fields:
         out.append(_diff(f + " (matched)", kl_r[f][mk], kl_g[f][mk]))
     return [o for o in out if o]
-
-
-# ---- the two sides ----------------------------------------------------------------------------------------------------
-class Bench:
-    """Two detected frames on the reference (two RefMap ring slots) and two GPU maps of one context.  The detector is the
-    reference's (its parity with the GPU detector is test_gpu_parity's business); every mapper stage below starts from a
-    state loaded identically on both sides."""
-
-    def __init__(self, cam, frames, kl_capacity=50000):
-        from oracle import refapi
-        from rebvo_b200 import capi
-        self.cam = cam
-        self.zfm = float(np.float32((np.float32(cam["zfx"]) + np.float32(cam["zfy"])) / np.float32(2)))
-        self.ref = [refapi.RefMap(cam["w"], cam["h"], cam["ppx"], cam["ppy"], cam["zfx"], cam["zfy"], CFG["sigma0"],
-                                  CFG["ksigma"]) for _ in range(2)]
-        t, l = CFG["thresh"], 0
-        self.kl, self.mask = [], []
-        for r, fr in zip(self.ref, frames):
-            r.rgb2bw(fr)
-            r.build()
-            _, t, l = r.detect(PLANE_FIT, POS_NEG, DOG_THRESH, CFG["kl_max"], t, l, CFG["kl_ref"], CFG["gain"],
-                               CFG["tmax"], CFG["tmin"])
-            self.kl.append(r.keylines())
-            self.mask.append(r.mask())
-        self.ctx = capi.Ctx(cam, CFG["sigma0"], CFG["ksigma"], kl_capacity=kl_capacity)
-        self.gpu = [self.ctx.new_map(), self.ctx.new_map()]
-
-    def load(self, i, kl, mask=None):
-        mask = self.mask[i] if mask is None else mask
-        kl = np.ascontiguousarray(kl)
-        self.ref[i].set_keylines(kl)
-        self.ref[i].set_mask(mask, len(kl))
-        self.gpu[i].load_keylines(kl, mask)
-
-    def close(self):
-        for g in self.gpu:
-            g.close()
-        self.ctx.close()
 
 
 def _cut(kl, mask, k):
@@ -135,26 +70,6 @@ def bench_kitti(built):
     assert min(len(k) for k in b.kl) > 2000
     yield b
     b.close()
-
-
-def _depth_state(kl, rng, new=False):
-    """Seeded depth state inside the flow's domain (module docstring)."""
-    kl = kl.copy()
-    k = len(kl)
-    rho = np.exp(rng.uniform(np.log(RHO_MIN), np.log(RHO_MAX), k))
-    u = rng.random(k)
-    rho[u < 0.03] = RHO_MIN
-    rho[(u >= 0.03) & (u < 0.06)] = 1.0
-    rho[(u >= 0.06) & (u < 0.09)] = RHO_MAX
-    for s in rng.choice(k, max(1, k // 64), replace=False):   # runs of equal values
-        rho[s:s + 8] = rho[s]
-    s_rho = np.exp(rng.uniform(np.log(1e-6), np.log(20.0), k))
-    kl["rho"] = rho
-    kl["s_rho"] = s_rho
-    kl["m_num"] = rng.integers(0, 11, k)
-    if new:
-        kl["m_id"] = -1
-    return kl
 
 
 # ---- 1. directed_matching ---------------------------------------------------------------------------------------------
