@@ -341,6 +341,38 @@ int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, int iters, fl
  * number.  k_prof is the depth scale the third thread passes (pbuf.K, rebvo_third_t.cpp:192). */
 int rb_map_pack_net_keylines(rb_map *m, double k_prof, void *dst, int capacity, int *n_out);
 
+/* Dense inverse-depth grid of a frame: the viewer's depth_filler on each net_keyline packet (src/visualizer/visualizer.cpp:436-440,
+ * depth_filler(cam, {block_w, block_h}, BOUND_NONE) at :303; src/visualizer/depth_filler.cpp):
+ *   ResetData; FillEdgeData(net_kl, n, {0,0}, thresh_rel_rho, thresh_match_num) (discart = true); InitCoarseFine;
+ *   Integrate(iter_num) (init_cf = true); computeDistance(Zeros)
+ * The grid is gw = w / block_w by gh = h / block_h cells (integer division); each cell holds the fused or filled inverse depth
+ * rho, its deviation s_rho, the distance |P| of its centre's 3D point from the camera (get3DPos, depth_filler.h:115-122) and
+ * whether a record fell into it.  min_dist is depth_filler::GetMinDist.  Bit-identical to the reference, with one deviation: a
+ * record whose cell index is >= gw * gh (qy / block_h >= gh) writes out of bounds in the reference (undefined behaviour) and is
+ * dropped here.  Every shipped viewer configuration uses block 10 x 10, thresh_rel_rho 1, thresh_match_num 5, iter_num 10.
+ * RB_ERR_ARG for a block < 1 or larger than the frame, and for iter_num < 0. */
+typedef struct rb_depth_params {
+    int32_t block_w, block_h;   /* depth_filler's blockSize */
+    double thresh_rel_rho;      /* DF_ThreshRelRho: records with s_rho / rho above it are skipped */
+    int32_t thresh_match_num;   /* DF_ThreshMatchNum: records with m_num below it are skipped */
+    int32_t iter_num;           /* DF_IterNum: Integrate1Step sweeps */
+} rb_depth_params;
+typedef struct rb_depth_cell {   /* df_point's rho, s_rho, dist, fixed; the grid is row-major gh x gw */
+    double rho, s_rho, dist;
+    int32_t fixed, _pad;
+} rb_depth_cell;
+/* the fill of n 15-byte net_keyline records in host memory on the context's camera; out receives gw * gh cells */
+int rb_depth_fill_net(rb_ctx *c, const void *records, int n, const rb_depth_params *p, rb_depth_cell *out, int *gw, int *gh,
+                      double *min_dist);
+/* Per-frame depth grid in the pipeline: with p set, every pushed frame's edge map is packed as net_keyline records with the
+ * frame's K (rebvo_third_t.cpp:191, pbuf.K; with mirror mode 2 the mirror's records are used) and filled by one CTA on a side
+ * stream while the following frames are tracked; the cells go straight into pinned host memory.  p == NULL: off, and the
+ * pushes run the batches of a pipeline that never had it.  Changing it drops the captured batches, like set_mirror.
+ * RB_ERR_ARG for invalid p (as rb_depth_fill_net) and in IMU mode.  rb_pipeline_depth(i): the grid of frame i of the last push,
+ * valid from the return of that push until the next one; RB_ERR_ARG when depth is off or i is out of range. */
+int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p);
+int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist);
+
 /* IMU fusion (BASELINE configs[2], REBVOParameters ImuMode = 2: samples from a dataset file).  After this call every push runs
  * the IMU branch of REBVO::SecondThread (rebvo_second_t.cpp:182-336: gyro pre-rotation, Minimizer_V, ExtRotVel, BiasCorrect,
  * scale / gravity / bias filter of scaleestimator.cpp, filtered pose of :521-551) instead of Minimizer_RV.  samples: n rows

@@ -69,6 +69,22 @@ ODOM = np.dtype([("relPosPose", "f8", 6), ("WrelPosPose", "f8", (6, 6)), ("AcelM
 # one record of the pose graph file (pose_graph::saveToFile): ODOM without `tracked`, unpadded
 PS_REC = np.dtype([(n, ODOM.fields[n][0]) for n in ODOM.names if n != "tracked"])
 
+# rb_depth_cell: one cell of the viewer's depth grid (depth_filler's df_point rho, s_rho, dist, fixed)
+DEPTH_CELL = np.dtype([("rho", "f8"), ("s_rho", "f8"), ("dist", "f8"), ("fixed", "i4"), ("_pad", "i4")])
+
+
+class DepthParams(C.Structure):
+    """rb_depth_params: depth_filler's block size and the viewer's DF_ThreshRelRho, DF_ThreshMatchNum, DF_IterNum."""
+    _fields_ = [("block_w", C.c_int32), ("block_h", C.c_int32), ("thresh_rel_rho", C.c_double),
+                ("thresh_match_num", C.c_int32), ("iter_num", C.c_int32)]
+
+
+def depth_params(block_w=10, block_h=10, thresh_rel_rho=1.0, thresh_match_num=5, iter_num=10):
+    """DepthParams; the defaults are every shipped viewer configuration's (visualizer.cpp:303, ThreshRelRho=1,
+    ThreshMatchNum=5, IterNum=10)."""
+    return DepthParams(block_w, block_h, thresh_rel_rho, thresh_match_num, iter_num)
+
+
 # struct KeyLine of the reference (168 bytes) == rb_keyline
 KEYLINE = np.dtype({
     "names": ["p_inx", "m_m", "u_m", "n_m", "score", "c_p", "rho", "s_rho", "rho_nr", "s_rho_nr",
@@ -100,7 +116,7 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_undistort_create", "rb_undistort_destroy", "rb_undistort_rgb", "rb_undistort_rgb_dev",
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
            "rb_nav_format_trajectory", "rb_nav_format_log", "rb_odometry_format_pose_graph", "rb_pipeline_set_odometry",
-           "rb_pipeline_odometry"]
+           "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth"]
 
 _lib = None
 
@@ -236,6 +252,18 @@ class Ctx:
 
     def new_map(self):
         return Map(self)
+
+    def depth_fill_net(self, records, params=None):
+        """The viewer's depth grid (depth_filler, visualizer.cpp:436-440) of uint8 [n, 15] net_keyline records on this
+        context's camera: (DEPTH_CELL [gh, gw], min_dist)."""
+        params = params if params is not None else depth_params()
+        rec = np.ascontiguousarray(records, np.uint8).reshape(-1, 15)
+        gw, gh = self.w // max(params.block_w, 1), self.h // max(params.block_h, 1)
+        out = np.zeros(max(gw * gh, 1), DEPTH_CELL)
+        cw, ch, md = C.c_int(0), C.c_int(0), C.c_double(0)
+        self.check(self.L.rb_depth_fill_net(self.h_, _p(rec), len(rec), C.byref(params), _p(out), C.byref(cw), C.byref(ch),
+                                            C.byref(md)))
+        return out[:cw.value * ch.value].reshape(ch.value, cw.value), md.value
 
     def close(self):
         if self.h_:
@@ -591,6 +619,19 @@ class Pipeline:
         self.check(self.L.rb_pipeline_odometry(self.h_, C.byref(p), C.byref(n)))
         buf = (C.c_char * (n.value * ODOM.itemsize)).from_address(p.value)
         return np.frombuffer(buf, dtype=ODOM, count=n.value).copy()
+
+    def set_depth(self, params):
+        """Per-frame depth grid (the viewer's depth_filler on every frame's net_keyline records) with every push:
+        DepthParams to switch it on, None to switch it off."""
+        self.check(self.L.rb_pipeline_set_depth(self.h_, C.byref(params) if params is not None else None))
+
+    def depth(self, i):
+        """(DEPTH_CELL [gh, gw], min_dist) of frame i of the last push (a copy)."""
+        p, gw, gh, md = C.c_void_p(0), C.c_int(0), C.c_int(0), C.c_double(0)
+        self.check(self.L.rb_pipeline_depth(self.h_, i, C.byref(p), C.byref(gw), C.byref(gh), C.byref(md)))
+        n = gw.value * gh.value
+        buf = (C.c_char * (n * DEPTH_CELL.itemsize)).from_address(p.value)
+        return np.frombuffer(buf, dtype=DEPTH_CELL, count=n).reshape(gh.value, gw.value).copy(), md.value
 
     def mirror(self, i):
         """View (no copy) of the records of frame `i` of the last push: KEYLINE[n] (mode 1) or uint8[n, 15] (mode 2); valid until

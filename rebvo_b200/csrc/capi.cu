@@ -273,6 +273,7 @@ extern "C" void rb_ctx_destroy(rb_ctx *c) {
     cudaFree(c->ticket);
     cudaFree(c->dev_small);
     cudaFree(c->boxtab);
+    cudaFree(c->depth_ws);
     if (c->pinned) cudaFreeHost(c->pinned);
     delete c->mtx;
     delete c;

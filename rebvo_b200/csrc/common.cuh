@@ -117,6 +117,8 @@ struct rb_ctx {
     size_t min_cluster_dyn_multi;
     int min_debug_abort;
     bool min_early;      // set by rb_pipeline around its Minimizer_RV launch: operands may be staged before the PDL wait  // test hook (env REBVO_B200_MIN_FORCE_ABORT=1): the kernel raises its abort flag at once
+    void *depth_ws;      // rb_depth_fill_net: records, cells and bucketing scratch of the largest call so far
+    size_t depth_ws_bytes;
 };
 // layout of rb_ctx::dev_small / pinned (byte offsets)
 #define RB_DS_REEST 0        // int[2 + nbins + 1]  reEstimateThresh min/max bits + histogram

@@ -12,6 +12,7 @@
 #include "lm.cuh"
 #include "tracker.cuh"
 #include "frame.cuh"
+#include "depth.cuh"
 
 int rb_map_alloc(rb_ctx *c, rb_map **out, bool with_ws);
 
@@ -111,6 +112,22 @@ struct rb_pipeline {
     rb_odometry *odom_dev, *odom_pin;             // [max_batch]
     int odom_n;                                   // records of the last push
     double rkp_last;                              // RKp of the last frame pushed: QK of the next push's first record
+    // optional per-frame depth grid (rb_pipeline_set_depth): right after its map update each frame's net_keyline records are
+    // packed into a staging slot (tracker stream; with mirror mode 2 the mirror's slot is read instead), then one fill CTA on
+    // a side stream writes the frame's cells and min_dist into mapped pinned host memory; both are part of the captured batch.
+    // Frame i's fill runs on depth_stream[i % RB_DEPTH_STREAMS] with that stream's workspace: one fill takes longer than a
+    // tracked frame, so the fills of consecutive frames run side by side on their own SMs
+    int depth_on;
+    DepthPlan depth_plan;
+    size_t depth_rec_stride;                      // bytes per frame staging slot (kcap records, multiple of 256)
+    unsigned char *depth_stage, *depth_host;      // [max_batch * stride]: device staging, mapped pinned host cells
+    unsigned char **depth_base_dev;               // device: {staging, host} address of frame 0 of the sub-batch being processed
+    unsigned char **depth_base_pin;               // pinned: one pair per sub-batch of the current push
+    void *depth_ws;                               // per stream: bucketing scratch (and the grid when it does not fit in smem)
+    size_t depth_ws_bytes, depth_host_bytes;      // (depth_ws_bytes: per stream)
+    cudaStream_t depth_stream[RB_DEPTH_STREAMS];
+    cudaEvent_t *ev_dpack, ev_djoin[RB_DEPTH_STREAMS];
+    int depth_n;                                  // frames of the last push
 };
 
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
@@ -383,6 +400,21 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     if (pl->ev_mjoin) cudaEventDestroy(pl->ev_mjoin);
     cudaFree(pl->mirror_base_dev);
     if (pl->mirror_base_pin) cudaFreeHost(pl->mirror_base_pin);
+    for (int k = 0; k < RB_DEPTH_STREAMS; k++)
+        if (pl->depth_stream[k]) {
+            cudaStreamSynchronize(pl->depth_stream[k]);
+            cudaStreamDestroy(pl->depth_stream[k]);
+        }
+    cudaFree(pl->depth_stage);
+    if (pl->depth_host) cudaFreeHost(pl->depth_host);
+    cudaFree(pl->depth_base_dev);
+    if (pl->depth_base_pin) cudaFreeHost(pl->depth_base_pin);
+    cudaFree(pl->depth_ws);
+    for (int i = 0; i < pl->max_batch; i++)
+        if (pl->ev_dpack && pl->ev_dpack[i]) cudaEventDestroy(pl->ev_dpack[i]);
+    delete[] pl->ev_dpack;
+    for (int k = 0; k < RB_DEPTH_STREAMS; k++)
+        if (pl->ev_djoin[k]) cudaEventDestroy(pl->ev_djoin[k]);
     rb_dogws_free(&pl->ws);
     cudaFree(pl->chain);
     cudaFree(pl->fs);
@@ -617,12 +649,34 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
             k_mirror_to_host<<<8, 256, 0, pl->mirror_stream>>>(pl->mirror_base_dev, ofs, &(pl->nav_dev + i)->kn, (int)pl->mirror_rec);
             RB_LAUNCH_CHECK();
         }
+        if (pl->depth_on) {   // the viewer's depth_filler on this frame's wire records (visualizer.cpp:436-440)
+            unsigned char *const *rec_pp = pl->mirror_base_dev;
+            size_t rec_ofs = (size_t)i * pl->mirror_stride;
+            if (pl->mirror_on != 2) {   // copy_net_keyline(..., pbuf.K) of the third thread (rebvo_third_t.cpp:191)
+                rec_pp = pl->depth_base_dev;
+                rec_ofs = (size_t)i * pl->depth_rec_stride;
+                if ((r = rb_map_pack_net_enqueue(c, neu, pl->depth_base_dev, rec_ofs, &(pl->nav_dev + i)->K))) return r;
+            }
+            const int k = i % RB_DEPTH_STREAMS;
+            RB_CUDA(cudaEventRecord(pl->ev_dpack[i], main_stream));
+            RB_CUDA(cudaStreamWaitEvent(pl->depth_stream[k], pl->ev_dpack[i], 0));
+            c->stream = pl->depth_stream[k];
+            r = rb_depth_fill_enqueue(c, pl->depth_plan, rec_pp, rec_ofs, nullptr, &(pl->nav_dev + i)->kn, 0, c->kcap,
+                                      (unsigned char *)pl->depth_ws + (size_t)k * pl->depth_ws_bytes, pl->depth_base_dev,
+                                      (size_t)i * pl->depth_plan.cells_bytes, nullptr);
+            c->stream = main_stream;
+            if (r) return r;
+        }
         if (ov && i + 2 < n) RB_CUDA(cudaEventRecord(pl->ev_trk[i], main_stream));
     }
     if ((r = resc_join(pl))) return r;   // the last frame's Kp / RKp are in its record before the nav copy
     if (pl->mirror_on) {   // the batch is complete when its last map has reached the host
         RB_CUDA(cudaEventRecord(pl->ev_mjoin, pl->mirror_stream));
         RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_mjoin, 0));
+    }
+    for (int k = 0; pl->depth_on && k < RB_DEPTH_STREAMS && k < n; k++) {   // and when its last grids have
+        RB_CUDA(cudaEventRecord(pl->ev_djoin[k], pl->depth_stream[k]));
+        RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_djoin[k], 0));
     }
     return RB_OK;
 }
@@ -638,6 +692,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     RB_CUDA(cudaSetDevice(c->device));
     int r;
     pl->odom_n = 0;
+    pl->depth_n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
         if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom_on ? pl->odom_pin : nullptr)))
             return r;
@@ -692,6 +747,12 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
             pl->mirror_base_pin[2 * j] = pl->mirror_dev + (size_t)off * pl->mirror_stride;
             pl->mirror_base_pin[2 * j + 1] = pl->mirror_host + (size_t)off * pl->mirror_stride;
             RB_CUDA(cudaMemcpyAsync(pl->mirror_base_dev, pl->mirror_base_pin + 2 * j, 2 * sizeof(void *), cudaMemcpyHostToDevice,
+                                    c->stream));
+        }
+        if (pl->depth_on) {
+            pl->depth_base_pin[2 * j] = pl->depth_stage + (size_t)off * pl->depth_rec_stride;
+            pl->depth_base_pin[2 * j + 1] = pl->depth_host + (size_t)off * pl->depth_plan.cells_bytes;
+            RB_CUDA(cudaMemcpyAsync(pl->depth_base_dev, pl->depth_base_pin + 2 * j, 2 * sizeof(void *), cudaMemcpyHostToDevice,
                                     c->stream));
         }
         const bool graph_ok = pl->use_graph && first_j > 0;
@@ -757,6 +818,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     }
     if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
     pl->mirror_n = pl->mirror_on ? n : 0;
+    pl->depth_n = pl->depth_on ? n : 0;
     // QK of a record: P_Kp as the frame found it = RKp of the previous frame's record, which holds the value after that frame's
     // rescaling also when the rescaling ran on the side stream (:382, :480-487)
     for (int i = 0; i < n && pl->odom_on; i++) {
@@ -842,6 +904,79 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     pl->mirror_rec = on == 2 ? 15 : sizeof(rb_keyline);
     pl->mirror_stride = stride;
     pl->mirror_n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    RB_CUDA(cudaSetDevice(c->device));
+    if (pl->imu) {
+        snprintf(c->err, sizeof(c->err), "set_depth: not available in IMU mode");
+        return RB_ERR_ARG;
+    }
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    if (!p) {
+        if (pl->depth_on) drop_graphs(pl);   // the captured batches contain the pack and fill kernels
+        pl->depth_on = 0;
+        pl->depth_n = 0;
+        return RB_OK;
+    }
+    DepthPlan plan;
+    int r = rb_depth_plan(c, p, &plan);
+    if (r) {
+        snprintf(c->err, sizeof(c->err), "set_depth: invalid parameters");
+        return r;
+    }
+    if (!pl->depth_stage) {
+        pl->depth_rec_stride = ((size_t)c->kcap * 15 + 255) & ~(size_t)255;
+        RB_CUDA(cudaMalloc(&pl->depth_stage, (size_t)pl->max_batch * pl->depth_rec_stride));
+        RB_CUDA(cudaMalloc(&pl->depth_base_dev, 2 * sizeof(void *)));
+        RB_CUDA(cudaMallocHost(&pl->depth_base_pin, 8 * sizeof(void *)));
+        // lowest priority: a fill CTA may hold a whole SM's shared memory, which the tracker's kernels get first
+        // (env REBVO_B200_DEPTH_PRIO=1: the tracker's own priority, for tools/bench_depth.py's comparison)
+        int lo = 0, hi = 0;
+        RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+        const char *dp = getenv("REBVO_B200_DEPTH_PRIO");
+        for (int k = 0; k < RB_DEPTH_STREAMS; k++) {
+            RB_CUDA(cudaStreamCreateWithPriority(&pl->depth_stream[k], cudaStreamNonBlocking, (dp && atoi(dp) == 1) ? hi : lo));
+            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_djoin[k], cudaEventDisableTiming));
+        }
+        pl->ev_dpack = new (std::nothrow) cudaEvent_t[pl->max_batch];
+        if (!pl->ev_dpack) return RB_ERR_ARG;
+        memset(pl->ev_dpack, 0, sizeof(cudaEvent_t) * pl->max_batch);
+        for (int i = 0; i < pl->max_batch; i++) RB_CUDA(cudaEventCreateWithFlags(&pl->ev_dpack[i], cudaEventDisableTiming));
+    }
+    const size_t host_bytes = (size_t)pl->max_batch * plan.cells_bytes, ws_bytes = rb_depth_ws_bytes(plan, c->kcap);
+    if (host_bytes > pl->depth_host_bytes) {
+        if (pl->depth_host) cudaFreeHost(pl->depth_host);
+        pl->depth_host = nullptr;
+        pl->depth_host_bytes = 0;
+        RB_CUDA(cudaHostAlloc(&pl->depth_host, host_bytes, cudaHostAllocMapped));
+        pl->depth_host_bytes = host_bytes;
+    }
+    if (ws_bytes > pl->depth_ws_bytes) {
+        cudaFree(pl->depth_ws);
+        pl->depth_ws = nullptr;
+        pl->depth_ws_bytes = 0;
+        RB_CUDA(cudaMalloc(&pl->depth_ws, ws_bytes * RB_DEPTH_STREAMS));
+        pl->depth_ws_bytes = ws_bytes;
+    }
+    drop_graphs(pl);   // the captured batches hold the fill's geometry
+    pl->depth_plan = plan;
+    pl->depth_on = 1;
+    pl->depth_n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
+    if (!pl || !pl->depth_on || !cells) return RB_ERR_ARG;
+    if (i < 0 || i >= pl->depth_n) return RB_ERR_ARG;
+    const unsigned char *slot = pl->depth_host + (size_t)i * pl->depth_plan.cells_bytes;
+    const size_t ncell = (size_t)pl->depth_plan.g.gw * pl->depth_plan.g.gh;
+    *cells = reinterpret_cast<const rb_depth_cell *>(slot);
+    if (gw) *gw = pl->depth_plan.g.gw;
+    if (gh) *gh = pl->depth_plan.g.gh;
+    if (min_dist) *min_dist = *reinterpret_cast<const double *>(slot + ncell * sizeof(rb_depth_cell));
     return RB_OK;
 }
 extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
