@@ -505,27 +505,35 @@ struct ResPtrs {
 struct Red28Smem {
     double part[TVR_T / 32][32];
 };
+// p ? a : b on values, never on addresses.  The butterfly used to pick `up ? v[k + o] : v[k]` in a loop over o >>= 1
+// that was not unrolled; the array (and the caller's acc) then lived in local memory, an L1 round trip per level.  Now
+// every index is a compile-time constant (one template per level, one array per level) and the choice is a selp.
+__device__ __forceinline__ double sel_f64(bool p, double a, double b) {
+    double r;
+    asm("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %1, 0;\n\tselp.f64 %0, %2, %3, q;\n\t}" : "=d"(r) : "r"((unsigned int)p), "d"(a), "d"(b));
+    return r;
+}
+// one butterfly level at distance O: lane keeps the upper or lower half of its 2*O values and trades the other half
+template <int O>
+__device__ __forceinline__ void transpose_level(const double (&in)[2 * O], double (&out)[O], int lane) {
+    const bool up = (lane & O) != 0;
+#pragma unroll
+    for (int k = 0; k < O; k++) {
+        const double lo = in[k], hi = in[k + O];
+        const double keep = sel_f64(up, hi, lo), send = sel_f64(up, lo, hi);
+        out[k] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+    }
+}
 __device__ __forceinline__ double warp_transpose_sum28(const double (&acc)[28], int lane) {
-    double v[16];
-    {
-        const bool up = (lane & 16) != 0;
+    double v32[32], v16[16], v8[8], v4[4], v2[2], v1[1];
 #pragma unroll
-        for (int k = 0; k < 16; k++) {
-            const double hi = (k + 16 < 28) ? acc[k + 16] : 0.0;
-            const double keep = up ? hi : acc[k], send = up ? acc[k] : hi;
-            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-        }
-    }
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) {
-        const bool up = (lane & o) != 0;
-#pragma unroll
-        for (int k = 0; k < o; k++) {
-            const double keep = up ? v[k + o] : v[k], send = up ? v[k] : v[k + o];
-            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-        }
-    }
-    return v[0];
+    for (int k = 0; k < 32; k++) v32[k] = k < 28 ? acc[k] : 0.0;
+    transpose_level<16>(v32, v16, lane);
+    transpose_level<8>(v16, v8, lane);
+    transpose_level<4>(v8, v4, lane);
+    transpose_level<2>(v4, v2, lane);
+    transpose_level<1>(v2, v1, lane);
+    return v1[0];
 }
 template <bool PJ>
 __device__ __forceinline__ void reduce28(const double (&acc)[28], Red28Smem &rs, int tid, int lane, int wid,
