@@ -388,6 +388,30 @@ typedef struct rb_imu_params {
     double Rc2i[9], Tc2i[3];
 } rb_imu_params;
 int rb_pipeline_set_imu(rb_pipeline *pl, const rb_imu_params *ip, const double *samples, int n);
+/* Live IMU input (REBVOParameters ImuMode = 1: ImuGrabber(CircBufferSize, SampleTime), imugrabber.cpp:34-40, fed by
+ * REBVO::pushIMU).  Switches the pipeline to IMU mode, like rb_pipeline_set_imu, with an empty ring of buffer_size samples
+ * (CircBufferSize; buffer_size + 1 slots) whose integration step is sample_time (SampleTime) instead of the mean sample spacing.
+ * Each call replaces the IMU setup of an earlier rb_pipeline_set_imu or rb_pipeline_set_imu_live.  RB_ERR_ARG for
+ * sample_time <= 0 and buffer_size < 1.
+ *
+ * rb_pipeline_push_imu appends n rows {t [s], gyro xyz [rad/s], accel xyz [m/s^2]} in time order (PushData,
+ * imugrabber.cpp:258-269), all of them or none:
+ *   RB_ERR_STATE  the ring cannot hold all n (a grabbed frame releases the samples before its last one); none is stored.
+ *                 Deviation: the reference stores the samples that fit and throws overflow_error at the first that does not.
+ *   RB_ERR_ARG    not in live IMU mode (off, or dataset mode), or a timestamp older than the one before it (this push's or the
+ *                 last one stored).
+ *
+ * A push of frames in live mode first checks, for every frame, that the ring covers (t_prev + TimeDesinc, t + TimeDesinc]:
+ * at least one sample after the window's start and one at or past its end.  If any frame is not covered, the push returns
+ * RB_ERR_STATE before it enqueues anything and leaves the ring, the filter, the maps and the frame count as they were; push
+ * the missing samples and repeat the push.  (The reference's FirstThr sleeps SampleTime and grabs again,
+ * rebvo_first_t.cpp:293-302; its failed GrabAndIntegrate also releases the samples before the window, this check releases
+ * none.)  The records are those of dataset mode with the same samples and the same integration step: rb_pipeline_set_imu on
+ * the same samples gives the same bytes when sample_time is their mean spacing.  rb_pipeline_reset resets the filter and
+ * keeps the ring: the samples it has not released and its read position.  Mono8 and device input and the odometry records
+ * work as in dataset mode; the mirror and the depth grid are not available in IMU mode. */
+int rb_pipeline_set_imu_live(rb_pipeline *pl, const rb_imu_params *ip, double sample_time, int buffer_size);
+int rb_pipeline_push_imu(rb_pipeline *pl, const double *samples, int n);
 
 #ifdef __cplusplus
 }

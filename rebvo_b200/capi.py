@@ -111,7 +111,7 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_push_mono_dev", "rb_pipeline_reset",
            "rb_pipeline_map", "rb_pipeline_launch_count", "rb_pipeline_stage_ms", "rb_pipeline_stream",
            "rb_pipeline_event_record", "rb_pipeline_event_elapsed", "rb_pipeline_event_elapsed_between", "rb_pipeline_bench_pass",
-           "rb_pipeline_set_imu", "rb_pipeline_set_mirror", "rb_pipeline_mirror", "rb_pipeline_set_undistort",
+           "rb_pipeline_set_imu", "rb_pipeline_set_imu_live", "rb_pipeline_push_imu", "rb_pipeline_set_mirror", "rb_pipeline_mirror", "rb_pipeline_set_undistort",
            "rb_pipeline_stage_profile",
            "rb_undistort_create", "rb_undistort_destroy", "rb_undistort_rgb", "rb_undistort_rgb_dev",
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
@@ -546,6 +546,19 @@ class Pipeline:
         samples = np.ascontiguousarray(samples, np.float64)
         ip = imu_params if imu_params is not None else default_imu_params()
         self.check(self.L.rb_pipeline_set_imu(self.h_, C.byref(ip), _p(samples), len(samples)))
+
+    def set_imu_live(self, imu_params=None, sample_time=0.005, buffer_size=1000):
+        """Live IMU mode (ImuMode=1): an empty ring of `buffer_size` samples (CircBufferSize) integrated with the step
+        `sample_time` (SampleTime), fed by push_imu.  The defaults are those of the reference's EuRoC ROS configuration."""
+        ip = imu_params if imu_params is not None else default_imu_params()
+        self.check(self.L.rb_pipeline_set_imu_live(self.h_, C.byref(ip), C.c_double(sample_time), int(buffer_size)))
+
+    def push_imu(self, samples):
+        """Append float64 [n, 7] rows {t, gyro xyz, accel xyz} in time order, all or none.  RbError when the ring cannot hold
+        them (push frames first), outside live IMU mode, or when a timestamp goes backwards.  A frame push that the samples do
+        not cover raises RbError and changes nothing: push the missing samples and repeat it."""
+        samples = np.ascontiguousarray(samples, np.float64).reshape(-1, 7)
+        self.check(self.L.rb_pipeline_push_imu(self.h_, _p(samples), len(samples)))
 
     def push_dev(self, dev_ptr, ts):
         ts = np.ascontiguousarray(ts, np.float64)

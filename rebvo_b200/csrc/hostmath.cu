@@ -69,4 +69,54 @@ int rb_hostmath_imu_integrate(const double *samples, int n, const double *ts, in
     }
     return 0;
 }
+// ImuGrabber live mode: the ring of rb_pipeline_set_imu_live (list_size samples, integration step tsample)
+struct HostImuRing {
+    std::vector<rbimu::ImuSample> slots;
+    rbimu::ImuBuffer b;
+};
+void *rb_hostmath_imu_ring_new(int list_size, double tsample) {
+    HostImuRing *r = new HostImuRing;
+    r->slots.resize((size_t)list_size + 1);
+    r->b.init_live(r->slots.data(), list_size, tsample, nullptr, nullptr);
+    return r;
+}
+void rb_hostmath_imu_ring_free(void *r) { delete (HostImuRing *)r; }
+// n rows {t, gyro, accel}: 1 when stored, 0 (nothing stored) when they do not fit
+int rb_hostmath_imu_ring_push(void *r, const double *rows, int n) {
+    std::vector<rbimu::ImuSample> s(n);
+    for (int i = 0; i < n; i++) {
+        s[i].t = rows[i * 7];
+        for (int k = 0; k < 3; k++) {
+            s[i].giro[k] = rows[i * 7 + 1 + k];
+            s[i].acel[k] = rows[i * 7 + 4 + k];
+        }
+    }
+    return ((HostImuRing *)r)->b.push(s.data(), n) ? 1 : 0;
+}
+// whether grab(tstart, tend) finds samples, without changing the ring (the check of a live-mode frame push)
+int rb_hostmath_imu_ring_covers(void *r, double tstart, double tend) {
+    rbimu::ImuBuffer probe = ((HostImuRing *)r)->b;
+    return probe.release(tstart, tend) ? 1 : 0;
+}
+// out: 20 doubles as rb_hostmath_imu_integrate's, plus dgiro[3] at 20..22
+void rb_hostmath_imu_ring_grab(void *r, double tstart, double tend, double *out) {
+    const rbimu::ImuIntegral d = ((HostImuRing *)r)->b.grab(tstart, tend);
+    out[0] = d.n;
+    out[1] = d.dt;
+    for (int k = 0; k < 9; k++) out[2 + k] = d.Rot[k];
+    for (int k = 0; k < 3; k++) {
+        out[11 + k] = d.giro[k];
+        out[14 + k] = d.acel[k];
+        out[17 + k] = d.cacel[k];
+        out[20 + k] = d.dgiro[k];
+    }
+}
+// {write_inx, read_inx, size, free slots}
+void rb_hostmath_imu_ring_state(const void *r, int *out) {
+    const rbimu::ImuBuffer &b = ((const HostImuRing *)r)->b;
+    out[0] = b.write_inx;
+    out[1] = b.read_inx;
+    out[2] = b.size;
+    out[3] = b.free_slots();
+}
 }

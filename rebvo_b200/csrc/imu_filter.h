@@ -156,7 +156,7 @@ inline void so3_from_two(const double *a, const double *b, double *R) {
     matmul(RbT, Ra, R, 3, 3, 3);
 }
 
-// ---- ImuGrabber (dataset mode) ----------------------------------------------------------------------------------------------
+// ---- ImuGrabber (dataset mode, ImuMode=2, and live mode, ImuMode=1) ---------------------------------------------------------
 struct ImuSample {
     double t, giro[3], acel[3];
 };
@@ -164,19 +164,52 @@ struct ImuIntegral {   // IntegratedImuData (include/UtilLib/imugrabber.h:56-67)
     int n;
     double dt, Rot[9], giro[3], acel[3], dgiro[3], cacel[3];
 };
-struct ImuBuffer {      // circular list of size n + 1 like ImuGrabber(const std::vector<ImuData>&) (imugrabber.cpp:47-68)
+// The circular list of ImuGrabber.  Both forms have one slot more than they can hold and share search / grab; they differ
+// only in who owns the samples and where writing starts:
+//   dataset  ImuGrabber(const std::vector<ImuData>&) (imugrabber.cpp:47-68): the caller's count samples, already written,
+//            tsample = their mean spacing
+//   live     ImuGrabber(list_size, tsamp) (imugrabber.cpp:34-40): list_size + 1 slots of the caller's, empty, filled by push
+//            (PushData); tsample = the configured SampleTime
+struct ImuBuffer {
     const ImuSample *s;
+    ImuSample *ring;   // live form: the writable slots (== s); nullptr in the dataset form
     int n, size, write_inx, read_inx;
     double tsample, Rc2i[9], Tc2i[3];
     void init(const ImuSample *samples, int count, const double *R, const double *T) {
         s = samples;
+        ring = nullptr;
         n = count;
         size = count + 1;
         write_inx = count % size;
         read_inx = size - 1;
         tsample = count > 1 ? (samples[count - 1].t - samples[0].t) / (count - 1) : 0;
+        set_se3(R, T);
+    }
+    void init_live(ImuSample *slots, int list_size, double tsamp, const double *R, const double *T) {
+        s = ring = slots;
+        n = 0;
+        size = list_size + 1;
+        write_inx = 0;
+        read_inx = size - 1;
+        tsample = tsamp;
+        set_se3(R, T);
+    }
+    void set_se3(const double *R, const double *T) {
         for (int i = 0; i < 9; i++) Rc2i[i] = R ? R[i] : (i % 4 == 0 ? 1.0 : 0.0);
         for (int i = 0; i < 3; i++) Tc2i[i] = T ? T[i] : 0.0;
+    }
+    // slots PushData can still fill before it meets read_inx (the slot of the last sample grabbed stays taken)
+    int free_slots() const { return (read_inx - write_inx + size) % size; }
+    // PushData (imugrabber.cpp:258-269) of count samples: all of them, or none when they do not fit (the reference stores
+    // the samples that fit and throws overflow_error at the first one that does not)
+    bool push(const ImuSample *in, int count) {
+        if (!ring || count > free_slots()) return false;
+        for (int i = 0; i < count; i++) {
+            ring[write_inx] = in[i];
+            write_inx = (write_inx + 1) % size;
+        }
+        n += count;
+        return true;
     }
     // SeachByTimeStamp (imugrabber.cpp:171-210): [begin, end) of the samples with tstart < t <= tend
     bool search(double tstart, double tend, int *begin, int *end) const {
@@ -193,6 +226,13 @@ struct ImuBuffer {      // circular list of size n + 1 like ImuGrabber(const std
         if (s[inx].t - tend < 1e-12) inx = (inx + 1) % size;
         *begin = b;
         *end = inx;
+        return true;
+    }
+    // the read position grab(tstart, tend) leaves, without the integration; false (and no change) where grab finds no sample
+    bool release(double tstart, double tend) {
+        int b = 0, e = 0;
+        if (!search(tstart, tend, &b, &e)) return false;
+        read_inx = (e - 1 + size) % size;
         return true;
     }
     // GrabAndIntegrate (imugrabber.cpp:217-253)

@@ -12,10 +12,12 @@
 
 struct ImuFlow {
     rb_imu_params ip;
-    std::vector<rbimu::ImuSample> samples;
+    std::vector<rbimu::ImuSample> samples;   // dataset mode: every sample; live mode: the ring's slots
     rbimu::ImuBuffer buf;
     rbimu::ImuFilterHist hist;
     bool enabled;
+    bool live;            // ImuMode=1 (rb_pipeline_set_imu_live): samples arrive through rb_pipeline_push_imu
+    double t_last;        // live mode: timestamp of the last sample pushed (-inf before the first)
     // SecondThread locals (:57-90)
     double V[3], W[3], Pos[3], R[9], Pose[9], Rgva[9], P_V[9], P_W[9];
     double K, Kp, P_Kp;
@@ -29,6 +31,17 @@ struct ImuFlow {
     int n_giro_init;
     double giro_init[3], g_init[3];
 };
+
+// n rows {t, gyro xyz, accel xyz} of the C interface -> samples
+static void imu_rows(const double *rows, int n, rbimu::ImuSample *out) {
+    for (int i = 0; i < n; i++) {
+        out[i].t = rows[i * 7];
+        for (int k = 0; k < 3; k++) {
+            out[i].giro[k] = rows[i * 7 + 1 + k];
+            out[i].acel[k] = rows[i * 7 + 4 + k];
+        }
+    }
+}
 
 static void imu_eye(double *M, double v) {
     for (int i = 0; i < 9; i++) M[i] = (i % 4 == 0) ? v : 0.0;
@@ -72,7 +85,9 @@ static void imu_flow_reset(ImuFlow &f) {
     for (int i = 0; i < 3; i++) f.g_est[i] = f.b_est[i] = f.giro_init[i] = f.g_init[i] = 0;
     f.init = false;
     f.n_giro_init = 0;
-    if (!f.samples.empty()) f.buf.init(f.samples.data(), (int)f.samples.size(), p.use_se3 ? p.Rc2i : nullptr, p.use_se3 ? p.Tc2i : nullptr);
+    // (live mode: the ring keeps the samples it has not released and its read position, so the next frame still finds them)
+    if (!f.live && !f.samples.empty())
+        f.buf.init(f.samples.data(), (int)f.samples.size(), p.use_se3 ? p.Rc2i : nullptr, p.use_se3 ? p.Tc2i : nullptr);
 }
 
 // one tracked frame: new = maps[fr % 3] (detected), old = maps[(fr-1) % 3]; returns the nav record and, with odom, the
@@ -284,6 +299,25 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
     o.retuned_thresh = ns.retuned;
     *nav = o;
     f.n_frame++;
+    return RB_OK;
+}
+
+// live mode, before a push enqueues anything: every frame's window (t_prev + TimeDesinc, t + TimeDesinc] must hold a sample
+// and end at or before the newest sample, replayed on a copy of the ring.  Where the reference's FirstThr sleeps and grabs again
+// (rebvo_first_t.cpp:293-302), the push fails with RB_ERR_STATE and changes nothing; the caller pushes more samples and repeats
+// it.  (The reference's failed GrabAndIntegrate also releases the samples before the window; this one releases none.)
+static int imu_live_check(rb_pipeline *pl, const ImuFlow &f, const double *ts, int n) {
+    rbimu::ImuBuffer probe = f.buf;
+    double t0 = f.t_prev_grab;
+    for (int i = 0; i < n; i++) {
+        if (!probe.release(t0 + f.ip.TimeDesinc, ts[i] + f.ip.TimeDesinc)) {
+            snprintf(pl->c->err, sizeof(pl->c->err),
+                     "IMU live mode: the samples pushed do not cover frame %d of the push (t=%.6f): push more samples and "
+                     "push the frames again", i, ts[i]);
+            return RB_ERR_STATE;
+        }
+        t0 = ts[i];
+    }
     return RB_OK;
 }
 

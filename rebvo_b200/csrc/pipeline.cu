@@ -4,6 +4,7 @@
 // The host only enqueues kernels: threshold feedback, LM driver, NaN / match-count decisions, pose
 // integration and the NavData record are all computed by 1-thread kernels from device state, so a batch of
 // frames costs one H2D copy, one stream of launches and one D2H copy of the nav records.
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <new>
@@ -44,7 +45,7 @@ extern "C" int rb_debug_fetch_trace(unsigned long long *out, unsigned int *n) {
 struct ImuFlow;
 struct rb_pipeline {
     rb_ctx *c;
-    ImuFlow *imu;         // IMU mode (rb_pipeline_set_imu), nullptr otherwise
+    ImuFlow *imu;         // IMU mode (rb_pipeline_set_imu, rb_pipeline_set_imu_live), nullptr otherwise
     rb_params p;
     int max_batch;
     DogWS ws;
@@ -345,15 +346,63 @@ extern "C" int rb_pipeline_set_imu(rb_pipeline *pl, const rb_imu_params *ip, con
     ImuFlow &f = *pl->imu;
     f.ip = *ip;
     f.samples.resize(n);
-    for (int i = 0; i < n; i++) {
-        f.samples[i].t = samples[i * 7];
-        for (int k = 0; k < 3; k++) {
-            f.samples[i].giro[k] = samples[i * 7 + 1 + k];
-            f.samples[i].acel[k] = samples[i * 7 + 4 + k];
-        }
-    }
+    imu_rows(samples, n, f.samples.data());
     f.enabled = true;
+    f.live = false;
     imu_flow_reset(f);
+    return RB_OK;
+}
+
+extern "C" int rb_pipeline_set_imu_live(rb_pipeline *pl, const rb_imu_params *ip, double sample_time, int buffer_size) {
+    if (!pl || !ip || !(sample_time > 0) || buffer_size < 1 || buffer_size == INT_MAX) return RB_ERR_ARG;
+    std::vector<rbimu::ImuSample> slots;
+    try {
+        slots.resize((size_t)buffer_size + 1);
+    } catch (const std::bad_alloc &) {
+        snprintf(pl->c->err, sizeof(pl->c->err), "set_imu_live: no host memory for %d samples", buffer_size);
+        return RB_ERR_ARG;
+    }
+    if (!pl->imu) pl->imu = new (std::nothrow) ImuFlow();
+    if (!pl->imu) return RB_ERR_ARG;
+    ImuFlow &f = *pl->imu;
+    f.samples.swap(slots);
+    f.ip = *ip;
+    f.enabled = true;
+    f.live = true;
+    f.t_last = -INFINITY;
+    f.buf.init_live(f.samples.data(), buffer_size, sample_time, ip->use_se3 ? ip->Rc2i : nullptr,
+                    ip->use_se3 ? ip->Tc2i : nullptr);
+    imu_flow_reset(f);
+    return RB_OK;
+}
+
+extern "C" int rb_pipeline_push_imu(rb_pipeline *pl, const double *samples, int n) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    if (!pl->imu || !pl->imu->live) {
+        snprintf(c->err, sizeof(c->err), "push_imu: the pipeline is not in live IMU mode (rb_pipeline_set_imu_live)");
+        return RB_ERR_ARG;
+    }
+    if (n < 0 || (n > 0 && !samples)) return RB_ERR_ARG;
+    ImuFlow &f = *pl->imu;
+    double t = f.t_last;
+    for (int i = 0; i < n; i++) {
+        if (!(samples[i * 7] >= t)) {   // (and NaN)
+            snprintf(c->err, sizeof(c->err), "push_imu: sample %d at t=%.9f is older than the one before it (t=%.9f)", i,
+                     samples[i * 7], t);
+            return RB_ERR_ARG;
+        }
+        t = samples[i * 7];
+    }
+    if (n > f.buf.free_slots()) {
+        snprintf(c->err, sizeof(c->err), "push_imu: %d samples do not fit in the ring (%d free slots): push frames to release "
+                 "samples, then push these again", n, f.buf.free_slots());
+        return RB_ERR_STATE;
+    }
+    std::vector<rbimu::ImuSample> rows(n);
+    imu_rows(samples, n, rows.data());
+    f.buf.push(rows.data(), n);
+    if (n > 0) f.t_last = t;
     return RB_OK;
 }
 
@@ -689,8 +738,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     if (n < 1 || n > pl->max_batch || !rgb || !ts) return RB_ERR_ARG;
     // (the mono kernels read the frames as 32-bit words; the RGB kernels have a byte-wise path for unaligned buffers)
     if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
-    RB_CUDA(cudaSetDevice(c->device));
     int r;
+    if (pl->imu && pl->imu->live && (r = imu_live_check(pl, *pl->imu, ts, n))) return r;
+    RB_CUDA(cudaSetDevice(c->device));
     pl->odom_n = 0;
     pl->depth_n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
