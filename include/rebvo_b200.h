@@ -373,6 +373,33 @@ int rb_depth_fill_net(rb_ctx *c, const void *records, int n, const rb_depth_para
 int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p);
 int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist);
 
+/* Dense inverse-depth image of a depth grid: pixel (x, y) of the w x h frame (x = 0..w-1, y = 0..h-1) holds
+ * depth_filler::getImgRho((float)x, (float)y, &s_rho) (include/visualizer/depth_filler.h:246-280) on the grid the same cells
+ * and rb_depth_params give, i.e. the reference's expressions in its order, without contraction:
+ *   x_histo = x / (float)block_w - 0.5    the quotient in float, the subtraction in double, stored as float (y likewise)
+ *   xf, xc = floor, ceil of x_histo, clamped to [0, gw - 1]   (yf, yc to [0, gh - 1])
+ *   dx = x_histo - xf                     in float (dy likewise)
+ *   r00, r10, r01, r11 = the rho of cells (xf, yf), (xc, yf), (xf, yc), (xc, yc), cast to float
+ *   rho = r00*(1-dx)*(1-dy) + r10*dx*(1-dy) + r01*(1-dx)*dy + r11*dx*dy   left to right in float
+ * and s_rho the same expression on the cells' s_rho.  The reference returns that float widened to double, so the float32
+ * planes hold it exactly.  The clamps are part of the definition: pixels left of or above the first cell centre
+ * (x < block_w / 2) take a negative dx (dy), and pixels past gw * block_w (gh * block_h), when the frame is not a multiple of
+ * the block, are clamped onto the last cell column (row), where dx (dy) may exceed 1.
+ *
+ * rb_depth_image: the planes of host cells (as rb_depth_fill_net / rb_pipeline_depth return them) on the context's camera;
+ * rho and s_rho receive w * h floats, row-major; s_rho may be NULL.  RB_ERR_ARG when gw / gh are not the grid size of p on
+ * this camera, and for the p rb_depth_fill_net rejects. */
+int rb_depth_image(rb_ctx *c, const rb_depth_cell *cells, int gw, int gh, const rb_depth_params *p, float *rho, float *s_rho);
+/* Per-frame images in the pipeline: mode 1 the rho plane, 2 the rho and s_rho planes, 0 off.  While the depth grid is on
+ * (rb_pipeline_set_depth), every pushed frame also gets its image: the pass runs on the frame's depth side stream right
+ * after its fill and writes straight into mapped pinned host memory; the batch's depth joins cover it.  May be called
+ * before or after rb_pipeline_set_depth.  Changing the mode drops the captured batches, like set_mirror / set_depth; mode 0
+ * gives the batches of a pipeline that never had it.  RB_ERR_ARG in IMU mode and for a mode outside 0..2.
+ * rb_pipeline_depth_image(i): the planes of frame i of the last push (row-major w x h floats, no padding; *s_rho is NULL in
+ * mode 1), valid until the next push; RB_ERR_ARG when the last push made no image or i is out of range. */
+int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode);
+int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho);
+
 /* IMU fusion (BASELINE configs[2], REBVOParameters ImuMode = 2: samples from a dataset file).  After this call every push runs
  * the IMU branch of REBVO::SecondThread (rebvo_second_t.cpp:182-336: gyro pre-rotation, Minimizer_V, ExtRotVel, BiasCorrect,
  * scale / gravity / bias filter of scaleestimator.cpp, filtered pose of :521-551) instead of Minimizer_RV.  samples: n rows

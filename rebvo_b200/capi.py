@@ -116,7 +116,8 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_undistort_create", "rb_undistort_destroy", "rb_undistort_rgb", "rb_undistort_rgb_dev",
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
            "rb_nav_format_trajectory", "rb_nav_format_log", "rb_odometry_format_pose_graph", "rb_pipeline_set_odometry",
-           "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth"]
+           "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth", "rb_depth_image",
+           "rb_pipeline_set_depth_image", "rb_pipeline_depth_image"]
 
 _lib = None
 
@@ -264,6 +265,19 @@ class Ctx:
         self.check(self.L.rb_depth_fill_net(self.h_, _p(rec), len(rec), C.byref(params), _p(out), C.byref(cw), C.byref(ch),
                                             C.byref(md)))
         return out[:cw.value * ch.value].reshape(ch.value, cw.value), md.value
+
+    def depth_image(self, cells, params=None, s_rho=True):
+        """The dense inverse-depth image of a grid (DEPTH_CELL [gh, gw], as depth_fill_net returns it): depth_filler::getImgRho
+        at every pixel of this context's frame.  (rho, s_rho or None) as float32 [h, w] arrays."""
+        params = params if params is not None else depth_params()
+        cells = np.ascontiguousarray(cells, DEPTH_CELL)
+        if cells.ndim != 2:
+            raise ValueError("cells: a [gh, gw] grid")
+        rho = np.zeros((self.h, self.w), np.float32)
+        srho = np.zeros((self.h, self.w), np.float32) if s_rho else None
+        self.check(self.L.rb_depth_image(self.h_, _p(cells), cells.shape[1], cells.shape[0], C.byref(params), _p(rho),
+                                         _p(srho) if s_rho else None))
+        return rho, srho
 
     def close(self):
         if self.h_:
@@ -645,6 +659,22 @@ class Pipeline:
         n = gw.value * gh.value
         buf = (C.c_char * (n * DEPTH_CELL.itemsize)).from_address(p.value)
         return np.frombuffer(buf, dtype=DEPTH_CELL, count=n).reshape(gh.value, gw.value).copy(), md.value
+
+    def set_depth_image(self, mode):
+        """Per-frame dense inverse-depth image of the depth grid (depth_filler::getImgRho at every pixel) with every push
+        while the grid is on: 1 = the rho plane, 2 = the rho and s_rho planes, 0 = off."""
+        self.check(self.L.rb_pipeline_set_depth_image(self.h_, int(mode)))
+
+    def depth_image(self, i):
+        """Views (no copy) of the image of frame i of the last push: (rho, s_rho or None) as float32 [h, w]; valid until the
+        next push."""
+        r, s = C.c_void_p(0), C.c_void_p(0)
+        self.check(self.L.rb_pipeline_depth_image(self.h_, i, C.byref(r), C.byref(s)))
+        n = self.w * self.h
+
+        def view(p):
+            return np.frombuffer((C.c_char * (4 * n)).from_address(p), dtype=np.float32).reshape(self.h, self.w)
+        return view(r.value), (view(s.value) if s.value else None)
 
     def mirror(self, i):
         """View (no copy) of the records of frame `i` of the last push: KEYLINE[n] (mode 1) or uint8[n, 15] (mode 2); valid until

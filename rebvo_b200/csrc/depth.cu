@@ -88,7 +88,7 @@ __device__ void sort_list(unsigned long long *a, int n) {
 __global__ void __launch_bounds__(RB_DEPTH_THREADS, 1)
     k_depth_fill(const unsigned char *const *rec_pp, size_t rec_ofs, const unsigned char *rec_direct, const int *kn_p,
                  int kn_direct, int kcap, DepthGeom g, int *cnt, unsigned long long *list, unsigned char *gwork,
-                 unsigned char *const *out_pp, size_t out_ofs, rb_depth_cell *out_direct) {
+                 unsigned char *const *out_pp, size_t out_ofs, rb_depth_cell *out_direct, double2 *grid_out) {
     extern __shared__ __align__(16) unsigned char dsm[];
     __shared__ int s_part[32];
     __shared__ double s_min[32];
@@ -288,6 +288,7 @@ __global__ void __launch_bounds__(RB_DEPTH_THREADS, 1)
         o.fixed = (int)DF_FIXED(c);
         o._pad = 0;
         out[c] = o;
+        if (grid_out) grid_out[c] = make_double2(r, o.s_rho);   // for the image pass (k_depth_image) on the same stream
     }
 #undef DF_FIXED
     for (int o = 16; o > 0; o >>= 1) {
@@ -347,22 +348,141 @@ int rb_depth_plan(rb_ctx *c, const rb_depth_params *p, DepthPlan *out) {
     return RB_OK;
 }
 
-// [cnt: ncell ints][list: kcap records][grid, when not in shared memory]
+// [cnt: ncell ints][list: kcap records][grid, when not in shared memory][final (rho, s_rho) per cell, for the image pass]
 static size_t ws_cnt_bytes(const DepthPlan &pl) { return (((size_t)pl.g.gw * pl.g.gh) * sizeof(int) + 255) & ~(size_t)255; }
 static size_t ws_list_bytes(int kcap) { return ((size_t)(kcap > 0 ? kcap : 1) * 8 + 255) & ~(size_t)255; }
+static size_t ws_grid_bytes(const DepthPlan &pl) { return (pl.g.in_smem ? 0 : (pl.grid_bytes + 255) & ~(size_t)255); }
 size_t rb_depth_ws_bytes(const DepthPlan &pl, int kcap) {
-    return ws_cnt_bytes(pl) + ws_list_bytes(kcap) + (pl.g.in_smem ? 0 : pl.grid_bytes);
+    return ws_cnt_bytes(pl) + ws_list_bytes(kcap) + ws_grid_bytes(pl) + (((size_t)pl.g.gw * pl.g.gh * 16 + 255) & ~(size_t)255);
+}
+double2 *rb_depth_ws_final(const DepthPlan &pl, int kcap, void *ws) {
+    return (double2 *)((unsigned char *)ws + ws_cnt_bytes(pl) + ws_list_bytes(kcap) + ws_grid_bytes(pl));
 }
 
 int rb_depth_fill_enqueue(rb_ctx *c, const DepthPlan &pl, const unsigned char *const *rec_pp, size_t rec_ofs,
                           const unsigned char *rec, const int *kn_p, int kn, int kcap, void *ws,
-                          unsigned char *const *out_pp, size_t out_ofs, rb_depth_cell *out) {
+                          unsigned char *const *out_pp, size_t out_ofs, rb_depth_cell *out, bool keep_final) {
     unsigned char *w = (unsigned char *)ws;
     int *cnt = (int *)w;
     unsigned long long *list = (unsigned long long *)(w + ws_cnt_bytes(pl));
     unsigned char *gwork = pl.g.in_smem ? nullptr : w + ws_cnt_bytes(pl) + ws_list_bytes(kcap);
     k_depth_fill<<<1, RB_DEPTH_THREADS, pl.dyn_smem, c->stream>>>(rec_pp, rec_ofs, rec, kn_p, kn, kcap, pl.g, cnt, list, gwork,
-                                                                  out_pp, out_ofs, out);
+                                                                  out_pp, out_ofs, out,
+                                                                  keep_final ? rb_depth_ws_final(pl, kcap, ws) : nullptr);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
+// ---- the dense inverse-depth image: depth_filler::getImgRho((float)x, (float)y, &s_rho) at every pixel (depth_filler.h:246-280)
+// Each CTA stages the whole grid as float (rho, s_rho) pairs in shared memory (8 B per cell) when it fits, else reads the
+// cells from global memory with the same code.  Thread t of the grid-stride loop computes 4 consecutive pixels of the
+// row-major w x h plane (a quad may span two rows) and writes them as one 16-byte store per plane; the planes start on
+// 16 bytes, so only a last partial quad (w * h not a multiple of 4) is written by scalar stores.
+struct ImgAxis {   // the reference's expressions along one axis, for integer pixel coordinate v
+    int f, c;
+    float d;
+};
+__device__ __forceinline__ ImgAxis img_axis(int v, int b, int n) {
+    // float x_histo = x / (float)bl_size.w - 0.5: a float quotient, the subtraction in double, stored as float
+    const float hist = (float)((double)((float)v / (float)b) - 0.5);
+    // int xf = std::min(std::max(floor(x_histo), 0.0), size.w - 1.0), xc likewise with ceil
+    ImgAxis a;
+    a.f = (int)fmin(fmax(floor((double)hist), 0.0), n - 1.0);
+    a.c = (int)fmin(fmax(ceil((double)hist), 0.0), n - 1.0);
+    a.d = hist - (float)a.f;   // float dx = x_histo - xf
+    return a;
+}
+__device__ __forceinline__ float img_bilin(float v00, float v10, float v01, float v11, float dx, float dy) {
+    // rho00*(1-dx)*(1-dy)+rho10*dx*(1-dy)+rho01*(1-dx)*dy+rho11*dx*dy, left to right in float (no contraction: -fmad=false)
+    return v00 * (1 - dx) * (1 - dy) + v10 * dx * (1 - dy) + v01 * (1 - dx) * dy + v11 * dx * dy;
+}
+
+__global__ void __launch_bounds__(RB_DEPTH_IMG_THREADS)
+    k_depth_image(const double *src, int stride, DepthImgGeom g, float *const *out_pp, size_t out_ofs, float *out_direct,
+                  size_t plane_floats) {
+    extern __shared__ __align__(16) float2 gsm[];
+    const int ncell = g.gw * g.gh;
+    if (g.in_smem) {
+        for (int c = threadIdx.x; c < ncell; c += blockDim.x)
+            gsm[c] = make_float2((float)src[(size_t)c * stride], (float)src[(size_t)c * stride + 1]);
+        __syncthreads();
+    }
+    float *rho = out_pp ? reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(out_pp[0]) + out_ofs) : out_direct;
+    float *srho = g.planes == 2 ? rho + plane_floats : nullptr;
+    const long long npx = (long long)g.w * g.h, nq = (npx + 3) >> 2;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += (long long)gridDim.x * blockDim.x) {
+        const long long p0 = q << 2;
+        int y = (int)(p0 / g.w), x = (int)(p0 - (long long)y * g.w);
+        float r[4], s[4];
+        ImgAxis ay = img_axis(y, g.bh, g.gh);
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            r[k] = s[k] = 0.f;
+            if (p0 + k < npx) {
+                const ImgAxis ax = img_axis(x, g.bw, g.gw);
+                const int i00 = ay.f * g.gw + ax.f, i10 = ay.f * g.gw + ax.c, i01 = ay.c * g.gw + ax.f, i11 = ay.c * g.gw + ax.c;
+                float2 c00, c10, c01, c11;
+                if (g.in_smem) {
+                    c00 = gsm[i00], c10 = gsm[i10], c01 = gsm[i01], c11 = gsm[i11];
+                } else {
+                    c00 = make_float2((float)src[(size_t)i00 * stride], (float)src[(size_t)i00 * stride + 1]);
+                    c10 = make_float2((float)src[(size_t)i10 * stride], (float)src[(size_t)i10 * stride + 1]);
+                    c01 = make_float2((float)src[(size_t)i01 * stride], (float)src[(size_t)i01 * stride + 1]);
+                    c11 = make_float2((float)src[(size_t)i11 * stride], (float)src[(size_t)i11 * stride + 1]);
+                }
+                r[k] = img_bilin(c00.x, c10.x, c01.x, c11.x, ax.d, ay.d);
+                if (srho) s[k] = img_bilin(c00.y, c10.y, c01.y, c11.y, ax.d, ay.d);
+            }
+            if (++x == g.w) {
+                x = 0;
+                ay = img_axis(++y, g.bh, g.gh);
+            }
+        }
+        if (p0 + 4 <= npx) {
+            *reinterpret_cast<float4 *>(rho + p0) = make_float4(r[0], r[1], r[2], r[3]);
+            if (srho) *reinterpret_cast<float4 *>(srho + p0) = make_float4(s[0], s[1], s[2], s[3]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                if (p0 + k >= npx) break;
+                rho[p0 + k] = r[k];
+                if (srho) srho[p0 + k] = s[k];
+            }
+        }
+    }
+}
+
+int rb_depth_image_plan(rb_ctx *c, const DepthGeom &fg, int planes, DepthImgPlan *out) {
+    DepthImgGeom &g = out->g;
+    g.w = c->w;
+    g.h = c->h;
+    g.gw = fg.gw;
+    g.gh = fg.gh;
+    g.bw = fg.bw;
+    g.bh = fg.bh;
+    g.planes = planes;
+    const size_t need = (size_t)g.gw * g.gh * sizeof(float2);
+    int optin = 0;
+    RB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    cudaFuncAttributes fa;
+    RB_CUDA(cudaFuncGetAttributes(&fa, k_depth_image));
+    const size_t max_dyn = (size_t)optin - fa.sharedSizeBytes;
+    g.in_smem = need <= max_dyn;
+    out->dyn_smem = g.in_smem ? need : 0;
+    // one value per kernel and device for the whole process: always the device's whole opt-in budget (as k_depth_fill's)
+    if (g.in_smem)
+        RB_CUDA(cudaFuncSetAttribute(k_depth_image, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_dyn));
+    // one CTA per SM at most: each CTA stages the whole grid, and the pass is bound by its stores, not by its arithmetic
+    const long long nq = ((long long)g.w * g.h + 3) / 4;
+    const long long ctas = (nq + RB_DEPTH_IMG_THREADS - 1) / RB_DEPTH_IMG_THREADS;
+    out->ctas = (int)(ctas < c->sm_count ? ctas : c->sm_count);
+    return RB_OK;
+}
+
+int rb_depth_image_enqueue(rb_ctx *c, const DepthImgPlan &ip, const double *src, int stride, float *const *out_pp,
+                           size_t out_ofs, float *out, size_t plane_floats) {
+    k_depth_image<<<ip.ctas, RB_DEPTH_IMG_THREADS, ip.dyn_smem, c->stream>>>(src, stride, ip.g, out_pp, out_ofs, out,
+                                                                             plane_floats);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
@@ -389,7 +509,7 @@ extern "C" int rb_depth_fill_net(rb_ctx *c, const void *records, int n, const rb
     rb_depth_cell *cells = (rb_depth_cell *)(recd + rec_bytes);
     if (n > 0) RB_CUDA(cudaMemcpyAsync(recd, records, (size_t)n * 15, cudaMemcpyHostToDevice, c->stream));
     if ((r = rb_depth_fill_enqueue(c, pl, nullptr, 0, recd, nullptr, n, n, (unsigned char *)cells + pl.cells_bytes, nullptr, 0,
-                                   cells)))
+                                   cells, false)))
         return r;
     RB_CUDA(cudaMemcpyAsync(out, cells, ncell * sizeof(rb_depth_cell), cudaMemcpyDeviceToHost, c->stream));
     double md = 0;
@@ -398,5 +518,41 @@ extern "C" int rb_depth_fill_net(rb_ctx *c, const void *records, int n, const rb
     if (gw) *gw = pl.g.gw;
     if (gh) *gh = pl.g.gh;
     if (min_dist) *min_dist = md;
+    return RB_OK;
+}
+
+// the stage call: cells from host memory (those rb_depth_fill_net / rb_pipeline_depth return), the planes back to host memory.
+// The kernel reads the uploaded cells in place: rho and s_rho are the first two of each cell's four doubles.
+static_assert(offsetof(rb_depth_cell, s_rho) == sizeof(double) && sizeof(rb_depth_cell) == 4 * sizeof(double),
+              "rb_depth_cell: rho, s_rho, then two more doubles' worth");
+extern "C" int rb_depth_image(rb_ctx *c, const rb_depth_cell *cells, int gw, int gh, const rb_depth_params *p, float *rho,
+                              float *s_rho) {
+    if (!c || !cells || !p || !rho) return RB_ERR_ARG;
+    RB_ENTER(c);
+    DepthPlan pl;
+    int r = rb_depth_plan(c, p, &pl);
+    if (r) return r;
+    if (gw != pl.g.gw || gh != pl.g.gh) return RB_ERR_ARG;
+    DepthImgPlan ip;
+    if ((r = rb_depth_image_plan(c, pl.g, s_rho ? 2 : 1, &ip))) return r;
+    const size_t ncell = (size_t)gw * gh, plane = ((size_t)c->N + 63) & ~(size_t)63;
+    const size_t cells_bytes = (ncell * sizeof(rb_depth_cell) + 255) & ~(size_t)255;
+    const size_t need = cells_bytes + 2 * plane * sizeof(float);
+    if (need > c->depth_ws_bytes) {
+        cudaFree(c->depth_ws);
+        c->depth_ws = nullptr;
+        c->depth_ws_bytes = 0;
+        RB_CUDA(cudaMalloc(&c->depth_ws, need));
+        c->depth_ws_bytes = need;
+    }
+    unsigned char *celld = (unsigned char *)c->depth_ws;
+    float *img = (float *)(celld + cells_bytes);
+    RB_CUDA(cudaMemcpyAsync(celld, cells, ncell * sizeof(rb_depth_cell), cudaMemcpyHostToDevice, c->stream));
+    if ((r = rb_depth_image_enqueue(c, ip, (const double *)celld, (int)(sizeof(rb_depth_cell) / sizeof(double)), nullptr, 0,
+                                    img, plane)))
+        return r;
+    RB_CUDA(cudaMemcpyAsync(rho, img, (size_t)c->N * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    if (s_rho) RB_CUDA(cudaMemcpyAsync(s_rho, img + plane, (size_t)c->N * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
     return RB_OK;
 }

@@ -122,13 +122,24 @@ struct rb_pipeline {
     DepthPlan depth_plan;
     size_t depth_rec_stride;                      // bytes per frame staging slot (kcap records, multiple of 256)
     unsigned char *depth_stage, *depth_host;      // [max_batch * stride]: device staging, mapped pinned host cells
-    unsigned char **depth_base_dev;               // device: {staging, host} address of frame 0 of the sub-batch being processed
-    unsigned char **depth_base_pin;               // pinned: one pair per sub-batch of the current push
+    unsigned char **depth_base_dev;               // device: {staging, host cells, host image} address of frame 0 of the
+                                                  // sub-batch being processed
+    unsigned char **depth_base_pin;               // pinned: one triple per sub-batch of the current push
     void *depth_ws;                               // per stream: bucketing scratch (and the grid when it does not fit in smem)
     size_t depth_ws_bytes, depth_host_bytes;      // (depth_ws_bytes: per stream)
     cudaStream_t depth_stream[RB_DEPTH_STREAMS];
     cudaEvent_t *ev_dpack, ev_djoin[RB_DEPTH_STREAMS];
     int depth_n;                                  // frames of the last push
+    // optional per-frame dense image of the grid (rb_pipeline_set_depth_image): right after each frame's fill, on the same
+    // side stream, k_depth_image reads the fill's final cells from that stream's workspace and writes 1 (rho) or 2 (rho,
+    // s_rho) w x h float planes into mapped pinned host memory; part of the captured batch, covered by its depth joins.
+    // A kernel of its own: the fill is one latency-bound CTA, the image pass writes megabytes from many CTAs.
+    int dimg_mode;                                // 0 off, 1 rho, 2 rho and s_rho
+    DepthImgPlan dimg_plan;                       // (of depth_plan's grid, when both are on)
+    size_t dimg_plane, dimg_stride;               // floats per plane (a multiple of 64); bytes per frame slot
+    unsigned char *dimg_host;                     // [max_batch * dimg_stride] mapped pinned host memory
+    size_t dimg_host_bytes;
+    int dimg_n;                                   // frames of the last push
 };
 
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
@@ -459,6 +470,7 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     cudaFree(pl->depth_base_dev);
     if (pl->depth_base_pin) cudaFreeHost(pl->depth_base_pin);
     cudaFree(pl->depth_ws);
+    if (pl->dimg_host) cudaFreeHost(pl->dimg_host);
     for (int i = 0; i < pl->max_batch; i++)
         if (pl->ev_dpack && pl->ev_dpack[i]) cudaEventDestroy(pl->ev_dpack[i]);
     delete[] pl->ev_dpack;
@@ -710,9 +722,13 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
             RB_CUDA(cudaEventRecord(pl->ev_dpack[i], main_stream));
             RB_CUDA(cudaStreamWaitEvent(pl->depth_stream[k], pl->ev_dpack[i], 0));
             c->stream = pl->depth_stream[k];
-            r = rb_depth_fill_enqueue(c, pl->depth_plan, rec_pp, rec_ofs, nullptr, &(pl->nav_dev + i)->kn, 0, c->kcap,
-                                      (unsigned char *)pl->depth_ws + (size_t)k * pl->depth_ws_bytes, pl->depth_base_dev,
-                                      (size_t)i * pl->depth_plan.cells_bytes, nullptr);
+            void *ws = (unsigned char *)pl->depth_ws + (size_t)k * pl->depth_ws_bytes;
+            r = rb_depth_fill_enqueue(c, pl->depth_plan, rec_pp, rec_ofs, nullptr, &(pl->nav_dev + i)->kn, 0, c->kcap, ws,
+                                      pl->depth_base_dev, (size_t)i * pl->depth_plan.cells_bytes, nullptr, pl->dimg_mode != 0);
+            if (!r && pl->dimg_mode)   // depth_filler::getImgRho at every pixel, from the cells the fill left in ws
+                r = rb_depth_image_enqueue(c, pl->dimg_plan, (const double *)rb_depth_ws_final(pl->depth_plan, c->kcap, ws), 2,
+                                           reinterpret_cast<float *const *>(pl->depth_base_dev + 2),
+                                           (size_t)i * pl->dimg_stride, nullptr, pl->dimg_plane);
             c->stream = main_stream;
             if (r) return r;
         }
@@ -743,6 +759,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     RB_CUDA(cudaSetDevice(c->device));
     pl->odom_n = 0;
     pl->depth_n = 0;
+    pl->dimg_n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
         if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom_on ? pl->odom_pin : nullptr)))
             return r;
@@ -800,9 +817,10 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
                                     c->stream));
         }
         if (pl->depth_on) {
-            pl->depth_base_pin[2 * j] = pl->depth_stage + (size_t)off * pl->depth_rec_stride;
-            pl->depth_base_pin[2 * j + 1] = pl->depth_host + (size_t)off * pl->depth_plan.cells_bytes;
-            RB_CUDA(cudaMemcpyAsync(pl->depth_base_dev, pl->depth_base_pin + 2 * j, 2 * sizeof(void *), cudaMemcpyHostToDevice,
+            pl->depth_base_pin[3 * j] = pl->depth_stage + (size_t)off * pl->depth_rec_stride;
+            pl->depth_base_pin[3 * j + 1] = pl->depth_host + (size_t)off * pl->depth_plan.cells_bytes;
+            pl->depth_base_pin[3 * j + 2] = pl->dimg_mode ? pl->dimg_host + (size_t)off * pl->dimg_stride : nullptr;
+            RB_CUDA(cudaMemcpyAsync(pl->depth_base_dev, pl->depth_base_pin + 3 * j, 3 * sizeof(void *), cudaMemcpyHostToDevice,
                                     c->stream));
         }
         const bool graph_ok = pl->use_graph && first_j > 0;
@@ -869,6 +887,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
     pl->mirror_n = pl->mirror_on ? n : 0;
     pl->depth_n = pl->depth_on ? n : 0;
+    pl->dimg_n = pl->depth_on && pl->dimg_mode ? n : 0;
     // QK of a record: P_Kp as the frame found it = RKp of the previous frame's record, which holds the value after that frame's
     // rescaling also when the rescaling ran on the side stream (:382, :480-487)
     for (int i = 0; i < n && pl->odom_on; i++) {
@@ -970,6 +989,7 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
         if (pl->depth_on) drop_graphs(pl);   // the captured batches contain the pack and fill kernels
         pl->depth_on = 0;
         pl->depth_n = 0;
+        pl->dimg_n = 0;
         return RB_OK;
     }
     DepthPlan plan;
@@ -981,8 +1001,8 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
     if (!pl->depth_stage) {
         pl->depth_rec_stride = ((size_t)c->kcap * 15 + 255) & ~(size_t)255;
         RB_CUDA(cudaMalloc(&pl->depth_stage, (size_t)pl->max_batch * pl->depth_rec_stride));
-        RB_CUDA(cudaMalloc(&pl->depth_base_dev, 2 * sizeof(void *)));
-        RB_CUDA(cudaMallocHost(&pl->depth_base_pin, 8 * sizeof(void *)));
+        RB_CUDA(cudaMalloc(&pl->depth_base_dev, 3 * sizeof(void *)));
+        RB_CUDA(cudaMallocHost(&pl->depth_base_pin, 12 * sizeof(void *)));
         // lowest priority: a fill CTA may hold a whole SM's shared memory, which the tracker's kernels get first
         // (env REBVO_B200_DEPTH_PRIO=1: the tracker's own priority, for tools/bench_depth.py's comparison)
         int lo = 0, hi = 0;
@@ -1012,10 +1032,12 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
         RB_CUDA(cudaMalloc(&pl->depth_ws, ws_bytes * RB_DEPTH_STREAMS));
         pl->depth_ws_bytes = ws_bytes;
     }
+    if (pl->dimg_mode && (r = rb_depth_image_plan(c, plan.g, pl->dimg_mode, &pl->dimg_plan))) return r;
     drop_graphs(pl);   // the captured batches hold the fill's geometry
     pl->depth_plan = plan;
     pl->depth_on = 1;
     pl->depth_n = 0;
+    pl->dimg_n = 0;
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
@@ -1027,6 +1049,44 @@ extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **c
     if (gw) *gw = pl->depth_plan.g.gw;
     if (gh) *gh = pl->depth_plan.g.gh;
     if (min_dist) *min_dist = *reinterpret_cast<const double *>(slot + ncell * sizeof(rb_depth_cell));
+    return RB_OK;
+}
+extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
+    if (!pl || mode < 0 || mode > 2) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    RB_CUDA(cudaSetDevice(c->device));
+    if (pl->imu) {
+        snprintf(c->err, sizeof(c->err), "set_depth_image: not available in IMU mode");
+        return RB_ERR_ARG;
+    }
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    if (mode) {
+        const size_t plane = ((size_t)c->N + 63) & ~(size_t)63, stride = (size_t)mode * plane * sizeof(float);
+        const size_t bytes = (size_t)pl->max_batch * stride;
+        if (bytes > pl->dimg_host_bytes) {
+            if (pl->dimg_host) cudaFreeHost(pl->dimg_host);
+            pl->dimg_host = nullptr;
+            pl->dimg_host_bytes = 0;
+            RB_CUDA(cudaHostAlloc(&pl->dimg_host, bytes, cudaHostAllocMapped));
+            pl->dimg_host_bytes = bytes;
+        }
+        int r;
+        if (pl->depth_on && (r = rb_depth_image_plan(c, pl->depth_plan.g, mode, &pl->dimg_plan))) return r;
+        pl->dimg_plane = plane;
+        pl->dimg_stride = stride;
+    }
+    if (mode != pl->dimg_mode) drop_graphs(pl);   // the captured batches contain (or not) the image pass
+    pl->dimg_mode = mode;
+    pl->dimg_n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
+    if (!pl || !rho) return RB_ERR_ARG;
+    if (i < 0 || i >= pl->dimg_n) return RB_ERR_ARG;
+    const float *p = reinterpret_cast<const float *>(pl->dimg_host + (size_t)i * pl->dimg_stride);
+    *rho = p;
+    if (s_rho) *s_rho = pl->dimg_mode == 2 ? p + pl->dimg_plane : nullptr;
     return RB_OK;
 }
 extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
