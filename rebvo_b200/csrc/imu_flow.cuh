@@ -330,9 +330,8 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bo
     const size_t fbytes = frame_bytes(c, fmt);
     if (!on_device)
         RB_CUDA(cudaMemcpyAsync(pl->ws.rgb, rgb, (size_t)n * fbytes, cudaMemcpyHostToDevice, c->stream));
-    const void *src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
-    RB_CUDA(cudaMemcpyAsync(pl->rgb_src_dev, &src, sizeof(void *), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaStreamSynchronize(c->stream));   // (&src is a stack variable)
+    pl->sb_pin[0].src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
+    RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
     if ((r = gray_pass(pl, fmt, n))) return r;
     if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
     for (int i = 0; i < n; i++) {

@@ -42,6 +42,14 @@ extern "C" int rb_debug_fetch_trace(unsigned long long *out, unsigned int *n) {
 #define RB_TRACE(stream, tag) do { } while (0)
 #endif
 
+// The device addresses a sub-batch's kernels read, so that one captured batch serves every region of a push: one table on
+// the device, rewritten by one H2D copy per sub-batch from its pinned entry
+struct SubBatchPtrs {
+    const void *src;            // the RGB24 (or mono) frames of the sub-batch
+    unsigned char *mirror[2];   // keyline mirror: {device staging, mapped host} slot of the sub-batch's first frame
+    unsigned char *depth[3];    // depth grid: {record staging, mapped host cells, mapped host image} of that frame
+};
+
 struct ImuFlow;
 struct rb_pipeline {
     rb_ctx *c;
@@ -50,10 +58,12 @@ struct rb_pipeline {
     int max_batch;
     DogWS ws;
     rb_map *maps[RB_NMAPS];   // ring: frame f lives in maps[f % RB_NMAPS]
+    // one event for every hand-over between two streams whose wait follows its record at once (stream_wait)
+    cudaEvent_t ev_hop;
     // detector stream: detect(f+1) (+ reEstimateThresh) runs beside the tracker/mapper of frame f; the third map is
-    // what lets it write while frame f still reads map f-1
+    // what lets it write while frame f still reads map f-1.  detect(f) waits for track(f-2): ev_trk[f % 2]
     cudaStream_t det_stream;
-    cudaEvent_t ev_dog, *ev_det, *ev_trk;
+    cudaEvent_t ev_trk[2];
     bool overlap;
     // FordwardMatch's apply + directed_matching in k_match, then gate + Regularize_1_iter + EKF + rotate_keylines in
     // k_reg_ekf (env REBVO_B200_MAP_CHAIN=0: the stage kernels in the reference's order, the bitwise reference of the two)
@@ -63,14 +73,14 @@ struct rb_pipeline {
     // before the next frame's first kernel after the minimiser (k_match, or k_fm_apply before k_rotate, which writes the
     // map's rho / s_rho, in the reference schedule)
     cudaStream_t resc_stream;     // nullptr: the rescaling stays in the frame's map-update kernel on the tracker stream
-    cudaEvent_t ev_rfork, ev_rjoin;
+    cudaEvent_t ev_rjoin;
     bool resc_open;               // a rescaling was forked and not joined yet
     // host-input pushes are cut into a short head and the rest: the H2D copy of the rest (copy stream) runs beside the
-    // kernels of the head.  The gray kernel reads its source through rgb_src_dev, so one graph serves every region.
+    // kernels of the head
     cudaStream_t copy_stream;
-    cudaEvent_t *ev_copy;
-    const void **rgb_src_dev;     // device: pointer to the RGB24 (or mono) frames of the sub-batch being processed
-    const void **rgb_src_pin;     // pinned: one pointer per sub-batch of the current push
+    cudaEvent_t ev_copy[2];       // per sub-batch: its frames are on the device
+    SubBatchPtrs *sb_dev;         // device: the table of the sub-batch being processed
+    SubBatchPtrs *sb_pin;         // pinned: one entry per sub-batch of the current push (at most two)
     int sub;                      // head sub-batch of a host-input push (env REBVO_B200_SUB, default 8 frames)
     DetChain *chain;      // device
     FrameState *fs;       // device
@@ -96,50 +106,55 @@ struct rb_pipeline {
     int pcap, pn;
     double pacc[16];
     long long pframes;
-    // optional per-frame host mirror of the edge map (rb_pipeline_set_mirror): every frame's keylines are packed into a device
-    // staging slot right after its map update (tracker stream), then a small kernel on mirror_stream writes exactly kn records
-    // into mapped pinned host memory while the next frames are tracked; both are part of the captured batch
-    int mirror_on;                                // 0 off, 1 = 168-byte KeyLine records, 2 = 15-byte net_keyline records
-    size_t mirror_rec, mirror_stride;             // bytes per record / per frame slot (multiple of 256)
-    unsigned char *mirror_dev, *mirror_host;      // [max_batch * mirror_stride]: device staging, mapped pinned host memory
-    unsigned char **mirror_base_dev;              // device: {staging, host} address of frame 0 of the sub-batch being processed
-    unsigned char **mirror_base_pin;              // pinned: one pair per sub-batch of the current push
-    cudaStream_t mirror_stream;
-    cudaEvent_t *ev_mpack, ev_mjoin;
-    int mirror_n;                                 // frames of the last push
-    rb_undistort *und;                            // UseUndistort=1 (rb_pipeline_set_undistort): fused into the gray pass
-    // optional per-frame odometry records (rb_pipeline_set_odometry): written beside the nav records, copied with them
-    int odom_on;
-    rb_odometry *odom_dev, *odom_pin;             // [max_batch]
-    int odom_n;                                   // records of the last push
-    double rkp_last;                              // RKp of the last frame pushed: QK of the next push's first record
-    // optional per-frame depth grid (rb_pipeline_set_depth): right after its map update each frame's net_keyline records are
-    // packed into a staging slot (tracker stream; with mirror mode 2 the mirror's slot is read instead), then one fill CTA on
-    // a side stream writes the frame's cells and min_dist into mapped pinned host memory; both are part of the captured batch.
-    // Frame i's fill runs on depth_stream[i % RB_DEPTH_STREAMS] with that stream's workspace: one fill takes longer than a
-    // tracked frame, so the fills of consecutive frames run side by side on their own SMs
-    int depth_on;
-    DepthPlan depth_plan;
-    size_t depth_rec_stride;                      // bytes per frame staging slot (kcap records, multiple of 256)
-    unsigned char *depth_stage, *depth_host;      // [max_batch * stride]: device staging, mapped pinned host cells
-    unsigned char **depth_base_dev;               // device: {staging, host cells, host image} address of frame 0 of the
-                                                  // sub-batch being processed
-    unsigned char **depth_base_pin;               // pinned: one triple per sub-batch of the current push
-    void *depth_ws;                               // per stream: bucketing scratch (and the grid when it does not fit in smem)
-    size_t depth_ws_bytes, depth_host_bytes;      // (depth_ws_bytes: per stream)
-    cudaStream_t depth_stream[RB_DEPTH_STREAMS];
-    cudaEvent_t *ev_dpack, ev_djoin[RB_DEPTH_STREAMS];
-    int depth_n;                                  // frames of the last push
-    // optional per-frame dense image of the grid (rb_pipeline_set_depth_image): right after each frame's fill, on the same
-    // side stream, k_depth_image reads the fill's final cells from that stream's workspace and writes 1 (rho) or 2 (rho,
-    // s_rho) w x h float planes into mapped pinned host memory; part of the captured batch, covered by its depth joins.
-    // A kernel of its own: the fill is one latency-bound CTA, the image pass writes megabytes from many CTAs.
-    int dimg_mode;                                // 0 off, 1 rho, 2 rho and s_rho
-    DepthImgPlan dimg_plan;                       // (of depth_plan's grid, when both are on)
-    size_t dimg_plane, dimg_stride;               // floats per plane (a multiple of 64); bytes per frame slot
-    unsigned char *dimg_host;                     // [max_batch * dimg_stride] mapped pinned host memory
-    size_t dimg_host_bytes;
-    int dimg_n;                                   // frames of the last push
+    rb_undistort *und;    // UseUndistort=1 (rb_pipeline_set_undistort): fused into the gray pass
+    // The optional per-frame outputs.  Each keeps its own frame count of the last push, which its set_* call clears (and
+    // set_depth the image's too: the images are of the grid).
+    // Keyline mirror (rb_pipeline_set_mirror): every frame's keylines are packed into a device staging slot right after its
+    // map update (tracker stream), then a small kernel on the mirror's stream writes exactly kn records into mapped pinned
+    // host memory while the next frames are tracked; both are part of the captured batch
+    struct {
+        int on;                        // 0 off, 1 = 168-byte KeyLine records, 2 = 15-byte net_keyline records
+        size_t rec, stride;            // bytes per record / per frame slot (multiple of 256)
+        unsigned char *dev, *host;     // [max_batch * stride]: device staging, mapped pinned host memory
+        size_t host_bytes;
+        cudaStream_t stream;
+        int n;                         // frames of the last push
+    } mirror;
+    // odometry records (rb_pipeline_set_odometry): written beside the nav records, copied with them
+    struct {
+        int on;
+        rb_odometry *dev, *pin;        // [max_batch]
+        int n;                         // records of the last push
+        double rkp_last;               // RKp of the last frame pushed: QK of the next push's first record
+    } odom;
+    // depth grid (rb_pipeline_set_depth): right after its map update each frame's net_keyline records are packed into a
+    // staging slot (tracker stream; with mirror mode 2 the mirror's slot is read instead), then one fill CTA on a side stream
+    // writes the frame's cells and min_dist into mapped pinned host memory; both are part of the captured batch.  Frame i's
+    // fill runs on stream[i % RB_DEPTH_STREAMS] with that stream's workspace: one fill takes longer than a tracked frame, so
+    // the fills of consecutive frames run side by side on their own SMs
+    struct {
+        int on;
+        DepthPlan plan;
+        size_t rec_stride;             // bytes per frame staging slot (kcap records, multiple of 256)
+        unsigned char *stage, *host;   // [max_batch * stride]: device staging, mapped pinned host cells
+        size_t host_bytes;
+        void *ws;                      // per stream: bucketing scratch (and the grid when it does not fit in smem)
+        size_t ws_bytes;               // (per stream)
+        cudaStream_t stream[RB_DEPTH_STREAMS];
+        int n;                         // frames of the last push
+    } depth;
+    // dense image of the grid (rb_pipeline_set_depth_image): right after each frame's fill, on the same side stream,
+    // k_depth_image reads the fill's final cells from that stream's workspace and writes 1 (rho) or 2 (rho, s_rho) w x h
+    // float planes into mapped pinned host memory; part of the captured batch, covered by its depth joins.  A kernel of its
+    // own: the fill is one latency-bound CTA, the image pass writes megabytes from many CTAs.
+    struct {
+        int mode;                      // 0 off, 1 rho, 2 rho and s_rho
+        DepthImgPlan plan;             // (of depth.plan's grid, when both are on)
+        size_t plane, stride;          // floats per plane (a multiple of 64); bytes per frame slot
+        unsigned char *host;           // [max_batch * stride] mapped pinned host memory
+        size_t host_bytes;
+        int n;                         // frames of the last push
+    } dimg;
 };
 
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
@@ -160,13 +175,31 @@ static void drop_graphs(rb_pipeline *pl) {
             pl->gexec[i] = nullptr;
         }
 }
-// the batch's gray plane from the frames at *rgb_src_dev (rebvo_first_t.cpp:231 undistortion + RGB -> BW)
+// `to` waits for the work enqueued on `from` so far.  One event serves every such hand-over: a wait (eager or captured)
+// takes the event's most recent record at the time of the call.
+static int stream_wait(rb_pipeline *pl, cudaStream_t from, cudaStream_t to) {
+    rb_ctx *c = pl->c;
+    RB_CUDA(cudaEventRecord(pl->ev_hop, from));
+    RB_CUDA(cudaStreamWaitEvent(to, pl->ev_hop, 0));
+    return RB_OK;
+}
+// *buf: mapped pinned host memory of at least `bytes`, kept when it is large enough (its contents are not kept otherwise)
+static int grow_mapped(rb_ctx *c, unsigned char **buf, size_t *have, size_t bytes) {
+    if (bytes <= *have) return RB_OK;
+    if (*buf) cudaFreeHost(*buf);
+    *buf = nullptr;
+    *have = 0;
+    RB_CUDA(cudaHostAlloc(buf, bytes, cudaHostAllocMapped));
+    *have = bytes;
+    return RB_OK;
+}
+// the batch's gray plane from the frames at sb_dev->src (rebvo_first_t.cpp:231 undistortion + RGB -> BW)
 static int gray_pass(rb_pipeline *pl, int fmt, int n) {
+    const void *const *src = &pl->sb_dev->src;
     if (pl->und)
-        return fmt == RB_IN_MONO ? rb_undistort_gray_mono_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, n)
-                                 : rb_undistort_gray_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, n);
-    return fmt == RB_IN_MONO ? rb_dog_gray_mono(pl->c, &pl->ws, n, pl->rgb_src_dev)
-                             : rb_dog_gray(pl->c, &pl->ws, n, pl->rgb_src_dev);
+        return fmt == RB_IN_MONO ? rb_undistort_gray_mono_enqueue(pl->und, src, pl->ws.gray, n)
+                                 : rb_undistort_gray_enqueue(pl->und, src, pl->ws.gray, n);
+    return fmt == RB_IN_MONO ? rb_dog_gray_mono(pl->c, &pl->ws, n, src) : rb_dog_gray(pl->c, &pl->ws, n, src);
 }
 #include "imu_flow.cuh"
 
@@ -303,7 +336,7 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
     if (pl->prof_on) {
         pl->use_graph = false;
         pl->pcap = max_batch * 12 + 8;
-        pl->pev = new (std::nothrow) cudaEvent_t[pl->pcap];
+        pl->pev = new (std::nothrow) cudaEvent_t[pl->pcap]();
         pl->ptag = new (std::nothrow) int[pl->pcap];
         if (!pl->pev || !pl->ptag) return RB_ERR_ARG;
         for (int i = 0; i < pl->pcap; i++) RB_CUDA(cudaEventCreate(&pl->pev[i]));
@@ -313,33 +346,23 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
         pl->map_chain = !(mc && atoi(mc) == 0);
         const char *ov = getenv("REBVO_B200_OVERLAP");
         pl->overlap = !(ov && ov[0] == '0') && !pl->prof_on;
-        pl->ev_det = new (std::nothrow) cudaEvent_t[max_batch];
-        pl->ev_trk = new (std::nothrow) cudaEvent_t[max_batch];
-        if (!pl->ev_det || !pl->ev_trk) return RB_ERR_ARG;
-        memset(pl->ev_det, 0, sizeof(cudaEvent_t) * max_batch);
-        memset(pl->ev_trk, 0, sizeof(cudaEvent_t) * max_batch);
         RB_CUDA(cudaStreamCreateWithFlags(&pl->det_stream, cudaStreamNonBlocking));
         RB_CUDA(cudaStreamCreateWithFlags(&pl->copy_stream, cudaStreamNonBlocking));
         const char *sb = getenv("REBVO_B200_SUB");
         pl->sub = sb ? atoi(sb) : 8;
         if (pl->sub < 1) pl->sub = max_batch;
-        pl->ev_copy = new (std::nothrow) cudaEvent_t[max_batch];
-        if (!pl->ev_copy) return RB_ERR_ARG;
-        memset(pl->ev_copy, 0, sizeof(cudaEvent_t) * max_batch);
-        for (int i = 0; i < max_batch; i++) RB_CUDA(cudaEventCreateWithFlags(&pl->ev_copy[i], cudaEventDisableTiming));
-        RB_CUDA(cudaMalloc(&pl->rgb_src_dev, sizeof(void *)));
-        RB_CUDA(cudaMallocHost(&pl->rgb_src_pin, sizeof(void *) * max_batch));
-        RB_CUDA(cudaEventCreateWithFlags(&pl->ev_dog, cudaEventDisableTiming));
-        for (int i = 0; i < max_batch; i++) {
-            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_det[i], cudaEventDisableTiming));
+        RB_CUDA(cudaMalloc(&pl->sb_dev, sizeof(SubBatchPtrs)));
+        RB_CUDA(cudaMallocHost(&pl->sb_pin, 2 * sizeof(SubBatchPtrs)));
+        RB_CUDA(cudaEventCreateWithFlags(&pl->ev_hop, cudaEventDisableTiming));
+        for (int i = 0; i < 2; i++) {
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
+            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_copy[i], cudaEventDisableTiming));
         }
         // (the inline schedule where the rescaled keylines feed the next frame, or everything runs on one stream)
         if (pl->overlap && p->DoReScaling <= 0) {
             int lo = 0, hi = 0;
             RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
             RB_CUDA(cudaStreamCreateWithPriority(&pl->resc_stream, cudaStreamNonBlocking, lo));   // minimiser blocks first
-            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_rfork, cudaEventDisableTiming));
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_rjoin, cudaEventDisableTiming));
         }
     }
@@ -422,80 +445,40 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     rb_ctx *c = pl->c;
     delete pl->imu;
     cudaSetDevice(c->device);
+    // every stream first, so that no work still uses what is freed below; whatever a create that failed halfway did not
+    // make yet is null.  (c->stream is the context's: rb_ctx_destroy destroys it.)
+    cudaStream_t own[4 + RB_DEPTH_STREAMS] = {pl->det_stream, pl->resc_stream, pl->copy_stream, pl->mirror.stream};
+    memcpy(own + 4, pl->depth.stream, sizeof(pl->depth.stream));
     cudaStreamSynchronize(c->stream);
-    if (pl->det_stream) cudaStreamSynchronize(pl->det_stream);
-    if (pl->resc_stream) cudaStreamSynchronize(pl->resc_stream);
+    for (cudaStream_t s : own)
+        if (s) cudaStreamSynchronize(s);
+    for (cudaStream_t s : own)
+        if (s) cudaStreamDestroy(s);
+    cudaEvent_t events[] = {pl->ev_hop, pl->ev_trk[0], pl->ev_trk[1], pl->ev_rjoin, pl->ev_copy[0], pl->ev_copy[1],
+                            pl->ev[0], pl->ev[1], pl->ev[2], pl->ev[3]};
+    for (cudaEvent_t e : events)
+        if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : pl->user_ev)
+        if (e) cudaEventDestroy(e);
+    for (int i = 0; pl->pev && i < pl->pcap; i++)
+        if (pl->pev[i]) cudaEventDestroy(pl->pev[i]);
+    delete[] pl->pev;
+    delete[] pl->ptag;
+    for (int i = 0; pl->gexec && i < graph_slots(pl); i++)
+        if (pl->gexec[i]) cudaGraphExecDestroy(pl->gexec[i]);
+    delete[] pl->gexec;
+    delete[] pl->glaunches;
     for (int i = 0; i < RB_NMAPS; i++)
         if (pl->maps[i]) rb_map_destroy(pl->maps[i]);
-    if (pl->ev_dog) cudaEventDestroy(pl->ev_dog);
-    for (int i = 0; i < pl->max_batch; i++) {
-        if (pl->ev_det && pl->ev_det[i]) cudaEventDestroy(pl->ev_det[i]);
-        if (pl->ev_trk && pl->ev_trk[i]) cudaEventDestroy(pl->ev_trk[i]);
-    }
-    delete[] pl->ev_det;
-    delete[] pl->ev_trk;
-    if (pl->det_stream) cudaStreamDestroy(pl->det_stream);
-    if (pl->resc_stream) cudaStreamDestroy(pl->resc_stream);
-    if (pl->ev_rfork) cudaEventDestroy(pl->ev_rfork);
-    if (pl->ev_rjoin) cudaEventDestroy(pl->ev_rjoin);
-    if (pl->copy_stream) {
-        cudaStreamSynchronize(pl->copy_stream);
-        cudaStreamDestroy(pl->copy_stream);
-    }
-    for (int i = 0; i < pl->max_batch; i++)
-        if (pl->ev_copy && pl->ev_copy[i]) cudaEventDestroy(pl->ev_copy[i]);
-    delete[] pl->ev_copy;
-    cudaFree(pl->rgb_src_dev);
-    if (pl->rgb_src_pin) cudaFreeHost(pl->rgb_src_pin);
-    if (pl->mirror_stream) {
-        cudaStreamSynchronize(pl->mirror_stream);
-        cudaStreamDestroy(pl->mirror_stream);
-    }
     if (pl->und) rb_undistort_destroy(pl->und);
-    cudaFree(pl->mirror_dev);
-    if (pl->mirror_host) cudaFreeHost(pl->mirror_host);
-    for (int i = 0; i < pl->max_batch; i++)
-        if (pl->ev_mpack && pl->ev_mpack[i]) cudaEventDestroy(pl->ev_mpack[i]);
-    delete[] pl->ev_mpack;
-    if (pl->ev_mjoin) cudaEventDestroy(pl->ev_mjoin);
-    cudaFree(pl->mirror_base_dev);
-    if (pl->mirror_base_pin) cudaFreeHost(pl->mirror_base_pin);
-    for (int k = 0; k < RB_DEPTH_STREAMS; k++)
-        if (pl->depth_stream[k]) {
-            cudaStreamSynchronize(pl->depth_stream[k]);
-            cudaStreamDestroy(pl->depth_stream[k]);
-        }
-    cudaFree(pl->depth_stage);
-    if (pl->depth_host) cudaFreeHost(pl->depth_host);
-    cudaFree(pl->depth_base_dev);
-    if (pl->depth_base_pin) cudaFreeHost(pl->depth_base_pin);
-    cudaFree(pl->depth_ws);
-    if (pl->dimg_host) cudaFreeHost(pl->dimg_host);
-    for (int i = 0; i < pl->max_batch; i++)
-        if (pl->ev_dpack && pl->ev_dpack[i]) cudaEventDestroy(pl->ev_dpack[i]);
-    delete[] pl->ev_dpack;
-    for (int k = 0; k < RB_DEPTH_STREAMS; k++)
-        if (pl->ev_djoin[k]) cudaEventDestroy(pl->ev_djoin[k]);
     rb_dogws_free(&pl->ws);
-    cudaFree(pl->chain);
-    cudaFree(pl->fs);
-    cudaFree(pl->nav_dev);
-    if (pl->nav_pin) cudaFreeHost(pl->nav_pin);
-    if (pl->abort_pin) cudaFreeHost(pl->abort_pin);
-    cudaFree(pl->fa_dev);
-    if (pl->fa_pin) cudaFreeHost(pl->fa_pin);
-    cudaFree(pl->odom_dev);
-    if (pl->odom_pin) cudaFreeHost(pl->odom_pin);
-    if (pl->gexec) {
-        for (int i = 0; i < graph_slots(pl); i++)
-            if (pl->gexec[i]) cudaGraphExecDestroy(pl->gexec[i]);
-        delete[] pl->gexec;
-    }
-    delete[] pl->glaunches;
-    for (int i = 0; i < 4; i++)
-        if (pl->ev[i]) cudaEventDestroy(pl->ev[i]);
-    for (int i = 0; i < 8; i++)
-        if (pl->user_ev[i]) cudaEventDestroy(pl->user_ev[i]);
+    void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->mirror.dev, pl->odom.dev, pl->depth.stage,
+                   pl->depth.ws};
+    for (void *p : dev) cudaFree(p);
+    void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->mirror.host, pl->odom.pin, pl->depth.host,
+                    pl->dimg.host};
+    for (void *p : host)
+        if (p) cudaFreeHost(p);
     rb_ctx_destroy(c);
     delete pl;
 }
@@ -575,7 +558,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
     // EKF, or with the rescaling stream, pose integration + NavData ride in the EKF kernel and the rescaling leaves the chain.
     // (Not with the 168-byte keyline mirror: there the inline schedule measured 2-3 % faster on H100, while the 15-byte
     // records gain from the side stream like the plain push; set_mirror drops the captured batches.)
-    const bool side = pl->resc_stream != nullptr && pl->mirror_on != 1;
+    const bool side = pl->resc_stream != nullptr && pl->mirror.on != 1;
     if (pl->map_chain) {
         // (the old map's rescaling is joined here although k_match only reads that map: joining it before k_reg_ekf
         // instead measured no faster on H100)
@@ -625,8 +608,7 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
     prof_mark(pl, ST_REG_EKF);
     if (side) {   // gated by the map's own copy of do_map; writes the map's Kp / RKp and the record's, no FrameState
         cudaStream_t main_stream = c->stream;
-        RB_CUDA(cudaEventRecord(pl->ev_rfork, main_stream));
-        RB_CUDA(cudaStreamWaitEvent(pl->resc_stream, pl->ev_rfork, 0));
+        if ((r = stream_wait(pl, main_stream, pl->resc_stream))) return r;
         c->stream = pl->resc_stream;
         r = rb_rescale_enqueue(c, neu, RB_RHO_MAX, 1, 0, &neu->st->do_map, nav_slot);
         c->stream = main_stream;
@@ -662,17 +644,15 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     // frame f.  detect(f) overwrites the map of frame f-3, which track(f-2) was the last to read.
     cudaStream_t main_stream = c->stream;
     const bool ov = pl->overlap;
-    if (ov) {
-        RB_CUDA(cudaEventRecord(pl->ev_dog, main_stream));
-        RB_CUDA(cudaStreamWaitEvent(pl->det_stream, pl->ev_dog, 0));
-    }
+    if (ov && (r = stream_wait(pl, main_stream, pl->det_stream))) return r;
+    SubBatchPtrs *tbl = pl->sb_dev;
     for (int i = 0; i < n; i++) {
         const long long fr = first_frame + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
         const float *img0 = pl->ws.img0 + (size_t)i * c->NP, *dog = pl->ws.dog + (size_t)i * c->NP;
         // FirstThr: detect + reEstimateThresh (rebvo_first_t.cpp:266-272)
         if (ov) {
-            if (i >= 2) RB_CUDA(cudaStreamWaitEvent(pl->det_stream, pl->ev_trk[i - 2], 0));
+            if (i >= 2) RB_CUDA(cudaStreamWaitEvent(pl->det_stream, pl->ev_trk[i % 2], 0));   // track(i-2)
             c->stream = pl->det_stream;
         }
         RB_TRACE(c->stream, 6);
@@ -687,62 +667,52 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
         RB_TRACE(c->stream, 7);
         c->stream = main_stream;
         if (r) return r;
-        if (ov) {
-            RB_CUDA(cudaEventRecord(pl->ev_det[i], pl->det_stream));
-            RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_det[i], 0));
-        }
+        if (ov && (r = stream_wait(pl, pl->det_stream, main_stream))) return r;
         if (fr == 0) {
             k_frame_first<<<1, 1, 0, c->stream>>>(pl->fs, neu->st, pl->nav_dev + i, pl->fa_dev + i);
             RB_LAUNCH_CHECK();
         } else {
-            if ((r = track_frame(pl, neu, old, pl->fa_dev + i, pl->nav_dev + i, pl->odom_on ? pl->odom_dev + i : nullptr)))
+            if ((r = track_frame(pl, neu, old, pl->fa_dev + i, pl->nav_dev + i, pl->odom.on ? pl->odom.dev + i : nullptr)))
                 return r;
         }
-        if (pl->mirror_on) {   // the frame's edge map as the reference's records, before the next frame touches it
-            const size_t ofs = (size_t)i * pl->mirror_stride;
-            if (pl->mirror_on == 1)
-                r = rb_map_pack_aos_enqueue(c, neu, pl->mirror_base_dev, ofs);
+        if (pl->mirror.on) {   // the frame's edge map as the reference's records, before the next frame touches it
+            const size_t ofs = (size_t)i * pl->mirror.stride;
+            if (pl->mirror.on == 1)
+                r = rb_map_pack_aos_enqueue(c, neu, tbl->mirror, ofs);
             else   // copy_net_keyline(..., pbuf.K) of the third thread (rebvo_third_t.cpp:192-197): K of this frame's nav record
-                r = rb_map_pack_net_enqueue(c, neu, pl->mirror_base_dev, ofs, &(pl->nav_dev + i)->K);
-            if (r) return r;
-            RB_CUDA(cudaEventRecord(pl->ev_mpack[i], main_stream));
-            RB_CUDA(cudaStreamWaitEvent(pl->mirror_stream, pl->ev_mpack[i], 0));
-            k_mirror_to_host<<<8, 256, 0, pl->mirror_stream>>>(pl->mirror_base_dev, ofs, &(pl->nav_dev + i)->kn, (int)pl->mirror_rec);
+                r = rb_map_pack_net_enqueue(c, neu, tbl->mirror, ofs, &(pl->nav_dev + i)->K);
+            if (r || (r = stream_wait(pl, main_stream, pl->mirror.stream))) return r;
+            k_mirror_to_host<<<8, 256, 0, pl->mirror.stream>>>(tbl->mirror, ofs, &(pl->nav_dev + i)->kn, (int)pl->mirror.rec);
             RB_LAUNCH_CHECK();
         }
-        if (pl->depth_on) {   // the viewer's depth_filler on this frame's wire records (visualizer.cpp:436-440)
-            unsigned char *const *rec_pp = pl->mirror_base_dev;
-            size_t rec_ofs = (size_t)i * pl->mirror_stride;
-            if (pl->mirror_on != 2) {   // copy_net_keyline(..., pbuf.K) of the third thread (rebvo_third_t.cpp:191)
-                rec_pp = pl->depth_base_dev;
-                rec_ofs = (size_t)i * pl->depth_rec_stride;
-                if ((r = rb_map_pack_net_enqueue(c, neu, pl->depth_base_dev, rec_ofs, &(pl->nav_dev + i)->K))) return r;
+        if (pl->depth.on) {   // the viewer's depth_filler on this frame's wire records (visualizer.cpp:436-440)
+            unsigned char *const *rec_pp = tbl->mirror;
+            size_t rec_ofs = (size_t)i * pl->mirror.stride;
+            if (pl->mirror.on != 2) {   // copy_net_keyline(..., pbuf.K) of the third thread (rebvo_third_t.cpp:191)
+                rec_pp = tbl->depth;
+                rec_ofs = (size_t)i * pl->depth.rec_stride;
+                if ((r = rb_map_pack_net_enqueue(c, neu, tbl->depth, rec_ofs, &(pl->nav_dev + i)->K))) return r;
             }
             const int k = i % RB_DEPTH_STREAMS;
-            RB_CUDA(cudaEventRecord(pl->ev_dpack[i], main_stream));
-            RB_CUDA(cudaStreamWaitEvent(pl->depth_stream[k], pl->ev_dpack[i], 0));
-            c->stream = pl->depth_stream[k];
-            void *ws = (unsigned char *)pl->depth_ws + (size_t)k * pl->depth_ws_bytes;
-            r = rb_depth_fill_enqueue(c, pl->depth_plan, rec_pp, rec_ofs, nullptr, &(pl->nav_dev + i)->kn, 0, c->kcap, ws,
-                                      pl->depth_base_dev, (size_t)i * pl->depth_plan.cells_bytes, nullptr, pl->dimg_mode != 0);
-            if (!r && pl->dimg_mode)   // depth_filler::getImgRho at every pixel, from the cells the fill left in ws
-                r = rb_depth_image_enqueue(c, pl->dimg_plan, (const double *)rb_depth_ws_final(pl->depth_plan, c->kcap, ws), 2,
-                                           reinterpret_cast<float *const *>(pl->depth_base_dev + 2),
-                                           (size_t)i * pl->dimg_stride, nullptr, pl->dimg_plane);
+            if ((r = stream_wait(pl, main_stream, pl->depth.stream[k]))) return r;
+            c->stream = pl->depth.stream[k];
+            void *ws = (unsigned char *)pl->depth.ws + (size_t)k * pl->depth.ws_bytes;
+            r = rb_depth_fill_enqueue(c, pl->depth.plan, rec_pp, rec_ofs, nullptr, &(pl->nav_dev + i)->kn, 0, c->kcap, ws,
+                                      tbl->depth, (size_t)i * pl->depth.plan.cells_bytes, nullptr, pl->dimg.mode != 0);
+            if (!r && pl->dimg.mode)   // depth_filler::getImgRho at every pixel, from the cells the fill left in ws
+                r = rb_depth_image_enqueue(c, pl->dimg.plan, (const double *)rb_depth_ws_final(pl->depth.plan, c->kcap, ws), 2,
+                                           reinterpret_cast<float *const *>(tbl->depth + 2), (size_t)i * pl->dimg.stride,
+                                           nullptr, pl->dimg.plane);
             c->stream = main_stream;
             if (r) return r;
         }
-        if (ov && i + 2 < n) RB_CUDA(cudaEventRecord(pl->ev_trk[i], main_stream));
+        if (ov && i + 2 < n) RB_CUDA(cudaEventRecord(pl->ev_trk[i % 2], main_stream));
     }
     if ((r = resc_join(pl))) return r;   // the last frame's Kp / RKp are in its record before the nav copy
-    if (pl->mirror_on) {   // the batch is complete when its last map has reached the host
-        RB_CUDA(cudaEventRecord(pl->ev_mjoin, pl->mirror_stream));
-        RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_mjoin, 0));
-    }
-    for (int k = 0; pl->depth_on && k < RB_DEPTH_STREAMS && k < n; k++) {   // and when its last grids have
-        RB_CUDA(cudaEventRecord(pl->ev_djoin[k], pl->depth_stream[k]));
-        RB_CUDA(cudaStreamWaitEvent(main_stream, pl->ev_djoin[k], 0));
-    }
+    // the batch is complete when its last map has reached the host, and its last grids
+    if (pl->mirror.on && (r = stream_wait(pl, pl->mirror.stream, main_stream))) return r;
+    for (int k = 0; pl->depth.on && k < RB_DEPTH_STREAMS && k < n; k++)
+        if ((r = stream_wait(pl, pl->depth.stream[k], main_stream))) return r;
     return RB_OK;
 }
 
@@ -757,15 +727,15 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     int r;
     if (pl->imu && pl->imu->live && (r = imu_live_check(pl, *pl->imu, ts, n))) return r;
     RB_CUDA(cudaSetDevice(c->device));
-    pl->odom_n = 0;
-    pl->depth_n = 0;
-    pl->dimg_n = 0;
+    pl->odom.n = 0;
+    pl->depth.n = 0;
+    pl->dimg.n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
-        if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom_on ? pl->odom_pin : nullptr)))
+        if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom.on ? pl->odom.pin : nullptr)))
             return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
         if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
-        pl->odom_n = pl->odom_on ? n : 0;
+        pl->odom.n = pl->odom.on ? n : 0;
         return RB_OK;
     }
     const long long first = pl->n_pushed;
@@ -792,43 +762,36 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
         nsub = 2;
     }
     const size_t fbytes = frame_bytes(c, fmt);   // (ws.rgb holds max_batch frames of either format)
-    for (int j = 0; j < nsub; j++) {
+    for (int j = 0; j < nsub && !on_device; j++) {
         const int off = soff[j], nj = soff[j + 1] - soff[j];
-        if (on_device) {
-            pl->rgb_src_pin[j] = rgb;
-        } else {
-            pl->rgb_src_pin[j] = pl->ws.rgb + (size_t)off * fbytes;
-            cudaStream_t cs = nsub > 1 ? pl->copy_stream : c->stream;
-            RB_CUDA(cudaMemcpyAsync(pl->ws.rgb + (size_t)off * fbytes, rgb + (size_t)off * fbytes, (size_t)nj * fbytes,
-                                    cudaMemcpyHostToDevice, cs));
-            if (nsub > 1) RB_CUDA(cudaEventRecord(pl->ev_copy[j], cs));
-        }
+        cudaStream_t cs = nsub > 1 ? pl->copy_stream : c->stream;
+        RB_CUDA(cudaMemcpyAsync(pl->ws.rgb + (size_t)off * fbytes, rgb + (size_t)off * fbytes, (size_t)nj * fbytes,
+                                cudaMemcpyHostToDevice, cs));
+        if (nsub > 1) RB_CUDA(cudaEventRecord(pl->ev_copy[j], cs));
     }
     for (int j = 0; j < nsub; j++) {
         const int off = soff[j], nj = soff[j + 1] - soff[j];
         const long long first_j = first + (long long)off;
         if (!on_device && nsub > 1) RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_copy[j], 0));
         RB_CUDA(cudaMemcpyAsync(pl->fa_dev, pl->fa_pin + off, sizeof(FrameArgs) * nj, cudaMemcpyHostToDevice, c->stream));
-        RB_CUDA(cudaMemcpyAsync(pl->rgb_src_dev, pl->rgb_src_pin + j, sizeof(void *), cudaMemcpyHostToDevice, c->stream));
-        if (pl->mirror_on) {
-            pl->mirror_base_pin[2 * j] = pl->mirror_dev + (size_t)off * pl->mirror_stride;
-            pl->mirror_base_pin[2 * j + 1] = pl->mirror_host + (size_t)off * pl->mirror_stride;
-            RB_CUDA(cudaMemcpyAsync(pl->mirror_base_dev, pl->mirror_base_pin + 2 * j, 2 * sizeof(void *), cudaMemcpyHostToDevice,
-                                    c->stream));
+        SubBatchPtrs &t = pl->sb_pin[j];
+        t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);
+        if (pl->mirror.on) {
+            t.mirror[0] = pl->mirror.dev + (size_t)off * pl->mirror.stride;
+            t.mirror[1] = pl->mirror.host + (size_t)off * pl->mirror.stride;
         }
-        if (pl->depth_on) {
-            pl->depth_base_pin[3 * j] = pl->depth_stage + (size_t)off * pl->depth_rec_stride;
-            pl->depth_base_pin[3 * j + 1] = pl->depth_host + (size_t)off * pl->depth_plan.cells_bytes;
-            pl->depth_base_pin[3 * j + 2] = pl->dimg_mode ? pl->dimg_host + (size_t)off * pl->dimg_stride : nullptr;
-            RB_CUDA(cudaMemcpyAsync(pl->depth_base_dev, pl->depth_base_pin + 3 * j, 3 * sizeof(void *), cudaMemcpyHostToDevice,
-                                    c->stream));
+        if (pl->depth.on) {
+            t.depth[0] = pl->depth.stage + (size_t)off * pl->depth.rec_stride;
+            t.depth[1] = pl->depth.host + (size_t)off * pl->depth.plan.cells_bytes;
+            t.depth[2] = pl->dimg.mode ? pl->dimg.host + (size_t)off * pl->dimg.stride : nullptr;
         }
+        RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
         const bool graph_ok = pl->use_graph && first_j > 0;
         if (!graph_ok) {
             if ((r = enqueue_batch(pl, fmt, nj, first_j, j == 0))) return r;
         } else {
             const int key = graph_slot(pl, fmt, (int)(first_j % RB_NMAPS), nj);
-            // capture the batch once per ring phase; replays only differ through fa_dev / rgb_src_dev contents.  All
+            // capture the batch once per ring phase; replays only differ through fa_dev / sb_dev contents.  All
             // phases of this format and batch size are instantiated together, so that no later push pays for a capture.
             // The other format's graphs are left as they are: a stream may alternate formats.
             const bool build = !pl->gexec[key];
@@ -864,8 +827,8 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
             c->launches += pl->glaunches[key];
         }
         RB_CUDA(cudaMemcpyAsync(pl->nav_pin + off, pl->nav_dev, sizeof(rb_nav) * nj, cudaMemcpyDeviceToHost, c->stream));
-        if (pl->odom_on)
-            RB_CUDA(cudaMemcpyAsync(pl->odom_pin + off, pl->odom_dev, sizeof(rb_odometry) * nj, cudaMemcpyDeviceToHost,
+        if (pl->odom.on)
+            RB_CUDA(cudaMemcpyAsync(pl->odom.pin + off, pl->odom.dev, sizeof(rb_odometry) * nj, cudaMemcpyDeviceToHost,
                                     c->stream));
     }
     for (int k = 0; k < RB_NMAPS; k++)
@@ -885,20 +848,20 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
         pl->pframes += n;
     }
     if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
-    pl->mirror_n = pl->mirror_on ? n : 0;
-    pl->depth_n = pl->depth_on ? n : 0;
-    pl->dimg_n = pl->depth_on && pl->dimg_mode ? n : 0;
+    pl->mirror.n = pl->mirror.on ? n : 0;
+    pl->depth.n = pl->depth.on ? n : 0;
+    pl->dimg.n = pl->depth.on && pl->dimg.mode ? n : 0;
     // QK of a record: P_Kp as the frame found it = RKp of the previous frame's record, which holds the value after that frame's
     // rescaling also when the rescaling ran on the side stream (:382, :480-487)
-    for (int i = 0; i < n && pl->odom_on; i++) {
+    for (int i = 0; i < n && pl->odom.on; i++) {
         if (first + i == 0) {   // the first frame of a sequence only initialises the ring (:109-121)
-            memset(&pl->odom_pin[i], 0, sizeof(rb_odometry));
+            memset(&pl->odom.pin[i], 0, sizeof(rb_odometry));
             continue;
         }
-        pl->odom_pin[i].QK = i == 0 ? pl->rkp_last : pl->nav_pin[i - 1].RKp;
+        pl->odom.pin[i].QK = i == 0 ? pl->odom.rkp_last : pl->nav_pin[i - 1].RKp;
     }
-    pl->odom_n = pl->odom_on ? n : 0;
-    pl->rkp_last = pl->nav_pin[n - 1].RKp;
+    pl->odom.n = pl->odom.on ? n : 0;
+    pl->odom.rkp_last = pl->nav_pin[n - 1].RKp;
     {   // did a minimiser of this push abort (an exchange between its CTAs timed out)?  Checked on every push.
         bool aborted = false;
         for (int k = 0; k < RB_NMAPS; k++) aborted = aborted || pl->abort_pin[k] != 0;
@@ -921,25 +884,34 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     return RB_OK;
 }
 
+// the opening of the set_* calls, under RB_ENTER: refused in IMU mode when `imu_refused` names the call, then the pushes
+// enqueued so far finish, so that the call may replace what they use
+static int set_begin(rb_pipeline *pl, const char *imu_refused) {
+    rb_ctx *c = pl->c;
+    RB_CUDA(cudaSetDevice(c->device));
+    if (imu_refused && pl->imu) {
+        snprintf(c->err, sizeof(c->err), "%s: not available in IMU mode", imu_refused);
+        return RB_ERR_ARG;
+    }
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    return RB_OK;
+}
 extern "C" int rb_pipeline_set_undistort(rb_pipeline *pl, const double kc[5]) {
     if (!pl) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
-    RB_CUDA(cudaSetDevice(c->device));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
+    int r = set_begin(pl, nullptr);
+    if (r) return r;
     if (pl->und) {
         rb_undistort_destroy(pl->und);
         pl->und = nullptr;
     }
     bool any = false;
     for (int i = 0; kc && i < 5; i++) any = any || kc[i] != 0.0;
-    if (any) {
-        int r = rb_undistort_create(c, kc, &pl->und);
-        if (r) {
-            if (pl->und) rb_undistort_destroy(pl->und);
-            pl->und = nullptr;
-            return r;
-        }
+    if (any && (r = rb_undistort_create(c, kc, &pl->und))) {
+        if (pl->und) rb_undistort_destroy(pl->und);
+        pl->und = nullptr;
+        return r;
     }
     drop_graphs(pl);   // the captured batches contain the other gray kernel (both input formats)
     return RB_OK;
@@ -948,173 +920,130 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     if (!pl || on < 0 || on > 2) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
-    RB_CUDA(cudaSetDevice(c->device));
-    if (pl->imu) {
-        snprintf(c->err, sizeof(c->err), "set_mirror: not available in IMU mode");
-        return RB_ERR_ARG;
-    }
-    RB_CUDA(cudaStreamSynchronize(c->stream));
+    int r = set_begin(pl, "set_mirror");
+    if (r) return r;
     const size_t stride = ((size_t)c->kcap * sizeof(rb_keyline) + 255) & ~(size_t)255;   // (sized for the larger record)
-    if (on && !pl->mirror_dev) {
-        const size_t bytes = (size_t)pl->max_batch * stride;
-        RB_CUDA(cudaMalloc(&pl->mirror_dev, bytes));
-        RB_CUDA(cudaHostAlloc(&pl->mirror_host, bytes, cudaHostAllocMapped));
-        RB_CUDA(cudaMalloc(&pl->mirror_base_dev, 2 * sizeof(void *)));
-        RB_CUDA(cudaMallocHost(&pl->mirror_base_pin, 8 * sizeof(void *)));
-        RB_CUDA(cudaStreamCreateWithFlags(&pl->mirror_stream, cudaStreamNonBlocking));
-        pl->ev_mpack = new (std::nothrow) cudaEvent_t[pl->max_batch];
-        if (!pl->ev_mpack) return RB_ERR_ARG;
-        memset(pl->ev_mpack, 0, sizeof(cudaEvent_t) * pl->max_batch);
-        for (int i = 0; i < pl->max_batch; i++) RB_CUDA(cudaEventCreateWithFlags(&pl->ev_mpack[i], cudaEventDisableTiming));
-        RB_CUDA(cudaEventCreateWithFlags(&pl->ev_mjoin, cudaEventDisableTiming));
+    if (on) {
+        if (!pl->mirror.dev) RB_CUDA(cudaMalloc(&pl->mirror.dev, (size_t)pl->max_batch * stride));
+        if ((r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, (size_t)pl->max_batch * stride))) return r;
+        if (!pl->mirror.stream) RB_CUDA(cudaStreamCreateWithFlags(&pl->mirror.stream, cudaStreamNonBlocking));
     }
-    if (on != pl->mirror_on) drop_graphs(pl);   // the captured batches contain (or not) the pack kernels
-    pl->mirror_on = on;
-    pl->mirror_rec = on == 2 ? 15 : sizeof(rb_keyline);
-    pl->mirror_stride = stride;
-    pl->mirror_n = 0;
+    if (on != pl->mirror.on) drop_graphs(pl);   // the captured batches contain (or not) the pack kernels
+    pl->mirror.on = on;
+    pl->mirror.rec = on == 2 ? 15 : sizeof(rb_keyline);
+    pl->mirror.stride = stride;
+    pl->mirror.n = 0;
     return RB_OK;
 }
 extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) {
     if (!pl) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
-    RB_CUDA(cudaSetDevice(c->device));
-    if (pl->imu) {
-        snprintf(c->err, sizeof(c->err), "set_depth: not available in IMU mode");
-        return RB_ERR_ARG;
-    }
-    RB_CUDA(cudaStreamSynchronize(c->stream));
+    int r = set_begin(pl, "set_depth");
+    if (r) return r;
     if (!p) {
-        if (pl->depth_on) drop_graphs(pl);   // the captured batches contain the pack and fill kernels
-        pl->depth_on = 0;
-        pl->depth_n = 0;
-        pl->dimg_n = 0;
+        if (pl->depth.on) drop_graphs(pl);   // the captured batches contain the pack and fill kernels
+        pl->depth.on = 0;
+        pl->depth.n = 0;
+        pl->dimg.n = 0;
         return RB_OK;
     }
     DepthPlan plan;
-    int r = rb_depth_plan(c, p, &plan);
-    if (r) {
+    if ((r = rb_depth_plan(c, p, &plan))) {
         snprintf(c->err, sizeof(c->err), "set_depth: invalid parameters");
         return r;
     }
-    if (!pl->depth_stage) {
-        pl->depth_rec_stride = ((size_t)c->kcap * 15 + 255) & ~(size_t)255;
-        RB_CUDA(cudaMalloc(&pl->depth_stage, (size_t)pl->max_batch * pl->depth_rec_stride));
-        RB_CUDA(cudaMalloc(&pl->depth_base_dev, 3 * sizeof(void *)));
-        RB_CUDA(cudaMallocHost(&pl->depth_base_pin, 12 * sizeof(void *)));
+    if (!pl->depth.stage) {
+        pl->depth.rec_stride = ((size_t)c->kcap * 15 + 255) & ~(size_t)255;
+        RB_CUDA(cudaMalloc(&pl->depth.stage, (size_t)pl->max_batch * pl->depth.rec_stride));
         // lowest priority: a fill CTA may hold a whole SM's shared memory, which the tracker's kernels get first
         // (env REBVO_B200_DEPTH_PRIO=1: the tracker's own priority, for tools/bench_depth.py's comparison)
         int lo = 0, hi = 0;
         RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
         const char *dp = getenv("REBVO_B200_DEPTH_PRIO");
-        for (int k = 0; k < RB_DEPTH_STREAMS; k++) {
-            RB_CUDA(cudaStreamCreateWithPriority(&pl->depth_stream[k], cudaStreamNonBlocking, (dp && atoi(dp) == 1) ? hi : lo));
-            RB_CUDA(cudaEventCreateWithFlags(&pl->ev_djoin[k], cudaEventDisableTiming));
-        }
-        pl->ev_dpack = new (std::nothrow) cudaEvent_t[pl->max_batch];
-        if (!pl->ev_dpack) return RB_ERR_ARG;
-        memset(pl->ev_dpack, 0, sizeof(cudaEvent_t) * pl->max_batch);
-        for (int i = 0; i < pl->max_batch; i++) RB_CUDA(cudaEventCreateWithFlags(&pl->ev_dpack[i], cudaEventDisableTiming));
+        for (int k = 0; k < RB_DEPTH_STREAMS; k++)
+            RB_CUDA(cudaStreamCreateWithPriority(&pl->depth.stream[k], cudaStreamNonBlocking, (dp && atoi(dp) == 1) ? hi : lo));
     }
-    const size_t host_bytes = (size_t)pl->max_batch * plan.cells_bytes, ws_bytes = rb_depth_ws_bytes(plan, c->kcap);
-    if (host_bytes > pl->depth_host_bytes) {
-        if (pl->depth_host) cudaFreeHost(pl->depth_host);
-        pl->depth_host = nullptr;
-        pl->depth_host_bytes = 0;
-        RB_CUDA(cudaHostAlloc(&pl->depth_host, host_bytes, cudaHostAllocMapped));
-        pl->depth_host_bytes = host_bytes;
+    if ((r = grow_mapped(c, &pl->depth.host, &pl->depth.host_bytes, (size_t)pl->max_batch * plan.cells_bytes))) return r;
+    const size_t ws_bytes = rb_depth_ws_bytes(plan, c->kcap);
+    if (ws_bytes > pl->depth.ws_bytes) {
+        cudaFree(pl->depth.ws);
+        pl->depth.ws = nullptr;
+        pl->depth.ws_bytes = 0;
+        RB_CUDA(cudaMalloc(&pl->depth.ws, ws_bytes * RB_DEPTH_STREAMS));
+        pl->depth.ws_bytes = ws_bytes;
     }
-    if (ws_bytes > pl->depth_ws_bytes) {
-        cudaFree(pl->depth_ws);
-        pl->depth_ws = nullptr;
-        pl->depth_ws_bytes = 0;
-        RB_CUDA(cudaMalloc(&pl->depth_ws, ws_bytes * RB_DEPTH_STREAMS));
-        pl->depth_ws_bytes = ws_bytes;
-    }
-    if (pl->dimg_mode && (r = rb_depth_image_plan(c, plan.g, pl->dimg_mode, &pl->dimg_plan))) return r;
+    if (pl->dimg.mode && (r = rb_depth_image_plan(c, plan.g, pl->dimg.mode, &pl->dimg.plan))) return r;
     drop_graphs(pl);   // the captured batches hold the fill's geometry
-    pl->depth_plan = plan;
-    pl->depth_on = 1;
-    pl->depth_n = 0;
-    pl->dimg_n = 0;
+    pl->depth.plan = plan;
+    pl->depth.on = 1;
+    pl->depth.n = 0;
+    pl->dimg.n = 0;
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
-    if (!pl || !pl->depth_on || !cells) return RB_ERR_ARG;
-    if (i < 0 || i >= pl->depth_n) return RB_ERR_ARG;
-    const unsigned char *slot = pl->depth_host + (size_t)i * pl->depth_plan.cells_bytes;
-    const size_t ncell = (size_t)pl->depth_plan.g.gw * pl->depth_plan.g.gh;
+    if (!pl || !pl->depth.on || !cells) return RB_ERR_ARG;
+    if (i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
+    const DepthGeom &g = pl->depth.plan.g;
+    const unsigned char *slot = pl->depth.host + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
-    if (gw) *gw = pl->depth_plan.g.gw;
-    if (gh) *gh = pl->depth_plan.g.gh;
-    if (min_dist) *min_dist = *reinterpret_cast<const double *>(slot + ncell * sizeof(rb_depth_cell));
+    if (gw) *gw = g.gw;
+    if (gh) *gh = g.gh;
+    if (min_dist) *min_dist = *reinterpret_cast<const double *>(slot + (size_t)g.gw * g.gh * sizeof(rb_depth_cell));
     return RB_OK;
 }
 extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
     if (!pl || mode < 0 || mode > 2) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
-    RB_CUDA(cudaSetDevice(c->device));
-    if (pl->imu) {
-        snprintf(c->err, sizeof(c->err), "set_depth_image: not available in IMU mode");
-        return RB_ERR_ARG;
-    }
-    RB_CUDA(cudaStreamSynchronize(c->stream));
+    int r = set_begin(pl, "set_depth_image");
+    if (r) return r;
     if (mode) {
         const size_t plane = ((size_t)c->N + 63) & ~(size_t)63, stride = (size_t)mode * plane * sizeof(float);
-        const size_t bytes = (size_t)pl->max_batch * stride;
-        if (bytes > pl->dimg_host_bytes) {
-            if (pl->dimg_host) cudaFreeHost(pl->dimg_host);
-            pl->dimg_host = nullptr;
-            pl->dimg_host_bytes = 0;
-            RB_CUDA(cudaHostAlloc(&pl->dimg_host, bytes, cudaHostAllocMapped));
-            pl->dimg_host_bytes = bytes;
-        }
-        int r;
-        if (pl->depth_on && (r = rb_depth_image_plan(c, pl->depth_plan.g, mode, &pl->dimg_plan))) return r;
-        pl->dimg_plane = plane;
-        pl->dimg_stride = stride;
+        if ((r = grow_mapped(c, &pl->dimg.host, &pl->dimg.host_bytes, (size_t)pl->max_batch * stride))) return r;
+        if (pl->depth.on && (r = rb_depth_image_plan(c, pl->depth.plan.g, mode, &pl->dimg.plan))) return r;
+        pl->dimg.plane = plane;
+        pl->dimg.stride = stride;
     }
-    if (mode != pl->dimg_mode) drop_graphs(pl);   // the captured batches contain (or not) the image pass
-    pl->dimg_mode = mode;
-    pl->dimg_n = 0;
+    if (mode != pl->dimg.mode) drop_graphs(pl);   // the captured batches contain (or not) the image pass
+    pl->dimg.mode = mode;
+    pl->dimg.n = 0;
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
     if (!pl || !rho) return RB_ERR_ARG;
-    if (i < 0 || i >= pl->dimg_n) return RB_ERR_ARG;
-    const float *p = reinterpret_cast<const float *>(pl->dimg_host + (size_t)i * pl->dimg_stride);
+    if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
+    const float *p = reinterpret_cast<const float *>(pl->dimg.host + (size_t)i * pl->dimg.stride);
     *rho = p;
-    if (s_rho) *s_rho = pl->dimg_mode == 2 ? p + pl->dimg_plane : nullptr;
+    if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
 }
 extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
     if (!pl || on < 0 || on > 1) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
-    RB_CUDA(cudaSetDevice(c->device));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
-    if (on && !pl->odom_dev) {
-        RB_CUDA(cudaMalloc(&pl->odom_dev, sizeof(rb_odometry) * pl->max_batch));
-        RB_CUDA(cudaMallocHost(&pl->odom_pin, sizeof(rb_odometry) * pl->max_batch));
+    int r = set_begin(pl, nullptr);
+    if (r) return r;
+    if (on && !pl->odom.dev) {
+        RB_CUDA(cudaMalloc(&pl->odom.dev, sizeof(rb_odometry) * pl->max_batch));
+        RB_CUDA(cudaMallocHost(&pl->odom.pin, sizeof(rb_odometry) * pl->max_batch));
     }
-    if (on != pl->odom_on) drop_graphs(pl);   // the captured batches pass (or not) the record slots to their kernels
-    pl->odom_on = on;
-    pl->odom_n = 0;
+    if (on != pl->odom.on) drop_graphs(pl);   // the captured batches pass (or not) the record slots to their kernels
+    pl->odom.on = on;
+    pl->odom.n = 0;
     return RB_OK;
 }
 extern "C" int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, int *n) {
     if (!pl || !recs || !n) return RB_ERR_ARG;
-    if (!pl->odom_n) return RB_ERR_STATE;
-    *recs = pl->odom_pin;
-    *n = pl->odom_n;
+    if (!pl->odom.n) return RB_ERR_STATE;
+    *recs = pl->odom.pin;
+    *n = pl->odom.n;
     return RB_OK;
 }
 extern "C" int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, int *n) {
-    if (!pl || !pl->mirror_on || !records || !n) return RB_ERR_ARG;
-    if (i < 0 || i >= pl->mirror_n) return RB_ERR_ARG;
-    *records = pl->mirror_host + (size_t)i * pl->mirror_stride;
+    if (!pl || !pl->mirror.on || !records || !n) return RB_ERR_ARG;
+    if (i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
+    *records = pl->mirror.host + (size_t)i * pl->mirror.stride;
     *n = pl->nav_pin[i].kn;
     return RB_OK;
 }
@@ -1170,14 +1099,14 @@ extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, in
         if (!pl->und) return RB_ERR_STATE;
         if (pass_id == 7) {
             bytes = 5.0 * c->N * nimg + 32.0 * c->N;
-            return rb_undistort_gray_mono_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, nimg);
+            return rb_undistort_gray_mono_enqueue(pl->und, &pl->sb_dev->src, pl->ws.gray, nimg);
         }
         bytes = 7.0 * c->N * nimg + 32.0 * c->N;
-        return rb_undistort_gray_enqueue(pl->und, pl->rgb_src_dev, pl->ws.gray, nimg);
+        return rb_undistort_gray_enqueue(pl->und, &pl->sb_dev->src, pl->ws.gray, nimg);
     };
     if (und_pass) {
-        const void *src = pl->ws.rgb;
-        RB_CUDA(cudaMemcpyAsync(pl->rgb_src_dev, &src, sizeof(void *), cudaMemcpyHostToDevice, c->stream));
+        pl->sb_pin[0].src = pl->ws.rgb;
+        RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
     }
     for (int i = 0; i < 3; i++)
         if ((r = one())) return r;
