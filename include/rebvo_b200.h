@@ -145,7 +145,9 @@ typedef struct rb_odometry {
 int rb_odometry_format_pose_graph(const rb_odometry *r, int n, void *buf, size_t cap, size_t *written);
 
 /* ---- context ---------------------------------------------------------------------------------- */
-/* RB_ERR_ARG for cam->w < 32, cam->h < 32 or kl_capacity < 1; every other frame size is accepted */
+/* RB_ERR_ARG for cam->w < 32, cam->h < 32, kl_capacity < 1 or kl_capacity > 50000 (the reference's KEYLINE_MAX); every
+ * other frame size is accepted.  RB_ERR_CUDA, with the reason in rb_last_error, when the device cannot run Minimizer_RV's
+ * 16-CTA thread-block cluster. */
 int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, double sigma0, double ksigma,
                   int kl_capacity);
 void rb_ctx_destroy(rb_ctx *c);
@@ -156,7 +158,7 @@ int rb_ctx_sync(rb_ctx *c);
 int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r);
 /* kernels launched on this context so far (bench.py's gpu_launches) */
 int64_t rb_ctx_launch_count(const rb_ctx *c);
-/* thread-block clusters of one Minimizer_RV launch (REBVO_B200_MIN_G when all fit, else 1); 0: one launch per evaluation */
+/* thread-block clusters of one Minimizer_RV launch: REBVO_B200_MIN_G (default 4) when all fit, else 1 */
 int rb_ctx_minimizer_clusters(const rb_ctx *c);
 
 /* ---- edge map (ring slot) ---------------------------------------------------------------------- */

@@ -249,6 +249,7 @@ class Ctx:
         return self.L.rb_ctx_launch_count(self.h_)
 
     def minimizer_clusters(self):
+        """thread-block clusters of one Minimizer_RV launch: REBVO_B200_MIN_G (default 4) when all fit, else 1"""
         return self.L.rb_ctx_minimizer_clusters(self.h_)
 
     def new_map(self):

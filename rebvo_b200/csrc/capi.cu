@@ -182,7 +182,7 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     *out = nullptr;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device >= ndev) return RB_ERR_NO_DEVICE;
-    if (cam->w < 32 || cam->h < 32 || kl_capacity < 1) return RB_ERR_ARG;
+    if (cam->w < 32 || cam->h < 32 || kl_capacity < 1 || kl_capacity > RB_KCAP_MAX) return RB_ERR_ARG;
     rb_ctx *c = new (std::nothrow) rb_ctx;
     if (!c) return RB_ERR_ARG;
     memset(c, 0, sizeof(*c));
@@ -207,8 +207,6 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     {
         const char *pd = getenv("REBVO_B200_PDL");
         c->pdl = !(pd && atoi(pd) == 0);
-        const char *mp = getenv("REBVO_B200_MIN_PERSIST");
-        c->min_persist = !(mp && atoi(mp) == 0);
     }
     // sspace::sspace (sspace.cpp:36-46): filter1 sigma = filter0.sigma_r * k_sigma
     box_plan_one(sigma0, 3, c->plan.d[0], &c->plan.sigma_r[0]);
@@ -231,7 +229,7 @@ extern "C" int rb_ctx_create(rb_ctx **out, int device, const rb_camera *cam, dou
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
     c->sm_count = prop.multiProcessorCount;
-    rb_minimizer_cluster_setup(c);
+    if ((r = rb_minimizer_cluster_setup(c))) return fail(r);
     {   // the context's stream carries the latency-critical tracker chain: highest priority, so that its kernels get SM slots
         // before the queued blocks of the detector / mirror streams (env REBVO_B200_PRIO=0: default priority)
         int lo = 0, hi = 0;
@@ -297,9 +295,7 @@ extern "C" int rb_ctx_box_plan(const rb_ctx *c, int *out_d, double *out_sigma_r)
 }
 
 extern "C" int64_t rb_ctx_launch_count(const rb_ctx *c) { return c->launches; }
-extern "C" int rb_ctx_minimizer_clusters(const rb_ctx *c) {
-    return c->min_persist && c->min_cluster_kpc > 0 ? c->min_cluster_g : 0;
-}
+extern "C" int rb_ctx_minimizer_clusters(const rb_ctx *c) { return c->min_cluster_g; }
 
 // ---- map ------------------------------------------------------------------------------------------
 int rb_map_alloc(rb_ctx *c, rb_map **out, bool with_ws) {

@@ -7,10 +7,9 @@
 #include "common.cuh"
 #include "tracker.cuh"
 
-int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, int buf);
-int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *X_dev, int reweight, int procjf,
-                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc,
-                           double k_huber);
+int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old);
+int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double X[6], int reweight, int procjf,
+                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber);
 
 static double *args_dev(rb_ctx *c) { return (double *)((char *)c->dev_small + RB_DS_ARGS); }
 static double *args_pin(rb_ctx *c) { return (double *)((char *)c->pinned + RB_DS_ARGS); }
@@ -94,17 +93,16 @@ extern "C" int rb_try_vel_rot(rb_map *fmap, rb_map *old, const double X[6], int 
     int r;
     if ((r = rb_read_map_state(old, &so))) return r;
     if ((r = rb_read_map_state(fmap, &sf))) return r;
-    if ((r = stage_in(c, X, 6, 0))) return r;
     if (res_in && so.kn > 0)
         RB_CUDA(cudaMemcpyAsync(fmap->res[0], res_in, sizeof(double) * so.kn, cudaMemcpyHostToDevice, c->stream));
     else
         RB_CUDA(cudaMemsetAsync(fmap->res[0], 0, sizeof(double) * (size_t)c->kcap, c->stream));
-    if ((r = rb_try_vel_rot_enqueue(c, fmap, old, args_dev(c), reweight, procjf, match_thresh, s_rho_min,
-                                    match_num_thresh, sf.frame_count, k_huber)))
+    if ((r = rb_try_vel_rot_enqueue(c, fmap, old, X, reweight, procjf, match_thresh, s_rho_min, match_num_thresh,
+                                    sf.frame_count, k_huber)))
         return r;
     LMState *lmh = (LMState *)((char *)c->pinned + 4096);
     RB_CUDA(cudaMemcpyAsync(lmh, &fmap->ts->lm, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
-    if (res_out && so.kn > 0 && (r = rb_resolve_res_enqueue(c, fmap, old, 1))) return r;
+    if (res_out && so.kn > 0 && (r = rb_resolve_res_enqueue(c, fmap, old))) return r;
     if (res_out && so.kn > 0)
         RB_CUDA(cudaMemcpyAsync(res_out, fmap->res[1], sizeof(double) * so.kn, cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));

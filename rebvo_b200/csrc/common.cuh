@@ -15,6 +15,7 @@
 #define RB_RHO_MIN 1e-3   // :39
 #define RB_RHO_INIT 1.0   // :40
 #define RB_MAX_IMG_VALUE 765  // edge_tracker(cam, 255*3), rebvo.cpp:300
+#define RB_KCAP_MAX 50000     // largest keyline capacity of a context: KEYLINE_MAX (edge_finder.h:43)
 
 // DetectorPlaneFitSize (build_mask's win_s): the detector has one kernel instance per radius 1..RB_PLANE_FIT_MAX
 #define RB_PLANE_FIT_MAX 4
@@ -109,8 +110,7 @@ struct rb_ctx {
     float *boxtab;       // 6 x 64 reciprocal clipped-area tables (iimage::build_average), see dog.cu
     bool counters_preset; // set by rb_pipeline: match / regularise counters are zeroed by its quantile kernel (d_frame_pre)
     bool pdl;            // programmatic dependent launch of the per-frame chain (env REBVO_B200_PDL=0 disables)
-    bool min_persist;    // whole Minimizer_RV in one launch (env REBVO_B200_MIN_PERSIST=0: one launch per evaluation)
-    int min_cluster_kpc; // keylines per CTA its shared memory is sized for (0: not available on this device / capacity)
+    int min_cluster_kpc; // keylines per CTA the one-cluster minimiser's shared memory is sized for
     size_t min_cluster_dyn;
     int min_cluster_g;   // clusters per minimisation (env REBVO_B200_MIN_G, default 4; 1 = one cluster, co-residency guaranteed)
     int min_cluster_kpc_multi;
@@ -158,7 +158,7 @@ struct TrackState {
     int *blk_has;
     double *blk_last_fi;  // per block: residual of its last matched keyline
     double *partials;     // per block x 28 reduction partials
-    double *carry;        // [3][256]: per residual buffer and block, the stale-fi value its leading misses inherit
+    double *carry;        // [256]: per block of rb_try_vel_rot's output, the stale-fi value its leading misses inherit
     int nblk;
     struct MinCtl *ctl;   // request slots / sequence base of the persistent minimiser kernel
     unsigned long long *ll;   // its inter-cluster slots

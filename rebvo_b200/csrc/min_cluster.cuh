@@ -47,8 +47,8 @@ extern "C" int rb_debug_fetch_gt(long long *out) { return (int)cudaMemcpyFromSym
 
 struct McPlan {
     int n, merge_round;              // merge_round: the round after which the better init try is picked (-1: none)
-    unsigned char sa[MIN_MAX_EVALS]; // zero-init try's step of the round (STEP_NONE when the round has one pose)
-    unsigned char sb[MIN_MAX_EVALS]; // prior-init try / main loop step
+    unsigned char sa[MIN_MAX_ROUNDS];   // zero-init try's step of the round (STEP_NONE when the round has one pose)
+    unsigned char sb[MIN_MAX_ROUNDS];   // prior-init try / main loop step
 };
 
 __device__ __forceinline__ unsigned int mc_smem_u32(const void *p) { return (unsigned int)__cvta_generic_to_shared(p); }
@@ -100,51 +100,6 @@ struct McView {
     int base, cnt, J;     // first keyline, keylines of this CTA, iterations per thread (uniform over the cluster)
 };
 
-// LM steps of the two init tries evaluated side by side (global_tracker.cpp:651-683 and :700-732)
-__device__ __forceinline__ void mc_lm_step_zero(LMState &z, int step) {
-    switch (step) {
-        case STEP_INIT_FIRST_ZERO:
-            lm_take_first(z);
-            if (z.init_iter > 0) {
-                lm_solve(z, true);
-                lm_request(z, z.Xnew, -1, z.iRt);
-            }
-            break;
-        case STEP_INIT_ITER_ZERO:
-            lm_update(z, true);
-            lm_solve(z, true);
-            lm_request(z, z.Xnew, -1, z.iRt);
-            break;
-        case STEP_INIT_LAST_ZERO:
-            lm_update(z, false);
-            break;
-        default:
-            break;
-    }
-}
-__device__ __forceinline__ void mc_lm_step_main(LMState &s, int step, MapState *fst) {
-    switch (step) {
-        case STEP_INIT_FIRST_PRIOR:
-            lm_take_first(s);
-            s.v = 2;
-            if (s.init_iter > 0) {
-                lm_solve(s, true);
-                lm_request(s, s.Xnew, -1, s.iRN);
-            }
-            break;
-        case STEP_INIT_ITER_PRIOR:
-            lm_update(s, true);
-            lm_solve(s, true);
-            lm_request(s, s.Xnew, -1, s.iRN);
-            break;
-        case STEP_INIT_LAST_PRIOR:
-            lm_update(s, false);
-            break;
-        default:
-            lm_step(s, step, fst);
-            break;
-    }
-}
 // "Save the scores in temporals" (:686-691) + "Check for the lowest score" (:734-747) once both tries are done
 __device__ __forceinline__ void mc_lm_merge(LMState &s, const LMState &z) {
     for (int i = 0; i < 6; i++) s.Xt[i] = z.X[i];
@@ -647,10 +602,10 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
                     L.n_eval++;
                     MC_STAMP(e, 5);
                     if (p == 0) {
-                        mc_lm_step_main(sm.lm, sb, first_cta ? f_st : nullptr);
+                        lm_step_main(sm.lm, sb, first_cta ? f_st : nullptr);
                         MC_STAMP(e, 6);
                     } else {
-                        mc_lm_step_zero(sm.lmz, sa);
+                        lm_step_zero(sm.lmz, sa);
                     }
                 }
                 __syncwarp();
@@ -699,7 +654,8 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
     if (first_cta && tid == 32 && post_fs) d_frame_post_min_pose(post_fs, sm.lm);
     __syncthreads();
     if (first_cta) {
-        if (tid == 0 && G > 1) ctl->gen = seq0 + MIN_MAX_EVALS + 1u;   // the next minimisation gets fresh sequence numbers
+        // the next minimisation gets fresh sequence numbers: this one used seq0 + 1 .. seq0 + plan.n <= seq0 + MIN_MAX_ROUNDS
+        if (tid == 0 && G > 1) ctl->gen = seq0 + MIN_MAX_ROUNDS + 1u;
         const double *src = reinterpret_cast<const double *>(&sm.lm);
         double *dst = reinterpret_cast<double *>(lm_out);
         for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += T) dst[k] = src[k];

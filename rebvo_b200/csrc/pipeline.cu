@@ -232,7 +232,6 @@ static void set_eye(double *M, double v) {
     M[0] = M[4] = M[8] = v;
 }
 
-__global__ void k_frame_post_min(FrameState *fs, const TrackState *ts) { d_frame_post_min(fs, ts->lm); }
 __global__ void k_frame_post_match(FrameState *fs, MapState *nst, int match_threshold, const TrackState *ts, rb_odometry *odom) {
     d_frame_post_match(fs, nst, match_threshold);
     nst->do_map = fs->do_map;   // for this map's rescaling on the side stream: the next frame rewrites FrameState
@@ -539,21 +538,15 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
     a.match_num_thresh = p.MatchNumThresh;
     // FrameCount comes from fa (written into neu->st by the folded loop-body start)
     RB_TRACE(c->stream, 2);
-    bool folded = false;
     // (since the old map's update only EstimateQuantile -- and build_field of the NEW map without the second stream -- ran
     // on this stream: the minimiser may stage the old map's operands while that kernel is still running)
     c->min_early = getenv("REBVO_B200_MIN_EARLY") ? atoi(getenv("REBVO_B200_MIN_EARLY")) != 0 : true;
-    // (folded: the one-thread stage after the minimiser and FordwardMatch's arg-max ran in its epilogue / last evaluation)
-    r = rb_minimizer_enqueue(c, neu, old, pl->fs->VW, &a, 0.0, true, 0, true, pl->fs, &folded);
+    // (the one-thread stage after the minimiser and FordwardMatch's arg-max run in its epilogue / last evaluation)
+    r = rb_minimizer_enqueue(c, neu, old, pl->fs->VW, &a, 0.0, true, 0, true, pl->fs);
     c->min_early = false;
     if (r) return r;
     RB_TRACE(c->stream, 3);
     prof_mark(pl, ST_MINIM);
-    if (!folded) {
-        k_frame_post_min<<<1, 1, 0, c->stream>>>(pl->fs, neu->ts);
-        RB_LAUNCH_CHECK();
-        if ((r = rb_forward_match_argmax_enqueue(c, old, neu))) return r;
-    }
     // :480-487 EstimateReScalingOpt and :545-585 pose integration + NavData: in one cluster kernel (k_map_update) after the
     // EKF, or with the rescaling stream, pose integration + NavData ride in the EKF kernel and the rescaling leaves the chain.
     // (Not with the 168-byte keyline mirror: there the inline schedule measured 2-3 % faster on H100, while the 15-byte

@@ -14,25 +14,21 @@
 #define TVR_T 256
 #define RES_SENTINEL 0x7FF8DEADBEEF0001ull
 
-// Cycle stamps of one evaluation kernel (build with -DRB_TVR_PROF, see scratch tooling); compiled out of the product.
+// Cycle stamps of the cluster minimiser (build with -DRB_TVR_PROF, read by tools/cluster_stamps.py); compiled out of the product.
 #ifdef RB_TVR_PROF
 __device__ long long g_tvr_prof[256 * 16];
-#define TVR_STAMP(k) do { if (threadIdx.x == 0) g_tvr_prof[blockIdx.x * 16 + (k)] = clock64(); } while (0)
 __device__ __forceinline__ long long tvr_gtime() {
     long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
     return t;
 }
-#define TVR_GSTAMP(k) do { if (threadIdx.x == 0) g_tvr_prof[blockIdx.x * 16 + (k)] = tvr_gtime(); } while (0)
 extern "C" int rb_debug_fetch(long long *out) {
     return (int)cudaMemcpyFromSymbol(out, g_tvr_prof, sizeof(long long) * 256 * 16);
 }
-#else
-#define TVR_STAMP(k) do { } while (0)
-#define TVR_GSTAMP(k) do { } while (0)
 #endif
-// Stage stamps of thread 0's first keyline of the cluster minimiser's last evaluation (CTA 0, round slot 14).  k_tvr_eval
-// runs the same body, so in such a build its block 0 stamps the same slots: read them after a cluster-kernel run only.
+// Stage stamps of thread 0's first keyline of the cluster minimiser's last evaluation (CTA 0, round slot 14).
+// k_try_vel_rot runs the same body, so in such a build its block 0 stamps the same slots: read them after a cluster-kernel
+// run only.
 #if defined(RB_TVR_PROF) && defined(MC_BODY_STAMPS)
 #define MC_BSTAMP(k) do { if (threadIdx.x == 0 && blockIdx.x == 0) g_tvr_prof[(14) * 16 + (k)] = clock64(); } while (0)
 #else
@@ -65,8 +61,8 @@ int rb_track_state_alloc(rb_ctx *c, rb_map *m) {
     RB_CUDA(cudaMalloc(&host.blk_has, sizeof(int) * nblk));
     RB_CUDA(cudaMalloc(&host.blk_last_fi, sizeof(double) * nblk));
     RB_CUDA(cudaMalloc(&host.partials, sizeof(double) * 28 * TVR_T));
-    RB_CUDA(cudaMalloc(&host.carry, sizeof(double) * 3 * TVR_T));
-    RB_CUDA(cudaMemsetAsync(host.carry, 0, sizeof(double) * 3 * TVR_T, c->stream));
+    RB_CUDA(cudaMalloc(&host.carry, sizeof(double) * TVR_T));
+    RB_CUDA(cudaMemsetAsync(host.carry, 0, sizeof(double) * TVR_T, c->stream));
     RB_CUDA(cudaMalloc(&host.ctl, sizeof(MinCtl)));
     RB_CUDA(cudaMemsetAsync(host.ctl, 0, sizeof(MinCtl), c->stream));
     // slots of the multi-cluster minimiser: [2][MC_GMAX][16][2][64]
@@ -224,7 +220,7 @@ int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool
 }
 
 // =====================================================================================================
-// Minimizer_RV: LM driver executed by the last block of every evaluation kernel
+// Minimizer_RV: the LM pieces the cluster kernel (min_cluster.cuh) runs between its rounds
 // =====================================================================================================
 __device__ __forceinline__ double max_element36(const double *M) {
     double m = M[0];
@@ -358,20 +354,6 @@ __device__ bool lm_update(LMState &s, bool gain_with_den) {
     s.v *= 2;
     return false;
 }
-__device__ void lm_after_zero_pass(LMState &s) {   // global_tracker.cpp:686-700
-    for (int i = 0; i < 6; i++) s.Xt[i] = s.X[i];
-    s.Ft = s.F;
-    s.F0t = s.F0;
-    s.ut = s.u;
-    s.vt = s.v;
-    s.eff_steps_t = s.eff_steps;
-    s.eff_steps = 0;
-    for (int i = 0; i < 3; i++) {
-        s.X[i] = s.Vel_in[i];
-        s.X[3 + i] = s.W0_in[i];
-    }
-    lm_request(s, s.X, -1, s.iRN);
-}
 __device__ void lm_after_prior_pass(LMState &s) {  // :734-747
     if (s.F > s.Ft) {
         for (int i = 0; i < 6; i++) s.X[i] = s.Xt[i];
@@ -426,32 +408,36 @@ __device__ void lm_finalize(LMState &s, MapState *fst) {   // :793-816; RVel / R
     if (fst) fst->frame_count = fst->frame_count + 1;   // FrameCount++ (one CTA of the cluster kernel does it)
 }
 
-__device__ __forceinline__ void lm_step(LMState &s, int step, MapState *fst) {
+// LM step after an evaluation.  The two init tries of init type 2 run side by side, one step each per round:
+// lm_step_zero is the zero-initialised try (global_tracker.cpp:651-683), lm_step_main the prior-initialised try
+// (:700-732) and then the main loop (:755-816); mc_lm_merge picks the better try (:686-691, :734-747).
+__device__ __forceinline__ void lm_step_zero(LMState &z, int step) {
     switch (step) {
         case STEP_INIT_FIRST_ZERO:
-            lm_take_first(s);   // v = 2 from the declaration (:620)
-            if (s.init_iter <= 0) {
-                lm_after_zero_pass(s);
-            } else {
-                lm_solve(s, true);
-                lm_request(s, s.Xnew, -1, s.iRt);
+            lm_take_first(z);   // v = 2 from the declaration (:620)
+            if (z.init_iter > 0) {
+                lm_solve(z, true);
+                lm_request(z, z.Xnew, -1, z.iRt);
             }
             break;
         case STEP_INIT_ITER_ZERO:
-            lm_update(s, true);
-            lm_solve(s, true);
-            lm_request(s, s.Xnew, -1, s.iRt);
+            lm_update(z, true);
+            lm_solve(z, true);
+            lm_request(z, z.Xnew, -1, z.iRt);
             break;
         case STEP_INIT_LAST_ZERO:
-            lm_update(s, false);
-            lm_after_zero_pass(s);
+            lm_update(z, false);
             break;
+        default:
+            break;
+    }
+}
+__device__ __forceinline__ void lm_step_main(LMState &s, int step, MapState *fst) {
+    switch (step) {
         case STEP_INIT_FIRST_PRIOR:
             lm_take_first(s);
             s.v = 2;
-            if (s.init_iter <= 0) {
-                lm_after_prior_pass(s);
-            } else {
+            if (s.init_iter > 0) {
                 lm_solve(s, true);
                 lm_request(s, s.Xnew, -1, s.iRN);
             }
@@ -463,7 +449,6 @@ __device__ __forceinline__ void lm_step(LMState &s, int step, MapState *fst) {
             break;
         case STEP_INIT_LAST_PRIOR:
             lm_update(s, false);
-            lm_after_prior_pass(s);
             break;
         case STEP_MAIN_FIRST:
             lm_take_first(s);
@@ -607,23 +592,8 @@ __device__ void lm_begin(LMState &s, const MapState *old_st, const MapState *f_s
         lm_request(s, s.X, -1, s.iRt);
     }
 }
-__global__ void k_lm_begin(TrackState *ts, const MapState *old_st, const MapState *f_st, const double *VW,
-                           rb_minimizer_args a, double max_r, double max_s_rho, int s_rho_from_state,
-                           unsigned int frame_count, int fc_from_state) {
-    LMState &s = ts->lm;
-    lm_begin(s, old_st, f_st, VW, a, max_r, max_s_rho, s_rho_from_state, frame_count, fc_from_state);
-    if (old_st->kn <= 0) {   // "if(klist.KNum()<=0) return 0;" (:598): the evaluations launched after this do nothing,
-        s.no_keylines = 1;   // Vel / W0 stay what the caller passed, no FrameCount++
-        s.score = 0;
-        for (int i = 0; i < 3; i++) {
-            s.Vel[i] = VW[i];
-            s.W0[i] = VW[3 + i];
-        }
-    }
-}
-
-// ---- pieces of one TryVelRot evaluation (global_tracker.cpp:285-543), shared by the one-launch-per-evaluation
-// kernel k_tvr_eval and by the whole-minimisation kernel k_minimizer_cluster ---------------------------------------
+// ---- pieces of one TryVelRot evaluation (global_tracker.cpp:285-543), shared by the single-evaluation kernel
+// k_try_vel_rot and by the whole-minimisation kernel k_minimizer_cluster ---------------------------------------------
 struct TvrConst {          // constants of one minimisation
     double max_r, match_thresh, s_rho_min, k_huber;
     unsigned int mnt;      // min(match_num_thresh, FrameCount)
@@ -666,12 +636,10 @@ struct TrackPtrs {         // the pointers inside TrackState, passed by value (n
     LMState *lm;
     int *blk_has;
     double *blk_last_fi, *partials, *carry;
-    struct MinCtl *ctl;
-    unsigned long long *ll;
 };
 
 // Per-keyline part of TryVelRot (global_tracker.cpp:350-463) for U keylines of one thread: projection, field lookup,
-// residual, Jacobian products added to acc.  k_tvr_eval runs one keyline per thread; the cluster kernel a thread's
+// residual, Jacobian products added to acc.  k_try_vel_rot runs one keyline per thread; the cluster kernel a thread's
 // keylines in turn, U = 1 at a time.  Written stage by stage over the U keylines with selects instead of branches: a
 // skipped keyline (or a lane without one, act false) runs the same path and adds zeros.  The stage-by-stage form is also
 // what keeps the cluster kernel's code as measured: the same body written for one scalar keyline compiles to different
@@ -828,8 +796,8 @@ __device__ __forceinline__ void tvr_keyline(const double (&x0)[U], const double 
 }
 
 // "DResidualNew[ikl]=fi" keeps the fi of the last matched keyline before ikl (fi is a function-level variable,
-// :341,399-408): in-block scan here; misses that precede the block's first match get RES_SENTINEL and are resolved
-// lazily by whoever reads the buffer, from the per-(buffer, block) carry table.  Then the block's 28 sums go to
+// :341,399-408): in-block scan here; misses that precede the block's first match get RES_SENTINEL, which k_resolve_res
+// replaces with the block's entry of the carry table.  Then the block's 28 sums go to
 // partials[k][vb] in a fixed order, and its "has a match / last matched fi" summary to blk_has / blk_last_fi.
 // matched / need / outside / fi_own: tvr_keyline's outputs for keyline i.
 template <bool PJ>
@@ -973,28 +941,28 @@ __device__ __forceinline__ void lm_ingest(LMState &L, const double *s_tot) {
     L.n_eval++;
 }
 
-// One TryVelRot evaluation + the LM step that follows it, one launch per evaluation (stage-level API rb_try_vel_rot,
-// every minimisation under REBVO_B200_MIN_PERSIST=0, and those whose keyline capacity exceeds what the cluster kernel
-// below can keep co-resident).
+struct TvrPose {
+    double X[6];          // VelRot: V, then W
+};
+// One TryVelRot evaluation (stage-level API rb_try_vel_rot): residuals rin (read when RW) -> rout, m_id_f of the old map.
+// The last block leaves the sums in the map's LMState (JtJn, JtFn, last_score) and the stale fi of each block's leading
+// misses in tp.carry.
 template <bool RW, bool PJ>
-__global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *__restrict__ old_st,
-                                                    const unsigned long long *__restrict__ field,
-                                                    const float4 *__restrict__ fpack, MapState *f_st, TrackPtrs tp,
-                                                    ResPtrs res, unsigned int *ticket, CamC cam, int step) {
+__global__ void __launch_bounds__(TVR_T) k_try_vel_rot(KLSoA old, const MapState *__restrict__ old_st,
+                                                       const unsigned long long *__restrict__ field,
+                                                       const float4 *__restrict__ fpack, TrackPtrs tp,
+                                                       const double *__restrict__ rin, double *__restrict__ rout,
+                                                       unsigned int *ticket, CamC cam, TvrPose pose, TvrConst tc) {
     __shared__ double sR[9], sV[3], sRM[4];
     __shared__ TvrSmem sm;
     __shared__ double s_tot[28];
     __shared__ bool s_last;
-    LMState &lm = *tp.lm;
-    if (lm.no_keylines) return;   // (the minimisation of an empty old map ended in k_lm_begin)
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) {   // the two exponentials run on two warps side by side (each is a serial sin/cos chain)
-        double X[6];
-        for (int i = 0; i < 6; i++) X[i] = lm.Xeval[i];
-        so3_exp(X + 3, sR);                        // SO3<> RotW0(VelRot.slice<3,3>())
-        for (int i = 0; i < 3; i++) sV[i] = X[i];
+        so3_exp(pose.X + 3, sR);                   // SO3<> RotW0(VelRot.slice<3,3>())
+        for (int i = 0; i < 3; i++) sV[i] = pose.X[i];
     } else if (tid == 32) {
-        double wz[3] = {0, 0, lm.Xeval[5]}, RMf[9];
+        double wz[3] = {0, 0, pose.X[5]}, RMf[9];
         so3_exp(wz, RMf);                          // SO3<> RotM(makeVector(0,0,VelRot[5]))
         sRM[0] = RMf[0];
         sRM[1] = RMf[1];
@@ -1002,15 +970,6 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
         sRM[3] = RMf[4];
     }
     __syncthreads();
-    const int res_in = lm.res_in, res_out = lm.res_out;
-    TvrConst tc;
-    tc.max_r = lm.max_r;
-    tc.match_thresh = lm.match_thresh;
-    tc.s_rho_min = lm.s_rho_min;
-    tc.k_huber = lm.k_huber;
-    tc.mnt = lm.match_num_thresh < lm.frame_count ? lm.match_num_thresh : lm.frame_count;
-    const double *__restrict__ rin = (RW && res_in >= 0) ? res.r[res_in] : nullptr;
-    double *__restrict__ rout = res.r[res_out];
 
     const int K0 = old_st->kn;
     const int i = blockIdx.x * TVR_T + tid;
@@ -1020,11 +979,7 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
     double r_prev = 0.0;
     if (act) {
         o = load_klop(old, i, cam);
-        if (RW && rin) {
-            r_prev = rin[i];
-            if ((unsigned long long)__double_as_longlong(r_prev) == RES_SENTINEL)
-                r_prev = tp.carry[res_in * TVR_T + blockIdx.x];   // stale-fi carry of the evaluation that wrote rin
-        }
+        if (RW) r_prev = rin[i];
     }
     const bool skip = !act || o.s_rho > tc.s_rho_min || (unsigned int)o.m_num < tc.mnt;   // :356
     double acc[28];
@@ -1032,8 +987,8 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
     for (int k = 0; k < 28; k++) acc[k] = 0;
     bool matched[1], need[1], outside[1];
     double fi_own[1];
-    tvr_keyline<RW, PJ, 1>({o.x0}, {o.y0}, {o.z0}, {o.s_rho}, {o.m}, {o.n_m}, {skip}, {act}, rin != nullptr, {r_prev}, sR, sV,
-                           sRM, tc, cam, field, fpack, old.m_id_f, {i}, acc, matched, need, fi_own, outside);
+    tvr_keyline<RW, PJ, 1>({o.x0}, {o.y0}, {o.z0}, {o.s_rho}, {o.m}, {o.n_m}, {skip}, {act}, RW, {r_prev}, sR, sV, sRM, tc,
+                           cam, field, fpack, old.m_id_f, {i}, acc, matched, need, fi_own, outside);
     tvr_block_tail<PJ>(matched[0], need[0], outside[0], fi_own[0], tc.max_r, rout, i, acc, sm, tp.partials + blockIdx.x, TVR_T,
                        tp.blk_has + blockIdx.x, tp.blk_last_fi + blockIdx.x, tid, lane, wid);
     __threadfence();
@@ -1041,52 +996,32 @@ __global__ void __launch_bounds__(TVR_T) k_tvr_eval(KLSoA old, const MapState *_
     if (tid == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
     __syncthreads();
     if (!s_last) return;
-    // ================= last block: grid reduction, stale-fi carries, LM step ==========================
+    // ================= last block: grid reduction, stale-fi carries ==========================
     __threadfence();
-    const int nb = gridDim.x;   // <= TVR_T (checked by the host)
+    const int nb = gridDim.x;   // <= TVR_T: at most 196 blocks for a capacity of RB_KCAP_MAX keylines
     tvr_grid_reduce<PJ>(tp.partials, nb, s_tot, lane, wid);
     __shared__ double s_blast[TVR_T];
     __shared__ unsigned int s_wmask[TVR_T / 32];
-    {
-        int has = 0;
-        double lastv = 0;
-        if (tid < nb) {
-            has = __ldcg(tp.blk_has + tid);
-            lastv = __ldcg(tp.blk_last_fi + tid);
-        }
-        tvr_carries(has, lastv, tp.carry + res_out * TVR_T, nb, s_blast, s_wmask, tid, lane, wid);
+    int has = 0;
+    double lastv = 0;
+    if (tid < nb) {
+        has = __ldcg(tp.blk_has + tid);
+        lastv = __ldcg(tp.blk_last_fi + tid);
     }
-    // the serial LM step works on a shared-memory copy of the state (global round trips would dominate it)
-    __shared__ LMState s_lm;
-    {
-        const double *src = reinterpret_cast<const double *>(&lm);
-        double *dst = reinterpret_cast<double *>(&s_lm);
-        for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += TVR_T) dst[k] = __ldcg(src + k);
-    }
-    __syncthreads();
+    tvr_carries(has, lastv, tp.carry, nb, s_blast, s_wmask, tid, lane, wid);   // (synchronises: s_tot is complete)
     if (tid == 0) {
-        lm_ingest<PJ>(s_lm, s_tot);
-        lm_step(s_lm, step, f_st);
+        lm_ingest<PJ>(*tp.lm, s_tot);
         *ticket = 0;
-    }
-    __syncthreads();
-    if (step == STEP_MAIN_LAST || (step == STEP_MAIN_FIRST && s_lm.iter_max <= 0)) {
-        lm_finalize_cov(s_lm, tid);
-        __syncthreads();
-    }
-    {
-        const double *src = reinterpret_cast<const double *>(&s_lm);
-        double *dst = reinterpret_cast<double *>(&lm);
-        for (int k = tid; k < (int)(sizeof(LMState) / sizeof(double)); k += TVR_T) dst[k] = src[k];
     }
 }
 
 // =====================================================================================================
 // Whole Minimizer_RV in ONE launch (min_cluster.cuh).  The ~12 evaluations of a frame are strictly dependent (each pose
-// comes out of the LM step on the previous sums), so with one launch per evaluation a frame pays 12x (launch + operand
+// comes out of the LM step on the previous sums), so with one launch per evaluation a frame would pay 12x (launch + operand
 // re-load + last-block hand-over through L2).  Declarations of the cluster kernel k_minimizer_cluster<T>:
 // =====================================================================================================
-#define MIN_MAX_EVALS 32
+#define MIN_MAX_EVALS 64                     // evaluations of one minimisation (rb_minimizer_enqueue refuses more)
+#define MIN_MAX_ROUNDS (MIN_MAX_EVALS - 1)   // rounds of such a minimisation: the init tries of type 2 share theirs
 struct MinSetup {
     rb_minimizer_args a;
     double max_r, max_s_rho;
@@ -1171,36 +1106,8 @@ __device__ __forceinline__ void d_fm_argmax_two(const KLSoA &old, int i0, int i1
 
 #include "min_cluster.cuh"
 
-static TrackPtrs track_ptrs(const rb_map *fmap) {
-    TrackPtrs tp;
-    tp.lm = &fmap->ts->lm;
-    tp.blk_has = fmap->ts_host.blk_has;
-    tp.blk_last_fi = fmap->ts_host.blk_last_fi;
-    tp.partials = fmap->ts_host.partials;
-    tp.carry = fmap->ts_host.carry;
-    tp.ctl = fmap->ts_host.ctl;
-    tp.ll = fmap->ts_host.ll;
-    return tp;
-}
-
-template <bool RW, bool PJ>
-static int launch_eval(rb_ctx *c, rb_map *fmap, rb_map *old, int step) {
-    ResPtrs rp;
-    for (int i = 0; i < 3; i++) rp.r[i] = fmap->res[i];
-    const int nblk = fmap->ts_host.nblk;
-    k_tvr_eval<RW, PJ><<<nblk, TVR_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, fmap->st,
-                                                     track_ptrs(fmap), rp, c->ticket + 1, make_cam(c), step);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-static int launch_eval_step(rb_ctx *c, rb_map *fmap, rb_map *old, int step) {
-    if (step >= STEP_MAIN_FIRST) return launch_eval<true, true>(c, fmap, old, step);
-    if (step == STEP_INIT_LAST_ZERO || step == STEP_INIT_LAST_PRIOR) return launch_eval<false, false>(c, fmap, old, step);
-    return launch_eval<false, true>(c, fmap, old, step);
-}
-
-// per-device set-up of the cluster minimiser (rb_ctx_create, after cudaSetDevice): opt-ins + how many keylines per CTA
-// fit.  Leaves c->min_cluster_kpc = 0 when the device cannot run it (the one-launch-per-evaluation path serves then).
+// per-device set-up of the cluster minimiser (rb_ctx_create, after cudaSetDevice, c->kcap <= RB_KCAP_MAX): opt-ins + how
+// many keylines per CTA fit.  RB_ERR_CUDA when the device cannot run the one-cluster form.
 void rb_mapper_cluster_setup();   // (defined after the mapper's cluster kernels)
 template <typename K>
 static bool mc_prepare(K kern, int threads, int clusters, size_t dyn, int dev_max) {
@@ -1218,30 +1125,30 @@ static bool mc_prepare(K kern, int threads, int clusters, size_t dyn, int dev_ma
 }
 int rb_minimizer_cluster_setup(rb_ctx *c) {
     rb_mapper_cluster_setup();
-    c->min_cluster_kpc = 0;
     c->min_cluster_g = 1;
     const char *fa_ = getenv("REBVO_B200_MIN_FORCE_ABORT");
     c->min_debug_abort = fa_ ? atoi(fa_) : 0;
     int dev_max = 0;
-    if (cudaDeviceGetAttribute(&dev_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device) != cudaSuccess) return RB_OK;
+    RB_CUDA(cudaDeviceGetAttribute(&dev_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
     int kfast = MC_KPC_FAST;                   // keylines per cluster rank kept in shared memory (the rest works from global memory)
     const char *kf = getenv("REBVO_B200_MIN_KPC");
     if (kf && atoi(kf) >= 32) kfast = atoi(kf) & ~31;
-    // one cluster of 512-thread CTAs: always possible when the capacity fits its virtual-warp tables
+    // one cluster of 512-thread CTAs: every capacity up to RB_KCAP_MAX fits its virtual-warp tables (MC_KPC_MAX)
     {
         int kpc = (c->kcap + MC_C - 1) / MC_C;
         kpc = (kpc + 31) & ~31;
-        if (kpc <= MC_KPC_MAX) {
-            if (kpc > kfast) kpc = kfast;
-            const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
-            if (mc_prepare(k_minimizer_cluster<512>, 512, 1, dyn, dev_max)) {
-                c->min_cluster_kpc = kpc;
-                c->min_cluster_dyn = dyn;
-            }
+        if (kpc > kfast) kpc = kfast;
+        const size_t dyn = (size_t)kpc * MC_BYTES_PER_KL + 64;
+        if (!mc_prepare(k_minimizer_cluster<512>, 512, 1, dyn, dev_max)) {
+            const cudaError_t e = cudaGetLastError();
+            snprintf(c->err, sizeof(c->err), "Minimizer_RV: the device cannot run a %d-CTA cluster of 512 threads with %zu "
+                     "bytes of dynamic shared memory (%s)", MC_C, dyn, cudaGetErrorString(e));
+            return RB_ERR_CUDA;
         }
+        c->min_cluster_kpc = kpc;
+        c->min_cluster_dyn = dyn;
     }
-    cudaGetLastError();
-    // several clusters of 256-thread CTAs (default 4 = 64 SMs): the per-evaluation keyline pass is the longest part of a
+    // several clusters of 256-thread CTAs (default 4 = 64 SMs): each evaluation's keyline pass is the longest part of a
     // round and scales with the SMs; the clusters exchange their sums through L2.  Needs all clusters co-resident: checked
     // here for an idle device (spins are bounded and abort otherwise), so contexts that share a GPU should ask for
     // REBVO_B200_MIN_G=1.
@@ -1249,7 +1156,7 @@ int rb_minimizer_cluster_setup(rb_ctx *c) {
     const char *ge = getenv("REBVO_B200_MIN_G");
     if (ge) G = atoi(ge);
     if (G > MC_GMAX) G = MC_GMAX;
-    if (c->min_cluster_kpc > 0 && G > 1) {
+    if (G > 1) {
         int kpc = (c->kcap + MC_C * G - 1) / (MC_C * G);
         kpc = (kpc + 31) & ~31;
         if (kpc <= MC_KPC_MAX) {
@@ -1299,64 +1206,41 @@ static int launch_minimizer_cluster(rb_ctx *c, rb_map *fmap, rb_map *old, const 
 
 int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_dev, const rb_minimizer_args *a,
                          double max_s_rho, bool s_rho_from_state, unsigned int frame_count, bool fc_from_state,
-                         FrameState *post_fs, bool *post_folded) {
-    if (post_folded) *post_folded = false;
+                         FrameState *post_fs) {
     if (fmap->field_radius <= 0) {
         snprintf(c->err, sizeof(c->err), "Minimizer_RV before build_field");
         return RB_ERR_STATE;
     }
-    const int nblk = fmap->ts_host.nblk;
-    if (nblk > TVR_T) return RB_ERR_ARG;
-    // the evaluation sequence of Minimizer_RV (global_tracker.cpp:640-791) is fixed by the configuration
+    // the evaluation sequence of Minimizer_RV (global_tracker.cpp:640-791) is fixed by the configuration.  At most
+    // MIN_MAX_EVALS evaluations, counting both init tries whatever the init type: at most MIN_MAX_ROUNDS rounds.
     const int n = a->init_iter, m = a->iter_max;
-    int steps[2 * MIN_MAX_EVALS], ns = 0;
-    if (n < 0 || m < 0 || 2 * (n + 1) + m + 1 > 2 * MIN_MAX_EVALS) return RB_ERR_ARG;
+    if (n < 0 || m < 0 || 2 * (n + 1) + m + 1 > MIN_MAX_EVALS) return RB_ERR_ARG;
+    // rounds of the cluster kernel: the two init tries of type 2 share their rounds
+    McPlan plan;
+    memset(&plan, 0, sizeof(plan));
+    plan.merge_round = -1;
+    int k = 0;
     if (a->init_type != 0 && a->init_type != 1) {
-        steps[ns++] = STEP_INIT_FIRST_ZERO;
-        for (int i = 0; i < n; i++) steps[ns++] = i == n - 1 ? STEP_INIT_LAST_ZERO : STEP_INIT_ITER_ZERO;
-        steps[ns++] = STEP_INIT_FIRST_PRIOR;
-        for (int i = 0; i < n; i++) steps[ns++] = i == n - 1 ? STEP_INIT_LAST_PRIOR : STEP_INIT_ITER_PRIOR;
-    }
-    steps[ns++] = STEP_MAIN_FIRST;
-    for (int j = 0; j < m; j++) steps[ns++] = j == m - 1 ? STEP_MAIN_LAST : STEP_MAIN_ITER;
-    int r;
-    if (c->min_persist && c->min_cluster_kpc > 0 && ns <= MIN_MAX_EVALS) {
-        // rounds of the cluster kernel: the two init tries of type 2 share their rounds
-        McPlan plan;
-        memset(&plan, 0, sizeof(plan));
-        plan.merge_round = -1;
-        int k = 0;
-        if (a->init_type != 0 && a->init_type != 1) {
-            for (int i = 0; i <= n; i++, k++) {
-                plan.sa[k] = i == 0 ? STEP_INIT_FIRST_ZERO : i == n ? STEP_INIT_LAST_ZERO : STEP_INIT_ITER_ZERO;
-                plan.sb[k] = i == 0 ? STEP_INIT_FIRST_PRIOR : i == n ? STEP_INIT_LAST_PRIOR : STEP_INIT_ITER_PRIOR;
-            }
-            plan.merge_round = k - 1;
+        for (int i = 0; i <= n; i++, k++) {
+            plan.sa[k] = i == 0 ? STEP_INIT_FIRST_ZERO : i == n ? STEP_INIT_LAST_ZERO : STEP_INIT_ITER_ZERO;
+            plan.sb[k] = i == 0 ? STEP_INIT_FIRST_PRIOR : i == n ? STEP_INIT_LAST_PRIOR : STEP_INIT_ITER_PRIOR;
         }
-        plan.sb[k++] = STEP_MAIN_FIRST;
-        for (int j = 0; j < m; j++) plan.sb[k++] = j == m - 1 ? STEP_MAIN_LAST : STEP_MAIN_ITER;
-        plan.n = k;
-        MinSetup su;
-        su.a = *a;
-        su.max_r = (double)fmap->field_radius;
-        su.max_s_rho = max_s_rho;
-        su.VW = VW_dev;
-        su.frame_count = frame_count;
-        su.s_rho_from_state = s_rho_from_state ? 1 : 0;
-        su.fc_from_state = fc_from_state ? 1 : 0;
-        su.debug_abort = c->min_debug_abort;
-        su.early_operands = c->min_early ? 1 : 0;
-        if ((r = launch_minimizer_cluster(c, fmap, old, plan, su, post_fs))) return r;
-        if (post_folded) *post_folded = post_fs != nullptr;
-        return RB_OK;
+        plan.merge_round = k - 1;
     }
-    RB_CUDA(cudaMemsetAsync(fmap->res[0], 0, sizeof(double) * (size_t)c->kcap, c->stream));   // Residual[i]=0 (:625)
-    k_lm_begin<<<1, 1, 0, c->stream>>>(fmap->ts, old->st, fmap->st, VW_dev, *a, (double)fmap->field_radius,
-                                       max_s_rho, s_rho_from_state ? 1 : 0, frame_count, fc_from_state ? 1 : 0);
-    RB_LAUNCH_CHECK();
-    for (int i = 0; i < ns; i++)
-        if ((r = launch_eval_step(c, fmap, old, steps[i]))) return r;
-    return RB_OK;
+    plan.sb[k++] = STEP_MAIN_FIRST;
+    for (int j = 0; j < m; j++) plan.sb[k++] = j == m - 1 ? STEP_MAIN_LAST : STEP_MAIN_ITER;
+    plan.n = k;
+    MinSetup su;
+    su.a = *a;
+    su.max_r = (double)fmap->field_radius;
+    su.max_s_rho = max_s_rho;
+    su.VW = VW_dev;
+    su.frame_count = frame_count;
+    su.s_rho_from_state = s_rho_from_state ? 1 : 0;
+    su.fc_from_state = fc_from_state ? 1 : 0;
+    su.debug_abort = c->min_debug_abort;
+    su.early_operands = c->min_early ? 1 : 0;
+    return launch_minimizer_cluster(c, fmap, old, plan, su, post_fs);
 }
 
 int rb_minimizer_check_abort(rb_ctx *c, rb_map *fmap) {
@@ -1370,45 +1254,38 @@ int rb_minimizer_check_abort(rb_ctx *c, rb_map *fmap) {
     return RB_ERR_CUDA;
 }
 
-// materialise the lazily resolved entries of a residual buffer (host export of DResidualNew in rb_try_vel_rot)
+// the leading misses of each block of rb_try_vel_rot's output (res[1]) get the stale fi of the blocks before them
 __global__ void __launch_bounds__(TVR_T) k_resolve_res(double *res, const double *carry, const MapState *old_st) {
     const int i = blockIdx.x * TVR_T + threadIdx.x;
     if (i >= old_st->kn) return;
     if (reinterpret_cast<unsigned long long *>(res)[i] == RES_SENTINEL) res[i] = carry[blockIdx.x];
 }
-int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, int buf) {
-    k_resolve_res<<<fmap->ts_host.nblk, TVR_T, 0, c->stream>>>(fmap->res[buf], fmap->ts_host.carry + buf * TVR_T, old->st);
+int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old) {
+    k_resolve_res<<<fmap->ts_host.nblk, TVR_T, 0, c->stream>>>(fmap->res[1], fmap->ts_host.carry, old->st);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
 
-// single evaluation for the parity tests (rb_try_vel_rot)
-__global__ void k_lm_single(TrackState *ts, const double *X, int res_in, int res_out, double max_r, double mt,
-                            double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber) {
-    LMState &s = ts->lm;
-    for (int i = 0; i < 6; i++) s.Xeval[i] = X[i];
-    s.res_in = res_in;
-    s.res_out = res_out;
-    s.max_r = max_r;
-    s.match_thresh = mt;
-    s.s_rho_min = s_rho_min;
-    s.match_num_thresh = mnt;
-    s.frame_count = fc;
-    s.k_huber = k_huber;
-    s.no_keylines = 0;
-}
-
-int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *X_dev, int reweight, int procjf,
-                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc,
-                           double k_huber) {
+// one TryVelRot evaluation at pose X from res[0] (the caller's residuals or zeros) to res[1] (rb_try_vel_rot)
+int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double X[6], int reweight, int procjf,
+                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber) {
     if (fmap->field_radius <= 0) return RB_ERR_STATE;
-    k_lm_single<<<1, 1, 0, c->stream>>>(fmap->ts, X_dev, 0, 1, (double)fmap->field_radius, match_thresh, s_rho_min,
-                                        mnt, fc, k_huber);
+    TvrPose pose;
+    for (int i = 0; i < 6; i++) pose.X[i] = X[i];
+    TvrConst tc;
+    tc.max_r = (double)fmap->field_radius;
+    tc.match_thresh = match_thresh;
+    tc.s_rho_min = s_rho_min;
+    tc.k_huber = k_huber;
+    tc.mnt = mnt < fc ? mnt : fc;
+    const TrackState &h = fmap->ts_host;
+    const TrackPtrs tp = {&fmap->ts->lm, h.blk_has, h.blk_last_fi, h.partials, h.carry};
+    auto kern = reweight ? (procjf ? k_try_vel_rot<true, true> : k_try_vel_rot<true, false>)
+                         : (procjf ? k_try_vel_rot<false, true> : k_try_vel_rot<false, false>);
+    kern<<<h.nblk, TVR_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, tp, fmap->res[0], fmap->res[1],
+                                          c->ticket + 1, make_cam(c), pose, tc);
     RB_LAUNCH_CHECK();
-    if (reweight && procjf) return launch_eval<true, true>(c, fmap, old, STEP_NONE);
-    if (reweight) return launch_eval<true, false>(c, fmap, old, STEP_NONE);
-    if (procjf) return launch_eval<false, true>(c, fmap, old, STEP_NONE);
-    return launch_eval<false, false>(c, fmap, old, STEP_NONE);
+    return RB_OK;
 }
 
 // =====================================================================================================
@@ -1520,7 +1397,7 @@ int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu) {
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
-int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
+static int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
     RB_KLAUNCH(k_fm_argmax, rb_div_up(c->kcap, 256), 256, 0, old->kl, (const MapState *)old->st,
                (const MapState *)neu->st, neu->ts_host.fm_best);
     return RB_OK;

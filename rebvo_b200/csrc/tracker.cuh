@@ -45,21 +45,19 @@ struct rb_minimizer_args {
 // (V then W); max_s_rho is read from old->st->s_rho_q when s_rho_from_state, else from the argument.
 // The optional FrameState / FrameArgs / rb_nav arguments below belong to the per-frame pipeline (frame.cuh): when given,
 // the one-thread glue stage next to the kernel runs inside it instead of as its own launch.
-// rb_minimizer_enqueue with post_fs: when *post_folded comes back set, the stage after the minimiser (d_frame_post_min)
-// and FordwardMatch's arg-max of old into fmap (rb_forward_match_argmax_enqueue; scratch cleared before) ran inside it.
+// rb_minimizer_enqueue with post_fs: the stage after the minimiser (d_frame_post_min) and FordwardMatch's arg-max of old
+// into fmap (its scratch cleared before by rb_forward_match_init_enqueue) run inside it.
 struct FrameState;
 struct FrameArgs;
 int rb_minimizer_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double *VW_dev,
                          const rb_minimizer_args *a, double max_s_rho, bool s_rho_from_state,
-                         unsigned int frame_count, bool frame_count_from_state, FrameState *post_fs = nullptr,
-                         bool *post_folded = nullptr);
+                         unsigned int frame_count, bool frame_count_from_state, FrameState *post_fs = nullptr);
 int rb_quantile_enqueue(rb_ctx *c, rb_map *m, double smin, double smax, double perc, int nbins,
                         FrameState *fs = nullptr, const unsigned int *frame_count_dev = nullptr, MapState *nst = nullptr);
 int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool min_mod_from_state);
 // FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu);
 // rb_forward_match_enqueue is the whole stage.
 int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu);
-int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev);

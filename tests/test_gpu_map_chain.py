@@ -61,10 +61,9 @@ def test_chain_mirror(built, stream, monkeypatch, mode):
     assert_runs_identical(*_two_schedules(monkeypatch, stream, 20, kc=EUROC_KC, mirror=mode), "mirror %d" % mode)
 
 
-@pytest.mark.parametrize("env", ["REBVO_B200_OVERLAP", "REBVO_B200_MIN_PERSIST", "REBVO_B200_NO_GRAPH"])
+@pytest.mark.parametrize("env", ["REBVO_B200_OVERLAP", "REBVO_B200_NO_GRAPH"])
 def test_chain_schedules(built, stream, monkeypatch, env):
-    """one stream without the side streams (OVERLAP=0), the one-launch-per-evaluation minimiser whose arg-max is its
-    own kernel (MIN_PERSIST=0), and eager launches (NO_GRAPH=1)"""
+    """one stream without the side streams (OVERLAP=0), and eager launches (NO_GRAPH=1)"""
     monkeypatch.setenv(env, "1" if env == "REBVO_B200_NO_GRAPH" else "0")
     assert_runs_identical(*_two_schedules(monkeypatch, stream, 20), env)
 

@@ -1,8 +1,8 @@
 """Every form of Minimizer_RV against the reference: the four-cluster kernel (the default), the one-cluster kernel
 (REBVO_B200_MIN_G=1), two and three clusters, the cluster kernels with a 32-keyline shared-memory slice (every other
-keyline spills to global memory, REBVO_B200_MIN_KPC=32), operands staged after the launch dependency
-(REBVO_B200_MIN_EARLY=0), and one k_tvr_eval launch per evaluation (REBVO_B200_MIN_PERSIST=0).  All share the per-keyline
-body and the LM steps.
+keyline spills to global memory, REBVO_B200_MIN_KPC=32), and operands staged after the launch dependency
+(REBVO_B200_MIN_EARLY=0).  Every form runs a minimisation in one launch, and shares the per-keyline body with the
+stage-level TryVelRot (rb_try_vel_rot, one launch of 256-keyline blocks).
 
 test_minimiser_form runs test_gpu_parity.py's tracker block on the EuRoC frame pair, with its bars: the stage-level
 TryVelRot at three poses x three (reweight, procjf) pairs, then Minimizer_RV, m_id_f exact.
@@ -13,9 +13,13 @@ sub-pixel jitter up to any K0 <= KEYLINE_MAX, with the depth, gate and gradient 
 are empty, partial, full and one past full, the s_rho and m_num gates (m_num beyond the kernel's 8-bit flag), runs of
 misses whose stale residual (DResidualNew[ikl] = fi of the last match, global_tracker.cpp:341,406) crosses every
 virtual-warp, slice, cluster, column and block boundary, projections on the image border, every LM schedule, degenerate
-maps and two minimisations on one new map.  Every case also runs a NumPy restatement of the LM driver
+maps, two minimisations on one new map, and schedules of more than 32 rounds.  Every case also runs a NumPy restatement of the LM driver
 (global_tracker.cpp:598-817) on the reference's own TryVelRot: it must agree with the reference, and its trace proves that
-the case reached its target (a vacuous case fails) and that no LM decision sits on a knife edge."""
+the case reached its target (a vacuous case fails) and that no LM decision sits on a knife edge.
+
+test_try_vel_rot_stale runs the stage-level TryVelRot on the stale-residual states against the reference: its misses
+inherit the fi of the last match across warp and block boundaries, and each evaluation reads the residuals of the one
+before it."""
 import numpy as np
 import pytest
 
@@ -23,13 +27,12 @@ from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG, Bench, Report
 
 pytestmark = pytest.mark.gpu
 
-FORMS = {"four_clusters": {}, "one_cluster": {"REBVO_B200_MIN_G": "1"}, "per_evaluation": {"REBVO_B200_MIN_PERSIST": "0"},
-         "two_clusters": {"REBVO_B200_MIN_G": "2"}, "three_clusters": {"REBVO_B200_MIN_G": "3"},
+FORMS = {"four_clusters": {}, "one_cluster": {"REBVO_B200_MIN_G": "1"}, "two_clusters": {"REBVO_B200_MIN_G": "2"}, "three_clusters": {"REBVO_B200_MIN_G": "3"},
          "spill_g4": {"REBVO_B200_MIN_KPC": "32"}, "spill_g1": {"REBVO_B200_MIN_G": "1", "REBVO_B200_MIN_KPC": "32"},
          "late_operands": {"REBVO_B200_MIN_EARLY": "0"}}
-CLUSTERS = {"four_clusters": 4, "one_cluster": 1, "per_evaluation": 0, "two_clusters": 2, "three_clusters": 3,
+CLUSTERS = {"four_clusters": 4, "one_cluster": 1, "two_clusters": 2, "three_clusters": 3,
             "spill_g4": 4, "spill_g1": 1, "late_operands": 4}
-ENV_KEYS = ("REBVO_B200_MIN_G", "REBVO_B200_MIN_PERSIST", "REBVO_B200_MIN_KPC", "REBVO_B200_MIN_EARLY")
+ENV_KEYS = ("REBVO_B200_MIN_G", "REBVO_B200_MIN_KPC", "REBVO_B200_MIN_EARLY")
 
 
 def _set_form_env(monkeypatch, form):
@@ -72,13 +75,12 @@ def test_minimiser_form(built, monkeypatch, form):
     gm[1].reestimate(cfg["track_points"], 100)
 
     m_r = tracker_parity(rep, cfg, refs, gm, rt)
-    # the switches took effect: the cluster forms run a minimisation in one launch, the other in one per evaluation
+    # a minimisation is one launch in every form
     n0 = ctx.launches()
     gm[1].minimizer_rv(gm[0], m_r["V"], m_r["W"], cfg["match_thresh"], cfg["iter_max"], cfg["init_type"],
                        cfg["reweight"], 1e3, cfg["match_num_thresh"], cfg["init_iter"])
     launches = ctx.launches() - n0
-    n_eval = 2 * (cfg["init_iter"] + 1) + cfg["iter_max"] + 1
-    assert launches >= n_eval if form == "per_evaluation" else launches <= 2, launches
+    assert launches <= 2, launches
     for g in gm:
         g.close()
     ctx.close()
@@ -95,7 +97,6 @@ MIN_HITS = 50            # keylines (misses, decisions ...) a case must put on i
 MARGIN = 1e-9            # least relative margin of an LM decision (gain > 0, F > Ft)
 H_TINY = 1e-11           # steps at most this long decide nothing that moves the pose
 MAX_R = 40.0             # build_field radius = TryVelRot's max_r
-MIN_MAX_EVALS = 32       # evaluations the cluster kernel runs in one launch (tracker.cu)
 V_FAR = np.array([0.02, -0.015, 0.01])       # a prior far from the frame pair's motion
 W_FAR = np.array([0.01, 0.012, -0.008])
 BASE = dict(mt=CFG["match_thresh"], iter_max=5, init_type=2, init_iter=2, k_huber=2.0, mnt=0, q=1e3, prior="zero")
@@ -106,12 +107,12 @@ def _kpc(K0, G):
     return min((k + 31) & ~31, 3584)
 
 
+BLOCKS = dict(G=0)       # the geometry of rb_try_vel_rot: 256-keyline blocks
+
+
 def _geometry(form, K0):
-    """How the form splits K0 keylines: cluster kernels -> (slice size kpc, shared-memory keylines S, clusters G, CTA
-    threads T); per_evaluation -> 256-keyline blocks."""
+    """How the form splits K0 keylines: slice size kpc, shared-memory keylines S, clusters G, CTA threads T"""
     G = CLUSTERS[form]
-    if G == 0:
-        return dict(G=0, unit=256)
     spill = "REBVO_B200_MIN_KPC" in FORMS[form]
     S = 32 if spill else {1: 1280, 2: 640, 3: 448, 4: 320}[G]
     kpc = _kpc(K0, G)
@@ -138,7 +139,7 @@ def _crossing(geo, j, i):
 
 
 def _classes(geo, K0):
-    """The boundary classes the form's geometry has at K0 keylines."""
+    """The boundary classes the geometry has at K0 keylines."""
     if geo["G"] == 0:
         return ["warp"] + (["block"] if K0 > 256 else [])
     c = ["vwarp", "column"]
@@ -289,6 +290,12 @@ for _n in (0, 1, 3):
 STATES["init2_n0_iter0_zero"] = dict(K0=8000, init_iter=0, iter_max=0, prior="far", fc=0, want=["eff0"])
 STATES["ns32"] = dict(K0=8000, init_iter=2, iter_max=25, prior="near", fc=0, want=["ns32"])
 STATES["ns33"] = dict(K0=8000, init_iter=2, iter_max=26, prior="near", fc=0, want=["ns33"])
+# the longest well-posed schedule near the API's limit (64 evaluations, 63 rounds at init_iter 0, iter_max 61), twice on
+# one map, so that the second minimisation's sequence numbers of the multi-cluster exchange follow those of a 48-round
+# one.  This map converges after one step and every later step is rejected: the 45th rejection in a row overflows u *= v
+# to inf, and every evaluation after it runs at a NaN pose.  So 46 iterations, the last of them that rejection: 49
+# evaluations in 48 rounds.
+STATES["ns49"] = dict(K0=8000, init_iter=0, iter_max=46, prior="near", fc=0, calls=["main", "main"], want=["ns49"])
 STATES["K0_then_gate"] = dict(K0=8000, fc=2, mnt=3, m_num=_mn2, calls=["empty", "main"], want=["empty"])
 STATES["back_to_back"] = dict(K0=8000, fc=2, mnt=3, m_num=_mn2, calls=["main", "main"], want=["gate_change"])
 STATES["all_skipped"] = dict(K0=3000, kind="all_skipped", fc=0, want=["degenerate"])
@@ -330,7 +337,7 @@ def _lm_driver(new_r, old_r, a, V, W):
         s, J, Fv, out = new_r.try_vel_rot(old_r, X, rw, pj, a["mt"], a["q"], a["mnt"], a["k_huber"], buf[rin])
         wrote = ~np.isnan(out)
         buf[rout] = np.where(wrote, out, buf[rout])
-        tr["evals"].append(dict(rw=rw, res=out[:K0].copy(), matched=old_r.keylines()["m_id_f"] >= 0,
+        tr["evals"].append(dict(X=np.array(X, np.float64), rw=rw, res=out[:K0].copy(), matched=old_r.keylines()["m_id_f"] >= 0,
                                 wrote=wrote[:K0]))
         return s, J, Fv
 
@@ -542,22 +549,9 @@ def _evidence(st, form):
             if gate > 0 and n_m < MIN_HITS:
                 msgs.append("m_num gate closes for %d keylines" % n_m)
         elif w == "stale":
-            cnt = {}
-            for e in tr["evals"]:
-                res, mt, wr = e["res"], e["matched"], e["wrote"]
-                idx = np.arange(K0)
-                lastm = np.maximum.accumulate(np.where(mt, idx, -1))
-                prev = np.concatenate([[-1], lastm[:-1]])
-                miss = wr & ~mt & (res != MAX_R)
-                cls = _crossing(geo, prev[miss], idx[miss])
-                big = np.abs(res[miss]) > sp["k_huber"]
-                for c in set(cls):
-                    sel = cls == c
-                    cnt[c] = cnt.get(c, 0) + int((sel & (big | (c == "start"))).sum())
+            cnt = _carried(geo, tr["evals"], K0, sp["k_huber"])
             info["carried misses"] = cnt
-            for c in _classes(geo, K0) + ["start"]:
-                if cnt.get(c, 0) < MIN_HITS:
-                    msgs.append("only %d carried misses across %s" % (cnt.get(c, 0), c))
+            msgs += _too_few_carried(geo, K0, cnt)
         elif w == "outside":
             e0 = tr["evals"][0]   # the zero-initialised try's first pose: X = 0
             n_out = int((e0["wrote"] & (e0["res"] == MAX_R) & ~e0["matched"]).sum())
@@ -576,7 +570,7 @@ def _evidence(st, form):
             info["eff_steps"] = tr.get("eff")
             if tr.get("eff") != 0:
                 msgs.append("eff_steps %s" % tr.get("eff"))
-        elif w in ("ns32", "ns33"):
+        elif w in ("ns32", "ns33", "ns49"):
             info["evals"] = len(tr["evals"])
             if len(tr["evals"]) != int(w[2:]):
                 msgs.append("%d evaluations" % len(tr["evals"]))
@@ -594,6 +588,29 @@ def _evidence(st, form):
             if usable >= 6:
                 msgs.append("%d usable keylines" % usable)
     return msgs, info
+
+
+def _carried(geo, evals, K0, k_huber):
+    """misses per boundary class between the miss and the last match before it whose inherited fi the evaluations wrote
+    (a miss at the start inherits 0; elsewhere only an fi beyond k_huber counts, one that changes a re-weighting)"""
+    cnt = {}
+    idx = np.arange(K0)
+    for e in evals:
+        res, mt, wr = e["res"], e["matched"], e["wrote"]
+        lastm = np.maximum.accumulate(np.where(mt, idx, -1))
+        prev = np.concatenate([[-1], lastm[:-1]])
+        miss = wr & ~mt & (res != MAX_R)
+        cls = _crossing(geo, prev[miss], idx[miss])
+        big = np.abs(res[miss]) > k_huber
+        for c in set(cls):
+            sel = cls == c
+            cnt[c] = cnt.get(c, 0) + int((sel & (big | (c == "start"))).sum())
+    return cnt
+
+
+def _too_few_carried(geo, K0, cnt):
+    return ["only %d carried misses across %s" % (cnt.get(c, 0), c) for c in _classes(geo, K0) + ["start"]
+            if cnt.get(c, 0) < MIN_HITS]
 
 
 def _knife(tr):
@@ -663,13 +680,69 @@ def test_minimiser_state(base, monkeypatch, state, form):
             mf = o.keylines()["m_id_f"]
             if not np.array_equal(run["m_id_f"], mf):
                 msgs.append("call %d: m_id_f differs at %d keylines" % (k, int((run["m_id_f"] != mf).sum())))
-            ns = len(run["tr"]["evals"])
-            if CLUSTERS[form] == 0:
-                if launches < ns:
-                    msgs.append("%d launches for %d evaluations" % (launches, ns))
-            elif (launches <= 2) != (ns <= MIN_MAX_EVALS):
-                msgs.append("%d launches for %d evaluations (cluster kernel up to %d)" % (launches, ns, MIN_MAX_EVALS))
+            if launches > 2:
+                msgs.append("%d launches for %d evaluations" % (launches, len(run["tr"]["evals"])))
     finally:
         for m in (new, old, empty):
             m.close()
     assert not msgs, "\n".join(msgs)
+
+
+# =====================================================================================================================
+# The stage-level TryVelRot on the stale-residual states
+# =====================================================================================================================
+@pytest.mark.parametrize("state", [k for k in STATES if STATES[k].get("kind") == "stale"])
+def test_try_vel_rot_stale(base, state):
+    """rb_try_vel_rot against the reference's TryVelRot at every pose of the state's minimisation, with (reweight,
+    procjf) in (0, 1), (1, 1), (0, 0), each evaluation reading the residuals of the one before it; tracker_parity's bars.
+    Its 256-keyline blocks hand the stale fi of a miss's last match across warps and blocks: MIN_HITS carried misses per
+    crossing class."""
+    st = base.state(state)
+    sp, kl = st["sp"], st["kl"]
+    K0 = sp["K0"]
+    r_new, r_old = base.ref_maps(kl, sp["fc"])
+    ctx = _ctx(base, "try_vel_rot")
+    new, old = ctx.new_map(), ctx.new_map()
+    msgs, evals = [], []
+    try:
+        new.load_keylines(base.kl11, base.mask11)
+        new.build_field(CFG["radius"], base.rt)
+        old.load_keylines(kl, base.empty)
+        new.set_frame_count(sp["fc"])
+        used = kl["s_rho"] <= sp["q"]
+        res_in = np.zeros((K0 + 3) & ~3)
+        for xi, e in enumerate(st["runs"][-1]["tr"]["evals"]):
+            for rw, pj in ((False, True), (True, True), (False, False)):
+                args = (e["X"], rw, pj, sp["mt"], sp["q"], sp["mnt"], sp["k_huber"], res_in)
+                s_r, J_r, F_r, res_r = r_new.try_vel_rot(r_old, *args)
+                mf_r = r_old.keylines()["m_id_f"].copy()
+                s_g, J_g, F_g, res_g = new.try_vel_rot(old, *args)
+                tag = "X%d rw=%d pj=%d " % (xi, rw, pj)
+                errs = _close("score", s_r, s_g, 1e-10, 0.0)
+                if pj:
+                    errs += _close("JtJ", J_r, J_g, 1e-9, 1e-9 * np.abs(J_r).max())
+                    errs += _close("JtF", F_r, F_g, 1e-9, 1e-9 * np.abs(F_r).max())
+                if not np.array_equal(mf_r, old.keylines()["m_id_f"]):
+                    errs.append("m_id_f differs")
+                errs += _close("DResidualNew", res_r[:K0][used], res_g[used], 1e-12, 1e-12)
+                msgs += [tag + m for m in errs]
+                wrote = ~np.isnan(res_r)
+                evals.append(dict(res=res_r[:K0], matched=mf_r >= 0, wrote=wrote[:K0]))
+                res_in = np.where(wrote, res_r, res_in)
+    finally:
+        new.close()
+        old.close()
+    cnt = _carried(BLOCKS, evals, K0, sp["k_huber"])
+    print("%s: %d evaluations, carried misses %s" % (state, len(evals), cnt))
+    assert not _too_few_carried(BLOCKS, K0, cnt), "vacuous case: %s" % _too_few_carried(BLOCKS, K0, cnt)
+    assert not msgs, "\n".join(msgs[:20])
+
+
+def test_kl_capacity_bound(built):
+    """a context holds up to the reference's KEYLINE_MAX keylines; rb_ctx_create refuses more with RB_ERR_ARG (-2)"""
+    from rebvo_b200 import capi
+    ctx = capi.Ctx(CFG["cam"], CFG["sigma0"], CFG["ksigma"], kl_capacity=KEYLINE_MAX)
+    assert ctx.minimizer_clusters() >= 1
+    ctx.close()
+    with pytest.raises(capi.RbError, match=r"rb_ctx_create failed \(-2\)"):
+        capi.Ctx(CFG["cam"], CFG["sigma0"], CFG["ksigma"], kl_capacity=KEYLINE_MAX + 1)

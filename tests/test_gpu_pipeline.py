@@ -99,11 +99,10 @@ def test_schedule_variants_do_not_change_the_result(built, stream, monkeypatch, 
 
 
 def test_fallback_paths_agree(built, stream, monkeypatch):
-    """The switches in DESIGN.md section 5 select the slower formulations of the same stages (one launch per TryVelRot
-    evaluation, detector on the tracker stream, plain stream order): same keylines and matches, poses equal to the
-    rounding of the differently ordered sums."""
+    """The switches in DESIGN.md section 5 select the slower formulations of the same stages (detector on the tracker
+    stream, plain stream order): same keylines and matches, poses equal to the rounding of the differently ordered sums."""
     a = _euroc_run(stream, 20).nav
-    for k in ("REBVO_B200_MIN_PERSIST", "REBVO_B200_OVERLAP", "REBVO_B200_PDL"):
+    for k in ("REBVO_B200_OVERLAP", "REBVO_B200_PDL"):
         monkeypatch.setenv(k, "0")
     b = _euroc_run(stream, 20).nav
     assert np.array_equal(a["kn"], b["kn"])                       # the detector does not depend on the tracker

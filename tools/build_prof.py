@@ -1,5 +1,5 @@
 """Build the profiling variant of the library (-DRB_TVR_PROF: clock64 stamps in the minimiser, %globaltimer marker kernels
-in the pipeline) into tools/_prof/ (git-ignored).  Used by minimiser_stamps.py and trace_run.py on a GPU box."""
+in the pipeline) into tools/_prof/ (git-ignored).  Used by cluster_stamps.py and trace_run.py on a GPU box."""
 import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rebvo_b200 import build as B
