@@ -402,6 +402,39 @@ int rb_depth_image(rb_ctx *c, const rb_depth_cell *cells, int gw, int gh, const 
 int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode);
 int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho);
 
+/* Where the per-frame outputs go: where = 0 (the default) mapped pinned host memory, read with rb_pipeline_mirror,
+ * rb_pipeline_depth and rb_pipeline_depth_image; where = 1 device memory, read with the _dev accessors below, for consumers
+ * that work on the GPU.  It applies to the keyline mirror, the depth grid and the depth image, whichever are on; the nav and
+ * odometry records stay on the host.  The same kernels write the same bytes in both modes: device mode only leaves out the
+ * mirror's copy into host memory (one launch per frame fewer with the mirror on).  May be called between pushes; changing it
+ * drops the captured batches, like set_mirror, and the outputs of the last push (the new mode's accessors return RB_ERR_ARG
+ * until the next push).  RB_ERR_ARG for a value outside 0..1 and in IMU mode, where these outputs are not available.
+ * In device mode the host accessors return RB_ERR_STATE; in host mode the _dev accessors do.
+ *
+ * Buffers: each mode's buffers are allocated by the set_* call that needs them, never by a push, and kept across switches.
+ * A device pointer the _dev accessors return stays the same from push to push until one of these calls has to grow its
+ * buffer: rb_pipeline_set_output_memory(pl, 1), when the grid or image was switched on or enlarged while in host mode;
+ * rb_pipeline_set_depth, for a grid with more cells than any before in device mode; rb_pipeline_set_depth_image, for mode 2
+ * after mode 1 in device mode.  The mirror's device slots are allocated once, by the first rb_pipeline_set_mirror, and
+ * never move. */
+int rb_pipeline_set_output_memory(rb_pipeline *pl, int where);
+/* Device mode: every push first makes its tracker stream wait for the work enqueued on `stream` (a cudaStream_t of the
+ * pipeline's device; NULL is the legacy default stream) at the time of the push, outside any captured batch, so that it
+ * writes no output before a consumer of the last push's outputs on that stream is done with them.  The push synchronises
+ * its own streams before it returns, so its outputs are complete on return and any stream may read them.  The stream must
+ * stay valid while it is set; rb_pipeline_stream(pl) (the default) waits for nothing.  Kept across pushes and switches;
+ * no effect in host mode. */
+int rb_pipeline_set_consumer_stream(rb_pipeline *pl, void *stream);
+/* Device pointers to the outputs of frame i of the last push, valid from the return of that push until the next push, in
+ * the layouts of the host accessors: the mirror's *n records (rb_keyline or 15-byte net_keyline), the grid's gw * gh
+ * row-major rb_depth_cell cells with *min_dist pointing at the double right after them, and the image's row-major w x h
+ * float planes, s_rho (mode 2; else NULL) starting a padded plane stride after rho: w * h rounded up to a multiple of 64
+ * floats.  Frame i + 1's planes start mode such strides after frame i's.  RB_ERR_ARG as the host accessors (output off or
+ * not made by the last push, i out of range, NULL out-pointer for the records / cells / rho); RB_ERR_STATE in host mode. */
+int rb_pipeline_mirror_dev(rb_pipeline *pl, int i, const void **records, int *n);
+int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, const double **min_dist);
+int rb_pipeline_depth_image_dev(rb_pipeline *pl, int i, const float **rho, const float **s_rho);
+
 /* IMU fusion (BASELINE configs[2], REBVOParameters ImuMode = 2: samples from a dataset file).  After this call every push runs
  * the IMU branch of REBVO::SecondThread (rebvo_second_t.cpp:182-336: gyro pre-rotation, Minimizer_V, ExtRotVel, BiasCorrect,
  * scale / gravity / bias filter of scaleestimator.cpp, filtered pose of :521-551) instead of Minimizer_RV.  samples: n rows

@@ -1,5 +1,6 @@
 """ctypes binding of librebvo_b200.so (include/rebvo_b200.h).  No fallback: if the CUDA library is missing
 or no CUDA device is present the calls raise."""
+import collections
 import ctypes as C
 import os
 
@@ -117,7 +118,8 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_try_vel", "rb_minimizer_v", "rb_ext_rot_vel", "rb_bias_correct", "rb_map_pack_net_keylines",
            "rb_nav_format_trajectory", "rb_nav_format_log", "rb_odometry_format_pose_graph", "rb_pipeline_set_odometry",
            "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth", "rb_depth_image",
-           "rb_pipeline_set_depth_image", "rb_pipeline_depth_image"]
+           "rb_pipeline_set_depth_image", "rb_pipeline_depth_image", "rb_pipeline_set_output_memory",
+           "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev"]
 
 _lib = None
 
@@ -503,6 +505,28 @@ class Map:
         return kp.value, rkp.value
 
 
+class _CudaArray:
+    """A device buffer for torch.as_tensor (__cuda_array_interface__): no copy, no ownership."""
+
+    def __init__(self, ptr, shape, typestr, strides):
+        self.__cuda_array_interface__ = dict(shape=tuple(shape), typestr=typestr, data=(int(ptr), False),
+                                             strides=tuple(strides) if shape else None, version=3)
+
+
+def _dev_view(ptr, shape, dtype, strides, device):
+    """torch CUDA tensor over device memory the pipeline owns on CUDA device `device`; strides in bytes."""
+    import torch
+    dev = torch.device("cuda", device)
+    if 0 in shape:
+        return torch.empty(shape, dtype=dtype, device=dev)
+    typestr = {torch.uint8: "|u1", torch.int32: "<i4", torch.float32: "<f4", torch.float64: "<f8"}[dtype]
+    return torch.as_tensor(_CudaArray(ptr, shape, typestr, strides), device=dev)
+
+
+# DEPTH_CELL fields of the grid's device views
+DepthDev = collections.namedtuple("DepthDev", "rho s_rho dist fixed min_dist")
+
+
 class Pipeline:
     """REBVO per-frame flow on one GPU (rb_pipeline_*)."""
 
@@ -511,6 +535,8 @@ class Pipeline:
         self.params = params
         self.w, self.h = params.cam.w, params.cam.h
         self.max_batch = max_batch
+        self.device = device
+        self._out_dev = False
         h = C.c_void_p()
         r = self.L.rb_pipeline_create(C.byref(h), device, C.byref(params), max_batch)
         self.h_ = h
@@ -532,6 +558,7 @@ class Pipeline:
             ptr = _p(rgb)
         else:
             ptr = C.c_void_p(int(rgb))
+        self._consumer_fence()
         self.check(self.L.rb_pipeline_push(self.h_, ptr, _p(ts), n, _p(nav)))
         return nav
 
@@ -546,6 +573,7 @@ class Pipeline:
             ptr = _p(frames)
         else:
             ptr = C.c_void_p(int(frames))
+        self._consumer_fence()
         self.check(self.L.rb_pipeline_push_mono(self.h_, ptr, _p(ts), n, _p(nav)))
         return nav
 
@@ -553,6 +581,7 @@ class Pipeline:
         """Mono frames already in device memory (4-byte aligned pointer), read in place."""
         ts = np.ascontiguousarray(ts, np.float64)
         nav = np.zeros(len(ts), NAV)
+        self._consumer_fence()
         self.check(self.L.rb_pipeline_push_mono_dev(self.h_, C.c_void_p(int(dev_ptr)), _p(ts), len(ts), _p(nav)))
         return nav
 
@@ -578,6 +607,7 @@ class Pipeline:
     def push_dev(self, dev_ptr, ts):
         ts = np.ascontiguousarray(ts, np.float64)
         nav = np.zeros(len(ts), NAV)
+        self._consumer_fence()
         self.check(self.L.rb_pipeline_push_dev(self.h_, C.c_void_p(int(dev_ptr)), _p(ts), len(ts), _p(nav)))
         return nav
 
@@ -690,6 +720,78 @@ class Pipeline:
         if net:
             return np.frombuffer(buf, dtype=np.uint8).reshape(kn.value, 15)
         return np.frombuffer(buf, dtype=KEYLINE, count=kn.value)
+
+    def set_output_memory(self, where):
+        """Where the mirror, the depth grid and the depth image go: "host" (the default; mirror(), depth(), depth_image()) or
+        "device" (mirror_dev(), depth_dev(), depth_image_dev(), depth_images_dev(): torch CUDA tensors, no copy).  Between
+        pushes; the outputs of the last push are dropped when it changes."""
+        if where not in ("host", "device"):
+            raise ValueError("where: 'host' or 'device'")
+        self.check(self.L.rb_pipeline_set_output_memory(self.h_, int(where == "device")))
+        self._out_dev = where == "device"
+
+    def set_consumer_stream(self, stream):
+        """Device mode: each push first waits for the work enqueued on `stream` (a cudaStream_t handle, as an int; 0 is the
+        legacy default stream) when it is called.  The push wrappers set torch.cuda.current_stream() before each push in
+        device mode; this call is for pushes made through the C functions.  self.stream() waits for nothing."""
+        self.check(self.L.rb_pipeline_set_consumer_stream(self.h_, C.c_void_p(int(stream))))
+
+    def _consumer_fence(self):
+        """Device mode: the push overwrites no output before the work torch enqueued so far on its current stream (which
+        may still read the last push's outputs) is done."""
+        if self._out_dev:
+            import torch
+            self.set_consumer_stream(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def mirror_dev(self, i):
+        """Device mode: the records of frame i of the last push as a uint8 CUDA tensor [kn, rec] (rec = 168 in mode 1,
+        15 in mode 2), no copy; valid until the next push."""
+        import torch
+        p, kn = C.c_void_p(0), C.c_int(0)
+        self.check(self.L.rb_pipeline_mirror_dev(self.h_, i, C.byref(p), C.byref(kn)))
+        rec = 15 if getattr(self, "_mirror_mode", 1) == 2 else KEYLINE.itemsize
+        return _dev_view(p.value, (kn.value, rec), torch.uint8, (rec, 1), self.device)
+
+    def depth_dev(self, i):
+        """Device mode: the grid of frame i of the last push as CUDA tensors over its DEPTH_CELL records, no copy:
+        DepthDev(rho, s_rho, dist: float64 [gh, gw]; fixed: int32 [gh, gw]; min_dist: float64 0-d); valid until the next
+        push."""
+        import torch
+        p, gw, gh, md = C.c_void_p(0), C.c_int(0), C.c_int(0), C.c_void_p(0)
+        self.check(self.L.rb_pipeline_depth_dev(self.h_, i, C.byref(p), C.byref(gw), C.byref(gh), C.byref(md)))
+        shape, strides = (gh.value, gw.value), (gw.value * DEPTH_CELL.itemsize, DEPTH_CELL.itemsize)
+        f = {n: (p.value + DEPTH_CELL.fields[n][1]) for n in ("rho", "s_rho", "dist", "fixed")}
+        return DepthDev(*(_dev_view(f[n], shape, torch.float64, strides, self.device) for n in ("rho", "s_rho", "dist")),
+                        _dev_view(f["fixed"], shape, torch.int32, strides, self.device),
+                        _dev_view(md.value, (), torch.float64, (), self.device))
+
+    def depth_image_dev(self, i):
+        """Device mode: the image of frame i of the last push as float32 CUDA tensors (rho, s_rho or None) [h, w], no copy;
+        valid until the next push."""
+        import torch
+        r, s = C.c_void_p(0), C.c_void_p(0)
+        self.check(self.L.rb_pipeline_depth_image_dev(self.h_, i, C.byref(r), C.byref(s)))
+
+        def view(ptr):
+            return _dev_view(ptr, (self.h, self.w), torch.float32, (4 * self.w, 4), self.device)
+        return view(r.value), (view(s.value) if s.value else None)
+
+    def depth_images_dev(self):
+        """Device mode: the images of every frame of the last push as float32 CUDA tensors (rho, s_rho or None) [n, h, w],
+        frame after frame a padded plane stride apart (no copy); valid until the next push."""
+        import torch
+        r, s = C.c_void_p(0), C.c_void_p(0)
+        self.check(self.L.rb_pipeline_depth_image_dev(self.h_, 0, C.byref(r), C.byref(s)))
+        n = 1
+        while n < self.max_batch and self.L.rb_pipeline_depth_image_dev(self.h_, n, C.byref(C.c_void_p()), None) == 0:
+            n += 1
+        plane = (self.w * self.h + 63) // 64 * 64
+        step = 4 * plane * (2 if s.value else 1)
+        strides = (step, 4 * self.w, 4)
+
+        def view(ptr):
+            return _dev_view(ptr, (n, self.h, self.w), torch.float32, strides, self.device)
+        return view(r.value), (view(s.value) if s.value else None)
 
     def map(self, age=0):
         """Edge map of the ring: age 0 = newest.  Returns a Map view bound to a throw-away context facade."""

@@ -47,7 +47,8 @@ extern "C" int rb_debug_fetch_trace(unsigned long long *out, unsigned int *n) {
 struct SubBatchPtrs {
     const void *src;            // the RGB24 (or mono) frames of the sub-batch
     unsigned char *mirror[2];   // keyline mirror: {device staging, mapped host} slot of the sub-batch's first frame
-    unsigned char *depth[3];    // depth grid: {record staging, mapped host cells, mapped host image} of that frame
+    unsigned char *depth[3];    // depth grid: {record staging, output cells, output image} of that frame (output: mapped
+                                // pinned host memory, or device memory with rb_pipeline_set_output_memory(pl, 1))
 };
 
 struct ImuFlow;
@@ -107,11 +108,19 @@ struct rb_pipeline {
     double pacc[16];
     long long pframes;
     rb_undistort *und;    // UseUndistort=1 (rb_pipeline_set_undistort): fused into the gray pass
+    // where the mirror, the depth grid and the depth image go (rb_pipeline_set_output_memory): 0 mapped pinned host memory,
+    // 1 device memory.  In device mode the mirror's staging slots are its output (no k_mirror_to_host), and the fill and
+    // the image pass write into depth.dev / dimg.dev instead of depth.host / dimg.host; no kernel changes.  Each mode's
+    // buffers are made by the set_* call that needs them and kept (grown, never shrunk) across switches.
+    int out_dev;
+    // device mode: each push first waits for the work enqueued on this stream so far (rb_pipeline_set_consumer_stream), so
+    // that it overwrites no output a consumer of the last push still reads; the pipeline's own stream = nothing to wait for
+    cudaStream_t consumer;
     // The optional per-frame outputs.  Each keeps its own frame count of the last push, which its set_* call clears (and
     // set_depth the image's too: the images are of the grid).
     // Keyline mirror (rb_pipeline_set_mirror): every frame's keylines are packed into a device staging slot right after its
-    // map update (tracker stream), then a small kernel on the mirror's stream writes exactly kn records into mapped pinned
-    // host memory while the next frames are tracked; both are part of the captured batch
+    // map update (tracker stream), then (host mode) a small kernel on the mirror's stream writes exactly kn records into
+    // mapped pinned host memory while the next frames are tracked; both are part of the captured batch
     struct {
         int on;                        // 0 off, 1 = 168-byte KeyLine records, 2 = 15-byte net_keyline records
         size_t rec, stride;            // bytes per record / per frame slot (multiple of 256)
@@ -138,6 +147,8 @@ struct rb_pipeline {
         size_t rec_stride;             // bytes per frame staging slot (kcap records, multiple of 256)
         unsigned char *stage, *host;   // [max_batch * stride]: device staging, mapped pinned host cells
         size_t host_bytes;
+        unsigned char *dev;            // [max_batch * cells_bytes]: the cells in device mode
+        size_t dev_bytes;
         void *ws;                      // per stream: bucketing scratch (and the grid when it does not fit in smem)
         size_t ws_bytes;               // (per stream)
         cudaStream_t stream[RB_DEPTH_STREAMS];
@@ -153,6 +164,8 @@ struct rb_pipeline {
         size_t plane, stride;          // floats per plane (a multiple of 64); bytes per frame slot
         unsigned char *host;           // [max_batch * stride] mapped pinned host memory
         size_t host_bytes;
+        unsigned char *dev;            // [max_batch * stride]: the planes in device mode
+        size_t dev_bytes;
         int n;                         // frames of the last push
     } dimg;
 };
@@ -192,6 +205,21 @@ static int grow_mapped(rb_ctx *c, unsigned char **buf, size_t *have, size_t byte
     RB_CUDA(cudaHostAlloc(buf, bytes, cudaHostAllocMapped));
     *have = bytes;
     return RB_OK;
+}
+// *buf: device memory of at least `bytes`, kept when it is large enough (its contents are not kept otherwise)
+static int grow_dev(rb_ctx *c, unsigned char **buf, size_t *have, size_t bytes) {
+    if (bytes <= *have) return RB_OK;
+    cudaFree(*buf);
+    *buf = nullptr;
+    *have = 0;
+    RB_CUDA(cudaMalloc(buf, bytes));
+    *have = bytes;
+    return RB_OK;
+}
+// an output buffer of `bytes` where the pipeline's outputs go now (rb_pipeline_set_output_memory)
+static int grow_out(rb_pipeline *pl, unsigned char **host, size_t *host_have, unsigned char **dev, size_t *dev_have,
+                    size_t bytes) {
+    return pl->out_dev ? grow_dev(pl->c, dev, dev_have, bytes) : grow_mapped(pl->c, host, host_have, bytes);
 }
 // the batch's gray plane from the frames at sb_dev->src (rebvo_first_t.cpp:231 undistortion + RGB -> BW)
 static int gray_pass(rb_pipeline *pl, int fmt, int n) {
@@ -367,6 +395,7 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
     }
     for (int i = 0; i < 4; i++) RB_CUDA(cudaEventCreate(&pl->ev[i]));
     for (int i = 0; i < 8; i++) RB_CUDA(cudaEventCreate(&pl->user_ev[i]));
+    pl->consumer = c->stream;
     if ((r = pl_reset_state(pl))) return r;
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return RB_OK;
@@ -472,7 +501,7 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     if (pl->und) rb_undistort_destroy(pl->und);
     rb_dogws_free(&pl->ws);
     void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->mirror.dev, pl->odom.dev, pl->depth.stage,
-                   pl->depth.ws};
+                   pl->depth.ws, pl->depth.dev, pl->dimg.dev};
     for (void *p : dev) cudaFree(p);
     void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->mirror.host, pl->odom.pin, pl->depth.host,
                     pl->dimg.host};
@@ -674,9 +703,13 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
                 r = rb_map_pack_aos_enqueue(c, neu, tbl->mirror, ofs);
             else   // copy_net_keyline(..., pbuf.K) of the third thread (rebvo_third_t.cpp:192-197): K of this frame's nav record
                 r = rb_map_pack_net_enqueue(c, neu, tbl->mirror, ofs, &(pl->nav_dev + i)->K);
-            if (r || (r = stream_wait(pl, main_stream, pl->mirror.stream))) return r;
-            k_mirror_to_host<<<8, 256, 0, pl->mirror.stream>>>(tbl->mirror, ofs, &(pl->nav_dev + i)->kn, (int)pl->mirror.rec);
-            RB_LAUNCH_CHECK();
+            if (r) return r;
+            if (!pl->out_dev) {   // (device mode: the staging slot is the output)
+                if ((r = stream_wait(pl, main_stream, pl->mirror.stream))) return r;
+                k_mirror_to_host<<<8, 256, 0, pl->mirror.stream>>>(tbl->mirror, ofs, &(pl->nav_dev + i)->kn,
+                                                                   (int)pl->mirror.rec);
+                RB_LAUNCH_CHECK();
+            }
         }
         if (pl->depth.on) {   // the viewer's depth_filler on this frame's wire records (visualizer.cpp:436-440)
             unsigned char *const *rec_pp = tbl->mirror;
@@ -703,7 +736,7 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     }
     if ((r = resc_join(pl))) return r;   // the last frame's Kp / RKp are in its record before the nav copy
     // the batch is complete when its last map has reached the host, and its last grids
-    if (pl->mirror.on && (r = stream_wait(pl, pl->mirror.stream, main_stream))) return r;
+    if (pl->mirror.on && !pl->out_dev && (r = stream_wait(pl, pl->mirror.stream, main_stream))) return r;
     for (int k = 0; pl->depth.on && k < RB_DEPTH_STREAMS && k < n; k++)
         if ((r = stream_wait(pl, pl->depth.stream[k], main_stream))) return r;
     return RB_OK;
@@ -731,6 +764,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
         pl->odom.n = pl->odom.on ? n : 0;
         return RB_OK;
     }
+    // device outputs: nothing of this push may overwrite them before the consumer's reads of the last push's are done.  The
+    // side streams that write them fork from the tracker stream, so one wait at its head covers them (outside any graph).
+    if (pl->out_dev && pl->consumer != c->stream && (r = stream_wait(pl, pl->consumer, c->stream))) return r;
     const long long first = pl->n_pushed;
     // per-frame scalars -> device (SecondThread :146-149 for dt; FrameCount of the reference's 8-slot ring:
     // frame fr is served by slot (fr+1)%8, whose global_tracker has run (fr-1)/8 minimisations before)
@@ -771,12 +807,14 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
         t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);
         if (pl->mirror.on) {
             t.mirror[0] = pl->mirror.dev + (size_t)off * pl->mirror.stride;
-            t.mirror[1] = pl->mirror.host + (size_t)off * pl->mirror.stride;
+            t.mirror[1] = pl->out_dev ? nullptr : pl->mirror.host + (size_t)off * pl->mirror.stride;
         }
         if (pl->depth.on) {
+            unsigned char *cells = pl->out_dev ? pl->depth.dev : pl->depth.host;
+            unsigned char *img = pl->out_dev ? pl->dimg.dev : pl->dimg.host;
             t.depth[0] = pl->depth.stage + (size_t)off * pl->depth.rec_stride;
-            t.depth[1] = pl->depth.host + (size_t)off * pl->depth.plan.cells_bytes;
-            t.depth[2] = pl->dimg.mode ? pl->dimg.host + (size_t)off * pl->dimg.stride : nullptr;
+            t.depth[1] = cells + (size_t)off * pl->depth.plan.cells_bytes;
+            t.depth[2] = pl->dimg.mode ? img + (size_t)off * pl->dimg.stride : nullptr;
         }
         RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
         const bool graph_ok = pl->use_graph && first_j > 0;
@@ -918,7 +956,9 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     const size_t stride = ((size_t)c->kcap * sizeof(rb_keyline) + 255) & ~(size_t)255;   // (sized for the larger record)
     if (on) {
         if (!pl->mirror.dev) RB_CUDA(cudaMalloc(&pl->mirror.dev, (size_t)pl->max_batch * stride));
-        if ((r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, (size_t)pl->max_batch * stride))) return r;
+        // (device mode: the staging slots are the output)
+        if (!pl->out_dev && (r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, (size_t)pl->max_batch * stride)))
+            return r;
         if (!pl->mirror.stream) RB_CUDA(cudaStreamCreateWithFlags(&pl->mirror.stream, cudaStreamNonBlocking));
     }
     if (on != pl->mirror.on) drop_graphs(pl);   // the captured batches contain (or not) the pack kernels
@@ -957,7 +997,9 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
         for (int k = 0; k < RB_DEPTH_STREAMS; k++)
             RB_CUDA(cudaStreamCreateWithPriority(&pl->depth.stream[k], cudaStreamNonBlocking, (dp && atoi(dp) == 1) ? hi : lo));
     }
-    if ((r = grow_mapped(c, &pl->depth.host, &pl->depth.host_bytes, (size_t)pl->max_batch * plan.cells_bytes))) return r;
+    if ((r = grow_out(pl, &pl->depth.host, &pl->depth.host_bytes, &pl->depth.dev, &pl->depth.dev_bytes,
+                      (size_t)pl->max_batch * plan.cells_bytes)))
+        return r;
     const size_t ws_bytes = rb_depth_ws_bytes(plan, c->kcap);
     if (ws_bytes > pl->depth.ws_bytes) {
         cudaFree(pl->depth.ws);
@@ -975,8 +1017,9 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
-    if (!pl || !pl->depth.on || !cells) return RB_ERR_ARG;
-    if (i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
+    if (!pl || !cells) return RB_ERR_ARG;
+    if (pl->out_dev) return RB_ERR_STATE;
+    if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
     const DepthGeom &g = pl->depth.plan.g;
     const unsigned char *slot = pl->depth.host + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
@@ -993,7 +1036,9 @@ extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
     if (r) return r;
     if (mode) {
         const size_t plane = ((size_t)c->N + 63) & ~(size_t)63, stride = (size_t)mode * plane * sizeof(float);
-        if ((r = grow_mapped(c, &pl->dimg.host, &pl->dimg.host_bytes, (size_t)pl->max_batch * stride))) return r;
+        if ((r = grow_out(pl, &pl->dimg.host, &pl->dimg.host_bytes, &pl->dimg.dev, &pl->dimg.dev_bytes,
+                          (size_t)pl->max_batch * stride)))
+            return r;
         if (pl->depth.on && (r = rb_depth_image_plan(c, pl->depth.plan.g, mode, &pl->dimg.plan))) return r;
         pl->dimg.plane = plane;
         pl->dimg.stride = stride;
@@ -1005,6 +1050,7 @@ extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
 }
 extern "C" int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
     if (!pl || !rho) return RB_ERR_ARG;
+    if (pl->out_dev) return RB_ERR_STATE;
     if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
     const float *p = reinterpret_cast<const float *>(pl->dimg.host + (size_t)i * pl->dimg.stride);
     *rho = p;
@@ -1034,10 +1080,74 @@ extern "C" int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, i
     return RB_OK;
 }
 extern "C" int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, int *n) {
-    if (!pl || !pl->mirror.on || !records || !n) return RB_ERR_ARG;
-    if (i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
+    if (!pl || !records || !n) return RB_ERR_ARG;
+    if (pl->out_dev) return RB_ERR_STATE;
+    if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
     *records = pl->mirror.host + (size_t)i * pl->mirror.stride;
     *n = pl->nav_pin[i].kn;
+    return RB_OK;
+}
+
+extern "C" int rb_pipeline_set_output_memory(rb_pipeline *pl, int where) {
+    if (!pl || where < 0 || where > 1) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    int r = set_begin(pl, "set_output_memory");
+    if (r) return r;
+    if (where == pl->out_dev) return RB_OK;
+    // the buffers of the products that are on, in the new place; the other place's stay for a switch back
+    const int was = pl->out_dev;
+    pl->out_dev = where;
+    const size_t mb = (size_t)pl->max_batch;
+    if (pl->mirror.on && !where)
+        r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, mb * pl->mirror.stride);
+    if (!r && pl->depth.on)
+        r = grow_out(pl, &pl->depth.host, &pl->depth.host_bytes, &pl->depth.dev, &pl->depth.dev_bytes,
+                     mb * pl->depth.plan.cells_bytes);
+    if (!r && pl->dimg.mode)
+        r = grow_out(pl, &pl->dimg.host, &pl->dimg.host_bytes, &pl->dimg.dev, &pl->dimg.dev_bytes, mb * pl->dimg.stride);
+    if (r) {
+        pl->out_dev = was;
+        return r;
+    }
+    drop_graphs(pl);   // the captured batches contain (or not) k_mirror_to_host and its join
+    pl->mirror.n = pl->depth.n = pl->dimg.n = 0;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_set_consumer_stream(rb_pipeline *pl, void *stream) {
+    if (!pl) return RB_ERR_ARG;
+    RB_ENTER(pl->c);
+    pl->consumer = (cudaStream_t)stream;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_mirror_dev(rb_pipeline *pl, int i, const void **records, int *n) {
+    if (!pl || !records || !n) return RB_ERR_ARG;
+    if (!pl->out_dev) return RB_ERR_STATE;
+    if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
+    *records = pl->mirror.dev + (size_t)i * pl->mirror.stride;
+    *n = pl->nav_pin[i].kn;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh,
+                                     const double **min_dist) {
+    if (!pl || !cells) return RB_ERR_ARG;
+    if (!pl->out_dev) return RB_ERR_STATE;
+    if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
+    const DepthGeom &g = pl->depth.plan.g;
+    const unsigned char *slot = pl->depth.dev + (size_t)i * pl->depth.plan.cells_bytes;
+    *cells = reinterpret_cast<const rb_depth_cell *>(slot);
+    if (gw) *gw = g.gw;
+    if (gh) *gh = g.gh;
+    if (min_dist) *min_dist = reinterpret_cast<const double *>(slot + (size_t)g.gw * g.gh * sizeof(rb_depth_cell));
+    return RB_OK;
+}
+extern "C" int rb_pipeline_depth_image_dev(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
+    if (!pl || !rho) return RB_ERR_ARG;
+    if (!pl->out_dev) return RB_ERR_STATE;
+    if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
+    const float *p = reinterpret_cast<const float *>(pl->dimg.dev + (size_t)i * pl->dimg.stride);
+    *rho = p;
+    if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
 }
 
