@@ -10,7 +10,8 @@
  *
  * Conventions: every function returns 0 on success, a negative rb_status otherwise, and never throws.
  * A CUDA failure is sticky per context (rb_last_error()).  Pointers are plain host pointers unless the
- * name says dev.  Images are row-major without stride (Image<T>, include/VideoLib/image.h:42-217).
+ * name says dev.  Images are row-major without stride (Image<T>, include/VideoLib/image.h:42-217), except the rb_frame
+ * ones of rb_pipeline_push_frames, which have a row step.
  * All calls on one context are ordered on the context's CUDA stream; functions that return values to
  * host memory synchronise that stream before returning.
  */
@@ -51,8 +52,9 @@ typedef struct rb_keyline {
 } rb_keyline;
 
 /* cam_model (include/UtilLib/cam_model.h:32-50): pinhole part used by the hot path.  Any w >= 32, h >= 32 (KITTI's
- * 1241x376 and 1226x370 included): frames are always packed (3*w*h or w*h bytes, no row stride); the device keeps the
- * scale-space planes in rows padded to a multiple of 4 floats, which no interface exposes. */
+ * 1241x376 and 1226x370 included): the push calls take packed frames (3*w*h or w*h bytes, no row stride), and
+ * rb_pipeline_push_frames / rb_pipeline_push_frames_dev take frames with a row step, one buffer per frame; the device keeps
+ * the scale-space planes in rows padded to a multiple of 4 floats, which no interface exposes. */
 typedef struct rb_camera {
     int32_t w, h;
     float ppx, ppy, zfx, zfy;
@@ -288,6 +290,32 @@ int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *
  * w*h is not a multiple of 4 the frames after the first start at unaligned bytes of that buffer; they are read correctly. */
 int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out);
 int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n, rb_nav *nav_out);
+/* Strided frames, one buffer per frame, as the reference's ROS nodelet reads a sensor_msgs/Image (data[step*y + x*3 + c] for
+ * rgb8, data[step*y + x] for mono8): pixel (x, y) of frame i is at frames[i].data + y * frames[i].step + x * bpp, bytes r, g, b
+ * for RB_FRAME_RGB24 (bpp 3), one byte for RB_FRAME_MONO8 (bpp 1).  Frames need not be adjacent, ordered or aligned, and each
+ * may have its own step.  The frames array itself is host memory in both calls; the _dev call's data pointers are device
+ * pointers on the pipeline's device.  A push reads only the bytes of each frame's span [data, data + (h-1)*step + w*bpp), and
+ * the bytes between rows never change a result: the records, maps, mirror, depth grids and images and the threshold feedback
+ * are those of rb_pipeline_push / push_mono / push_dev / push_mono_dev of the same pixels packed, with and without
+ * undistortion, at every frame size, and in IMU mode (dataset and live).
+ *   rb_pipeline_push_frames: each frame is copied into the pipeline's packed staging with one 2D copy, then the batch runs
+ *     exactly as a packed push of that format (same kernels, same captured batches).
+ *   rb_pipeline_push_frames_dev: the frames are read in place.  A device table of max_batch {data, step} entries is written
+ *     before the batch runs; the gray pass (with or without undistortion) reads each frame through it.  Such pushes have
+ *     captured batches of their own, so a pipeline may alternate packed and strided pushes, and they launch as many kernels
+ *     as a packed device push of the same size and format.
+ * RB_ERR_ARG, before anything is enqueued and with the state unchanged, for a format other than the two below, n outside
+ * 1..max_batch, a NULL frames, ts or data, a step < w * bpp, and, for the _dev call with undistortion on, frames wider or
+ * higher than 65535 pixels.  Live IMU mode checks the samples' coverage as for a packed
+ * push.  Synchronous, like rb_pipeline_push. */
+typedef struct rb_frame {
+    const uint8_t *data; /* first byte of row 0 */
+    int64_t step;        /* bytes from the start of one row to the next (sensor_msgs/Image step); >= w * bytes per pixel */
+} rb_frame;
+enum { RB_FRAME_RGB24 = 0, RB_FRAME_MONO8 = 1 };
+int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out);
+int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
+                                rb_nav *nav_out);
 /* REBVO::Reset (rebvo_second_t.cpp:609-620) */
 int rb_pipeline_reset(rb_pipeline *pl);
 /* newest / previous edge map of the ring (valid until the next push) */

@@ -119,9 +119,80 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_nav_format_trajectory", "rb_nav_format_log", "rb_odometry_format_pose_graph", "rb_pipeline_set_odometry",
            "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth", "rb_depth_image",
            "rb_pipeline_set_depth_image", "rb_pipeline_depth_image", "rb_pipeline_set_output_memory",
-           "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev"]
+           "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev",
+           "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev"]
 
 _lib = None
+
+
+# rb_frame: the first byte of row 0 and the bytes from one row to the next
+FRAME = np.dtype([("data", "<u8"), ("step", "<i8")])
+
+
+FRAME_RGB24, FRAME_MONO8 = 0, 1
+
+
+def _array_layout(a):
+    """(on_device, shape, byte strides, dtype is uint8, address of element 0) of a NumPy array, a torch CUDA tensor or an
+    object with __cuda_array_interface__ (torch tensors are read directly: building the interface dict costs more than
+    the rest of a frame's checks)"""
+    if isinstance(a, np.ndarray):
+        return False, a.shape, a.strides, a.dtype == np.uint8, a.__array_interface__["data"][0]
+    if type(a).__module__.startswith("torch") and hasattr(a, "data_ptr"):
+        if not a.is_cuda:
+            raise ValueError("frames: a torch tensor in host memory (pass tensor.numpy())")
+        return True, tuple(a.shape), tuple(a.stride()), str(a.dtype) == "torch.uint8", a.data_ptr()
+    if not hasattr(a, "__cuda_array_interface__"):
+        raise ValueError("frames: NumPy arrays (host) or CUDA arrays (__cuda_array_interface__), not %s" % type(a).__name__)
+    ai = a.__cuda_array_interface__
+    shape, strides = tuple(ai["shape"]), ai.get("strides")
+    if strides is None:   # C-contiguous
+        strides = tuple(int(np.prod(shape[k + 1:], dtype=np.int64)) * np.dtype(ai["typestr"]).itemsize
+                        for k in range(len(shape)))
+    return True, shape, tuple(strides), np.dtype(ai["typestr"]) == np.uint8, int(ai["data"][0])
+
+
+def frame_table(frames, w, h):
+    """How push_frames passes `frames` to rb_pipeline_push_frames(_dev), without copying anything: (format, on_device,
+    [(data pointer, step)] per frame).  `frames` is a sequence of per-frame arrays or one array of frames, with any frame
+    stride; a frame is uint8 (h, w, 3) RGB24 or (h, w) mono8.  NumPy arrays are host frames, objects with
+    __cuda_array_interface__ (torch CUDA tensors among them) device frames.  Within a frame the channel and pixel strides
+    must be 1 and 3 bytes (RGB24) or the pixel stride 1 byte (mono8), and the row stride is the step, at least one row of
+    pixels.  Anything else -- another dtype, shape or stride, host and device frames or two formats in one push, an empty
+    push -- raises ValueError."""
+    batch = not isinstance(frames, (list, tuple))
+    items = [frames] if batch else list(frames)
+    if not items:
+        raise ValueError("frames: no frames")
+    fmt = dev = None
+    table = []
+    for a in items:
+        on_dev, shape, strides, u8, base = _array_layout(a)
+        if not u8:
+            raise ValueError("frames: dtype %s, not uint8" % (a.dtype if hasattr(a, "dtype") else "?"))
+        fshape, fstrides = (shape[1:], strides[1:]) if batch else (shape, strides)
+        if fshape == (h, w, 3):
+            f, ok = FRAME_RGB24, fstrides[1:] == (3, 1)
+        elif fshape == (h, w):
+            f, ok = FRAME_MONO8, fstrides[1] == 1
+        else:
+            raise ValueError("frames: frame shape %s, not (%d, %d, 3) (RGB24) or (%d, %d) (mono8)" % (fshape, h, w, h, w))
+        if not ok:
+            raise ValueError("frames: pixel / channel strides %s bytes; the frames must have 3, 1 (RGB24) or 1 (mono8)"
+                             % (fstrides[1:],))
+        step = int(fstrides[0])
+        if step < w * (3 if f == FRAME_RGB24 else 1):
+            raise ValueError("frames: row stride %d bytes is shorter than a row" % step)
+        if fmt is not None and (f, on_dev) != (fmt, dev):
+            raise ValueError("frames: one format, all in host or all in device memory, in one push")
+        fmt, dev = f, on_dev
+        if batch:
+            table += [(base + i * int(strides[0]), step) for i in range(shape[0])]
+        else:
+            table.append((base, step))
+    if not table:
+        raise ValueError("frames: no frames")
+    return fmt, dev, table
 
 
 def _format_nav(fn, nav, *args):
@@ -576,6 +647,38 @@ class Pipeline:
         self._consumer_fence()
         self.check(self.L.rb_pipeline_push_mono(self.h_, ptr, _p(ts), n, _p(nav)))
         return nav
+
+    def push_frames(self, frames, ts):
+        """Strided frames, read where they are (no copy): a sequence of per-frame arrays or one array of frames with any
+        frame stride, uint8 (h, w, 3) RGB24 or (h, w) mono8 frames whose row stride is the step (see frame_table).  NumPy
+        arrays go through rb_pipeline_push_frames, CUDA arrays (torch tensors, __cuda_array_interface__) through
+        rb_pipeline_push_frames_dev.  Device frames are ordered after the work torch enqueued so far on its current stream of
+        the pipeline's device: the pipeline's stream waits for an event recorded there (no host synchronisation); frames
+        written on another stream must be complete before the call.  Same records as push / push_mono of the same pixels."""
+        fmt, on_dev, table = frame_table(frames, self.w, self.h)
+        ts = np.ascontiguousarray(ts, np.float64)
+        n = len(ts)
+        if len(table) != n:
+            raise ValueError("push_frames: %d frames, %d timestamps" % (len(table), n))
+        if on_dev:
+            self._after_torch_stream()
+        fr = np.array(table, FRAME)
+        nav = np.zeros(n, NAV)
+        self._consumer_fence()
+        fn = self.L.rb_pipeline_push_frames_dev if on_dev else self.L.rb_pipeline_push_frames
+        self.check(fn(self.h_, fmt, _p(fr), _p(ts), n, _p(nav)))
+        return nav
+
+    def _after_torch_stream(self):
+        """The pipeline's stream waits for the work torch enqueued so far on its current stream of this device: an event
+        recorded there (one event, reused: a wait takes the record made just before it)."""
+        import torch
+        if getattr(self, "_order", None) is None:
+            dev = torch.device("cuda", self.device)
+            self._order = (dev, torch.cuda.ExternalStream(self.stream(), device=dev), torch.cuda.Event())
+        dev, ext, ev = self._order
+        ev.record(torch.cuda.current_stream(dev))
+        ext.wait_event(ev)
 
     def push_mono_dev(self, dev_ptr, ts):
         """Mono frames already in device memory (4-byte aligned pointer), read in place."""

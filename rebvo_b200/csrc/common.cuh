@@ -259,6 +259,7 @@ int rb_dogws_alloc(rb_ctx *c, DogWS *ws, int B);
 void rb_dogws_free(DogWS *ws);
 int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // rgb -> gray
 int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // mono -> gray
+int rb_dog_gray_strided(rb_ctx *c, DogWS *ws, int nimg, const rb_frame *frames_dev, bool mono);   // strided frames -> gray
 int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg);          // gray -> img0, dog
 int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img);            // Img(1), dx, dy into ws->aux
 int rb_dog_make_tables(rb_ctx *c);

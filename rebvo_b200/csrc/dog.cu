@@ -105,21 +105,10 @@ __device__ __forceinline__ uint32_t in_word(const uint8_t *__restrict__ p0, long
         if (b + k >= lo && b + k < hi) v |= (uint32_t)__ldg(p0 + b + k) << (8 * k);
     return v;
 }
+// the float4 of the nv (1..4) pixels whose first byte is t of the word array p0, of which the bytes [lo, hi) may be read
 template <bool MONO>
-__global__ void __launch_bounds__(256) k_gray_pitched(const uint8_t *__restrict__ src_fixed,
-                                                      const uint8_t *const *__restrict__ src_pp,
-                                                      float4 *__restrict__ gray, int w, int h, int pitch, int nimg) {
-    const int pv = pitch >> 2;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the pitched batch
-    if (i >= (long long)nimg * h * pv) return;
-    const uint8_t *src = src_pp ? *src_pp : src_fixed;
-    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+__device__ __forceinline__ float4 gray4(const uint8_t *__restrict__ p0, long long t, int nv, long long lo, long long hi) {
     const int cb = MONO ? 1 : 3;   // bytes per pixel
-    const long long lo = (long long)(src - p0), hi = lo + (long long)nimg * cb * w * h;
-    const long long row = i / pv;  // frame * h + y: frames are packed, so the pixel index of the row's start is row * w
-    const int x = 4 * (int)(i - row * pv);
-    const int nv = w - x < 4 ? w - x : 4;   // valid pixels of this float4 (1..4)
-    const long long t = lo + (long long)cb * (row * w + x);   // byte of the first pixel
     const long long wi = t >> 2, we = (t + cb * nv - 1) >> 2;   // first / last word holding a wanted byte
     const int sh = (int)(t & 3) * 8;
     float4 o;
@@ -147,7 +136,46 @@ __global__ void __launch_bounds__(256) k_gray_pitched(const uint8_t *__restrict_
         if (nv < 3) o.z = 0.f;
         if (nv < 2) o.y = 0.f;
     }
-    gray[i] = o;
+    return o;
+}
+template <bool MONO>
+__global__ void __launch_bounds__(256) k_gray_pitched(const uint8_t *__restrict__ src_fixed,
+                                                      const uint8_t *const *__restrict__ src_pp,
+                                                      float4 *__restrict__ gray, int w, int h, int pitch, int nimg) {
+    const int pv = pitch >> 2;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the pitched batch
+    if (i >= (long long)nimg * h * pv) return;
+    const uint8_t *src = src_pp ? *src_pp : src_fixed;
+    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+    const int cb = MONO ? 1 : 3;   // bytes per pixel
+    const long long lo = (long long)(src - p0), hi = lo + (long long)nimg * cb * w * h;
+    const long long row = i / pv;  // frame * h + y: frames are packed, so the pixel index of the row's start is row * w
+    const int x = 4 * (int)(i - row * pv);
+    const int nv = w - x < 4 ? w - x : 4;   // valid pixels of this float4 (1..4)
+    gray[i] = gray4<MONO>(p0, lo + (long long)cb * (row * w + x), nv, lo, hi);
+}
+
+// Strided frames (rb_pipeline_push_frames_dev): frame f of the batch starts at frames[f].data and its rows are
+// frames[f].step bytes apart, each frame read where it is.  A thread makes the float4 of 4 pixels of one gray row, pitched
+// or not (pitch == w), as k_gray_pitched does, but word indices count from the frame's own first byte rounded down to 4 and
+// loads are bounded by the frame's span [data, data + (h-1)*step + w*bpp): the row padding and the bytes around a frame are
+// never read (the padding columns of the last float4 of a row get +0 whatever was loaded).
+template <bool MONO>
+__global__ void __launch_bounds__(256) k_gray_strided(const rb_frame *__restrict__ frames, float4 *__restrict__ gray, int w,
+                                                      int h, int pitch, int nimg) {
+    const int pv = pitch >> 2;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the (pitched) batch
+    if (i >= (long long)nimg * h * pv) return;
+    const long long row = i / pv;   // frame * h + y
+    const int f = (int)(row / h), y = (int)(row - (long long)f * h);
+    const int x = 4 * (int)(i - row * pv);
+    const uint8_t *src = frames[f].data;
+    const long long step = frames[f].step;
+    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+    const int cb = MONO ? 1 : 3;
+    const long long lo = (long long)(src - p0), hi = lo + (long long)(h - 1) * step + (long long)cb * w;
+    const int nv = w - x < 4 ? w - x : 4;
+    gray[i] = gray4<MONO>(p0, lo + (long long)y * step + (long long)cb * x, nv, lo, hi);
 }
 
 // Column pass, software-pipelined: VW adjacent columns per thread, the next U rows are in flight while the current U are added
@@ -489,6 +517,15 @@ int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
     k_rgb2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
                                                                    (const uint32_t *const *)src_pp,
                                                                    (float4 *)ws->gray, n4);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
+// strided RGB24 / mono frames -> gray (rb_pipeline_push_frames_dev): frame f of the batch is frames_dev[f], a device table
+int rb_dog_gray_strided(rb_ctx *c, DogWS *ws, int nimg, const rb_frame *frames_dev, bool mono) {
+    const size_t n4 = (size_t)nimg * c->NP / 4;
+    (mono ? k_gray_strided<true> : k_gray_strided<false>)<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>(
+        frames_dev, (float4 *)ws->gray, c->w, c->h, c->pitch, nimg);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }

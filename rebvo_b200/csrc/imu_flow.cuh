@@ -322,14 +322,14 @@ static int imu_live_check(rb_pipeline *pl, const ImuFlow &f, const double *ts, i
 }
 
 // a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking
-static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, int fmt, bool on_device, const double *ts, int n,
-                    rb_nav *nav_out, rb_odometry *odom_out) {
+// (rgb, frames, fmt as push_impl's)
+static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device,
+                    const double *ts, int n, rb_nav *nav_out, rb_odometry *odom_out) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
-    const size_t fbytes = frame_bytes(c, fmt);
-    if (!on_device)
-        RB_CUDA(cudaMemcpyAsync(pl->ws.rgb, rgb, (size_t)n * fbytes, cudaMemcpyHostToDevice, c->stream));
+    if (!on_device && (r = stage_host_frames(pl, rgb, frames, fmt, 0, n, c->stream))) return r;
+    if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;
     pl->sb_pin[0].src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
     RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
     if ((r = gray_pass(pl, fmt, n))) return r;

@@ -82,6 +82,11 @@ struct rb_pipeline {
     cudaEvent_t ev_copy[2];       // per sub-batch: its frames are on the device
     SubBatchPtrs *sb_dev;         // device: the table of the sub-batch being processed
     SubBatchPtrs *sb_pin;         // pinned: one entry per sub-batch of the current push (at most two)
+    // strided device input (rb_pipeline_push_frames_dev): frame i of the push is frames_dev[i], written from frames_pin
+    // before the batch runs, so that one captured batch serves every push of that layout.  Apart from SubBatchPtrs: the
+    // packed pushes' per-sub-batch copy does not grow.
+    rb_frame *frames_dev;         // device [max_batch]
+    rb_frame *frames_pin;         // pinned [max_batch]
     int sub;                      // head sub-batch of a host-input push (env REBVO_B200_SUB, default 8 frames)
     DetChain *chain;      // device
     FrameState *fs;       // device
@@ -172,10 +177,15 @@ struct rb_pipeline {
 
 int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
 int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
+int rb_undistort_gray_strided_enqueue(rb_undistort *u, const rb_frame *frames_dev, float *gray, int nimg, bool mono);
 
-// input formats of a push: RGB24 (3 bytes per pixel) or mono8, which stands for the RGB24 frame (m, m, m)
-enum { RB_IN_RGB = 0, RB_IN_MONO = 1, RB_NFMT = 2 };
-static inline size_t frame_bytes(const rb_ctx *c, int fmt) { return (fmt == RB_IN_MONO ? (size_t)1 : (size_t)3) * c->N; }
+// input layouts of a push: packed RGB24 (3 bytes per pixel) or mono8, which stands for the RGB24 frame (m, m, m), at
+// sb_dev->src; or the same two formats as strided device frames, one {data, step} entry per frame in frames_dev.  Each
+// layout has graph slots of its own.
+enum { RB_IN_RGB = 0, RB_IN_MONO = 1, RB_IN_RGB_STRIDED = 2, RB_IN_MONO_STRIDED = 3, RB_NFMT = 4 };
+static inline bool in_mono(int fmt) { return fmt == RB_IN_MONO || fmt == RB_IN_MONO_STRIDED; }
+static inline bool in_strided(int fmt) { return fmt == RB_IN_RGB_STRIDED || fmt == RB_IN_MONO_STRIDED; }
+static inline size_t frame_bytes(const rb_ctx *c, int fmt) { return (in_mono(fmt) ? (size_t)1 : (size_t)3) * c->N; }
 static inline int graph_slots(const rb_pipeline *pl) { return RB_NFMT * RB_NMAPS * (pl->max_batch + 1); }
 static inline int graph_slot(const rb_pipeline *pl, int fmt, int phase, int n) {
     return (fmt * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
@@ -221,13 +231,40 @@ static int grow_out(rb_pipeline *pl, unsigned char **host, size_t *host_have, un
                     size_t bytes) {
     return pl->out_dev ? grow_dev(pl->c, dev, dev_have, bytes) : grow_mapped(pl->c, host, host_have, bytes);
 }
-// the batch's gray plane from the frames at sb_dev->src (rebvo_first_t.cpp:231 undistortion + RGB -> BW)
+// the batch's gray plane from the frames at sb_dev->src, or through frames_dev for the strided layouts (rebvo_first_t.cpp:231
+// undistortion + RGB -> BW)
 static int gray_pass(rb_pipeline *pl, int fmt, int n) {
+    if (in_strided(fmt))
+        return pl->und ? rb_undistort_gray_strided_enqueue(pl->und, pl->frames_dev, pl->ws.gray, n, in_mono(fmt))
+                       : rb_dog_gray_strided(pl->c, &pl->ws, n, pl->frames_dev, in_mono(fmt));
     const void *const *src = &pl->sb_dev->src;
     if (pl->und)
         return fmt == RB_IN_MONO ? rb_undistort_gray_mono_enqueue(pl->und, src, pl->ws.gray, n)
                                  : rb_undistort_gray_enqueue(pl->und, src, pl->ws.gray, n);
     return fmt == RB_IN_MONO ? rb_dog_gray_mono(pl->c, &pl->ws, n, src) : rb_dog_gray(pl->c, &pl->ws, n, src);
+}
+// host frames of a push into the packed staging, frames [i0, i0 + count) of `frames` (strided, one 2D copy each) or of the
+// packed buffer `rgb`, on stream s
+static int stage_host_frames(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, int i0, int count,
+                             cudaStream_t s) {
+    rb_ctx *c = pl->c;
+    const size_t fbytes = frame_bytes(c, fmt), row = fbytes / c->h;
+    uint8_t *dst = pl->ws.rgb + (size_t)i0 * fbytes;
+    if (!frames) {
+        RB_CUDA(cudaMemcpyAsync(dst, rgb + (size_t)i0 * fbytes, (size_t)count * fbytes, cudaMemcpyHostToDevice, s));
+        return RB_OK;
+    }
+    for (int i = 0; i < count; i++)
+        RB_CUDA(cudaMemcpy2DAsync(dst + (size_t)i * fbytes, row, frames[i0 + i].data, (size_t)frames[i0 + i].step, row, c->h,
+                                  cudaMemcpyHostToDevice, s));
+    return RB_OK;
+}
+// strided device frames: the push's {data, step} table into frames_dev, on the tracker stream before the batch
+static int write_frame_table(rb_pipeline *pl, const rb_frame *frames, int n) {
+    rb_ctx *c = pl->c;
+    memcpy(pl->frames_pin, frames, sizeof(rb_frame) * n);
+    RB_CUDA(cudaMemcpyAsync(pl->frames_dev, pl->frames_pin, sizeof(rb_frame) * n, cudaMemcpyHostToDevice, c->stream));
+    return RB_OK;
 }
 #include "imu_flow.cuh"
 
@@ -380,6 +417,8 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
         if (pl->sub < 1) pl->sub = max_batch;
         RB_CUDA(cudaMalloc(&pl->sb_dev, sizeof(SubBatchPtrs)));
         RB_CUDA(cudaMallocHost(&pl->sb_pin, 2 * sizeof(SubBatchPtrs)));
+        RB_CUDA(cudaMalloc(&pl->frames_dev, sizeof(rb_frame) * max_batch));
+        RB_CUDA(cudaMallocHost(&pl->frames_pin, sizeof(rb_frame) * max_batch));
         RB_CUDA(cudaEventCreateWithFlags(&pl->ev_hop, cudaEventDisableTiming));
         for (int i = 0; i < 2; i++) {
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
@@ -500,11 +539,11 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
         if (pl->maps[i]) rb_map_destroy(pl->maps[i]);
     if (pl->und) rb_undistort_destroy(pl->und);
     rb_dogws_free(&pl->ws);
-    void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->mirror.dev, pl->odom.dev, pl->depth.stage,
-                   pl->depth.ws, pl->depth.dev, pl->dimg.dev};
+    void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->frames_dev, pl->mirror.dev, pl->odom.dev,
+                   pl->depth.stage, pl->depth.ws, pl->depth.dev, pl->dimg.dev};
     for (void *p : dev) cudaFree(p);
-    void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->mirror.host, pl->odom.pin, pl->depth.host,
-                    pl->dimg.host};
+    void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->frames_pin, pl->mirror.host, pl->odom.pin,
+                    pl->depth.host, pl->dimg.host};
     for (void *p : host)
         if (p) cudaFreeHost(p);
     rb_ctx_destroy(c);
@@ -742,12 +781,13 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     return RB_OK;
 }
 
-// rgb: n frames of frame_bytes(fmt) each, host or device memory
-static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_device, const double *ts, int n,
-                     rb_nav *nav_out) {
+// rgb: n packed frames of frame_bytes(fmt) each, host or device memory; or (rgb == nullptr) frames: n strided frames, checked
+// by push_frames, whose layout is fmt (device memory) or whose packed format is fmt (host memory)
+static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
+                     int n, rb_nav *nav_out) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
-    if (n < 1 || n > pl->max_batch || !rgb || !ts) return RB_ERR_ARG;
+    if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts) return RB_ERR_ARG;
     // (the mono kernels read the frames as 32-bit words; the RGB kernels have a byte-wise path for unaligned buffers)
     if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
     int r;
@@ -757,7 +797,8 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     pl->depth.n = 0;
     pl->dimg.n = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
-        if ((r = imu_push(pl, *pl->imu, rgb, fmt, on_device, ts, n, pl->nav_pin, pl->odom.on ? pl->odom.pin : nullptr)))
+        if ((r = imu_push(pl, *pl->imu, rgb, frames, fmt, on_device, ts, n, pl->nav_pin,
+                          pl->odom.on ? pl->odom.pin : nullptr)))
             return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
         if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
@@ -794,17 +835,17 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, int fmt, bool on_devic
     for (int j = 0; j < nsub && !on_device; j++) {
         const int off = soff[j], nj = soff[j + 1] - soff[j];
         cudaStream_t cs = nsub > 1 ? pl->copy_stream : c->stream;
-        RB_CUDA(cudaMemcpyAsync(pl->ws.rgb + (size_t)off * fbytes, rgb + (size_t)off * fbytes, (size_t)nj * fbytes,
-                                cudaMemcpyHostToDevice, cs));
+        if ((r = stage_host_frames(pl, rgb, frames, fmt, off, nj, cs))) return r;
         if (nsub > 1) RB_CUDA(cudaEventRecord(pl->ev_copy[j], cs));
     }
+    if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;   // (device input: one sub-batch)
     for (int j = 0; j < nsub; j++) {
         const int off = soff[j], nj = soff[j + 1] - soff[j];
         const long long first_j = first + (long long)off;
         if (!on_device && nsub > 1) RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_copy[j], 0));
         RB_CUDA(cudaMemcpyAsync(pl->fa_dev, pl->fa_pin + off, sizeof(FrameArgs) * nj, cudaMemcpyHostToDevice, c->stream));
         SubBatchPtrs &t = pl->sb_pin[j];
-        t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);
+        t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);   // (strided: unused)
         if (pl->mirror.on) {
             t.mirror[0] = pl->mirror.dev + (size_t)off * pl->mirror.stride;
             t.mirror[1] = pl->out_dev ? nullptr : pl->mirror.host + (size_t)off * pl->mirror.stride;
@@ -1152,18 +1193,51 @@ extern "C" int rb_pipeline_depth_image_dev(rb_pipeline *pl, int i, const float *
 }
 
 extern "C" int rb_pipeline_push(rb_pipeline *pl, const uint8_t *rgb, const double *ts, int n, rb_nav *nav_out) {
-    return push_impl(pl, rgb, RB_IN_RGB, false, ts, n, nav_out);
+    return push_impl(pl, rgb, nullptr, RB_IN_RGB, false, ts, n, nav_out);
 }
 extern "C" int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *ts, int n,
                                     rb_nav *nav_out) {
-    return push_impl(pl, rgb_dev, RB_IN_RGB, true, ts, n, nav_out);
+    return push_impl(pl, rgb_dev, nullptr, RB_IN_RGB, true, ts, n, nav_out);
 }
 extern "C" int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out) {
-    return push_impl(pl, mono, RB_IN_MONO, false, ts, n, nav_out);
+    return push_impl(pl, mono, nullptr, RB_IN_MONO, false, ts, n, nav_out);
 }
 extern "C" int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n,
                                          rb_nav *nav_out) {
-    return push_impl(pl, mono_dev, RB_IN_MONO, true, ts, n, nav_out);
+    return push_impl(pl, mono_dev, nullptr, RB_IN_MONO, true, ts, n, nav_out);
+}
+// strided frames: every argument is checked before anything is enqueued; host frames then run the packed format's batches,
+// device frames the strided layout's
+static int push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out,
+                       bool on_device) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    if (format != RB_FRAME_RGB24 && format != RB_FRAME_MONO8) {
+        snprintf(c->err, sizeof(c->err), "push_frames: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", format);
+        return RB_ERR_ARG;
+    }
+    if (n < 1 || n > pl->max_batch || !frames || !ts) return RB_ERR_ARG;
+    const int64_t row = (int64_t)(format == RB_FRAME_MONO8 ? 1 : 3) * c->w;
+    for (int i = 0; i < n; i++)
+        if (!frames[i].data || frames[i].step < row) {
+            snprintf(c->err, sizeof(c->err), "push_frames: frame %d has %s (rows need %lld bytes)", i,
+                     frames[i].data ? "a step shorter than a row" : "no data", (long long)row);
+            return RB_ERR_ARG;
+        }
+    if (on_device && pl->und && (c->w > 65535 || c->h > 65535)) {   // (the strided undistortion's 16-bit tap coordinates)
+        snprintf(c->err, sizeof(c->err), "push_frames_dev: undistorted frames wider or higher than 65535 pixels");
+        return RB_ERR_ARG;
+    }
+    const int fmt = format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB;
+    return push_impl(pl, nullptr, frames, on_device ? fmt + RB_IN_RGB_STRIDED : fmt, on_device, ts, n, nav_out);
+}
+extern "C" int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
+                                       rb_nav *nav_out) {
+    return push_frames(pl, format, frames, ts, n, nav_out, false);
+}
+extern "C" int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
+                                           rb_nav *nav_out) {
+    return push_frames(pl, format, frames, ts, n, nav_out, true);
 }
 
 extern "C" int rb_pipeline_event_record(rb_pipeline *pl, int slot) {

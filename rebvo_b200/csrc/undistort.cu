@@ -19,6 +19,8 @@
 struct rb_undistort {
     rb_ctx *c;
     int4 *inx, *iw;
+    int4 *ixy;                   // the taps of inx as x | y << 16, for the strided kernel (built with the map; frames of up
+                                 // to 65535 x 65535 pixels, rb_pipeline_push_frames_dev)
     uint8_t *tmp_in, *tmp_out;   // staging for the host-pointer entry point
 };
 
@@ -119,29 +121,36 @@ __device__ __forceinline__ unsigned int ug_word(const uint8_t *__restrict__ p0, 
         if (b + k >= lo && b + k < hi) v |= (unsigned int)__ldg(p0 + b + k) << (8 * k);
     return v;
 }
-__device__ __forceinline__ float ug_pixel_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
-                                              const int4 ix, const int4 w) {
+// The four taps at bytes ofs[k] of the word array p0; pairs: taps 0, 1 and taps 2, 3 are two runs of two adjacent pixels
+__device__ __forceinline__ float ug_taps_rgb(const uint8_t *__restrict__ p0, const long long ofs[4], bool pairs, long long lo,
+                                             long long hi, const int4 w) {
     int r = 0, g = 0, b = 0;
-    if (ix.y == ix.x + 1 && ix.w == ix.z + 1) {   // two runs of two adjacent pixels, as ug_pixel
+    if (pairs) {   // as ug_pixel
 #pragma unroll
         for (int row = 0; row < 2; row++) {
-            const long long ofs = t0 + 3 * (row ? ix.z : ix.x), wi = ofs >> 2;
-            const int sh = (int)(ofs & 3) * 8;
+            const long long o = ofs[2 * row], wi = o >> 2;
+            const int sh = (int)(o & 3) * 8;
             const unsigned int w0 = ug_word(p0, wi, lo, hi), w1 = ug_word(p0, wi + 1, lo, hi), w2 = ug_word(p0, wi + 2, lo, hi);
             const unsigned int l = __funnelshift_r(w0, w1, sh), m = __funnelshift_r(w1, w2, sh);
             ug_acc(l, row ? w.z : w.x, r, g, b);
             ug_acc(__funnelshift_r(l, m, 24), row ? w.w : w.y, r, g, b);
         }
     } else {
-        const int t[4] = {ix.x, ix.y, ix.z, ix.w}, ww[4] = {w.x, w.y, w.z, w.w};
+        const int ww[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            const long long ofs = t0 + 3 * t[k], wi = ofs >> 2;
-            ug_acc(__funnelshift_r(ug_word(p0, wi, lo, hi), ug_word(p0, wi + 1, lo, hi), (int)(ofs & 3) * 8), ww[k], r, g, b);
+            const long long wi = ofs[k] >> 2;
+            ug_acc(__funnelshift_r(ug_word(p0, wi, lo, hi), ug_word(p0, wi + 1, lo, hi), (int)(ofs[k] & 3) * 8), ww[k], r, g,
+                   b);
         }
     }
     const unsigned int s = (unsigned int)((uint8_t)(r >> 16)) + (unsigned int)((uint8_t)(g >> 16)) + (unsigned int)((uint8_t)(b >> 16));
     return (float)s;
+}
+__device__ __forceinline__ float ug_pixel_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
+                                              const int4 ix, const int4 w) {
+    const long long ofs[4] = {t0 + 3 * ix.x, t0 + 3 * ix.y, t0 + 3 * ix.z, t0 + 3 * ix.w};
+    return ug_taps_rgb(p0, ofs, ix.y == ix.x + 1 && ix.w == ix.z + 1, lo, hi, w);
 }
 // IMGS frames per thread: the 32-byte map entry of a pixel (L2-resident, but 739 MB of L2 reads per 64-frame launch when every
 // frame fetches it again) is loaded once for IMGS frames.  ANYW: any width (see ug_pixel_any); otherwise w % 4 == 0, the plane
@@ -220,23 +229,29 @@ __device__ __forceinline__ float ug_pixel_mono(const uint8_t *__restrict__ src, 
 // keeps its rule that the source is 4-byte aligned, so lo = 0 there; the frames after the first start at any byte when
 // N % 4 != 0).  The pair's second byte t0 + ix.x + 1 is inside the frame, so when the pair straddles a word boundary its
 // second word holds a byte of the batch and ug_word reads it whole or byte by byte.
-__device__ __forceinline__ float ug_pixel_mono_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
-                                                   const int4 ix, const int4 w) {
+// (the mono taps at bytes ofs[k], as ug_taps_rgb)
+__device__ __forceinline__ float ug_taps_mono(const uint8_t *__restrict__ p0, const long long ofs[4], bool pairs, long long lo,
+                                              long long hi, const int4 w) {
     int s;
-    if (ix.y == ix.x + 1 && ix.w == ix.z + 1) {
+    if (pairs) {
         s = 0;
 #pragma unroll
         for (int row = 0; row < 2; row++) {
-            const long long ofs = t0 + (row ? ix.z : ix.x), wi = ofs >> 2;
-            const unsigned int w0 = ug_word(p0, wi, lo, hi), w1 = (ofs & 3) == 3 ? ug_word(p0, wi + 1, lo, hi) : w0;
-            const unsigned int v = __funnelshift_r(w0, w1, (int)(ofs & 3) * 8);   // bytes ofs, ofs + 1 in the low half
+            const long long o = ofs[2 * row], wi = o >> 2;
+            const unsigned int w0 = ug_word(p0, wi, lo, hi), w1 = (o & 3) == 3 ? ug_word(p0, wi + 1, lo, hi) : w0;
+            const unsigned int v = __funnelshift_r(w0, w1, (int)(o & 3) * 8);   // bytes o, o + 1 in the low half
             s += (row ? w.z : w.x) * (int)(v & 0xffu) + (row ? w.w : w.y) * (int)((v >> 8) & 0xffu);
         }
     } else {
-        s = w.x * (int)__ldg(p0 + t0 + ix.x) + w.y * (int)__ldg(p0 + t0 + ix.y) + w.z * (int)__ldg(p0 + t0 + ix.z) +
-            w.w * (int)__ldg(p0 + t0 + ix.w);
+        s = w.x * (int)__ldg(p0 + ofs[0]) + w.y * (int)__ldg(p0 + ofs[1]) + w.z * (int)__ldg(p0 + ofs[2]) +
+            w.w * (int)__ldg(p0 + ofs[3]);
     }
     return (float)(3u * (unsigned int)(uint8_t)(s >> 16));
+}
+__device__ __forceinline__ float ug_pixel_mono_any(const uint8_t *__restrict__ p0, long long t0, long long lo, long long hi,
+                                                   const int4 ix, const int4 w) {
+    const long long ofs[4] = {t0 + ix.x, t0 + ix.y, t0 + ix.z, t0 + ix.w};
+    return ug_taps_mono(p0, ofs, ix.y == ix.x + 1 && ix.w == ix.z + 1, lo, hi, w);
 }
 template <int IMGS, bool ANYW>
 __global__ void __launch_bounds__(256) k_undistort_gray_mono(const uint8_t *const *__restrict__ src_pp,
@@ -284,6 +299,67 @@ int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, f
     return RB_OK;
 }
 
+// Strided frames (rb_pipeline_push_frames_dev), RGB24 or mono: frame f of the batch is frames[f] = {data, step}.  The map's
+// taps as (x, y) -- ixy, the packed indices of inx split once when the map is built, so the kernel reads as many map bytes
+// as k_undistort_gray and divides nothing -- are shared by the thread's IMGS frames (the map entry is loaded once, as in
+// k_undistort_gray); tap k of a frame is then at byte y*step + x*bpp of that frame.  Word indices count from the frame's
+// first byte rounded down to 4, and ug_word bounds every load by the frame's span [data, data + (h-1)*step + w*bpp), so
+// frames may start at any byte and the row padding is never read.  The two-runs path needs the taps of a pair on one row.
+// The gray plane is written as k_undistort_gray's any-width one (rows of `pitch` floats; pitch == w: unpitched).
+template <int IMGS, bool MONO>
+__global__ void __launch_bounds__(256) k_undistort_gray_strided(const rb_frame *__restrict__ frames, float *__restrict__ gray,
+                                                                const int4 *__restrict__ ixy, const int4 *__restrict__ iw,
+                                                                int N, int nimg, int wd, int pitch) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int img0 = blockIdx.y * IMGS;
+    if (i >= N) return;
+    const int4 xy = ixy[i], w = iw[i];
+    const int t[4] = {xy.x, xy.y, xy.z, xy.w};
+    int tx[4], ty[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        tx[k] = t[k] & 0xffff;
+        ty[k] = (int)((unsigned int)t[k] >> 16);
+    }
+    const bool pairs = ty[1] == ty[0] && tx[1] == tx[0] + 1 && ty[3] == ty[2] && tx[3] == tx[2] + 1;
+    const int cb = MONO ? 1 : 3, h = N / wd;
+    float v[IMGS];
+#pragma unroll
+    for (int k = 0; k < IMGS; k++) {
+        v[k] = 0.f;
+        if (img0 + k >= nimg) continue;
+        const uint8_t *src = frames[img0 + k].data;
+        const long long step = frames[img0 + k].step;
+        const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
+        const long long lo = (long long)(src - p0), hi = lo + (long long)(h - 1) * step + (long long)cb * wd;
+        long long ofs[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) ofs[j] = lo + (long long)ty[j] * step + (long long)cb * tx[j];
+        v[k] = MONO ? ug_taps_mono(p0, ofs, pairs, lo, hi, w) : ug_taps_rgb(p0, ofs, pairs, lo, hi, w);
+    }
+    const int y = i / wd;
+    const size_t o = (size_t)y * pitch + (i - y * wd), plane = (size_t)pitch * h;
+#pragma unroll
+    for (int k = 0; k < IMGS; k++)
+        if (img0 + k < nimg) gray[(size_t)(img0 + k) * plane + o] = v[k];
+}
+int rb_undistort_gray_strided_enqueue(rb_undistort *u, const rb_frame *frames_dev, float *gray, int nimg, bool mono) {
+    rb_ctx *c = u->c;
+#define UGS_LAUNCH(K, M)                                                                                           \
+    k_undistort_gray_strided<K, M><<<dim3(rb_div_up(c->N, 256), rb_div_up(nimg, K)), 256, 0, c->stream>>>(        \
+        frames_dev, gray, u->ixy, u->iw, c->N, nimg, c->w, c->pitch)
+    if (nimg >= 4) {
+        if (mono) UGS_LAUNCH(4, true);
+        else UGS_LAUNCH(4, false);
+    } else {
+        if (mono) UGS_LAUNCH(1, true);
+        else UGS_LAUNCH(1, false);
+    }
+#undef UGS_LAUNCH
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+}
+
 static inline bool inx_valid_f(float fx, float fy, int w, int h) {
     // Image::isInxValid takes `const uint&`: the float is converted to unsigned (x86-64: through a 64-bit
     // truncation, so negatives wrap to huge values and fail the upper bound)
@@ -307,7 +383,7 @@ extern "C" int rb_undistort_create(rb_ctx *c, const double kc[5], rb_undistort *
     const double Kc2 = kc[0], Kc4 = kc[1], Kc6 = kc[2], P1 = kc[3], P2 = kc[4];
     const float ppx = c->cam.ppx, ppy = c->cam.ppy, zfx = c->cam.zfx, zfy = c->cam.zfy;
     const double zfm = c->zfm;
-    std::vector<int4> hinx(N), hiw(N);
+    std::vector<int4> hinx(N), hiw(N), hxy(N);
     const float i_mult = (float)(1 << 16);
     for (int x = 0; x < w; x++)
         for (int y = 0; y < h; y++) {
@@ -361,15 +437,20 @@ extern "C" int rb_undistort_create(rb_ctx *c, const double kc[5], rb_undistort *
             const int o = y * w + x;                                  // umap(x,y)
             hinx[o] = make_int4(inx[0], inx[1], inx[2], inx[3]);
             hiw[o] = make_int4(iw[0], iw[1], iw[2], iw[3]);
+            int xy[4];
+            for (int i = 0; i < 4; i++) xy[i] = (int)((unsigned int)(inx[i] % w) | (unsigned int)(inx[i] / w) << 16);
+            hxy[o] = make_int4(xy[0], xy[1], xy[2], xy[3]);
         }
     *out = u;
     RB_CUDA(cudaSetDevice(c->device));
     RB_CUDA(cudaMalloc(&u->inx, sizeof(int4) * (size_t)N));
     RB_CUDA(cudaMalloc(&u->iw, sizeof(int4) * (size_t)N));
+    RB_CUDA(cudaMalloc(&u->ixy, sizeof(int4) * (size_t)N));
     RB_CUDA(cudaMalloc(&u->tmp_in, (size_t)3 * N));
     RB_CUDA(cudaMalloc(&u->tmp_out, (size_t)3 * N));
     RB_CUDA(cudaMemcpy(u->inx, hinx.data(), sizeof(int4) * (size_t)N, cudaMemcpyHostToDevice));
     RB_CUDA(cudaMemcpy(u->iw, hiw.data(), sizeof(int4) * (size_t)N, cudaMemcpyHostToDevice));
+    RB_CUDA(cudaMemcpy(u->ixy, hxy.data(), sizeof(int4) * (size_t)N, cudaMemcpyHostToDevice));
     return RB_OK;
 }
 
@@ -379,6 +460,7 @@ extern "C" void rb_undistort_destroy(rb_undistort *u) {
     cudaStreamSynchronize(u->c->stream);
     cudaFree(u->inx);
     cudaFree(u->iw);
+    cudaFree(u->ixy);
     cudaFree(u->tmp_in);
     cudaFree(u->tmp_out);
     delete u;
