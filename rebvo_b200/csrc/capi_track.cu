@@ -156,7 +156,11 @@ extern "C" int rb_minimizer_rv(rb_map *fmap, rb_map *old, double V[3], double W[
 extern "C" int rb_forward_match(rb_map *old, rb_map *neu, int *nmatch) {
     if (!old || !neu) return RB_ERR_ARG;
     RB_ENTER(old->c);
-    int r = rb_forward_match_enqueue(old->c, old, neu);
+    // *nmatch counts this call's matches: a pipeline context leaves the counter to its per-frame kernel, which the IMU
+    // flow (the caller inside a pipeline) does not run, so the count would add up over the frames that reuse neu
+    rb_ctx *c = old->c;
+    RB_CUDA(cudaMemsetAsync(&neu->st->fwd_match, 0, sizeof(int), c->stream));
+    int r = rb_forward_match_enqueue(c, old, neu);
     if (r) return r;
     MapState s;
     if ((r = rb_read_map_state(neu, &s))) return r;

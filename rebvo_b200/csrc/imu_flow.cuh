@@ -140,7 +140,9 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
     if (p.TrackerInitType == 0)
         for (int i = 0; i < 3; i++) f.Vg[i] = 0;
     double score = 0;
-    if (os.kn > 0)   // global_tracker::Minimizer_V returns at once on an empty map
+    // On an empty old map the reference's Minimizer_V runs iter_max rejected NaN steps: Vel stays as it is and P_Vg
+    // becomes NaN.  P_Vg is never read (rebvo_second_t.cpp only writes it), so skipping the call gives the same frame.
+    if (os.kn > 0)
         if ((r = rb_minimizer_v(neu, old, f.Vg, f.P_Vg, p.TrackerMatchThresh, p.TrackerIterNum, s_rho_q, p.MatchNumThresh,
                                 p.ReweigthDistance, os.retuned, &score)))
             return r;

@@ -344,8 +344,13 @@ static int pl_reset_state(rb_pipeline *pl) {
     ch.l_kl_num = 0;
     ch.pad = 0;
     RB_CUDA(cudaMemcpy(pl->chain, &ch, sizeof(ch), cudaMemcpyHostToDevice));
+    // FrameCount 0 in every ring map: the vision flow rewrites it each frame, but the IMU flow only reads it (the
+    // reference raises FrameCount in Minimizer_RV alone, so its IMU mode never gates on m_num)
     for (int k = 0; k < RB_NMAPS; k++)
-        if (pl->maps[k]) RB_CUDA(cudaMemset(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int)));
+        if (pl->maps[k]) {
+            RB_CUDA(cudaMemset(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int)));
+            RB_CUDA(cudaMemset(&pl->maps[k]->st->frame_count, 0, sizeof(unsigned int)));
+        }
     if (pl->imu) imu_flow_reset(*pl->imu);
     pl->n_pushed = 0;
     pl->t_prev = 0;
