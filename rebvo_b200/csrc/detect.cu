@@ -163,8 +163,7 @@ __global__ void __launch_bounds__(1024) k_seg_scan(int *__restrict__ seg, int ns
     if (tid == 0) {
         const int total = base;
         int kn = total;
-        if (kn > kl_max) kn = kl_max;   // build_mask stops when ++kn >= kl_max (:203)
-        if (kn < 0) kn = 0;
+        if (kn > kl_max) kn = kl_max;   // build_mask stops when ++kn >= kl_max (:203); kl_max >= 1 here
         st->total_cand = total;
         st->kn = kn;
         st->nmatch = 0;
@@ -179,14 +178,22 @@ __global__ void __launch_bounds__(256) k_detect_b(int *__restrict__ mask, const 
     const int lane = threadIdx.x & 31;
     const int seg = blockIdx.x * 8 + (threadIdx.x >> 5);
     const int y = seg / nchunk, ch = seg - y * nchunk;
-    if (y < border || y >= h - border) return;
+    if (y >= h) return;
     const int x = ch * 32 + lane;
-    const bool interior = (x >= border && x < w - border);
+    const bool interior = (y >= border && y < h - border && x >= border && x < w - border);
     const size_t idx = (size_t)y * w + x;
     const bool is_cand = interior && mask[idx] == -2;
     const unsigned bal = __ballot_sync(0xffffffffu, is_cand);
-    if (!is_cand) return;
-    const int id = seg_off[seg] + __popc(bal & ((1u << lane) - 1u));
+    const int off = seg_off[seg];
+    const int id = off + __popc(bal & ((1u << lane) - 1u));
+    // The cut clears every pixel after the kl_max-th keyline, the border included (:205-207).  Interior non-candidates
+    // are -1 already; a border pixel holds an id only if one was loaded there (rb_map_load_keylines).
+    const unsigned cut = __ballot_sync(0xffffffffu, is_cand && id == kl_max - 1);
+    const bool past = off >= kl_max || (cut && lane > __ffs(cut) - 1);
+    if (!is_cand) {
+        if (past && !interior && x < w) mask[idx] = -1;
+        return;
+    }
     if (id >= kl_max) {   // past the cut: the reference never visits these pixels and clears the mask (:205-207)
         mask[idx] = -1;
         return;
@@ -343,7 +350,10 @@ int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
     }
     const int w = c->w, h = c->h;
     const int nchunk = rb_div_up(w, 32);
-    int kl_max = p->kl_max > c->kcap ? c->kcap : p->kl_max;   // build_mask: kl_max>kl_size -> kl_size (:105)
+    // build_mask: kl_max>kl_size -> kl_size (:105).  It appends a keyline before it tests ++kn >= kl_max (:203), so any
+    // kl_max <= 0 keeps the first candidate: the cut is at least 1.
+    int kl_max = p->kl_max > c->kcap ? c->kcap : p->kl_max;
+    if (kl_max < 1) kl_max = 1;
     k_update_thresh<<<1, 1, 0, c->stream>>>(chain_dev, m->st, p->gain, p->kl_ref, p->thresh_max,
                                             p->thresh_min);
     RB_LAUNCH_CHECK();
