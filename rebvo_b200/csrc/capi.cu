@@ -444,7 +444,7 @@ extern "C" int rb_map_upload_rgb(rb_map *m, const uint8_t *rgb) {
     rb_ctx *c = m->c;
     if (!m->owns_ws) return RB_ERR_STATE;
     RB_CUDA(cudaMemcpyAsync(m->ws.rgb, rgb, (size_t)3 * c->N, cudaMemcpyHostToDevice, c->stream));
-    return rb_dog_gray(c, &m->ws, 1);
+    return rb_gray_enqueue(c, &m->ws, nullptr, false, nullptr, nullptr, 1);
 }
 
 extern "C" int rb_map_upload_mono(rb_map *m, const uint8_t *mono) {
@@ -453,7 +453,7 @@ extern "C" int rb_map_upload_mono(rb_map *m, const uint8_t *mono) {
     rb_ctx *c = m->c;
     if (!m->owns_ws) return RB_ERR_STATE;
     RB_CUDA(cudaMemcpyAsync(m->ws.rgb, mono, (size_t)c->N, cudaMemcpyHostToDevice, c->stream));
-    return rb_dog_gray_mono(c, &m->ws, 1);
+    return rb_gray_enqueue(c, &m->ws, nullptr, true, nullptr, nullptr, 1);
 }
 
 extern "C" int rb_map_upload_gray(rb_map *m, const float *gray) {

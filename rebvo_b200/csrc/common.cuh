@@ -257,13 +257,14 @@ static inline cudaError_t rb_klaunch(bool pdl, void (*kernel)(KArgs...), dim3 gr
 // dog.cu
 int rb_dogws_alloc(rb_ctx *c, DogWS *ws, int B);
 void rb_dogws_free(DogWS *ws);
-int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // rgb -> gray
-int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp = nullptr);   // mono -> gray
-int rb_dog_gray_strided(rb_ctx *c, DogWS *ws, int nimg, const rb_frame *frames_dev, bool mono);   // strided frames -> gray
 int rb_dog_build_batch(rb_ctx *c, DogWS *ws, int nimg);          // gray -> img0, dog
 int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img);            // Img(1), dx, dy into ws->aux
 int rb_dog_make_tables(rb_ctx *c);
 int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws);
+// gray.cu: nimg RGB24 / mono8 frames -> ws->gray, undistorted through und unless it is null.  The frames are the strided
+// device frames of the table frames_dev, or else packed at *src_pp (at ws->rgb when src_pp is null; undistortion needs src_pp).
+int rb_gray_enqueue(rb_ctx *c, DogWS *ws, const rb_undistort *und, bool mono, const void *const *src_pp,
+                    const rb_frame *frames_dev, int nimg);
 // detect.cu
 int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
                       const rb_detect_params *p, DetChain *chain_dev);

@@ -52,132 +52,6 @@ __device__ __forceinline__ float box_avg(const float *__restrict__ I, int x, int
     return r * tab[(cy - d2 - 1) * BOX_TAB_W + (cx - d2 - 1)];
 }
 
-// Image<float>::ConvertRGB2BW (image.h:197-203): b+g+r as float, 4 pixels per thread
-// src_pp (optional): the RGB source is read through a device-resident pointer, so that one captured graph serves
-// whichever staging region / caller buffer a push uses (rb_pipeline)
-__global__ void __launch_bounds__(256) k_rgb2gray(const uint32_t *__restrict__ rgb_fixed,
-                                                  const uint32_t *const *__restrict__ src_pp,
-                                                  float4 *__restrict__ gray, size_t n4) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
-    const uint32_t *__restrict__ rgb = src_pp ? *src_pp : rgb_fixed;
-    uint32_t a = rgb[3 * i], b = rgb[3 * i + 1], c = rgb[3 * i + 2];
-    // bytes: a = p0.0 p0.1 p0.2 p1.0 | b = p1.1 p1.2 p2.0 p2.1 | c = p2.2 p3.0 p3.1 p3.2
-    float4 o;
-    o.x = (float)((a & 0xff) + ((a >> 8) & 0xff) + ((a >> 16) & 0xff));
-    o.y = (float)((a >> 24) + (b & 0xff) + ((b >> 8) & 0xff));
-    o.z = (float)(((b >> 16) & 0xff) + (b >> 24) + (c & 0xff));
-    o.w = (float)(((c >> 8) & 0xff) + ((c >> 16) & 0xff) + (c >> 24));
-    gray[i] = o;
-}
-
-// The same for 8-bit grayscale input (rb_pipeline_push_mono): a mono frame m stands for the RGB24 frame (m, m, m), so a
-// pixel's b+g+r is the integer 3v and the plane is bit-identical to k_rgb2gray's on the replicated frame.  4 pixels per
-// thread: one 32-bit load, one float4 store; the source is read through src_pp like k_rgb2gray's.
-__global__ void __launch_bounds__(256) k_mono2gray(const uint32_t *__restrict__ mono_fixed,
-                                                   const uint32_t *const *__restrict__ src_pp,
-                                                   float4 *__restrict__ gray, size_t n4) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
-    const uint32_t *__restrict__ mono = src_pp ? *src_pp : mono_fixed;
-    const uint32_t a = mono[i];
-    float4 o;
-    o.x = (float)(3u * (a & 0xff));
-    o.y = (float)(3u * ((a >> 8) & 0xff));
-    o.z = (float)(3u * ((a >> 16) & 0xff));
-    o.w = (float)(3u * (a >> 24));
-    gray[i] = o;
-}
-
-// The same two conversions for widths that are not a multiple of 4 (rows of the gray plane are then pitched, DogWS).  The
-// frames stay packed as pushed (3wh or wh bytes, no stride), so a row -- and, past the first, a frame -- starts at any byte
-// offset, in the staging buffer (the rest of a head / rest push starts mid-buffer) and in a caller's device buffer alike.
-// A thread makes the float4 of 4 pixels of one pitched row (zeros in the padding columns) from the aligned 32-bit words
-// that hold its 12 (RGB) / 4 (mono) source bytes and funnel shifts.  Word indices count from the source rounded down to 4
-// bytes; a word is loaded whole only when it lies inside the batch's bytes [lo, hi), so the (at most two) words that
-// straddle an end of the buffer are assembled from its bytes that do -- no load touches a byte outside the frames.
-__device__ __forceinline__ uint32_t in_word(const uint8_t *__restrict__ p0, long long wi, long long lo, long long hi) {
-    const long long b = 4 * wi;
-    if (b >= lo && b + 4 <= hi) return __ldg(reinterpret_cast<const uint32_t *>(p0) + wi);
-    uint32_t v = 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++)
-        if (b + k >= lo && b + k < hi) v |= (uint32_t)__ldg(p0 + b + k) << (8 * k);
-    return v;
-}
-// the float4 of the nv (1..4) pixels whose first byte is t of the word array p0, of which the bytes [lo, hi) may be read
-template <bool MONO>
-__device__ __forceinline__ float4 gray4(const uint8_t *__restrict__ p0, long long t, int nv, long long lo, long long hi) {
-    const int cb = MONO ? 1 : 3;   // bytes per pixel
-    const long long wi = t >> 2, we = (t + cb * nv - 1) >> 2;   // first / last word holding a wanted byte
-    const int sh = (int)(t & 3) * 8;
-    float4 o;
-    if (MONO) {
-        const uint32_t w0 = in_word(p0, wi, lo, hi), w1 = we > wi ? in_word(p0, wi + 1, lo, hi) : 0u;
-        const uint32_t a = __funnelshift_r(w0, w1, sh);   // bytes t .. t+3
-        o.x = (float)(3u * (a & 0xff));
-        o.y = (float)(3u * ((a >> 8) & 0xff));
-        o.z = (float)(3u * ((a >> 16) & 0xff));
-        o.w = (float)(3u * (a >> 24));
-    } else {
-        uint32_t wd[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) wd[k] = wi + k <= we ? in_word(p0, wi + k, lo, hi) : 0u;
-        const uint32_t a = __funnelshift_r(wd[0], wd[1], sh), b = __funnelshift_r(wd[1], wd[2], sh),
-                       c = __funnelshift_r(wd[2], wd[3], sh);   // bytes t .. t+11, as k_rgb2gray's a, b, c
-        o.x = (float)((a & 0xff) + ((a >> 8) & 0xff) + ((a >> 16) & 0xff));
-        o.y = (float)((a >> 24) + (b & 0xff) + ((b >> 8) & 0xff));
-        o.z = (float)(((b >> 16) & 0xff) + (b >> 24) + (c & 0xff));
-        o.w = (float)(((c >> 8) & 0xff) + ((c >> 16) & 0xff) + (c >> 24));
-    }
-    // pixels past w came from the next row's bytes (or zeros): the padding columns get +0
-    if (nv < 4) {
-        o.w = 0.f;
-        if (nv < 3) o.z = 0.f;
-        if (nv < 2) o.y = 0.f;
-    }
-    return o;
-}
-template <bool MONO>
-__global__ void __launch_bounds__(256) k_gray_pitched(const uint8_t *__restrict__ src_fixed,
-                                                      const uint8_t *const *__restrict__ src_pp,
-                                                      float4 *__restrict__ gray, int w, int h, int pitch, int nimg) {
-    const int pv = pitch >> 2;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the pitched batch
-    if (i >= (long long)nimg * h * pv) return;
-    const uint8_t *src = src_pp ? *src_pp : src_fixed;
-    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
-    const int cb = MONO ? 1 : 3;   // bytes per pixel
-    const long long lo = (long long)(src - p0), hi = lo + (long long)nimg * cb * w * h;
-    const long long row = i / pv;  // frame * h + y: frames are packed, so the pixel index of the row's start is row * w
-    const int x = 4 * (int)(i - row * pv);
-    const int nv = w - x < 4 ? w - x : 4;   // valid pixels of this float4 (1..4)
-    gray[i] = gray4<MONO>(p0, lo + (long long)cb * (row * w + x), nv, lo, hi);
-}
-
-// Strided frames (rb_pipeline_push_frames_dev): frame f of the batch starts at frames[f].data and its rows are
-// frames[f].step bytes apart, each frame read where it is.  A thread makes the float4 of 4 pixels of one gray row, pitched
-// or not (pitch == w), as k_gray_pitched does, but word indices count from the frame's own first byte rounded down to 4 and
-// loads are bounded by the frame's span [data, data + (h-1)*step + w*bpp): the row padding and the bytes around a frame are
-// never read (the padding columns of the last float4 of a row get +0 whatever was loaded).
-template <bool MONO>
-__global__ void __launch_bounds__(256) k_gray_strided(const rb_frame *__restrict__ frames, float4 *__restrict__ gray, int w,
-                                                      int h, int pitch, int nimg) {
-    const int pv = pitch >> 2;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the (pitched) batch
-    if (i >= (long long)nimg * h * pv) return;
-    const long long row = i / pv;   // frame * h + y
-    const int f = (int)(row / h), y = (int)(row - (long long)f * h);
-    const int x = 4 * (int)(i - row * pv);
-    const uint8_t *src = frames[f].data;
-    const long long step = frames[f].step;
-    const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)3);
-    const int cb = MONO ? 1 : 3;
-    const long long lo = (long long)(src - p0), hi = lo + (long long)(h - 1) * step + (long long)cb * w;
-    const int nv = w - x < 4 ? w - x : 4;
-    gray[i] = gray4<MONO>(p0, lo + (long long)y * step + (long long)cb * x, nv, lo, hi);
-}
-
 // Column pass, software-pipelined: VW adjacent columns per thread, the next U rows are in flight while the current U are added
 // and stored (the add chain per column is the reference's: top to bottom, one float add per row)
 template <int VW> struct ColVec;
@@ -503,44 +377,6 @@ void rb_dogws_free(DogWS *ws) {
     memset(ws, 0, sizeof(*ws));
 }
 
-static int gray_pitched(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp, bool mono) {
-    const size_t n4 = (size_t)nimg * c->NP / 4;
-    (mono ? k_gray_pitched<true> : k_gray_pitched<false>)<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>(
-        ws->rgb, (const uint8_t *const *)src_pp, (float4 *)ws->gray, c->w, c->h, c->pitch, nimg);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
-int rb_dog_gray(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
-    if (c->pitch != c->w) return gray_pitched(c, ws, nimg, src_pp, false);
-    const size_t n4 = (size_t)nimg * c->N / 4;
-    k_rgb2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
-                                                                   (const uint32_t *const *)src_pp,
-                                                                   (float4 *)ws->gray, n4);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
-// strided RGB24 / mono frames -> gray (rb_pipeline_push_frames_dev): frame f of the batch is frames_dev[f], a device table
-int rb_dog_gray_strided(rb_ctx *c, DogWS *ws, int nimg, const rb_frame *frames_dev, bool mono) {
-    const size_t n4 = (size_t)nimg * c->NP / 4;
-    (mono ? k_gray_strided<true> : k_gray_strided<false>)<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>(
-        frames_dev, (float4 *)ws->gray, c->w, c->h, c->pitch, nimg);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
-// mono -> gray: nimg frames of N bytes (the source must be 4-byte aligned; k_mono2gray when N is a multiple of 4)
-int rb_dog_gray_mono(rb_ctx *c, DogWS *ws, int nimg, const void *const *src_pp) {
-    if (c->pitch != c->w) return gray_pitched(c, ws, nimg, src_pp, true);
-    const size_t n4 = (size_t)nimg * c->N / 4;
-    k_mono2gray<<<(unsigned)((n4 + 255) / 256), 256, 0, c->stream>>>((const uint32_t *)ws->rgb,
-                                                                    (const uint32_t *const *)src_pp,
-                                                                    (float4 *)ws->gray, n4);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
 // ---------------------------------------------------------------------------------------------------
 // Row pass on TMA tiles.  One warp = one 32-row band of one image (the sequential float add chain of iimage.cpp:56-60 runs
 // along x, one row per lane), one warp per CTA so that the CTAs spread evenly over the SMs.  A chunk costs ~80 (plain) / ~370
@@ -853,7 +689,7 @@ int rb_dog_aux_planes(rb_ctx *c, DogWS *ws, int img) {
     return RB_OK;
 }
 
-// measurement hook used by rb_pipeline_bench_pass
+// measurement hook used by rb_pipeline_bench_pass (passes 0-3; the gray passes 4-7 are measured there)
 int rb_dog_single_pass(rb_ctx *c, DogWS *ws, int pass_id, int nimg, double *bytes) {
     const double N = (double)c->N;
     switch (pass_id) {
@@ -869,12 +705,6 @@ int rb_dog_single_pass(rb_ctx *c, DogWS *ws, int pass_id, int nimg, double *byte
         case 3:
             *bytes = 16.0 * N * nimg;      // read I of both filters 8N, write img0 + dog 8N
             return blur_dog(c, ws, nimg, nullptr);
-        case 4:
-            *bytes = 7.0 * N * nimg;       // read RGB 3N, write gray 4N
-            return rb_dog_gray(c, ws, nimg);
-        case 6:
-            *bytes = 5.0 * N * nimg;       // read mono N, write gray 4N
-            return rb_dog_gray_mono(c, ws, nimg);
         default:
             return RB_ERR_ARG;
     }

@@ -334,7 +334,9 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_fr
     if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;
     pl->sb_pin[0].src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
     RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
-    if ((r = gray_pass(pl, fmt, n))) return r;
+    if ((r = rb_gray_enqueue(c, &pl->ws, pl->und, in_mono(fmt), &pl->sb_dev->src, in_strided(fmt) ? pl->frames_dev : nullptr,
+                             n)))
+        return r;
     if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
     for (int i = 0; i < n; i++) {
         const long long fr = pl->n_pushed + i;

@@ -175,10 +175,6 @@ struct rb_pipeline {
     } dimg;
 };
 
-int rb_undistort_gray_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
-int rb_undistort_gray_mono_enqueue(rb_undistort *u, const void *const *src_pp, float *gray, int nimg);
-int rb_undistort_gray_strided_enqueue(rb_undistort *u, const rb_frame *frames_dev, float *gray, int nimg, bool mono);
-
 // input layouts of a push: packed RGB24 (3 bytes per pixel) or mono8, which stands for the RGB24 frame (m, m, m), at
 // sb_dev->src; or the same two formats as strided device frames, one {data, step} entry per frame in frames_dev.  Each
 // layout has graph slots of its own.
@@ -230,18 +226,6 @@ static int grow_dev(rb_ctx *c, unsigned char **buf, size_t *have, size_t bytes) 
 static int grow_out(rb_pipeline *pl, unsigned char **host, size_t *host_have, unsigned char **dev, size_t *dev_have,
                     size_t bytes) {
     return pl->out_dev ? grow_dev(pl->c, dev, dev_have, bytes) : grow_mapped(pl->c, host, host_have, bytes);
-}
-// the batch's gray plane from the frames at sb_dev->src, or through frames_dev for the strided layouts (rebvo_first_t.cpp:231
-// undistortion + RGB -> BW)
-static int gray_pass(rb_pipeline *pl, int fmt, int n) {
-    if (in_strided(fmt))
-        return pl->und ? rb_undistort_gray_strided_enqueue(pl->und, pl->frames_dev, pl->ws.gray, n, in_mono(fmt))
-                       : rb_dog_gray_strided(pl->c, &pl->ws, n, pl->frames_dev, in_mono(fmt));
-    const void *const *src = &pl->sb_dev->src;
-    if (pl->und)
-        return fmt == RB_IN_MONO ? rb_undistort_gray_mono_enqueue(pl->und, src, pl->ws.gray, n)
-                                 : rb_undistort_gray_enqueue(pl->und, src, pl->ws.gray, n);
-    return fmt == RB_IN_MONO ? rb_dog_gray_mono(pl->c, &pl->ws, n, src) : rb_dog_gray(pl->c, &pl->ws, n, src);
 }
 // host frames of a push into the packed staging, frames [i0, i0 + count) of `frames` (strided, one 2D copy each) or of the
 // packed buffer `rgb`, on stream s
@@ -699,7 +683,11 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     int r;
     pl->resc_open = false;   // (a batch joins its last rescaling at its end; a failed enqueue must not leave a join behind)
     prof_mark(pl, ST_H2D);
-    if ((r = gray_pass(pl, fmt, n))) return r;
+    // the batch's gray plane (rebvo_first_t.cpp:231 undistortion + RGB -> BW) from the frames at sb_dev->src, or through
+    // frames_dev for the strided layouts
+    if ((r = rb_gray_enqueue(c, &pl->ws, pl->und, in_mono(fmt), &pl->sb_dev->src, in_strided(fmt) ? pl->frames_dev : nullptr,
+                             n)))
+        return r;
     prof_mark(pl, ST_GRAY);
     if (with_events) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
     if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
@@ -1272,19 +1260,16 @@ extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, in
     if (nimg < 1 || nimg > pl->max_batch || iters < 1) return RB_ERR_ARG;
     int r;
     double bytes = 0;
-    // pass 5: the gray pass with the undistortion fused in (needs rb_pipeline_set_undistort; source = the workspace's RGB);
-    // algorithmic bytes: 3N in + 4N out per frame + the 32N-byte map once per launch.  Pass 7: the same from mono frames
-    // (N in + 4N out per frame + the map)
-    const bool und_pass = pass_id == 5 || pass_id == 7;
+    // passes 4-7: the gray pass on the workspace's frames, 4 and 5 from RGB24, 6 and 7 from mono8; 5 and 7 with the
+    // undistortion fused in (needs rb_pipeline_set_undistort; the frames are read through sb_dev->src).  Algorithmic bytes:
+    // 3N (RGB) / N (mono) in + 4N out per frame, + the 32N-byte map once per launch
+    const bool gray = pass_id >= 4 && pass_id <= 7, mono = pass_id >= 6, und_pass = pass_id == 5 || pass_id == 7;
+    if (und_pass && !pl->und) return RB_ERR_STATE;
     auto one = [&]() -> int {
-        if (!und_pass) return rb_dog_single_pass(c, &pl->ws, pass_id, nimg, &bytes);
-        if (!pl->und) return RB_ERR_STATE;
-        if (pass_id == 7) {
-            bytes = 5.0 * c->N * nimg + 32.0 * c->N;
-            return rb_undistort_gray_mono_enqueue(pl->und, &pl->sb_dev->src, pl->ws.gray, nimg);
-        }
-        bytes = 7.0 * c->N * nimg + 32.0 * c->N;
-        return rb_undistort_gray_enqueue(pl->und, &pl->sb_dev->src, pl->ws.gray, nimg);
+        if (!gray) return rb_dog_single_pass(c, &pl->ws, pass_id, nimg, &bytes);
+        bytes = (mono ? 5.0 : 7.0) * c->N * nimg + (und_pass ? 32.0 * c->N : 0.0);
+        return rb_gray_enqueue(c, &pl->ws, und_pass ? pl->und : nullptr, mono, und_pass ? &pl->sb_dev->src : nullptr, nullptr,
+                               nimg);
     };
     if (und_pass) {
         pl->sb_pin[0].src = pl->ws.rgb;

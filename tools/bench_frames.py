@@ -17,7 +17,7 @@ packed input.  In one invocation:
   - kernel times from a separate torch.profiler run with eager launches (REBVO_B200_NO_GRAPH=1): the gray and undistortion
     passes of packed and strided device pushes of 64 frames, in picoseconds per pixel, at 752x480 and at 1226x370 (the
     any-width path; there the strided pushes read packed frames, step w*bpp and frames frame_bytes apart, to compare
-    k_gray_strided with k_gray_pitched on the same bytes);
+    the strided layout with the packed any-width one on the same bytes);
   - whether every arm's nav records equal its packed twin's (exit status 1 if not).
 
 Prints one JSON line (and writes it to --out if given).  Needs a CUDA device: there is no CPU path.
@@ -264,9 +264,10 @@ def kernel_times(torch, capi, bench, B, reps=4):
                     pl.close()
                     for e in prof.key_averages():
                         key = e.key
-                        if not any(k in key for k in ("gray", "k_rgb2gray", "k_mono2gray")):
+                        if "gray" not in key:
                             continue
-                        short = key.split("(")[0].replace("void ", "")
+                        short = key.replace("void ", "")   # the name with its template arguments, which may hold "("
+                        short = short[:short.index(">") + 1] if "<" in short.split("(")[0] else short.split("(")[0]
                         tot = getattr(e, "device_time_total", 0) or getattr(e, "cuda_time_total", 0)   # us
                         ent = res.setdefault(name, {}).setdefault("%s%s" % ("und_" if kc is not None else "", fmt), {})
                         ent[short] = {"ps_per_pixel": tot * 1e6 / (e.count * B * w * h), "launches": e.count}

@@ -122,7 +122,7 @@ def main():
     pl.push_mono(host["mono"][0].data_ptr(), ts[:B])
     pl.push(host["rgb"][B].data_ptr(), ts[B:2 * B])
     passes = {}
-    names = {4: "k_rgb2gray", 5: "k_undistort_gray", 6: "k_mono2gray", 7: "k_undistort_gray_mono"}
+    names = {4: "k_gray<rgb>", 5: "k_undistort_gray<rgb>", 6: "k_gray<mono>", 7: "k_undistort_gray<mono>"}
     for rep in range(3):   # (interleaved, best of three per pass)
         for pid in (4, 6, 5, 7):
             ms, by = pl.bench_pass(pid, B, args.pass_iters)
