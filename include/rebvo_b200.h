@@ -278,7 +278,9 @@ const char *rb_pipeline_last_error(const rb_pipeline *pl);
  * batched, tracking runs frame by frame in order; nav_out[n] receives one record per frame (the first
  * frame ever pushed only initialises the ring: estimation_ok = 0).  Synchronous. */
 int rb_pipeline_push(rb_pipeline *pl, const uint8_t *rgb, const double *ts, int n, rb_nav *nav_out);
-/* same with frames already resident in device memory (device pointer) */
+/* same with frames already resident in device memory (device pointer), read in place.  rgb_dev may be at any byte address,
+ * with and without undistortion and at every frame size: the kernels test the buffer's alignment on the device, so one
+ * captured batch serves buffers of every alignment, and the records are those of the same frames pushed from host memory. */
 int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *ts, int n,
                          rb_nav *nav_out);
 /* Mono input (8-bit grayscale cameras such as EuRoC cam0): n frames of w*h bytes, row-major, no stride.  A mono frame m is
@@ -287,7 +289,9 @@ int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *
  * undistortion, and in IMU mode.  The host copy and the device staging are a third of the RGB24 ones.  A pipeline may
  * alternate formats from push to push.  Arguments are checked like rb_pipeline_push's; the device variant also returns
  * RB_ERR_ARG for a pointer that is not 4-byte aligned (the kernels read 32-bit words), before anything is enqueued.  When
- * w*h is not a multiple of 4 the frames after the first start at unaligned bytes of that buffer; they are read correctly. */
+ * w*h is not a multiple of 4 the frames after the first start at unaligned bytes of that buffer; they are read correctly.
+ * (The mono rule stays where the RGB24 call takes any address: device allocators return aligned buffers, and mono frames at
+ * any address can be pushed in place with rb_pipeline_push_frames_dev, whose kernels read sources at any byte.) */
 int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out);
 int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n, rb_nav *nav_out);
 /* Strided frames, one buffer per frame, as the reference's ROS nodelet reads a sensor_msgs/Image (data[step*y + x*3 + c] for
@@ -364,6 +368,11 @@ int rb_pipeline_event_elapsed(rb_pipeline *pl, int a, int b, float *ms);
  * bytes_per_launch receives the algorithmic bytes of one launch (DESIGN.md section 4). */
 int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, int iters, float *ms_per_launch,
                            double *bytes_per_launch);
+/* Test and debug accessor, like rb_map_get_plane: plane `which` (0 Img(0), 2 ImgDOG, 5 gray) of slot `slot` of the last
+ * scale-space batch the pipeline built, w*h floats.  The last push's frames in order, except after a host push cut into a
+ * head and the rest (REBVO_B200_SUB): the slots then hold the rest, frames sub..n-1.  RB_ERR_ARG for a slot not below the
+ * size of that batch (none after creation, a failed push or rb_pipeline_bench_pass) or another `which`.  Synchronous. */
+int rb_pipeline_batch_plane(rb_pipeline *pl, int slot, int which, float *out);
 
 /* Wire egress of an edge map (monocular): the 15-byte packed net_keyline records of copy_net_keyline +
  * copy_net_keyline_nextid (src/CommLib/net_keypoint.cpp:29-107, struct net_keyline include/CommLib/net_keypoint.h:37-62,

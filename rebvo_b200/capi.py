@@ -120,7 +120,7 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth", "rb_depth_image",
            "rb_pipeline_set_depth_image", "rb_pipeline_depth_image", "rb_pipeline_set_output_memory",
            "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev",
-           "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev"]
+           "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev", "rb_pipeline_batch_plane"]
 
 _lib = None
 
@@ -749,6 +749,14 @@ class Pipeline:
         names = ["copies", "gray", "scale_space", "detect", "reestimate", "quantile+field", "minimizer",
                  "fwdmatch+rotate", "directed_match", "regularize+ekf", "rescale", "pose/nav", "nav_copy"]
         return {n: 1e3 * out[i] / max(fr.value, 1) for i, n in enumerate(names)}, fr.value
+
+    def batch_plane(self, slot, which):
+        """Plane `which` ("gray", "img0" or "dog") of slot `slot` of the last scale-space batch, (h, w) float32.  After a host
+        push cut into a head and the rest (REBVO_B200_SUB) the slots hold the rest."""
+        idx = {"img0": 0, "dog": 2, "gray": 5}[which]
+        out = np.empty((self.h, self.w), np.float32)
+        self.check(self.L.rb_pipeline_batch_plane(self.h_, int(slot), idx, _p(out)))
+        return out
 
     def bench_pass(self, pass_id, nimg, iters):
         ms, by = C.c_float(0), C.c_double(0)

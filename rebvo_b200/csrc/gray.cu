@@ -82,7 +82,8 @@ __device__ __forceinline__ float4 gray4(const uint8_t *__restrict__ p0, long lon
 }
 
 // 4 pixels per thread, one float4 of the plane.  The packed layouts read *src_pp, or src_fixed when src_pp is null.
-//   GRAY_ALIGNED : float4 i of the n4 of the batch from 3 (RGB) / 1 (mono) aligned words.
+//   GRAY_ALIGNED : float4 i of the n4 of the batch from 3 (RGB) / 1 (mono) aligned words; an RGB source that is not
+//   4-byte aligned through gray4 instead.
 //   GRAY_ANYW, GRAY_STRIDED : the float4 of 4 pixels of one pitched row (gray4, zeros in the padding columns).  Word indices
 //   count from the batch's source (GRAY_ANYW) / the frame's own first byte (GRAY_STRIDED) rounded down to 4, and loads are
 //   bounded by the batch's bytes / the frame's span [data, data + (h-1)*step + w*bpp): the row padding and the bytes around a
@@ -94,9 +95,20 @@ __global__ void __launch_bounds__(256) k_gray(const uint8_t *__restrict__ src_fi
     if constexpr (L == GRAY_ALIGNED) {
         size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
         if (i >= n4) return;
-        const uint32_t *__restrict__ src = reinterpret_cast<const uint32_t *>(src_pp ? *src_pp : src_fixed);
-        if constexpr (MONO) gray[i] = mono_gray4(src[i]);
-        else gray[i] = rgb_gray4(src[3 * i], src[3 * i + 1], src[3 * i + 2]);
+        const uint8_t *s = src_pp ? *src_pp : src_fixed;
+        const uint32_t *__restrict__ src = reinterpret_cast<const uint32_t *>(s);
+        if constexpr (MONO) {
+            gray[i] = mono_gray4(src[i]);   // (rb_pipeline_push_mono_dev refuses sources that are not 4-byte aligned)
+        } else if ((reinterpret_cast<uintptr_t>(s) & 3) == 0) {
+            gray[i] = rgb_gray4(src[3 * i], src[3 * i + 1], src[3 * i + 2]);
+        } else {
+            // a caller's device buffer at any byte address (rb_pipeline_push_dev): the aligned words around the 12 bytes,
+            // bounded by the batch's 12 * n4 bytes, as GRAY_ANYW reads them.  Decided here, per launch and warp-uniformly,
+            // because one captured graph serves pushes whose sources differ in alignment.
+            const uint8_t *p0 = reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(s) & ~(uintptr_t)3);
+            const long long lo = (long long)(s - p0);
+            gray[i] = gray4<false>(p0, lo + 12 * (long long)i, 4, lo, lo + 12 * (long long)n4);
+        }
     } else {
         const int pv = pitch >> 2;
         const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // float4 of the pitched batch

@@ -88,6 +88,7 @@ struct rb_pipeline {
     rb_frame *frames_dev;         // device [max_batch]
     rb_frame *frames_pin;         // pinned [max_batch]
     int sub;                      // head sub-batch of a host-input push (env REBVO_B200_SUB, default 8 frames)
+    int last_sub;                 // frames of the last scale-space batch (the rest of a head / rest push): ws slots in use
     DetChain *chain;      // device
     FrameState *fs;       // device
     rb_nav *nav_dev;
@@ -781,7 +782,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts) return RB_ERR_ARG;
-    // (the mono kernels read the frames as 32-bit words; the RGB kernels have a byte-wise path for unaligned buffers)
+    // (the packed mono kernels read a device buffer as aligned 32-bit words; the RGB kernels test the alignment of the source
+    // on the device -- k_gray<false, GRAY_ALIGNED> and ug_pixel take a path for unaligned sources -- and the any-width kernels
+    // read every source through aligned words around it)
     if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
     int r;
     if (pl->imu && pl->imu->live && (r = imu_live_check(pl, *pl->imu, ts, n))) return r;
@@ -789,11 +792,13 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
     pl->odom.n = 0;
     pl->depth.n = 0;
     pl->dimg.n = 0;
+    pl->last_sub = 0;
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
         if ((r = imu_push(pl, *pl->imu, rgb, frames, fmt, on_device, ts, n, pl->nav_pin,
                           pl->odom.on ? pl->odom.pin : nullptr)))
             return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
+        pl->last_sub = n;   // (one scale-space batch)
         if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
         pl->odom.n = pl->odom.on ? n : 0;
         return RB_OK;
@@ -913,6 +918,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
         pl->pframes += n;
     }
     if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
+    pl->last_sub = soff[nsub] - soff[nsub - 1];
     pl->mirror.n = pl->mirror.on ? n : 0;
     pl->depth.n = pl->depth.on ? n : 0;
     pl->dimg.n = pl->depth.on && pl->dimg.mode ? n : 0;
@@ -1254,6 +1260,21 @@ extern "C" int rb_pipeline_event_elapsed_between(rb_pipeline *pa, int a, rb_pipe
     RB_CUDA(cudaEventElapsedTime(ms, pa->user_ev[a], pb->user_ev[b]));
     return RB_OK;
 }
+// the batch's planes stay in the workspace until the next push: the detector and the side streams only read img0 / dog, and
+// the mirror and depth passes write buffers of their own
+extern "C" int rb_pipeline_batch_plane(rb_pipeline *pl, int slot, int which, float *out) {
+    if (!pl || !out) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    if (slot < 0 || slot >= pl->last_sub || (which != 0 && which != 2 && which != 5)) return RB_ERR_ARG;
+    const float *src = (which == 0 ? pl->ws.img0 : which == 2 ? pl->ws.dog : pl->ws.gray) + (size_t)slot * c->NP;
+    // the pitched plane without its padding columns: w * h floats (as rb_map_get_plane)
+    RB_CUDA(cudaMemcpy2DAsync(out, (size_t)4 * c->w, src, (size_t)4 * c->pitch, (size_t)4 * c->w, c->h,
+                              cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    return RB_OK;
+}
+
 extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, int iters, float *ms_per_launch,
                                       double *bytes_per_launch) {
     rb_ctx *c = pl->c;
@@ -1265,6 +1286,7 @@ extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, in
     // 3N (RGB) / N (mono) in + 4N out per frame, + the 32N-byte map once per launch
     const bool gray = pass_id >= 4 && pass_id <= 7, mono = pass_id >= 6, und_pass = pass_id == 5 || pass_id == 7;
     if (und_pass && !pl->und) return RB_ERR_STATE;
+    pl->last_sub = 0;   // (the passes overwrite the workspace's planes: rb_pipeline_batch_plane has nothing to show)
     auto one = [&]() -> int {
         if (!gray) return rb_dog_single_pass(c, &pl->ws, pass_id, nimg, &bytes);
         bytes = (mono ? 5.0 : 7.0) * c->N * nimg + (und_pass ? 32.0 * c->N : 0.0);

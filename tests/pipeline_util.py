@@ -45,6 +45,8 @@ def push(pl, frames, ts, how="host", offset=0):
     flat = torch.from_numpy(np.ascontiguousarray(frames).reshape(-1))
     buf = torch.zeros(flat.numel() + offset + 8, dtype=torch.uint8, device="cuda")
     buf[offset:offset + flat.numel()] = flat.cuda()
+    # the pipeline's stream does not wait for torch's: the frames must be in the buffer before the push reads them
+    torch.cuda.synchronize()
     try:
         return (pl.push_mono_dev if mono else pl.push_dev)(buf.data_ptr() + offset, ts)
     finally:

@@ -3,6 +3,7 @@ the reference's bit for bit, including the frame border where taps fall outside 
 import numpy as np
 import pytest
 
+import ingress_states
 from pipeline_util import EUROC_KC
 
 pytestmark = pytest.mark.gpu
@@ -26,3 +27,25 @@ def test_undistort_matches_reference(built, kc):
         assert np.array_equal(ref, got), "mismatch in %d bytes" % int((ref != got).sum())
     und.close()
     ctx.close()
+
+
+@pytest.mark.parametrize("name", sorted(ingress_states.MAPS))
+def test_undistort_maps_match_reference(built, name):
+    """The maps of tests/ingress_states.py: every tap count the map can have (0, 1, 2, 4), principal points on integers and
+    on x.5, kc = 0 (exact weights), the KITTI and odd-width geometries, on random, edge and all-255 frames."""
+    from oracle import refapi
+    from rebvo_b200 import capi
+    if not refapi.available():
+        pytest.skip("oracle/_ref not built")
+    c = ingress_states.MAPS[name]
+    ctx = capi.Ctx(c["cam"], 3.56359, 1.2599)
+    und = capi.Undistort(ctx, c["kc"])
+    try:
+        for key in (("rand", 0), ("edge", 1), ("white",)):
+            im = ingress_states.frame(c["cam"], key)
+            ref = refapi.undistort_rgb(c["cam"], c["kc"], im)
+            got = und.apply(im)
+            assert np.array_equal(ref, got), "%s %s: mismatch in %d bytes" % (name, key, int((ref != got).sum()))
+    finally:
+        und.close()
+        ctx.close()
