@@ -209,7 +209,7 @@ int rb_map_build_field(rb_map *m, int radius, float min_mod);
 int rb_map_get_field(rb_map *m, int32_t *out);
 /* one global_tracker::TryVelRot<double,ReWeight,ProcJF,false> evaluation (global_tracker.cpp:285-543).
  * fmap holds the field (new map), old is the map being moved.  res_in / res_out: K0 doubles (may be
- * NULL when !reweight / not wanted). */
+ * NULL when !reweight / not wanted).  JtJ / JtF are written only when procjf, as the reference leaves them. */
 int rb_try_vel_rot(rb_map *fmap, rb_map *old, const double X[6], int reweight, int procjf,
                    double match_thresh, double s_rho_min, uint32_t match_num_thresh, double k_huber,
                    const double *res_in, double *res_out, double JtJ[36], double JtF[6], double *score);

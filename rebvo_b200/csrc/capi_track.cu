@@ -7,9 +7,9 @@
 #include "common.cuh"
 #include "tracker.cuh"
 
-int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old);
 int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double X[6], int reweight, int procjf,
-                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber);
+                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber,
+                           double *tot_dev);
 
 static double *args_dev(rb_ctx *c) { return (double *)((char *)c->dev_small + RB_DS_ARGS); }
 static double *args_pin(rb_ctx *c) { return (double *)((char *)c->pinned + RB_DS_ARGS); }
@@ -98,17 +98,32 @@ extern "C" int rb_try_vel_rot(rb_map *fmap, rb_map *old, const double X[6], int 
     else
         RB_CUDA(cudaMemsetAsync(fmap->res[0], 0, sizeof(double) * (size_t)c->kcap, c->stream));
     if ((r = rb_try_vel_rot_enqueue(c, fmap, old, X, reweight, procjf, match_thresh, s_rho_min, match_num_thresh,
-                                    sf.frame_count, k_huber)))
+                                    sf.frame_count, k_huber, args_dev(c))))
         return r;
-    LMState *lmh = (LMState *)((char *)c->pinned + 4096);
-    RB_CUDA(cudaMemcpyAsync(lmh, &fmap->ts->lm, sizeof(LMState), cudaMemcpyDeviceToHost, c->stream));
-    if (res_out && so.kn > 0 && (r = rb_resolve_res_enqueue(c, fmap, old))) return r;
+    RB_CUDA(cudaMemcpyAsync(args_pin(c), args_dev(c), sizeof(double) * 28, cudaMemcpyDeviceToHost, c->stream));
     if (res_out && so.kn > 0)
         RB_CUDA(cudaMemcpyAsync(res_out, fmap->res[1], sizeof(double) * so.kn, cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
-    if (JtJ) memcpy(JtJ, lmh->JtJn, sizeof(double) * 36);
-    if (JtF) memcpy(JtF, lmh->JtFn, sizeof(double) * 6);
-    if (score) *score = lmh->last_score;
+    const double *s = args_pin(c);
+    if (procjf) {   // JtJ upper triangle and JtF, their sign fix-ups and the symmetric fill (:484-490, :492-496)
+        double J[36], F[6];
+        int k = 0;
+        for (int a = 0; a < 6; a++)
+            for (int b = a; b < 6; b++) J[a * 6 + b] = s[k++];
+        for (int a = 0; a < 6; a++) F[a] = s[21 + a];
+        for (int a = 0; a < 2; a++) {
+            F[a + 2] = -F[a + 2];
+            for (int b = 0; b < 2; b++) {
+                J[(a + 0) * 6 + (b + 2)] = -J[(a + 0) * 6 + (b + 2)];
+                J[(a + 2) * 6 + (b + 4)] = -J[(a + 2) * 6 + (b + 4)];
+            }
+        }
+        for (int a = 0; a < 6; a++)
+            for (int b = a + 1; b < 6; b++) J[b * 6 + a] = J[a * 6 + b];
+        if (JtJ) memcpy(JtJ, J, sizeof(J));
+        if (JtF) memcpy(JtF, F, sizeof(F));
+    }
+    if (score) *score = s[27];
     return RB_OK;
 }
 

@@ -158,7 +158,6 @@ struct TrackState {
     int *blk_has;
     double *blk_last_fi;  // per block: residual of its last matched keyline
     double *partials;     // per block x 28 reduction partials
-    double *carry;        // [256]: per block of rb_try_vel_rot's output, the stale-fi value its leading misses inherit
     int nblk;
     struct MinCtl *ctl;   // request slots / sequence base of the persistent minimiser kernel
     unsigned long long *ll;   // its inter-cluster slots

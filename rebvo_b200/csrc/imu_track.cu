@@ -12,43 +12,21 @@
 #include "common.cuh"
 #include "lm.cuh"
 #include "tracker.cuh"
-
-#define TV_T 256
-#define TV_SENTINEL 0x7FF8DEADBEEF0002ull
-
-template <int NV>
-__device__ __forceinline__ void block_sum_to(const double (&acc)[NV], double (*s_part)[TV_T / 32], int lane, int wid,
-                                             double *dst, int dst_stride) {
-#pragma unroll
-    for (int k = 0; k < NV; k++) {
-        double v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_part[k][wid] = v;
-    }
-    __syncthreads();
-    if (wid == 0 && lane < NV) {
-        double t = 0;
-#pragma unroll
-        for (int ww = 0; ww < TV_T / 32; ww++) t += s_part[lane][ww];
-        dst[lane * dst_stride] = t;
-    }
-}
+#include "stage_reduce.cuh"
 
 // One TryVel evaluation.  partials[k][block], k = 0..9: JtJ(0,0),(1,1),(2,2),(0,1),(0,2),(1,2), JtF[0..2], score.
-__global__ void __launch_bounds__(TV_T) k_tv_eval(KLSoA old, const MapState *__restrict__ old_st,
-                                                  const unsigned long long *__restrict__ field,
-                                                  const float4 *__restrict__ fpack, const MapState *__restrict__ f_st,
-                                                  const double *__restrict__ velp, double *__restrict__ res,
-                                                  double *__restrict__ partials, int *blk_has, double *blk_last,
-                                                  double zfm, float ppx, float ppy, int w, int h, double max_r,
-                                                  double match_thresh, double s_rho_min, unsigned int mnt_arg,
-                                                  double rw_dist, float min_mod) {
-    __shared__ double s_part[10][TV_T / 32];
-    __shared__ int s_whas[TV_T / 32];
-    __shared__ double s_wlast[TV_T / 32];
+__global__ void __launch_bounds__(STAGE_T) k_tv_eval(KLSoA old, const MapState *__restrict__ old_st,
+                                                     const unsigned long long *__restrict__ field,
+                                                     const float4 *__restrict__ fpack, const MapState *__restrict__ f_st,
+                                                     const double *__restrict__ velp, double *__restrict__ res,
+                                                     double *__restrict__ partials, int *blk_has, double *blk_last,
+                                                     double zfm, float ppx, float ppy, int w, int h, double max_r,
+                                                     double match_thresh, double s_rho_min, unsigned int mnt_arg,
+                                                     double rw_dist, float min_mod) {
+    __shared__ double s_part[10][STAGE_T / 32];
+    __shared__ StaleSmem sm;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int i = blockIdx.x * TV_T + tid;
+    const int i = blockIdx.x * STAGE_T + tid;
     const int K0 = old_st->kn;
     const double V0 = velp[0], V1 = velp[1], V2 = velp[2];
     const unsigned int fc = f_st->frame_count;
@@ -125,72 +103,11 @@ __global__ void __launch_bounds__(TV_T) k_tv_eval(KLSoA old, const MapState *__r
         }
         old.m_id_f[i] = mid_f;
     }
-    // Residuals[ikl]=fabs(fi): fi is the last matched keyline's value on a miss (function-level variable, :836)
-    const unsigned int bal = __ballot_sync(0xffffffffu, matched);
-    const unsigned int lower = bal & ((1u << lane) - 1u);
-    const double prev_fi = __shfl_sync(0xffffffffu, fi_own, lower ? 31 - __clz(lower) : 0);
-    const double wl = __shfl_sync(0xffffffffu, fi_own, bal ? 31 - __clz(bal) : 0);
-    if (lane == 0) {
-        s_whas[wid] = bal != 0;
-        s_wlast[wid] = wl;
-    }
-    __syncthreads();
-    if (i < K0) {
-        if (matched) {
-            res[i] = fabs(fi_own);
-        } else if (need) {
-            bool found = lower != 0;
-            double v = prev_fi;
-            if (!found)
-                for (int ww = wid - 1; ww >= 0; ww--)
-                    if (s_whas[ww]) {
-                        v = s_wlast[ww];
-                        found = true;
-                        break;
-                    }
-            if (found) res[i] = fabs(v);
-            else reinterpret_cast<unsigned long long *>(res)[i] = TV_SENTINEL;
-        }
-    }
-    if (tid == 0) {
-        int has = 0;
-        double lv = 0;
-        for (int ww = 0; ww < TV_T / 32; ww++)
-            if (s_whas[ww]) {
-                has = 1;
-                lv = s_wlast[ww];
-            }
-        blk_has[blockIdx.x] = has;
-        blk_last[blockIdx.x] = lv;
-    }
-    __syncthreads();
-    block_sum_to<10>(acc, s_part, lane, wid, partials + blockIdx.x, TV_T);
-}
-
-// second pass: fold the per-block partials in block order and patch the residuals that inherit the stale fi of an
-// earlier block (host-driven loop, so a separate tiny kernel keeps the buffer fully resolved between evaluations)
-__global__ void __launch_bounds__(TV_T) k_tv_finish(double *__restrict__ res, const double *__restrict__ partials,
-                                                    const int *__restrict__ blk_has, const double *__restrict__ blk_last,
-                                                    const MapState *__restrict__ old_st, int nb, double *out10) {
-    __shared__ double s_carry[TV_T];
-    const int tid = threadIdx.x;
-    if (blockIdx.x == 0 && tid < 10) {
-        double t = 0;
-        for (int b = 0; b < nb; b++) t += partials[tid * TV_T + b];
-        out10[tid] = t;
-    }
-    if (tid < nb) {
-        double carry = 0;
-        for (int b = tid - 1; b >= 0; b--)
-            if (blk_has[b]) {
-                carry = blk_last[b];
-                break;
-            }
-        s_carry[tid] = carry;
-    }
-    __syncthreads();
-    const int i = blockIdx.x * TV_T + tid;
-    if (i < old_st->kn && reinterpret_cast<unsigned long long *>(res)[i] == TV_SENTINEL) res[i] = fabs(s_carry[blockIdx.x]);
+    // Residuals[ikl]=fabs(fi), fi of the last match on a miss (:836)
+    const double stale = block_stale_fi(matched, fi_own, true, sm, blk_has, blk_last, lane, wid);
+    if (matched) res[i] = fabs(fi_own);
+    else if (need) res[i] = stale;
+    block_sum_to<10>(acc, s_part, lane, wid, partials + blockIdx.x, STAGE_T);
 }
 
 static int tv_eval(rb_ctx *c, rb_map *fmap, rb_map *old, const double vel[3], double match_thresh, double s_rho_min,
@@ -199,13 +116,13 @@ static int tv_eval(rb_ctx *c, rb_map *fmap, rb_map *old, const double vel[3], do
     memcpy(pin, vel, sizeof(double) * 3);
     RB_CUDA(cudaMemcpyAsync(args, pin, sizeof(double) * 3, cudaMemcpyHostToDevice, c->stream));
     const int nb = fmap->ts_host.nblk;
-    k_tv_eval<<<nb, TV_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, fmap->st, args, fmap->res[0],
-                                          fmap->ts_host.partials, fmap->ts_host.blk_has, fmap->ts_host.blk_last_fi, c->zfm,
-                                          c->ppx, c->ppy, c->w, c->h, (double)fmap->field_radius, match_thresh, s_rho_min,
-                                          mnt, rw_dist, min_mod);
+    k_tv_eval<<<nb, STAGE_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, fmap->st, args, fmap->res[0],
+                                             fmap->ts_host.partials, fmap->ts_host.blk_has, fmap->ts_host.blk_last_fi, c->zfm,
+                                             c->ppx, c->ppy, c->w, c->h, (double)fmap->field_radius, match_thresh, s_rho_min,
+                                             mnt, rw_dist, min_mod);
     RB_LAUNCH_CHECK();
-    k_tv_finish<<<nb, TV_T, 0, c->stream>>>(fmap->res[0], fmap->ts_host.partials, fmap->ts_host.blk_has,
-                                            fmap->ts_host.blk_last_fi, old->st, nb, args + 8);
+    k_blocks_finish<10><<<nb, STAGE_T, 0, c->stream>>>(fmap->ts_host.partials, nb, args + 8, fmap->res[0],
+                                                       fmap->ts_host.blk_has, fmap->ts_host.blk_last_fi, old->st, true);
     RB_LAUNCH_CHECK();
     RB_CUDA(cudaMemcpyAsync(pin + 8, args + 8, sizeof(double) * 10, cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
@@ -295,12 +212,12 @@ extern "C" int rb_minimizer_v(rb_map *fmap, rb_map *old, double Vel[3], double R
 }
 
 // ---- ExtRotVel (edge_tracker.cpp:1207-1301): sums of Phi^T Phi (21) and Phi^T Y (6) over the matched keylines ------
-__global__ void __launch_bounds__(TV_T) k_extrotvel(KLSoA kl, const MapState *__restrict__ st,
-                                                    const double *__restrict__ velp, double *__restrict__ partials,
-                                                    double zf, double loc_unc, double hub) {
-    __shared__ double s_part[27][TV_T / 32];
+__global__ void __launch_bounds__(STAGE_T) k_extrotvel(KLSoA kl, const MapState *__restrict__ st,
+                                                       const double *__restrict__ velp, double *__restrict__ partials,
+                                                       double zf, double loc_unc, double hub) {
+    __shared__ double s_part[27][STAGE_T / 32];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int i = blockIdx.x * TV_T + tid;
+    const int i = blockIdx.x * STAGE_T + tid;
     double acc[27];
 #pragma unroll
     for (int k = 0; k < 27; k++) acc[k] = 0;
@@ -337,14 +254,7 @@ __global__ void __launch_bounds__(TV_T) k_extrotvel(KLSoA kl, const MapState *__
 #pragma unroll
         for (int a = 0; a < 6; a++) acc[21 + a] = P[a] * Y;
     }
-    block_sum_to<27>(acc, s_part, lane, wid, partials + blockIdx.x, TV_T);
-}
-__global__ void k_fold27(const double *__restrict__ partials, int nb, double *out) {
-    const int k = threadIdx.x;
-    if (k >= 27) return;
-    double t = 0;
-    for (int b = 0; b < nb; b++) t += partials[k * TV_T + b];
-    out[k] = t;
+    block_sum_to<27>(acc, s_part, lane, wid, partials + blockIdx.x, STAGE_T);
 }
 
 // edge_tracker::ExtRotVel(vel, Wx, Rx, X, LocUncert, HubReweigth); returns *ok = 0 when the estimate is NaN (the reference
@@ -358,9 +268,10 @@ extern "C" int rb_ext_rot_vel(rb_map *m, const double vel[3], double Wx[36], dou
     memcpy(pin, vel, sizeof(double) * 3);
     RB_CUDA(cudaMemcpyAsync(args, pin, sizeof(double) * 3, cudaMemcpyHostToDevice, c->stream));
     const int nb = m->ts_host.nblk;
-    k_extrotvel<<<nb, TV_T, 0, c->stream>>>(m->kl, m->st, args, m->ts_host.partials, c->zfm, loc_uncertainty, hub_reweight);
+    k_extrotvel<<<nb, STAGE_T, 0, c->stream>>>(m->kl, m->st, args, m->ts_host.partials, c->zfm, loc_uncertainty, hub_reweight);
     RB_LAUNCH_CHECK();
-    k_fold27<<<1, 32, 0, c->stream>>>(m->ts_host.partials, nb, args + 8);
+    k_blocks_finish<27><<<1, 32, 0, c->stream>>>(m->ts_host.partials, nb, args + 8, nullptr, nullptr, nullptr, nullptr,
+                                                 false);
     RB_LAUNCH_CHECK();
     RB_CUDA(cudaMemcpyAsync(pin + 8, args + 8, sizeof(double) * 27, cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));

@@ -10,9 +10,7 @@
 #include "tracker.cuh"
 #include "lm.cuh"
 #include "frame.cuh"
-
-#define TVR_T 256
-#define RES_SENTINEL 0x7FF8DEADBEEF0001ull
+#include "stage_reduce.cuh"
 
 // Cycle stamps of the cluster minimiser (build with -DRB_TVR_PROF, read by tools/cluster_stamps.py); compiled out of the product.
 #ifdef RB_TVR_PROF
@@ -55,14 +53,12 @@ static CamC make_cam(const rb_ctx *c) {
 int rb_track_state_alloc(rb_ctx *c, rb_map *m) {
     TrackState host;
     memset(&host, 0, sizeof(host));
-    const int nblk = rb_div_up(c->kcap, TVR_T);
+    const int nblk = rb_div_up(c->kcap, STAGE_T);
     const size_t K = c->kcap + 32;
     host.nblk = nblk;
     RB_CUDA(cudaMalloc(&host.blk_has, sizeof(int) * nblk));
     RB_CUDA(cudaMalloc(&host.blk_last_fi, sizeof(double) * nblk));
-    RB_CUDA(cudaMalloc(&host.partials, sizeof(double) * 28 * TVR_T));
-    RB_CUDA(cudaMalloc(&host.carry, sizeof(double) * TVR_T));
-    RB_CUDA(cudaMemsetAsync(host.carry, 0, sizeof(double) * TVR_T, c->stream));
+    RB_CUDA(cudaMalloc(&host.partials, sizeof(double) * 28 * STAGE_T));
     RB_CUDA(cudaMalloc(&host.ctl, sizeof(MinCtl)));
     RB_CUDA(cudaMemsetAsync(host.ctl, 0, sizeof(MinCtl), c->stream));
     // slots of the multi-cluster minimiser: [2][MC_GMAX][16][2][64]
@@ -84,7 +80,6 @@ void rb_track_state_free(rb_map *m) {
     cudaFree(h.blk_has);
     cudaFree(h.blk_last_fi);
     cudaFree(h.partials);
-    cudaFree(h.carry);
     cudaFree(h.ctl);
     cudaFree(h.ll);
     cudaFree(h.fm_best);
@@ -483,13 +478,9 @@ struct ResPtrs {
     double *r[3];
 };
 
-// Sum 28 per-thread values over the block in a fixed order.  Inside a warp: a transposing butterfly -- at distance
-// 16, 8, .. 1 every lane keeps one half of its values and trades the other half with its partner, so after 5 steps
-// (16+8+4+2+1 = 31 exchanges instead of 28 x 5) lane l holds the warp's sum of value l.  Across warps: one
-// shared-memory hop, thread k < 28 adds the warps' sums of value k in warp order.  dst[k * dst_stride] = sum k.
-struct Red28Smem {
-    double part[TVR_T / 32][32];
-};
+// Sum 28 per-thread values over a warp in a fixed order (the cluster minimiser's block sums): a transposing butterfly --
+// at distance 16, 8, .. 1 every lane keeps one half of its values and trades the other half with its partner, so after
+// 5 steps (16+8+4+2+1 = 31 exchanges instead of 28 x 5) lane l holds the warp's sum of value l.
 // p ? a : b on values, never on addresses.  The butterfly used to pick `up ? v[k + o] : v[k]` in a loop over o >>= 1
 // that was not unrolled; the array (and the caller's acc) then lived in local memory, an L1 round trip per level.  Now
 // every index is a compile-time constant (one template per level, one array per level) and the choice is a selp.
@@ -519,35 +510,6 @@ __device__ __forceinline__ double warp_transpose_sum28(const double (&acc)[28], 
     transpose_level<2>(v4, v2, lane);
     transpose_level<1>(v2, v1, lane);
     return v1[0];
-}
-template <bool PJ>
-__device__ __forceinline__ void reduce28(const double (&acc)[28], Red28Smem &rs, int tid, int lane, int wid,
-                                         double *dst, int dst_stride) {
-    if (PJ) {
-        const double w = warp_transpose_sum28(acc, lane);
-        __syncthreads();   // the previous user of rs is done
-        rs.part[wid][lane] = w;
-        __syncthreads();
-        if (tid < 28) {
-            double t = rs.part[0][tid];
-#pragma unroll
-            for (int ww = 1; ww < TVR_T / 32; ww++) t += rs.part[ww][tid];
-            dst[tid * dst_stride] = t;
-        }
-    } else {
-        double v = acc[27];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        __syncthreads();
-        if (lane == 0) rs.part[0][wid] = v;
-        __syncthreads();
-        if (tid == 0) {
-            double t = 0;
-#pragma unroll
-            for (int ww = 0; ww < TVR_T / 32; ww++) t += rs.part[0][ww];
-            dst[27 * dst_stride] = t;
-        }
-    }
 }
 
 // Minimizer_RV preamble (global_tracker.cpp:596-650): configuration, LM variables, request of the first evaluation
@@ -627,16 +589,6 @@ __device__ __forceinline__ double div_with_rcp(double a, double b, double y) {
     const double r = fma(-b, q, a);
     return fma(r, y, q);
 }
-struct TvrSmem {
-    Red28Smem red;
-    double wlast[TVR_T / 32];
-    int whas[TVR_T / 32];
-};
-struct TrackPtrs {         // the pointers inside TrackState, passed by value (no dependent load to reach them)
-    LMState *lm;
-    int *blk_has;
-    double *blk_last_fi, *partials, *carry;
-};
 
 // Per-keyline part of TryVelRot (global_tracker.cpp:350-463) for U keylines of one thread: projection, field lookup,
 // residual, Jacobian products added to acc.  k_try_vel_rot runs one keyline per thread; the cluster kernel a thread's
@@ -795,168 +747,22 @@ __device__ __forceinline__ void tvr_keyline(const double (&x0)[U], const double 
     }
 }
 
-// "DResidualNew[ikl]=fi" keeps the fi of the last matched keyline before ikl (fi is a function-level variable,
-// :341,399-408): in-block scan here; misses that precede the block's first match get RES_SENTINEL, which k_resolve_res
-// replaces with the block's entry of the carry table.  Then the block's 28 sums go to
-// partials[k][vb] in a fixed order, and its "has a match / last matched fi" summary to blk_has / blk_last_fi.
-// matched / need / outside / fi_own: tvr_keyline's outputs for keyline i.
-template <bool PJ>
-__device__ __forceinline__ void tvr_block_tail(bool matched, bool need, bool outside, double fi_own, double max_r,
-                                               double *__restrict__ rout, int i, const double (&acc)[28],
-                                               TvrSmem &sm, double *dst, int dst_stride, int *has_out,
-                                               double *last_out, int tid, int lane, int wid) {
-    const unsigned int bal = __ballot_sync(0xffffffffu, matched);
-    const unsigned int lower = bal & ((1u << lane) - 1u);
-    const int src = lower ? 31 - __clz(lower) : 0;
-    const double prev_fi = __shfl_sync(0xffffffffu, fi_own, src);
-    const int hi = bal ? 31 - __clz(bal) : 0;
-    const double wl = __shfl_sync(0xffffffffu, fi_own, hi);
-    __syncthreads();   // the previous user of sm is done
-    if (lane == 0) {
-        sm.whas[wid] = bal != 0;
-        sm.wlast[wid] = wl;
-    }
-    __syncthreads();
-    if (matched) {
-        rout[i] = fi_own;
-    } else if (need) {
-        double v = prev_fi;
-        bool found = lower != 0;
-        if (!found) {
-            for (int ww = wid - 1; ww >= 0; ww--)
-                if (sm.whas[ww]) {
-                    v = sm.wlast[ww];
-                    found = true;
-                    break;
-                }
-        }
-        if (!found) v = __longlong_as_double((long long)RES_SENTINEL);
-        reinterpret_cast<unsigned long long *>(rout)[i] = (unsigned long long)__double_as_longlong(v);
-    } else if (outside) {
-        rout[i] = max_r;
-    }
-    if (tid == 0) {
-        int has = 0;
-        double lastv = 0;
-        for (int ww = 0; ww < TVR_T / 32; ww++)
-            if (sm.whas[ww]) {
-                has = 1;
-                lastv = sm.wlast[ww];
-            }
-        *has_out = has;
-        *last_out = lastv;
-    }
-    reduce28<PJ>(acc, sm.red, tid, lane, wid, dst, dst_stride);
-}
-
-// grid reduction of the per-block partials (layout [28][TVR_T], nb <= TVR_T blocks) in a fixed order: warp w owns sums
-// w, w+8, ...; its lanes add the lane-strided entries (every load in flight at once), then one xor tree per sum.
-// The caller synchronises before reading s_tot.
-template <bool PJ>
-__device__ __forceinline__ void tvr_grid_reduce(const double *partials, int nb, double *s_tot, int lane, int wid) {
-    constexpr int NW = TVR_T / 32;
-    if (PJ) {
-        double v[4];
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            const int k = wid + NW * q;
-            double x[NW];
-#pragma unroll
-            for (int j = 0; j < NW; j++) {
-                const int b = lane + 32 * j;
-                x[j] = (k < 28 && b < nb) ? __ldcg(partials + k * TVR_T + b) : 0.0;
-            }
-            double t = x[0];
-#pragma unroll
-            for (int j = 1; j < NW; j++) t += x[j];
-            v[q] = t;
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-            for (int q = 0; q < 4; q++) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-        if (lane == 0)
-#pragma unroll
-            for (int q = 0; q < 4; q++)
-                if (wid + NW * q < 28) s_tot[wid + NW * q] = v[q];
-    } else if (wid == 0) {
-        double t = 0;
-#pragma unroll
-        for (int j = 0; j < NW; j++) {
-            const int b = lane + 32 * j;
-            t += (b < nb) ? __ldcg(partials + 27 * TVR_T + b) : 0.0;
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-        if (lane == 0) s_tot[27] = t;
-    }
-}
-
-// stale-fi carries: block b inherits the last matched fi of the nearest earlier block that has one (0 at the start);
-// one ballot per warp finds it.  blockDim.x == TVR_T >= nb; thread b brings block b's summary (0 beyond nb).
-__device__ __forceinline__ double tvr_carries(int has, double lastv, double *carry_out, int nb, double *s_blast,
-                                            unsigned int *s_wmask, int tid, int lane, int wid) {
-    const unsigned int mask = __ballot_sync(0xffffffffu, has != 0);
-    s_blast[tid] = lastv;
-    if (lane == 0) s_wmask[wid] = mask;
-    __syncthreads();
-    double cy = 0;
-    if (tid < nb) {
-        const unsigned int lower = mask & ((1u << lane) - 1u);
-        if (lower) {
-            cy = s_blast[wid * 32 + 31 - __clz(lower)];
-        } else {
-            for (int ww = wid - 1; ww >= 0; ww--) {
-                const unsigned int mm = s_wmask[ww];
-                if (mm) {
-                    cy = s_blast[ww * 32 + 31 - __clz(mm)];
-                    break;
-                }
-            }
-        }
-        carry_out[tid] = cy;
-    }
-    return cy;
-}
-
-// totals -> JtJn / JtFn / score of the evaluation (sign fix-ups :484-490)
-template <bool PJ>
-__device__ __forceinline__ void lm_ingest(LMState &L, const double *s_tot) {
-    if (PJ) {
-        int k = 0;
-        for (int a = 0; a < 6; a++)
-            for (int b = a; b < 6; b++) L.JtJn[a * 6 + b] = s_tot[k++];
-        for (int a = 0; a < 6; a++) L.JtFn[a] = s_tot[21 + a];
-        for (int a = 0; a < 2; a++) {
-            L.JtFn[a + 2] = -L.JtFn[a + 2];
-            for (int b = 0; b < 2; b++) {
-                L.JtJn[(a + 0) * 6 + (b + 2)] = -L.JtJn[(a + 0) * 6 + (b + 2)];
-                L.JtJn[(a + 2) * 6 + (b + 4)] = -L.JtJn[(a + 2) * 6 + (b + 4)];
-            }
-        }
-        for (int a = 0; a < 6; a++)
-            for (int b = a + 1; b < 6; b++) L.JtJn[b * 6 + a] = L.JtJn[a * 6 + b];
-    }
-    L.last_score = s_tot[27];
-    L.n_eval++;
-}
-
 struct TvrPose {
     double X[6];          // VelRot: V, then W
 };
-// One TryVelRot evaluation (stage-level API rb_try_vel_rot): residuals rin (read when RW) -> rout, m_id_f of the old map.
-// The last block leaves the sums in the map's LMState (JtJn, JtFn, last_score) and the stale fi of each block's leading
-// misses in tp.carry.
+// One TryVelRot evaluation (stage-level API rb_try_vel_rot): residuals rin (read when RW) -> rout, m_id_f of the old map,
+// the block's 28 sums (JtJ upper triangle, JtF, score; before the sign fix-ups) to partials[k][block].
+// "DResidualNew[ikl]=fi" on a miss: the fi of the last match before it (:341,399-408), across blocks by k_blocks_finish.
 template <bool RW, bool PJ>
-__global__ void __launch_bounds__(TVR_T) k_try_vel_rot(KLSoA old, const MapState *__restrict__ old_st,
-                                                       const unsigned long long *__restrict__ field,
-                                                       const float4 *__restrict__ fpack, TrackPtrs tp,
-                                                       const double *__restrict__ rin, double *__restrict__ rout,
-                                                       unsigned int *ticket, CamC cam, TvrPose pose, TvrConst tc) {
+__global__ void __launch_bounds__(STAGE_T) k_try_vel_rot(KLSoA old, const MapState *__restrict__ old_st,
+                                                         const unsigned long long *__restrict__ field,
+                                                         const float4 *__restrict__ fpack,
+                                                         const double *__restrict__ rin, double *__restrict__ rout,
+                                                         double *__restrict__ partials, int *blk_has, double *blk_last_fi,
+                                                         CamC cam, TvrPose pose, TvrConst tc) {
     __shared__ double sR[9], sV[3], sRM[4];
-    __shared__ TvrSmem sm;
-    __shared__ double s_tot[28];
-    __shared__ bool s_last;
+    __shared__ StaleSmem sm;
+    __shared__ double s_part[28][STAGE_T / 32];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) {   // the two exponentials run on two warps side by side (each is a serial sin/cos chain)
         so3_exp(pose.X + 3, sR);                   // SO3<> RotW0(VelRot.slice<3,3>())
@@ -972,7 +778,7 @@ __global__ void __launch_bounds__(TVR_T) k_try_vel_rot(KLSoA old, const MapState
     __syncthreads();
 
     const int K0 = old_st->kn;
-    const int i = blockIdx.x * TVR_T + tid;
+    const int i = blockIdx.x * STAGE_T + tid;
     const bool act = i < K0;
     // a thread without a keyline runs on harmless operands and contributes zeros
     KlOp o = {make_float2(0.f, 0.f), 0.0, 0.0, 1.0, 1.0, 0, 0.f};
@@ -989,30 +795,11 @@ __global__ void __launch_bounds__(TVR_T) k_try_vel_rot(KLSoA old, const MapState
     double fi_own[1];
     tvr_keyline<RW, PJ, 1>({o.x0}, {o.y0}, {o.z0}, {o.s_rho}, {o.m}, {o.n_m}, {skip}, {act}, RW, {r_prev}, sR, sV, sRM, tc,
                            cam, field, fpack, old.m_id_f, {i}, acc, matched, need, fi_own, outside);
-    tvr_block_tail<PJ>(matched[0], need[0], outside[0], fi_own[0], tc.max_r, rout, i, acc, sm, tp.partials + blockIdx.x, TVR_T,
-                       tp.blk_has + blockIdx.x, tp.blk_last_fi + blockIdx.x, tid, lane, wid);
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-    __syncthreads();
-    if (!s_last) return;
-    // ================= last block: grid reduction, stale-fi carries ==========================
-    __threadfence();
-    const int nb = gridDim.x;   // <= TVR_T: at most 196 blocks for a capacity of RB_KCAP_MAX keylines
-    tvr_grid_reduce<PJ>(tp.partials, nb, s_tot, lane, wid);
-    __shared__ double s_blast[TVR_T];
-    __shared__ unsigned int s_wmask[TVR_T / 32];
-    int has = 0;
-    double lastv = 0;
-    if (tid < nb) {
-        has = __ldcg(tp.blk_has + tid);
-        lastv = __ldcg(tp.blk_last_fi + tid);
-    }
-    tvr_carries(has, lastv, tp.carry, nb, s_blast, s_wmask, tid, lane, wid);   // (synchronises: s_tot is complete)
-    if (tid == 0) {
-        lm_ingest<PJ>(*tp.lm, s_tot);
-        *ticket = 0;
-    }
+    const double stale = block_stale_fi(matched[0], fi_own[0], false, sm, blk_has, blk_last_fi, lane, wid);
+    if (matched[0]) rout[i] = fi_own[0];
+    else if (need[0]) rout[i] = stale;
+    else if (outside[0]) rout[i] = tc.max_r;
+    block_sum_to<28>(acc, s_part, lane, wid, partials + blockIdx.x, STAGE_T);
 }
 
 // =====================================================================================================
@@ -1039,11 +826,6 @@ __device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned lon
 }
 __device__ __forceinline__ void st_volatile_u64(unsigned long long *p, unsigned long long v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned int ld_volatile_u32(const unsigned int *p) {
-    unsigned int v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
 }
 
 // =====================================================================================================
@@ -1254,21 +1036,11 @@ int rb_minimizer_check_abort(rb_ctx *c, rb_map *fmap) {
     return RB_ERR_CUDA;
 }
 
-// the leading misses of each block of rb_try_vel_rot's output (res[1]) get the stale fi of the blocks before them
-__global__ void __launch_bounds__(TVR_T) k_resolve_res(double *res, const double *carry, const MapState *old_st) {
-    const int i = blockIdx.x * TVR_T + threadIdx.x;
-    if (i >= old_st->kn) return;
-    if (reinterpret_cast<unsigned long long *>(res)[i] == RES_SENTINEL) res[i] = carry[blockIdx.x];
-}
-int rb_resolve_res_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old) {
-    k_resolve_res<<<fmap->ts_host.nblk, TVR_T, 0, c->stream>>>(fmap->res[1], fmap->ts_host.carry, old->st);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-}
-
-// one TryVelRot evaluation at pose X from res[0] (the caller's residuals or zeros) to res[1] (rb_try_vel_rot)
+// one TryVelRot evaluation at pose X from res[0] (the caller's residuals or zeros) to res[1] (rb_try_vel_rot); the 28
+// totals go to tot_dev
 int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double X[6], int reweight, int procjf,
-                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber) {
+                           double match_thresh, double s_rho_min, unsigned int mnt, unsigned int fc, double k_huber,
+                           double *tot_dev) {
     if (fmap->field_radius <= 0) return RB_ERR_STATE;
     TvrPose pose;
     for (int i = 0; i < 6; i++) pose.X[i] = X[i];
@@ -1279,11 +1051,13 @@ int rb_try_vel_rot_enqueue(rb_ctx *c, rb_map *fmap, rb_map *old, const double X[
     tc.k_huber = k_huber;
     tc.mnt = mnt < fc ? mnt : fc;
     const TrackState &h = fmap->ts_host;
-    const TrackPtrs tp = {&fmap->ts->lm, h.blk_has, h.blk_last_fi, h.partials, h.carry};
     auto kern = reweight ? (procjf ? k_try_vel_rot<true, true> : k_try_vel_rot<true, false>)
                          : (procjf ? k_try_vel_rot<false, true> : k_try_vel_rot<false, false>);
-    kern<<<h.nblk, TVR_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, tp, fmap->res[0], fmap->res[1],
-                                          c->ticket + 1, make_cam(c), pose, tc);
+    kern<<<h.nblk, STAGE_T, 0, c->stream>>>(old->kl, old->st, fmap->field, fmap->kl.pack, fmap->res[0], fmap->res[1],
+                                            h.partials, h.blk_has, h.blk_last_fi, make_cam(c), pose, tc);
+    RB_LAUNCH_CHECK();
+    k_blocks_finish<28><<<h.nblk, STAGE_T, 0, c->stream>>>(h.partials, h.nblk, tot_dev, fmap->res[1], h.blk_has,
+                                                           h.blk_last_fi, old->st, false);
     RB_LAUNCH_CHECK();
     return RB_OK;
 }

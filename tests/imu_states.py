@@ -28,7 +28,7 @@ RW = CFG["reweight"]     # ReweigthDistance (also ExtRotVel's Huber threshold in
 Q = 0.3                  # s_rho_min
 LOC_UNC = 1.0            # LocationUncertainty
 V_FAR = np.array([0.02, -0.015, 0.01])
-BLOCK, WARP = 256, 32    # k_tv_eval / k_extrotvel: 256-keyline blocks of eight warps
+BLOCK, WARP = 256, 32    # STAGE_T (csrc/stage_reduce.cuh): k_tv_eval / k_extrotvel run 256-keyline blocks of eight warps
 
 # path codes of tv_setup
 P_MOD, P_SRHO, P_MNUM, P_ZP, P_BORDER, P_IN = range(6)

@@ -1,14 +1,14 @@
 """The IMU-mode device stages against the reference on the seeded states of tests/imu_states.py (their validity, hit counts
 and LM margins are checked on the CPU by tests/test_cpu_imu_states.py):
 
-- rb_try_vel (k_tv_eval + k_tv_finish): m_id_f and the whole in-place residual buffer bit for bit, at every evaluation of
+- rb_try_vel (k_tv_eval + k_blocks_finish<10>): m_id_f and the whole in-place residual buffer bit for bit, at every evaluation of
   a chain whose residuals feed the next evaluation's reweighting.  Misses inherit the fi of the last match before them
   across warps, blocks and gated keylines, or 0 before the first match.  The per-keyline arithmetic is sequential double
   on both sides; the sums differ only in order: score rel 1e-11, JtJ(a,b) within 1e-11 sqrt(JtJ(a,a) JtJ(b,b)), JtF(a)
   within 1e-11 sqrt(JtJ(a,a) score) (Cauchy-Schwarz bounds on the sums of |terms|).
 - rb_minimizer_v: V abs 1e-10 / rel 1e-8 where every LM decision clears the margin, F rel 1e-10, RVel rel 1e-8 where JtJ is
   non-singular (else the same NaN / inf positions), m_id_f of the last evaluation exact.
-- rb_ext_rot_vel (k_extrotvel + k_fold27): ok equal, Wx(a,b) within 1e-11 sqrt(Wx(a,a) Wx(b,b)); X and Rx rel 1e-8 where
+- rb_ext_rot_vel (k_extrotvel + k_blocks_finish<27>): ok equal, Wx(a,b) within 1e-11 sqrt(Wx(a,a) Wx(b,b)); X and Rx rel 1e-8 where
   cond(Wx) <= 1e6 and rel 1e-14 cond above; on rank-deficient systems the same number of kept singular values and X, Rx
   equal on the kept subspace.
 - The IMU pipeline with MatchNumThresh = 3: after vision frames and a reset it runs as a fresh pipeline does, and a fresh
