@@ -100,8 +100,249 @@ struct McView {
     int base, cnt, J;     // first keyline, keylines of this CTA, iterations per thread (uniform over the cluster)
 };
 
-// "Save the scores in temporals" (:686-691) + "Check for the lowest score" (:734-747) once both tries are done
-__device__ __forceinline__ void mc_lm_merge(LMState &s, const LMState &z) {
+// ---- a chain's LM variables in the registers of its warp (warp 0: main / prior-init chain, warp 1: zero-init chain) -----
+// Lane k < 27 holds sum k in the layout the totals arrive in (k < 21: the upper triangle of JtJ row by row, 21..26: JtF):
+// `acc` the accepted JtJ / JtF, `nw` the newest evaluation's JtJn / JtFn, so accepting a step is a select per lane instead
+// of a 42-element copy.  Lanes 0-5 hold X, Xnew and h; the scalars are warp-uniform (every lane evaluates the same
+// expression).  The LMState in shared memory is the hand-off: the merge reads the zero-init chain's try from it, and the
+// epilogue reads the main chain from it once the rounds are over.  Fields nothing reads during the rounds (Xeval, res_in /
+// res_out, Fnew, gain, last_score, Xt ..) are stored there as they are produced and never loaded back.
+struct McChain {
+    double acc, nw;        // lane k < 27: JtJ | JtF, JtJn | JtFn
+    double x, xn, h;       // lane i < 6: X[i], Xnew[i], h[i]
+    double F, F0, u, v;
+    int eff, iR, iRN, iRt, n_eval;
+};
+struct McReq {             // the pose a step requests (uniform): Xeval and its residual buffers
+    double x[6];
+    int ri, ro;
+};
+#define MC_FULL 0xffffffffu
+__device__ __forceinline__ int mc_up_row(int k) { return k < 6 ? 0 : k < 11 ? 1 : k < 15 ? 2 : k < 18 ? 3 : k < 20 ? 4 : 5; }
+__device__ __forceinline__ int mc_up_col(int k, int a) {
+    return k - (a == 0 ? 0 : a == 1 ? 6 : a == 2 ? 11 : a == 3 ? 15 : a == 4 ? 18 : 20) + a;
+}
+__device__ __forceinline__ double mc_lane6(const double (&a)[6], int lane) {   // a[lane] for lanes 0-5, no local memory
+    double r = a[0];
+#pragma unroll
+    for (int i = 1; i < 6; i++) r = lane == i ? a[i] : r;
+    return r;
+}
+__device__ __forceinline__ void mc_gather6(double v, double (&a)[6]) {   // lanes 0-5's v to every lane
+#pragma unroll
+    for (int i = 0; i < 6; i++) a[i] = __shfl_sync(MC_FULL, v, i);
+}
+__device__ __forceinline__ void mc_chain_load(McChain &c, const LMState &L, int lane) {
+    {   // (every field is assigned on every lane, so nothing of the previous contents stays live)
+        const int k = lane < 27 ? lane : 0;
+        const int a = mc_up_row(k), b = mc_up_col(k, a);
+        const int ij = k < 21 ? a * 6 + b : 0, jf = k < 21 ? 0 : k - 21;
+        c.acc = k < 21 ? L.JtJ[ij] : L.JtF[jf];
+        c.nw = k < 21 ? L.JtJn[ij] : L.JtFn[jf];
+    }
+    const int i = lane < 6 ? lane : 0;
+    c.x = L.X[i];
+    c.xn = L.Xnew[i];
+    c.h = L.h[i];
+    c.F = L.F;
+    c.F0 = L.F0;
+    c.u = L.u;
+    c.v = L.v;
+    c.eff = L.eff_steps;
+    c.iR = L.iR;
+    c.iRN = L.iRN;
+    c.iRt = L.iRt;
+    c.n_eval = L.n_eval;
+}
+__device__ __forceinline__ void mc_chain_store(const McChain &c, LMState &L, int lane) {
+    if (lane < 21) {
+        const int a = mc_up_row(lane), b = mc_up_col(lane, a);
+        L.JtJ[a * 6 + b] = c.acc;
+        L.JtJ[b * 6 + a] = c.acc;
+        L.JtJn[a * 6 + b] = c.nw;
+        L.JtJn[b * 6 + a] = c.nw;
+    } else if (lane < 27) {
+        L.JtF[lane - 21] = c.acc;
+        L.JtFn[lane - 21] = c.nw;
+    }
+    if (lane < 6) {
+        L.X[lane] = c.x;
+        L.Xnew[lane] = c.xn;
+        L.h[lane] = c.h;
+    }
+    if (lane == 0) {
+        L.F = c.F;
+        L.F0 = c.F0;
+        L.u = c.u;
+        L.v = c.v;
+        L.eff_steps = c.eff;
+        L.iR = c.iR;
+        L.iRN = c.iRN;
+        L.iRt = c.iRt;
+        L.n_eval = c.n_eval;
+    }
+}
+// lm_request: the pose of the next evaluation; Xeval also goes to shared memory, where warps 3 / 4 read W.z
+__device__ __forceinline__ void mc_request(McReq &q, LMState &L, const double (&X)[6], int ri, int ro, int lane) {
+#pragma unroll
+    for (int i = 0; i < 6; i++) q.x[i] = X[i];
+    q.ri = ri;
+    q.ro = ro;
+    if (lane < 6) L.Xeval[lane] = mc_lane6(X, lane);
+    if (lane == 0) {
+        L.res_in = ri;
+        L.res_out = ro;
+    }
+}
+// F = TryVelRot(JtJ, JtF, X ...); F0 = F; u = tau*max(JtJ).  max_element36 scans JtJ row by row and keeps the first of the
+// largest elements (a NaN is skipped unless it is JtJ[0]); the upper triangle in row order has the same first maximum
+// (a mirrored element repeats an earlier one), and a butterfly that keeps the earlier operand unless the later one is
+// larger, NaN as "no element", finds it in any grouping.
+__device__ __forceinline__ void mc_take_first(McChain &c, double last, int lane) {
+    c.F = last;
+    c.acc = c.nw;
+    c.F0 = c.F;
+    double m = lane < 21 ? c.acc : __longlong_as_double(0x7FF8000000000000ll);
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const double q = __shfl_xor_sync(MC_FULL, m, o);
+        const bool hi = (lane & o) != 0;
+        const double lo_v = hi ? q : m, hi_v = hi ? m : q;
+        m = isnan(lo_v) ? hi_v : (hi_v > lo_v ? hi_v : lo_v);
+    }
+    const double m0 = __shfl_sync(MC_FULL, c.acc, 0);
+    c.u = 1e-3 * (isnan(m0) ? m0 : m);
+}
+// lm_update; returns true when the step was accepted
+__device__ __forceinline__ bool mc_update(McChain &c, LMState &L, double last, bool gain_with_den, int lane) {
+    const double Fnew = last;
+    double gain;
+    if (gain_with_den) {
+        const double jf = __shfl_sync(MC_FULL, c.acc, (lane + 21) & 31);   // JtF[lane]
+        const double p = (0.5 * c.h) * (c.u * c.h - jf);
+        double den = 0;   // 0.5*h*(u*h-JtF): TooN dot of (0.5*h) and (u*h-JtF), left to right
+#pragma unroll
+        for (int i = 0; i < 6; i++) den += __shfl_sync(MC_FULL, p, i);
+        gain = (c.F - Fnew) / den;
+    } else {
+        gain = c.F - Fnew;
+    }
+    if (lane == 0) {
+        L.Fnew = Fnew;
+        L.gain = gain;
+    }
+    if (gain > 0) {
+        c.F = Fnew;
+        c.x = c.xn;
+        c.acc = c.nw;
+        const double g = 2 * gain - 1;
+        const double f = 1 - (g * g * g);
+        c.u *= (0.33 > f ? 0.33 : f);  // std::max(0.33, ...)
+        c.v = 2;
+        c.eff++;
+        return true;
+    }
+    c.u *= c.v;
+    c.v *= 2;
+    return false;
+}
+// lm_solve: h = (JtJ + u I)^-1 (-JtF), Xnew = X + h.  Every lane gathers ApI and factors it (chol6_solve_reg, the same
+// operations in the same order), so h and Xnew need no broadcast; the SVD replacement stays serial and cold.
+__device__ __forceinline__ void mc_solve(McChain &c, LMState &L, bool use_svd, int lane, double (&xn)[6]) {
+    double A[36], rhs[6], hh[6], xg[6], dmin, dmax;
+    mc_gather6(c.x, xg);
+#pragma unroll
+    for (int a = 0; a < 6; a++)
+#pragma unroll
+        for (int b = a; b < 6; b++) {
+            const double t = __shfl_sync(MC_FULL, c.acc, a * 6 - a * (a - 1) / 2 + (b - a));
+            A[a * 6 + b] = t;
+            A[b * 6 + a] = t;
+        }
+#pragma unroll
+    for (int i = 0; i < 6; i++) {
+        A[i * 6 + i] = A[i * 6 + i] + c.u;  // ApI = JtJ + Identity*u
+        rhs[i] = -__shfl_sync(MC_FULL, c.acc, 21 + i);
+    }
+    chol6_solve_reg(A, rhs, hh, dmin, dmax);
+    if (use_svd && !(dmin > 0 && dmin * 1e7 > dmax)) {   // (uniform) rank-deficient ApI: SVD<> pseudo-inverse semantics
+        if (lane < 21) {
+            const int a = mc_up_row(lane), b = mc_up_col(lane, a);
+            L.JtJ[a * 6 + b] = c.acc;
+            L.JtJ[b * 6 + a] = c.acc;
+        } else if (lane < 27) {
+            L.JtF[lane - 21] = c.acc;
+        }
+        if (lane == 0) L.u = c.u;
+        __syncwarp();
+        if (lane == 0) lm_solve_fallback(L);
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < 6; i++) hh[i] = L.h[i];
+        __syncwarp();
+    }
+#pragma unroll
+    for (int i = 0; i < 6; i++) xn[i] = xg[i] + hh[i];
+    c.h = mc_lane6(hh, lane);
+    c.xn = mc_lane6(xn, lane);
+}
+// the LM step of a chain after an evaluation (global_tracker.cpp:651-683 zero-initialised try, :700-732 prior-initialised
+// try, :755-816 main loop).  Returns whether it requested a pose; *fin: the main loop ended (lm_finalize follows the
+// rounds).
+__device__ __forceinline__ bool mc_step(McChain &c, McReq &q, LMState &L, int step, double last, int init_iter,
+                                        int iter_max, bool &fin, int lane) {
+    if (step == STEP_NONE) return false;
+    const bool zero = step <= STEP_INIT_LAST_ZERO, init = step < STEP_MAIN_FIRST;
+    const bool first = step == STEP_INIT_FIRST_ZERO || step == STEP_INIT_FIRST_PRIOR || step == STEP_MAIN_FIRST;
+    const bool init_last = step == STEP_INIT_LAST_ZERO || step == STEP_INIT_LAST_PRIOR;
+    if (first) {
+        mc_take_first(c, last, lane);
+        if (!zero) c.v = 2;   // (zero-init try: v = 2 from the declaration, :620)
+    } else if (mc_update(c, L, last, !init_last, lane) && !init) {   // main loop: std::swap(ResidualNew,Residual)
+        const int t = c.iRN;
+        c.iRN = c.iR;
+        c.iR = t;
+    }
+    // a first step solves when its loop iterates at all; the last step of each loop solves nothing
+    const bool solve = first ? (init ? init_iter > 0 : iter_max > 0) : !(init_last || step == STEP_MAIN_LAST);
+    fin = fin || (!init && !solve);
+    if (!solve) return false;
+    double xn[6];
+    mc_solve(c, L, init, lane, xn);   // (init tries: SVD<> semantics; main loop: Cholesky<6>)
+    mc_request(q, L, xn, init ? -1 : c.iR, zero ? c.iRt : c.iRN, lane);
+    return true;
+}
+// "Save the scores in temporals" (:686-691) + "Check for the lowest score" (:734-747) once both tries are done: the
+// main chain's warp reads the zero-init chain's try from z (which its warp stored before the named barrier)
+__device__ __forceinline__ void mc_merge(McChain &c, McReq &q, LMState &s, const LMState &z, int lane) {
+    const double Xt = z.X[lane < 6 ? lane : 0];
+    const double Ft = z.F, F0t = z.F0, ut = z.u, vt = z.v;
+    const int eff_t = z.eff_steps;
+    if (lane < 6) s.Xt[lane] = Xt;
+    if (lane == 0) {
+        s.Ft = Ft;
+        s.F0t = F0t;
+        s.ut = ut;
+        s.vt = vt;
+        s.eff_steps_t = eff_t;
+    }
+    if (c.F > Ft) {
+        c.x = Xt;
+        c.F = Ft;
+        c.F0 = F0t;
+        c.u = ut;
+        c.v = vt;
+        c.eff = eff_t;
+        c.iRN = c.iRt;
+    }
+    const int t = c.iRN;
+    c.iRN = c.iR;
+    c.iR = t;
+    double X[6];
+    mc_gather6(c.x, X);
+    mc_request(q, s, X, c.iR, c.iRN, lane);
+}
+__device__ __forceinline__ void mc_lm_merge(LMState &s, const LMState &z) {   // the same on LMStates, one lane
     for (int i = 0; i < 6; i++) s.Xt[i] = z.X[i];
     s.Ft = z.F;
     s.F0t = z.F0;
@@ -109,6 +350,16 @@ __device__ __forceinline__ void mc_lm_merge(LMState &s, const LMState &z) {
     s.vt = z.v;
     s.eff_steps_t = z.eff_steps;
     lm_after_prior_pass(s);
+}
+__device__ __forceinline__ void mc_merge_publish(const McChain &z, LMState &Z, int lane) {   // what mc_merge reads
+    if (lane < 6) Z.X[lane] = z.x;
+    if (lane == 0) {
+        Z.F = z.F;
+        Z.F0 = z.F0;
+        Z.u = z.u;
+        Z.v = z.v;
+        Z.eff_steps = z.eff;
+    }
 }
 
 
@@ -294,11 +545,11 @@ __device__ __forceinline__ void mc_eval_pose(McSmem<T> &sm, const McView &v, int
 
 // next pose of a chain: R = exp(W), V, residual buffer ids (:309-311) / the z rotation RotM = exp((0,0,W.z)) (:313-314)
 template <int T>
-__device__ __forceinline__ void mc_req_R(McSmem<T> &sm, int p, const LMState &s) {
-    so3_exp(s.Xeval + 3, sm.req[p]);
-    for (int k = 0; k < 3; k++) sm.req[p][9 + k] = s.Xeval[k];
-    sm.req_res[p][0] = s.res_in;
-    sm.req_res[p][1] = s.res_out;
+__device__ __forceinline__ void mc_req_R(McSmem<T> &sm, int p, const double *X, int res_in, int res_out) {
+    so3_exp(X + 3, sm.req[p]);
+    for (int k = 0; k < 3; k++) sm.req[p][9 + k] = X[k];
+    sm.req_res[p][0] = res_in;
+    sm.req_res[p][1] = res_out;
 }
 template <int T>
 __device__ __forceinline__ void mc_req_RM(McSmem<T> &sm, int p, const LMState &s) {
@@ -421,15 +672,23 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
         mc_mbar_init(&sm.mbar[0], 1);
         mc_mbar_init(&sm.mbar[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        mc_req_R(sm, 0, sm.lm);
+        mc_req_R(sm, 0, sm.lm.Xeval, sm.lm.res_in, sm.lm.res_out);
         mc_req_RM(sm, 0, sm.lm);
     } else if (tid == 32 && fused) {
         lm_begin(sm.lmz, old_st, f_st, su.VW, su.a, su.max_r, su.max_s_rho, su.s_rho_from_state, su.frame_count,
                  su.fc_from_state);   // X = 0, request {0, -1, Rest}
-        mc_req_R(sm, 1, sm.lmz);
+        mc_req_R(sm, 1, sm.lmz.Xeval, sm.lmz.res_in, sm.lmz.res_out);
         mc_req_RM(sm, 1, sm.lmz);
     }
     __syncthreads();
+    // REG: the chains' LM variables live in registers of warps 0 / 1 for the whole minimisation (McChain).  The compiler
+    // allocates registers per kernel, not per warp, and the solve on every lane holds ApI in registers: the 512-thread
+    // form (capped at 128 registers) would spill 600 bytes instead of 172, so it keeps the LMState in shared memory and
+    // runs the LM step on one lane (lm_step_main / lm_step_zero).
+    constexpr bool REG = T <= 256;
+    McChain ch;
+    if (REG && wid < 2) mc_chain_load(ch, wid == 0 ? sm.lm : sm.lmz, lane);
+    bool fin = false;   // the main loop ended: lm_finalize after the rounds
     mc_cluster_sync();   // every CTA's barriers exist before anybody sends
     MC_STAMP(15, 2);
 
@@ -575,52 +834,100 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
             } else if (wid == 0 || two) {   // totals in rank order, then this chain's LM step and next pose
                 const int p = wid;
                 LMState &L = p == 0 ? sm.lm : sm.lmz;
-                if (lane < 28) {   // lane k: total k in rank order, filed straight into JtJn / JtFn (lm_ingest, sign fix-ups :484-490)
-                    double t = sm.gather[par][0][p * MC_PW + lane];
+                if constexpr (REG) {
+                    // lane k: total k in rank order, filed straight into this lane's JtJn / JtFn (lm_ingest, sign fix-ups
+                    // :484-490); lane 27: the score
+                    double t = 0;
+                    if (lane < 28) {
+                        t = sm.gather[par][0][p * MC_PW + lane];
 #pragma unroll
-                    for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
-                    if (lane == 27) {
-                        L.last_score = t;
-                    } else if (PJ && lane < 27) {
+                        for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
+                    }
+                    if (lane == 27) L.last_score = t;
+                    if (PJ && lane < 27) {
                         if (lane < 21) {
-                            // upper-triangle index -> (row, column), branch-free
-                            const int a = lane < 6 ? 0 : lane < 11 ? 1 : lane < 15 ? 2 : lane < 18 ? 3 : lane < 20 ? 4 : 5;
-                            const int b = lane - (a == 0 ? 0 : a == 1 ? 6 : a == 2 ? 11 : a == 3 ? 15 : a == 4 ? 18 : 20) + a;
+                            const int a = mc_up_row(lane), b = mc_up_col(lane, a);
                             const bool neg = (a < 2 && (b == 2 || b == 3)) || ((a == 2 || a == 3) && b >= 4);
-                            t = neg ? -t : t;
-                            L.JtJn[a * 6 + b] = t;
-                            L.JtJn[b * 6 + a] = t;
+                            ch.nw = neg ? -t : t;
                         } else {
                             const int a = lane - 21;
-                            L.JtFn[a] = (a == 2 || a == 3) ? -t : t;
+                            ch.nw = (a == 2 || a == 3) ? -t : t;
                         }
                     }
-                }
-                __syncwarp();
-                MC_STAMP(e, 4);
-                if (lane == 0 && !sm.abort) {
-                    L.n_eval++;
-                    MC_STAMP(e, 5);
-                    if (p == 0) {
-                        lm_step_main(sm.lm, sb, first_cta ? f_st : nullptr);
-                        MC_STAMP(e, 6);
-                    } else {
-                        lm_step_zero(sm.lmz, sa);
+                    const double last_score = __shfl_sync(MC_FULL, t, 27);
+                    MC_STAMP(e, 4);
+                    const bool ab = __any_sync(MC_FULL, sm.abort != 0);   // (one decision for the whole warp)
+                    McReq q;
+                    bool req = false;
+                    if (!ab) {
+                        ch.n_eval++;
+                        MC_STAMP(e, 5);
+                        req = mc_step(ch, q, L, p == 0 ? sb : sa, last_score, su.a.init_iter, su.a.iter_max, fin, lane);
+                        if (p == 0) MC_STAMP(e, 6);
                     }
-                }
-                __syncwarp();
-                if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
-                    asm volatile("bar.sync 3, 64;" ::: "memory");
-                    if (p == 0 && lane == 0 && !sm.abort) mc_lm_merge(sm.lm, sm.lmz);
+                    if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
+                        if (p == 1) mc_merge_publish(ch, sm.lmz, lane);
+                        asm volatile("bar.sync 3, 64;" ::: "memory");
+                        if (p == 0 && !ab) {
+                            mc_merge(ch, q, sm.lm, sm.lmz, lane);
+                            req = true;
+                        }
+                    }
+                    if (!last) {
+                        if (p == 0) {
+                            asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
+                            if (lane == 0 && req) mc_req_R(sm, 0, q.x, q.ri, q.ro);
+                        } else if (next_two) {
+                            asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
+                            if (lane == 0 && req) mc_req_R(sm, 1, q.x, q.ri, q.ro);
+                        }
+                    }
+                } else {   // the 512-thread form: the LMState in shared memory, the step on one lane
+                    if (lane < 28) {   // lane k: total k in rank order, filed straight into JtJn / JtFn (lm_ingest, sign fix-ups :484-490)
+                        double t = sm.gather[par][0][p * MC_PW + lane];
+#pragma unroll
+                        for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
+                        if (lane == 27) {
+                            L.last_score = t;
+                        } else if (PJ && lane < 27) {
+                            if (lane < 21) {
+                                const int a = mc_up_row(lane), b = mc_up_col(lane, a);
+                                const bool neg = (a < 2 && (b == 2 || b == 3)) || ((a == 2 || a == 3) && b >= 4);
+                                t = neg ? -t : t;
+                                L.JtJn[a * 6 + b] = t;
+                                L.JtJn[b * 6 + a] = t;
+                            } else {
+                                const int a = lane - 21;
+                                L.JtFn[a] = (a == 2 || a == 3) ? -t : t;
+                            }
+                        }
+                    }
                     __syncwarp();
-                }
-                if (!last) {
-                    if (p == 0) {
-                        asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
-                        if (lane == 0) mc_req_R(sm, 0, sm.lm);
-                    } else if (next_two) {
-                        asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
-                        if (lane == 0) mc_req_R(sm, 1, sm.lmz);
+                    MC_STAMP(e, 4);
+                    if (lane == 0 && !sm.abort) {
+                        L.n_eval++;
+                        MC_STAMP(e, 5);
+                        if (p == 0) {
+                            lm_step_main(sm.lm, sb, first_cta ? f_st : nullptr);
+                            MC_STAMP(e, 6);
+                        } else {
+                            lm_step_zero(sm.lmz, sa);
+                        }
+                    }
+                    __syncwarp();
+                    if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
+                        asm volatile("bar.sync 3, 64;" ::: "memory");
+                        if (p == 0 && lane == 0 && !sm.abort) mc_lm_merge(sm.lm, sm.lmz);
+                        __syncwarp();
+                    }
+                    if (!last) {
+                        if (p == 0) {
+                            asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
+                            if (lane == 0) mc_req_R(sm, 0, sm.lm.Xeval, sm.lm.res_in, sm.lm.res_out);
+                        } else if (next_two) {
+                            asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
+                            if (lane == 0) mc_req_R(sm, 1, sm.lmz.Xeval, sm.lmz.res_in, sm.lmz.res_out);
+                        }
                     }
                 }
                 MC_STAMP(e, 7);
@@ -644,6 +951,11 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
         if (sm.abort) break;
     }
     // ---- epilogue ------------------------------------------------------------------------------------------------
+    if (REG && wid == 0) {   // the main chain's registers -> sm.lm, then the outputs of the main loop (:793-816)
+        mc_chain_store(ch, sm.lm, lane);
+        __syncwarp();
+        if (lane == 0 && fin) lm_finalize(sm.lm, first_cta ? f_st : nullptr);
+    }
     if (sm.abort && tid == 0) {
         *abort_out = 1;
         for (int k = 0; k < 3; k++) sm.lm.Vel[k] = sm.lm.W0[k] = __longlong_as_double(0x7FF8000000000000ll);
