@@ -194,7 +194,7 @@ __device__ __forceinline__ void mc_request(McReq &q, LMState &L, const double (&
         L.res_out = ro;
     }
 }
-// F = TryVelRot(JtJ, JtF, X ...); F0 = F; u = tau*max(JtJ).  max_element36 scans JtJ row by row and keeps the first of the
+// F = TryVelRot(JtJ, JtF, X ...); F0 = F; u = tau*max_element(JtJ).  A row-by-row scan of JtJ keeps the first of the
 // largest elements (a NaN is skipped unless it is JtJ[0]); the upper triangle in row order has the same first maximum
 // (a mirrored element repeats an earlier one), and a butterfly that keeps the earlier operand unless the later one is
 // larger, NaN as "no element", finds it in any grouping.
@@ -213,7 +213,8 @@ __device__ __forceinline__ void mc_take_first(McChain &c, double last, int lane)
     const double m0 = __shfl_sync(MC_FULL, c.acc, 0);
     c.u = 1e-3 * (isnan(m0) ? m0 : m);
 }
-// lm_update; returns true when the step was accepted
+// gain, then accept (F, X, JtJ / JtF from the evaluation, u shrinks) or reject (u *= v, v *= 2); returns true when the
+// step was accepted
 __device__ __forceinline__ bool mc_update(McChain &c, LMState &L, double last, bool gain_with_den, int lane) {
     const double Fnew = last;
     double gain;
@@ -246,8 +247,11 @@ __device__ __forceinline__ bool mc_update(McChain &c, LMState &L, double last, b
     c.v *= 2;
     return false;
 }
-// lm_solve: h = (JtJ + u I)^-1 (-JtF), Xnew = X + h.  Every lane gathers ApI and factors it (chol6_solve_reg, the same
-// operations in the same order), so h and Xnew need no broadcast; the SVD replacement stays serial and cold.
+// h = (JtJ + u I)^-1 (-JtF), Xnew = X + h.  Every lane gathers ApI and factors it (chol6_solve_reg, the same operations in
+// the same order), so h and Xnew need no broadcast.  The main loop solves with Cholesky<6> (:766-767), the init tries with
+// SVD<> (:659-661): ApI is SPD with a condition number far below SVD.h's 1e9 cut, so the pseudo-inverse is the inverse and
+// the LDL^T solve returns the same vector up to rounding; the Jacobi pseudo-inverse (lm_solve_fallback) is kept for
+// rank-deficient input, serial and cold.
 __device__ __forceinline__ void mc_solve(McChain &c, LMState &L, bool use_svd, int lane, double (&xn)[6]) {
     double A[36], rhs[6], hh[6], xg[6], dmin, dmax;
     mc_gather6(c.x, xg);
@@ -341,15 +345,6 @@ __device__ __forceinline__ void mc_merge(McChain &c, McReq &q, LMState &s, const
     double X[6];
     mc_gather6(c.x, X);
     mc_request(q, s, X, c.iR, c.iRN, lane);
-}
-__device__ __forceinline__ void mc_lm_merge(LMState &s, const LMState &z) {   // the same on LMStates, one lane
-    for (int i = 0; i < 6; i++) s.Xt[i] = z.X[i];
-    s.Ft = z.F;
-    s.F0t = z.F0;
-    s.ut = z.u;
-    s.vt = z.v;
-    s.eff_steps_t = z.eff_steps;
-    lm_after_prior_pass(s);
 }
 __device__ __forceinline__ void mc_merge_publish(const McChain &z, LMState &Z, int lane) {   // what mc_merge reads
     if (lane < 6) Z.X[lane] = z.x;
@@ -681,13 +676,10 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
         mc_req_RM(sm, 1, sm.lmz);
     }
     __syncthreads();
-    // REG: the chains' LM variables live in registers of warps 0 / 1 for the whole minimisation (McChain).  The compiler
-    // allocates registers per kernel, not per warp, and the solve on every lane holds ApI in registers: the 512-thread
-    // form (capped at 128 registers) would spill 600 bytes instead of 172, so it keeps the LMState in shared memory and
-    // runs the LM step on one lane (lm_step_main / lm_step_zero).
-    constexpr bool REG = T <= 256;
+    // the chains' LM variables live in registers of warps 0 / 1 for the whole minimisation (McChain).  Registers are
+    // allocated per kernel, not per warp: the 512-thread form (capped at 128) spills part of the step (DESIGN.md §5)
     McChain ch;
-    if (REG && wid < 2) mc_chain_load(ch, wid == 0 ? sm.lm : sm.lmz, lane);
+    if (wid < 2) mc_chain_load(ch, wid == 0 ? sm.lm : sm.lmz, lane);
     bool fin = false;   // the main loop ended: lm_finalize after the rounds
     mc_cluster_sync();   // every CTA's barriers exist before anybody sends
     MC_STAMP(15, 2);
@@ -834,100 +826,51 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
             } else if (wid == 0 || two) {   // totals in rank order, then this chain's LM step and next pose
                 const int p = wid;
                 LMState &L = p == 0 ? sm.lm : sm.lmz;
-                if constexpr (REG) {
-                    // lane k: total k in rank order, filed straight into this lane's JtJn / JtFn (lm_ingest, sign fix-ups
-                    // :484-490); lane 27: the score
-                    double t = 0;
-                    if (lane < 28) {
-                        t = sm.gather[par][0][p * MC_PW + lane];
+                // lane k: total k in rank order, filed straight into this lane's JtJn / JtFn (lm_ingest, sign fix-ups
+                // :484-490); lane 27: the score
+                double t = 0;
+                if (lane < 28) {
+                    t = sm.gather[par][0][p * MC_PW + lane];
 #pragma unroll
-                        for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
+                    for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
+                }
+                if (lane == 27) L.last_score = t;
+                if (PJ && lane < 27) {
+                    if (lane < 21) {
+                        const int a = mc_up_row(lane), b = mc_up_col(lane, a);
+                        const bool neg = (a < 2 && (b == 2 || b == 3)) || ((a == 2 || a == 3) && b >= 4);
+                        ch.nw = neg ? -t : t;
+                    } else {
+                        const int a = lane - 21;
+                        ch.nw = (a == 2 || a == 3) ? -t : t;
                     }
-                    if (lane == 27) L.last_score = t;
-                    if (PJ && lane < 27) {
-                        if (lane < 21) {
-                            const int a = mc_up_row(lane), b = mc_up_col(lane, a);
-                            const bool neg = (a < 2 && (b == 2 || b == 3)) || ((a == 2 || a == 3) && b >= 4);
-                            ch.nw = neg ? -t : t;
-                        } else {
-                            const int a = lane - 21;
-                            ch.nw = (a == 2 || a == 3) ? -t : t;
-                        }
+                }
+                const double last_score = __shfl_sync(MC_FULL, t, 27);
+                MC_STAMP(e, 4);
+                const bool ab = __any_sync(MC_FULL, sm.abort != 0);   // (one decision for the whole warp)
+                McReq q;
+                bool req = false;
+                if (!ab) {
+                    ch.n_eval++;
+                    MC_STAMP(e, 5);
+                    req = mc_step(ch, q, L, p == 0 ? sb : sa, last_score, su.a.init_iter, su.a.iter_max, fin, lane);
+                    if (p == 0) MC_STAMP(e, 6);
+                }
+                if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
+                    if (p == 1) mc_merge_publish(ch, sm.lmz, lane);
+                    asm volatile("bar.sync 3, 64;" ::: "memory");
+                    if (p == 0 && !ab) {
+                        mc_merge(ch, q, sm.lm, sm.lmz, lane);
+                        req = true;
                     }
-                    const double last_score = __shfl_sync(MC_FULL, t, 27);
-                    MC_STAMP(e, 4);
-                    const bool ab = __any_sync(MC_FULL, sm.abort != 0);   // (one decision for the whole warp)
-                    McReq q;
-                    bool req = false;
-                    if (!ab) {
-                        ch.n_eval++;
-                        MC_STAMP(e, 5);
-                        req = mc_step(ch, q, L, p == 0 ? sb : sa, last_score, su.a.init_iter, su.a.iter_max, fin, lane);
-                        if (p == 0) MC_STAMP(e, 6);
-                    }
-                    if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
-                        if (p == 1) mc_merge_publish(ch, sm.lmz, lane);
-                        asm volatile("bar.sync 3, 64;" ::: "memory");
-                        if (p == 0 && !ab) {
-                            mc_merge(ch, q, sm.lm, sm.lmz, lane);
-                            req = true;
-                        }
-                    }
-                    if (!last) {
-                        if (p == 0) {
-                            asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
-                            if (lane == 0 && req) mc_req_R(sm, 0, q.x, q.ri, q.ro);
-                        } else if (next_two) {
-                            asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
-                            if (lane == 0 && req) mc_req_R(sm, 1, q.x, q.ri, q.ro);
-                        }
-                    }
-                } else {   // the 512-thread form: the LMState in shared memory, the step on one lane
-                    if (lane < 28) {   // lane k: total k in rank order, filed straight into JtJn / JtFn (lm_ingest, sign fix-ups :484-490)
-                        double t = sm.gather[par][0][p * MC_PW + lane];
-#pragma unroll
-                        for (int r = 1; r < MC_C; r++) t += sm.gather[par][r][p * MC_PW + lane];
-                        if (lane == 27) {
-                            L.last_score = t;
-                        } else if (PJ && lane < 27) {
-                            if (lane < 21) {
-                                const int a = mc_up_row(lane), b = mc_up_col(lane, a);
-                                const bool neg = (a < 2 && (b == 2 || b == 3)) || ((a == 2 || a == 3) && b >= 4);
-                                t = neg ? -t : t;
-                                L.JtJn[a * 6 + b] = t;
-                                L.JtJn[b * 6 + a] = t;
-                            } else {
-                                const int a = lane - 21;
-                                L.JtFn[a] = (a == 2 || a == 3) ? -t : t;
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    MC_STAMP(e, 4);
-                    if (lane == 0 && !sm.abort) {
-                        L.n_eval++;
-                        MC_STAMP(e, 5);
-                        if (p == 0) {
-                            lm_step_main(sm.lm, sb, first_cta ? f_st : nullptr);
-                            MC_STAMP(e, 6);
-                        } else {
-                            lm_step_zero(sm.lmz, sa);
-                        }
-                    }
-                    __syncwarp();
-                    if (merge) {   // (uniform) the main chain picks the better try once both LM steps are done
-                        asm volatile("bar.sync 3, 64;" ::: "memory");
-                        if (p == 0 && lane == 0 && !sm.abort) mc_lm_merge(sm.lm, sm.lmz);
-                        __syncwarp();
-                    }
-                    if (!last) {
-                        if (p == 0) {
-                            asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
-                            if (lane == 0) mc_req_R(sm, 0, sm.lm.Xeval, sm.lm.res_in, sm.lm.res_out);
-                        } else if (next_two) {
-                            asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
-                            if (lane == 0) mc_req_R(sm, 1, sm.lmz.Xeval, sm.lmz.res_in, sm.lmz.res_out);
-                        }
+                }
+                if (!last) {
+                    if (p == 0) {
+                        asm volatile("bar.sync 1, 64;" ::: "memory");      // releases warp 3
+                        if (lane == 0 && req) mc_req_R(sm, 0, q.x, q.ri, q.ro);
+                    } else if (next_two) {
+                        asm volatile("bar.sync 2, 64;" ::: "memory");      // releases warp 4
+                        if (lane == 0 && req) mc_req_R(sm, 1, q.x, q.ri, q.ro);
                     }
                 }
                 MC_STAMP(e, 7);
@@ -951,7 +894,7 @@ __global__ void __cluster_dims__(MC_C, 1, 1) __launch_bounds__(T, 1)
         if (sm.abort) break;
     }
     // ---- epilogue ------------------------------------------------------------------------------------------------
-    if (REG && wid == 0) {   // the main chain's registers -> sm.lm, then the outputs of the main loop (:793-816)
+    if (wid == 0) {   // the main chain's registers -> sm.lm, then the outputs of the main loop (:793-816)
         mc_chain_store(ch, sm.lm, lane);
         __syncwarp();
         if (lane == 0 && fin) lm_finalize(sm.lm, first_cta ? f_st : nullptr);

@@ -217,12 +217,6 @@ int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool
 // =====================================================================================================
 // Minimizer_RV: the LM pieces the cluster kernel (min_cluster.cuh) runs between its rounds
 // =====================================================================================================
-__device__ __forceinline__ double max_element36(const double *M) {
-    double m = M[0];
-    for (int i = 1; i < 36; i++)
-        if (M[i] > m) m = M[i];
-    return m;
-}
 __device__ void lm_build_api(const LMState &s, double *A, double *rhs) {
     for (int i = 0; i < 36; i++) A[i] = s.JtJ[i];
     for (int i = 0; i < 6; i++) {
@@ -291,78 +285,10 @@ __device__ __noinline__ void lm_solve_fallback(LMState &s) {   // rank-deficient
     sym_svd_backsub(A, 6, rhs, h);
     for (int i = 0; i < 6; i++) s.h[i] = h[i];
 }
-__device__ void lm_solve(LMState &s, bool use_svd) {
-    double A[36], rhs[6], h[6], dmin, dmax;
-#pragma unroll
-    for (int i = 0; i < 36; i++) A[i] = s.JtJ[i];
-#pragma unroll
-    for (int i = 0; i < 6; i++) {
-        A[i * 6 + i] = s.JtJ[i * 6 + i] + s.u;  // ApI = JtJ + Identity*u
-        rhs[i] = -s.JtF[i];
-    }
-    // Cholesky<6> svdApI(ApI); h = svdApI.backsub(-JtF)   (main loop, global_tracker.cpp:766-767)
-    // SVD<> svdApI(ApI); h = svdApI.backsub(-JtF)          (init iterations, :659-661): ApI is SPD with a condition
-    // number far below SVD.h's 1e9 cut, so the pseudo-inverse is the inverse and the LDL^T solve returns the same
-    // vector up to rounding; the Jacobi pseudo-inverse is kept for rank-deficient input.
-    chol6_solve_reg(A, rhs, h, dmin, dmax);
-#pragma unroll
-    for (int i = 0; i < 6; i++) s.h[i] = h[i];
-    if (use_svd && !(dmin > 0 && dmin * 1e7 > dmax)) lm_solve_fallback(s);
-#pragma unroll
-    for (int i = 0; i < 6; i++) s.Xnew[i] = s.X[i] + s.h[i];
-}
 __device__ void lm_request(LMState &s, const double *X, int res_in, int res_out) {
     for (int i = 0; i < 6; i++) s.Xeval[i] = X[i];
     s.res_in = res_in;
     s.res_out = res_out;
-}
-__device__ void lm_take_first(LMState &s) {   // F = TryVelRot(JtJ, JtF, X ...); F0 = F; u = tau*max(JtJ)
-    s.F = s.last_score;
-    for (int i = 0; i < 36; i++) s.JtJ[i] = s.JtJn[i];
-    for (int i = 0; i < 6; i++) s.JtF[i] = s.JtFn[i];
-    s.F0 = s.F;
-    s.u = 1e-3 * max_element36(s.JtJ);
-}
-// returns true when the step was accepted
-__device__ bool lm_update(LMState &s, bool gain_with_den) {
-    s.Fnew = s.last_score;
-    if (gain_with_den) {
-        double den = 0;  // 0.5*h*(u*h-JtF): TooN dot of (0.5*h) and (u*h-JtF)
-        for (int i = 0; i < 6; i++) den += (0.5 * s.h[i]) * (s.u * s.h[i] - s.JtF[i]);
-        s.gain = (s.F - s.Fnew) / den;
-    } else {
-        s.gain = s.F - s.Fnew;
-    }
-    if (s.gain > 0) {
-        s.F = s.Fnew;
-        for (int i = 0; i < 6; i++) s.X[i] = s.Xnew[i];
-        for (int i = 0; i < 36; i++) s.JtJ[i] = s.JtJn[i];
-        for (int i = 0; i < 6; i++) s.JtF[i] = s.JtFn[i];
-        const double g = 2 * s.gain - 1;
-        const double f = 1 - (g * g * g);
-        s.u *= (0.33 > f ? 0.33 : f);  // std::max(0.33, ...)
-        s.v = 2;
-        s.eff_steps++;
-        return true;
-    }
-    s.u *= s.v;
-    s.v *= 2;
-    return false;
-}
-__device__ void lm_after_prior_pass(LMState &s) {  // :734-747
-    if (s.F > s.Ft) {
-        for (int i = 0; i < 6; i++) s.X[i] = s.Xt[i];
-        s.F = s.Ft;
-        s.F0 = s.F0t;
-        s.u = s.ut;
-        s.v = s.vt;
-        s.eff_steps = s.eff_steps_t;
-        s.iRN = s.iRt;
-    }
-    const int t = s.iRN;
-    s.iRN = s.iR;
-    s.iR = t;
-    lm_request(s, s.X, s.iR, s.iRN);
 }
 // RRV = Cholesky<6>(JtJ).get_inverse() (:795-801): column c = backsub(e_c) with the matrix overload's y *= 1/diag.
 // Threads 0..5 of the calling block each factorise (registers) and solve one column.
@@ -401,77 +327,6 @@ __device__ void lm_finalize(LMState &s, MapState *fst) {   // :793-816; RVel / R
     }
     s.score = s.F;
     if (fst) fst->frame_count = fst->frame_count + 1;   // FrameCount++ (one CTA of the cluster kernel does it)
-}
-
-// LM step after an evaluation.  The two init tries of init type 2 run side by side, one step each per round:
-// lm_step_zero is the zero-initialised try (global_tracker.cpp:651-683), lm_step_main the prior-initialised try
-// (:700-732) and then the main loop (:755-816); mc_lm_merge picks the better try (:686-691, :734-747).
-__device__ __forceinline__ void lm_step_zero(LMState &z, int step) {
-    switch (step) {
-        case STEP_INIT_FIRST_ZERO:
-            lm_take_first(z);   // v = 2 from the declaration (:620)
-            if (z.init_iter > 0) {
-                lm_solve(z, true);
-                lm_request(z, z.Xnew, -1, z.iRt);
-            }
-            break;
-        case STEP_INIT_ITER_ZERO:
-            lm_update(z, true);
-            lm_solve(z, true);
-            lm_request(z, z.Xnew, -1, z.iRt);
-            break;
-        case STEP_INIT_LAST_ZERO:
-            lm_update(z, false);
-            break;
-        default:
-            break;
-    }
-}
-__device__ __forceinline__ void lm_step_main(LMState &s, int step, MapState *fst) {
-    switch (step) {
-        case STEP_INIT_FIRST_PRIOR:
-            lm_take_first(s);
-            s.v = 2;
-            if (s.init_iter > 0) {
-                lm_solve(s, true);
-                lm_request(s, s.Xnew, -1, s.iRN);
-            }
-            break;
-        case STEP_INIT_ITER_PRIOR:
-            lm_update(s, true);
-            lm_solve(s, true);
-            lm_request(s, s.Xnew, -1, s.iRN);
-            break;
-        case STEP_INIT_LAST_PRIOR:
-            lm_update(s, false);
-            break;
-        case STEP_MAIN_FIRST:
-            lm_take_first(s);
-            s.v = 2;
-            if (s.iter_max <= 0) {
-                lm_finalize(s, fst);
-            } else {
-                lm_solve(s, false);
-                lm_request(s, s.Xnew, s.iR, s.iRN);
-            }
-            break;
-        case STEP_MAIN_ITER:
-        case STEP_MAIN_LAST:
-            if (lm_update(s, true)) {   // std::swap(ResidualNew,Residual)
-                const int t = s.iRN;
-                s.iRN = s.iR;
-                s.iR = t;
-            }
-            if (step == STEP_MAIN_LAST) {
-                lm_finalize(s, fst);
-            } else {
-                lm_solve(s, false);
-                lm_request(s, s.Xnew, s.iR, s.iRN);
-            }
-            break;
-        default:
-            break;
-    }
 }
 
 struct ResPtrs {
