@@ -512,6 +512,52 @@ int rb_pipeline_set_imu(rb_pipeline *pl, const rb_imu_params *ip, const double *
 int rb_pipeline_set_imu_live(rb_pipeline *pl, const rb_imu_params *ip, double sample_time, int buffer_size);
 int rb_pipeline_push_imu(rb_pipeline *pl, const double *samples, int n);
 
+/* ---- session checkpoints ------------------------------------------------------------------------
+ * A tracking session as a versioned blob in host memory, written by one pipeline and loaded into any pipeline of the same
+ * geometry, on any device and in any process: after the load the pushes continue the session exactly, with the bytes an
+ * uninterrupted run would have produced (nav and odometry records, mirrors, depth grids and images).  Use it to survive a
+ * process restart, to move a live stream to another GPU or worker, or to start a test or a debugging session at frame N of
+ * a long stream without replaying the frames before it.
+ *
+ * The blob holds the session: the newest edge map (its live keylines and scalars; the keyline mask is rebuilt from them on
+ * load), pose, velocity and their covariances, K / Kp / P_Kp, the detector's threshold feedback, the frame count, the last
+ * timestamp, and in IMU mode the filter, the scale estimator's history and the sample ring's read position (live mode: also
+ * the samples it has not released).  It does not hold the configuration, which stays with the pipeline object: mirror, depth
+ * grid and image, odometry records, undistortion, output memory, consumer stream, and the rb_params fields other than the
+ * geometry.  About 120 bytes per keyline (2 MB at 15 k keylines).  Layout: DESIGN.md §5.
+ *
+ * rb_pipeline_save_state writes the blob into buf and its size into *written.  When cap is too small it writes nothing,
+ * still reports the size needed and returns RB_ERR_ARG (buf = NULL, cap = 0 asks for the size).  Between pushes;
+ * synchronous.  It changes nothing in the pipeline: the pushes after it give what they would have given.
+ *
+ * rb_pipeline_load_state replaces the session of pl with the blob's.  RB_ERR_ARG, with pl unchanged (its next push gives what
+ * it would have given), when the blob is truncated or corrupt (checksum), of another version, of another camera (w, h, pp, zf),
+ * Sigma0, KSigma or kl_capacity, or of another mode (vision only, IMU dataset, IMU live: rb_pipeline_set_imu /
+ * rb_pipeline_set_imu_live must come before the load); in dataset mode when pl's samples are not the source's (count and
+ * checksum); in live mode when pl's ring cannot hold the samples the source had not released.  The other rb_params fields may
+ * differ: the session then continues with pl's parameters from its next frame on (a fork with other tracker settings, which
+ * no uninterrupted run reproduces).  After a load the outputs of the last push are gone, as after the set_* calls: their
+ * accessors return RB_ERR_ARG until the next push; rb_pipeline_map(pl, 0) is the restored map and rb_pipeline_map(pl, 1) is
+ * NULL until the next push.  Neither call changes a push's captured batches: pushes launch what they launched before.
+ * rb_pipeline_reset keeps its meaning (a new session).
+ *
+ * rb_state_info: host only, no device needed.  Checks the header and the checksum (RB_ERR_ARG otherwise) and describes the
+ * blob. */
+enum { RB_STATE_VISION = 0, RB_STATE_IMU_DATASET = 1, RB_STATE_IMU_LIVE = 2 };
+struct rb_state_info {   /* (a struct tag, not a typedef: the function below has its name) */
+    uint32_t version;
+    int32_t mode;          /* RB_STATE_* */
+    uint64_t bytes;        /* size of the blob */
+    rb_camera cam;
+    double Sigma0, KSigma;
+    int32_t kl_capacity;
+    int32_t kn;            /* keylines of the newest edge map */
+    int64_t n_pushed;      /* frames pushed in the session */
+};
+int rb_pipeline_save_state(rb_pipeline *pl, void *buf, size_t cap, size_t *written);
+int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n);
+int rb_state_info(const void *buf, size_t n, struct rb_state_info *out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librebvo_b200.so")
 SOURCES = ["dog.cu", "detect.cu", "tracker.cu", "capi.cu", "capi_track.cu", "pipeline.cu", "hostmath.cu",
-           "undistort.cu", "gray.cu", "imu_track.cu", "netpack.cu", "logfmt.cu", "depth.cu"]
+           "undistort.cu", "gray.cu", "imu_track.cu", "netpack.cu", "logfmt.cu", "depth.cu",
+           "state.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference is built without FMA contraction (x86-64 -O2, no -march); bit parity of the
 # float32 scale space and of the per-keyline float64 arithmetic depends on it.

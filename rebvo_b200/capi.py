@@ -120,7 +120,8 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_odometry", "rb_depth_fill_net", "rb_pipeline_set_depth", "rb_pipeline_depth", "rb_depth_image",
            "rb_pipeline_set_depth_image", "rb_pipeline_depth_image", "rb_pipeline_set_output_memory",
            "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev",
-           "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev", "rb_pipeline_batch_plane"]
+           "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev", "rb_pipeline_batch_plane", "rb_pipeline_save_state",
+           "rb_pipeline_load_state", "rb_state_info"]
 
 _lib = None
 
@@ -242,6 +243,29 @@ def read_pose_graph(path):
         out[k] = ps[k]
     out["tracked"] = 1
     return out
+
+
+# rb_state_info (include/rebvo_b200.h, session checkpoints); mode: STATE_VISION, STATE_IMU_DATASET or STATE_IMU_LIVE
+class StateInfo(C.Structure):
+    _fields_ = [("version", C.c_uint32), ("mode", C.c_int32), ("bytes", C.c_uint64), ("cam", Camera), ("Sigma0", C.c_double),
+                ("KSigma", C.c_double), ("kl_capacity", C.c_int32), ("kn", C.c_int32), ("n_pushed", C.c_int64)]
+
+
+STATE_VISION, STATE_IMU_DATASET, STATE_IMU_LIVE = 0, 1, 2
+
+
+def state_info(blob):
+    """What a session blob (Pipeline.save_state) holds: version, bytes, camera, Sigma0, KSigma, kl_capacity, mode, frames
+    pushed (n_pushed) and the newest map's keyline count (kn).  Host only.  RbError for a blob whose header or checksum is
+    wrong."""
+    blob = bytes(blob)
+    out = StateInfo()
+    r = lib().rb_state_info(blob, C.c_size_t(len(blob)), C.byref(out))
+    if r:
+        raise RbError("rb_state_info: not a valid state blob (%d)" % r)
+    d = {k: getattr(out, k) for k, _ in StateInfo._fields_ if k != "cam"}
+    d.update({k: getattr(out.cam, k) for k, _ in Camera._fields_})
+    return d
 
 
 def lib():
@@ -716,6 +740,23 @@ class Pipeline:
 
     def reset(self):
         self.check(self.L.rb_pipeline_reset(self.h_))
+
+    def save_state(self):
+        """The tracking session as a blob (bytes): load it into a pipeline of the same geometry, here or in another process
+        or on another GPU, and the pushes continue the session exactly (rb_pipeline_save_state)."""
+        need = C.c_size_t(0)
+        r = self.L.rb_pipeline_save_state(self.h_, None, C.c_size_t(0), C.byref(need))
+        if r and need.value == 0:
+            self.check(r)
+        buf = C.create_string_buffer(need.value)
+        self.check(self.L.rb_pipeline_save_state(self.h_, buf, C.c_size_t(need.value), C.byref(need)))
+        return buf.raw[:need.value]
+
+    def load_state(self, blob):
+        """Replace this pipeline's session with the blob's (rb_pipeline_load_state).  RbError, with the pipeline unchanged,
+        for a corrupt blob or one of another version, geometry or mode."""
+        blob = bytes(blob)
+        self.check(self.L.rb_pipeline_load_state(self.h_, blob, C.c_size_t(len(blob))))
 
     def launches(self):
         return self.L.rb_pipeline_launch_count(self.h_)

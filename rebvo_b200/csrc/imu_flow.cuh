@@ -10,14 +10,9 @@
 
 #include "imu_filter.h"
 
-struct ImuFlow {
-    rb_imu_params ip;
-    std::vector<rbimu::ImuSample> samples;   // dataset mode: every sample; live mode: the ring's slots
-    rbimu::ImuBuffer buf;
+// the session part of the IMU flow: plain data, which a state blob carries as it is (rb_pipeline_save_state)
+struct ImuSession {
     rbimu::ImuFilterHist hist;
-    bool enabled;
-    bool live;            // ImuMode=1 (rb_pipeline_set_imu_live): samples arrive through rb_pipeline_push_imu
-    double t_last;        // live mode: timestamp of the last sample pushed (-inf before the first)
     // SecondThread locals (:57-90)
     double V[3], W[3], Pos[3], R[9], Pose[9], Rgva[9], P_V[9], P_W[9];
     double K, Kp, P_Kp;
@@ -30,6 +25,14 @@ struct ImuFlow {
     bool init;
     int n_giro_init;
     double giro_init[3], g_init[3];
+};
+struct ImuFlow : ImuSession {
+    rb_imu_params ip;
+    std::vector<rbimu::ImuSample> samples;   // dataset mode: every sample; live mode: the ring's slots
+    rbimu::ImuBuffer buf;
+    bool enabled;
+    bool live;            // ImuMode=1 (rb_pipeline_set_imu_live): samples arrive through rb_pipeline_push_imu
+    double t_last;        // live mode: timestamp of the last sample pushed (-inf before the first)
 };
 
 // n rows {t, gyro xyz, accel xyz} of the C interface -> samples
@@ -373,5 +376,6 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_fr
     }
     pl->t_prev = ts[n - 1];
     pl->n_pushed += n;
+    pl->restored = false;
     return RB_OK;
 }

@@ -14,6 +14,7 @@
 #include "tracker.cuh"
 #include "frame.cuh"
 #include "depth.cuh"
+#include "state.cuh"
 
 int rb_map_alloc(rb_ctx *c, rb_map **out, bool with_ws);
 
@@ -96,6 +97,9 @@ struct rb_pipeline {
     int *abort_pin;       // pinned: abort flags of the three maps' minimisers, read back with every push
     uint8_t *rgb_pin;     // optional pinned staging (unused when the caller's buffer is pinned)
     long long n_pushed;   // frames pushed so far
+    bool restored;        // rb_pipeline_load_state since the last push: the ring holds the newest map alone
+    unsigned char *state_host;    // mapped pinned staging of a state blob's device section (rb_pipeline_save_state)
+    size_t state_host_bytes;
     double t_prev;
     cudaEvent_t ev[4];
     cudaEvent_t user_ev[8];
@@ -338,6 +342,7 @@ static int pl_reset_state(rb_pipeline *pl) {
         }
     if (pl->imu) imu_flow_reset(*pl->imu);
     pl->n_pushed = 0;
+    pl->restored = false;
     pl->t_prev = 0;
     return RB_OK;
 }
@@ -533,7 +538,7 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
                    pl->depth.stage, pl->depth.ws, pl->depth.dev, pl->dimg.dev};
     for (void *p : dev) cudaFree(p);
     void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->frames_pin, pl->mirror.host, pl->odom.pin,
-                    pl->depth.host, pl->dimg.host};
+                    pl->depth.host, pl->dimg.host, pl->state_host};
     for (void *p : host)
         if (p) cudaFreeHost(p);
     rb_ctx_destroy(c);
@@ -544,7 +549,7 @@ extern "C" const char *rb_pipeline_last_error(const rb_pipeline *pl) { return pl
 extern "C" int64_t rb_pipeline_launch_count(const rb_pipeline *pl) { return pl->c->launches; }
 extern "C" void *rb_pipeline_stream(rb_pipeline *pl) { return (void *)pl->c->stream; }
 extern "C" rb_map *rb_pipeline_map(rb_pipeline *pl, int age) {
-    if (age < 0 || age > 1 || pl->n_pushed <= age) return nullptr;
+    if (age < 0 || age > 1 || pl->n_pushed <= age || (age == 1 && pl->restored)) return nullptr;
     return pl->maps[(pl->n_pushed - 1 - age) % RB_NMAPS];
 }
 extern "C" int rb_pipeline_stage_ms(const rb_pipeline *pl, float out[6]) {
@@ -906,6 +911,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
                                 c->stream));
     pl->t_prev = ts[n - 1];
     pl->n_pushed += n;
+    pl->restored = false;
     prof_mark(pl, ST_NAV);
     RB_CUDA(cudaEventRecord(pl->ev[3], c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
@@ -1315,5 +1321,178 @@ extern "C" int rb_pipeline_stage_profile(rb_pipeline *pl, double out_ms[16], lon
     if (!pl->prof_on) return RB_ERR_STATE;
     for (int i = 0; i < 16; i++) out_ms[i] = pl->pacc[i];
     if (frames) *frames = pl->pframes;
+    return RB_OK;
+}
+
+// ---- session checkpoints (rb_pipeline_save_state / rb_pipeline_load_state; blob layout: state.cuh, DESIGN.md §5) ----------
+static int state_mode(const rb_pipeline *pl) {
+    return !pl->imu ? RB_STATE_VISION : pl->imu->live ? RB_STATE_IMU_LIVE : RB_STATE_IMU_DATASET;
+}
+// live ring: the samples pushed and not released yet, s[read_inx + 1 ..] up to write_inx
+static int live_pending(const rbimu::ImuBuffer &b) { return (b.write_inx - b.read_inx - 1 + 2 * b.size) % b.size; }
+// host section: t_prev, odometry's rkp_last; in IMU mode then ImuSession, the ring's read position (dataset mode), t_last and
+// the count of pending samples (live mode), and those samples
+#define RB_STATE_HOST_VISION 16
+static size_t state_host_bytes(int mode, long long n_pending) {
+    if (mode == RB_STATE_VISION) return RB_STATE_HOST_VISION;
+    return RB_STATE_HOST_VISION + state_align8(sizeof(ImuSession)) + 24 + sizeof(rbimu::ImuSample) * (size_t)n_pending;
+}
+static uint64_t imu_samples_checksum(const ImuFlow &f) {
+    return state_checksum(f.samples.data(), sizeof(rbimu::ImuSample) * f.samples.size());
+}
+
+extern "C" int rb_pipeline_save_state(rb_pipeline *pl, void *buf, size_t cap, size_t *written) {
+    if (!pl || !written || (cap && !buf)) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    rb_map *m = pl->n_pushed > 0 ? pl->maps[(pl->n_pushed - 1) % RB_NMAPS] : nullptr;
+    MapState ms;
+    memset(&ms, 0, sizeof(ms));
+    int r;
+    if (m && (r = rb_read_map_state(m, &ms))) return r;
+    const int mode = state_mode(pl);
+    const int pending = mode == RB_STATE_IMU_LIVE ? live_pending(pl->imu->buf) : 0;
+    const size_t dev_b = state_dev_bytes(ms.kn), off_host = sizeof(StateHeader) + dev_b;
+    const size_t total = off_host + state_host_bytes(mode, pending);
+    *written = total;
+    if (cap < total) {
+        snprintf(c->err, sizeof(c->err), "save_state: the blob needs %zu bytes, the buffer holds %zu", total, cap);
+        return RB_ERR_ARG;
+    }
+    // the device section: one kernel writes the live prefix straight into mapped pinned memory
+    if ((r = grow_mapped(c, &pl->state_host, &pl->state_host_bytes, dev_b))) return r;
+    if ((r = rb_state_pack_enqueue(c, m, pl->fs, pl->chain, pl->state_host))) return r;
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    unsigned char *out = static_cast<unsigned char *>(buf);
+    memcpy(out + sizeof(StateHeader), pl->state_host, dev_b);
+    unsigned char *q = out + off_host;
+    memset(q, 0, total - off_host);
+    memcpy(q, &pl->t_prev, 8);
+    memcpy(q + 8, &pl->odom.rkp_last, 8);
+    StateHeader h;
+    memset(&h, 0, sizeof(h));
+    if (pl->imu) {
+        const ImuFlow &f = *pl->imu;
+        q += RB_STATE_HOST_VISION;
+        memcpy(q, static_cast<const ImuSession *>(&f), sizeof(ImuSession));
+        q += state_align8(sizeof(ImuSession));
+        const int64_t read_inx = f.live ? -1 : f.buf.read_inx, npend = pending;
+        const double t_last = f.live ? f.t_last : 0.0;
+        memcpy(q, &read_inx, 8);
+        memcpy(q + 8, &t_last, 8);
+        memcpy(q + 16, &npend, 8);
+        q += 24;
+        for (int k = 0; k < pending; k++)
+            memcpy(q + sizeof(rbimu::ImuSample) * k, &f.buf.s[(f.buf.read_inx + 1 + k) % f.buf.size], sizeof(rbimu::ImuSample));
+        if (!f.live) {
+            h.imu_count = f.samples.size();
+            h.imu_checksum = imu_samples_checksum(f);
+        }
+    }
+    memcpy(h.magic, RB_STATE_MAGIC, 8);
+    h.version = RB_STATE_VERSION;
+    h.header_bytes = sizeof(StateHeader);
+    h.total_bytes = total;
+    h.cam = c->cam;
+    h.kl_capacity = c->kcap;
+    h.mode = mode;
+    h.sigma0 = c->sigma0;
+    h.ksigma = c->ksigma;
+    h.n_pushed = pl->n_pushed;
+    h.kn = ms.kn;
+    h.det_r = m ? m->det_r : 0;
+    h.off_dev = sizeof(StateHeader);
+    h.off_host = off_host;
+    memcpy(out, &h, sizeof(h));
+    h.checksum = state_checksum(out + RB_STATE_SUMMED, total - RB_STATE_SUMMED);
+    memcpy(out, &h, sizeof(h));
+    return RB_OK;
+}
+
+extern "C" int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    int r = rb_state_check(buf, n, c->err, sizeof(c->err));
+    if (r) return r;
+    const unsigned char *b = static_cast<const unsigned char *>(buf);
+    StateHeader h;
+    memcpy(&h, b, sizeof(h));
+#define REFUSE(...)                                         \
+    do {                                                    \
+        snprintf(c->err, sizeof(c->err), __VA_ARGS__);      \
+        return RB_ERR_ARG;                                  \
+    } while (0)
+    // everything is checked before anything of the pipeline changes
+    if (memcmp(&h.cam, &c->cam, sizeof(rb_camera)) != 0 || h.sigma0 != c->sigma0 || h.ksigma != c->ksigma ||
+        h.kl_capacity != c->kcap)
+        REFUSE("load_state: the blob's camera, Sigma0, KSigma or kl_capacity are not this pipeline's");
+    const int mode = state_mode(pl);
+    if (h.mode != mode) REFUSE("load_state: a blob of mode %d, the pipeline runs mode %d", h.mode, mode);
+    if (h.det_r < 0 || h.det_r > RB_PLANE_FIT_MAX || h.off_host - h.off_dev != state_dev_bytes(h.kn))
+        REFUSE("load_state: inconsistent device section");
+    MapState ms;
+    memcpy(&ms, b + h.off_dev + state_align8(sizeof(FrameState)) + state_align8(sizeof(DetChain)), sizeof(ms));
+    if (ms.kn != h.kn) REFUSE("load_state: inconsistent keyline count");
+    const size_t host_b = n - h.off_host;
+    if (host_b < RB_STATE_HOST_VISION) REFUSE("load_state: truncated host section");
+    const unsigned char *q = b + h.off_host;
+    int64_t read_inx = -1, npend = 0;
+    double t_last = 0;
+    const unsigned char *imu_q = q + RB_STATE_HOST_VISION;
+    if (pl->imu) {
+        const ImuFlow &f = *pl->imu;
+        if (host_b < state_host_bytes(mode, 0)) REFUSE("load_state: truncated IMU section");
+        const unsigned char *t = imu_q + state_align8(sizeof(ImuSession));
+        memcpy(&read_inx, t, 8);
+        memcpy(&t_last, t + 8, 8);
+        memcpy(&npend, t + 16, 8);
+        if (!f.live) {
+            if (h.imu_count != f.samples.size() || h.imu_checksum != imu_samples_checksum(f))
+                REFUSE("load_state: the pipeline's IMU samples are not those of the blob's session");
+            if (read_inx < 0 || read_inx >= f.buf.size || npend != 0) REFUSE("load_state: inconsistent IMU ring position");
+        } else if (npend < 0 || npend > f.buf.size - 1) {
+            REFUSE("load_state: %lld samples pending, the pipeline's ring holds %d", (long long)npend, f.buf.size - 1);
+        }
+    }
+    if (host_b != state_host_bytes(mode, npend)) REFUSE("load_state: inconsistent host section");
+#undef REFUSE
+    // the device section through mapped pinned memory into the slot of the restored newest frame
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    const size_t dev_b = h.off_host - h.off_dev;
+    if ((r = grow_mapped(c, &pl->state_host, &pl->state_host_bytes, dev_b))) return r;
+    memcpy(pl->state_host, b + h.off_dev, dev_b);
+    rb_map *m = h.n_pushed > 0 ? pl->maps[(h.n_pushed - 1) % RB_NMAPS] : nullptr;
+    // the other ring maps as rb_pipeline_reset leaves them: each frame detects its own map before it reads one
+    for (int k = 0; k < RB_NMAPS; k++) {
+        RB_CUDA(cudaMemsetAsync(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int), c->stream));
+        if (pl->maps[k] != m) RB_CUDA(cudaMemsetAsync(&pl->maps[k]->st->frame_count, 0, sizeof(unsigned int), c->stream));
+        pl->abort_pin[k] = 0;
+    }
+    if ((r = rb_state_unpack_enqueue(c, m, pl->fs, pl->chain, pl->state_host, h.kn))) return r;
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    if (m) m->det_r = h.det_r;
+    pl->n_pushed = h.n_pushed;
+    pl->restored = true;
+    memcpy(&pl->t_prev, q, 8);
+    memcpy(&pl->odom.rkp_last, q + 8, 8);
+    if (pl->imu) {
+        ImuFlow &f = *pl->imu;
+        memcpy(static_cast<ImuSession *>(&f), imu_q, sizeof(ImuSession));
+        if (!f.live) {
+            f.buf.read_inx = (int)read_inx;
+        } else {   // the pending samples, oldest first, at the start of the ring
+            const unsigned char *s = imu_q + state_align8(sizeof(ImuSession)) + 24;
+            for (int k = 0; k < (int)npend; k++) memcpy(&f.samples[k], s + sizeof(rbimu::ImuSample) * k, sizeof(rbimu::ImuSample));
+            f.buf.write_inx = (int)npend;
+            f.buf.read_inx = f.buf.size - 1;
+            f.buf.n = (int)npend;
+            f.t_last = t_last;
+        }
+    }
+    // the outputs of the last push are not this session's
+    pl->mirror.n = pl->depth.n = pl->dimg.n = pl->odom.n = 0;
+    pl->last_sub = 0;
     return RB_OK;
 }
