@@ -254,6 +254,30 @@ void ref_so3_ln(const double *R, double *w) {
 }
 }  // extern "C"
 
+// ---- TooN::Cholesky<N> (Cholesky.h): x = backsub(b) and inv = get_inverse(), for the sizes the product solves ------------
+#include <TooN/Cholesky.h>
+template <int N>
+static void ref_cholesky(const double *A, const double *b, double *x, double *inv) {
+    Matrix<N, N> m;
+    Vector<N> v;
+    for (int i = 0; i < N; i++) {
+        v[i] = b[i];
+        for (int j = 0; j < N; j++) m(i, j) = A[i * N + j];
+    }
+    Cholesky<N> ch(m);
+    const Vector<N> r = ch.backsub(v);
+    const Matrix<N, N> mi = ch.get_inverse();
+    for (int i = 0; i < N; i++) {
+        x[i] = r[i];
+        for (int j = 0; j < N; j++) inv[i * N + j] = mi(i, j);
+    }
+}
+extern "C" {
+void ref_cholesky3(const double *A, const double *b, double *x, double *inv) { ref_cholesky<3>(A, b, x, inv); }
+void ref_cholesky6(const double *A, const double *b, double *x, double *inv) { ref_cholesky<6>(A, b, x, inv); }
+void ref_cholesky7(const double *A, const double *b, double *x, double *inv) { ref_cholesky<7>(A, b, x, inv); }
+}
+
 // ---- image_undistort (SURVEY.md 8(f) rank 1): reference undistort<true> on RGB24 -------------------------
 #include "VideoLib/image_undistort.h"
 extern "C" void ref_undistort_rgb(int w, int h, float ppx, float ppy, float zfx, float zfy, const double *kc,

@@ -288,6 +288,16 @@ def so3_ln(R):
     return w
 
 
+def cholesky(A, b):
+    """TooN::Cholesky<N>(A) for N = 3, 6, 7: (backsub(b), get_inverse())."""
+    A = np.ascontiguousarray(A, np.float64)
+    b = np.ascontiguousarray(b, np.float64)
+    n = len(b)
+    x, inv = np.zeros(n), np.zeros((n, n))
+    getattr(lib(), "ref_cholesky%d" % n)(_p(A), _p(b), _p(x), _p(inv))
+    return x, inv
+
+
 OUTREC = np.dtype([("t", "f8"), ("Pos", "f8", 3), ("PoseLie", "f8", 3), ("Pose", "f8", 9), ("Vel", "f8", 3),
                    ("RotLie", "f8", 3), ("dtp0", "f8"), ("dtp1", "f8"), ("K", "f8"), ("Kp", "f8"),
                    ("s_rho_p", "f8"), ("kn", "i4"), ("matches", "i4"), ("est_ok", "i4"), ("p_id", "i4"),

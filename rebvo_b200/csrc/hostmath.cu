@@ -1,24 +1,36 @@
-// hostmath.cu -- C exports of the host/device algebra in lm.cuh so that the CPU test-suite can check it
-// (SO3 exp/ln, LDL^T solve, symmetric pseudo-inverse solve) against the reference's TooN results without a GPU.
+// hostmath.cu -- C exports of the host/device algebra in lm.cuh so that the CPU test-suite can check it without a GPU
+// against the reference's TooN results and numpy: SO3 exp/ln, and the solver instances the minimiser, the IMU stages and the
+// IMU filter run (the LDL^T of lm.cuh with and without TooN's zero-pivot stop, its pivot rule, the Jacobi pseudo-inverse).
 #include "lm.cuh"
 #include "imu_filter.h"
 #include <vector>
 
+template <int N>
+static const double (&arr(const double *p))[N] { return *(const double (*)[N])p; }
+template <int N>
+static double (&arr(double *p))[N] { return *(double (*)[N])p; }
+
 extern "C" {
 void rb_hostmath_so3_exp(const double *w, double *R) { so3_exp(w, R); }
 void rb_hostmath_so3_ln(const double *R, double *w) { so3_ln_of_matrix(R, w); }
-void rb_hostmath_chol6_solve(const double *A, const double *b, double *x) {
-    Chol6 ch;
-    chol6_compute(A, &ch);
-    chol6_backsub(&ch, b, x);
+// the minimiser's solve (mc_solve): x = A^-1 b without the zero-pivot stop; piv = {smallest, largest} pivot
+void rb_hostmath_ldlt6_solve(const double *A, const double *b, double *x, double *piv) {
+    double a[36];
+    ldlt_factor<6, false>(arr<36>(A), a, piv[0], piv[1]);
+    ldlt_backsub<6>(a, arr<6>(b), arr<6>(x));
 }
-void rb_hostmath_chol6_inverse(const double *A, double *inv) {
-    Chol6 ch;
-    chol6_compute(A, &ch);
-    chol6_inverse(&ch, inv);
+// get_inverse without the zero-pivot stop (N = 3, 6, 7: the IMU filter, the IMU flow's R_Xgv) and with it (rb_bias_correct)
+void rb_hostmath_ldlt3_inverse(const double *A, double *inv) { ldlt_inverse<3, false>(arr<9>(A), arr<9>(inv)); }
+void rb_hostmath_ldlt6_inverse(const double *A, double *inv) { ldlt_inverse<6, false>(arr<36>(A), arr<36>(inv)); }
+void rb_hostmath_ldlt7_inverse(const double *A, double *inv) { ldlt_inverse<7, false>(arr<49>(A), arr<49>(inv)); }
+void rb_hostmath_ldlt6_inverse_stop(const double *A, double *inv) { ldlt_inverse<6, true>(arr<36>(A), arr<36>(inv)); }
+int rb_hostmath_ldlt_solves_like_svd(double dmin, double dmax) { return ldlt_solves_like_svd(dmin, dmax) ? 1 : 0; }
+void rb_hostmath_sym_svd_backsub6(const double *A, const double *b, double *x) {
+    sym_svd_backsub<6>(arr<36>(A), arr<6>(b), arr<6>(x));
 }
-void rb_hostmath_sym_svd_backsub(const double *A, int n, const double *b, double *x) { sym_svd_backsub(A, n, b, x); }
-void rb_hostmath_solve_sym6_like_svd(const double *A, const double *b, double *x) { solve_sym6_like_svd(A, b, x); }
+void rb_hostmath_sym_svd_backsub7(const double *A, const double *b, double *x) {
+    sym_svd_backsub<7>(arr<49>(A), arr<7>(b), arr<7>(x));
+}
 void rb_hostmath_mat3_inv(const double *A, double *B) { mat3_inv(A, B); }
 
 // IMU-mode host filter chain (imu_filter.h) for the CPU parity test against the reference's ScaleEstimator / ImuGrabber

@@ -6,7 +6,8 @@
 // This is small serial algebra (7 x 7, 11 x 11) once per frame; it stays on the host like in the reference and feeds
 // the device stages through the stage-level entry points.  The reference's function-static histories (EstAcelLsq4's
 // V..V3 / T / Dt, MeanAcel4's A..A2) live in ImuFilterHist, one per pipeline.  TooN's LAPACK-backed SVD<7> of the
-// Gauss-Newton step is replaced by a Jacobi pseudo-inverse (sym_svd_backsub, lm.cuh): the matrix is symmetric.
+// Gauss-Newton step is replaced by a Jacobi pseudo-inverse (sym_svd_backsub<7>, lm.cuh): the matrix is symmetric.  Its
+// Cholesky<3/6/7>::get_inverse calls are lm.cuh's ldlt_inverse without TooN's stop at a zero pivot (lm.cuh lists the sites).
 // Agreement with the reference: rounding level (tests/test_cpu_imu_filter.py, rel 1e-9 on the filter state).
 #pragma once
 #include <math.h>
@@ -40,92 +41,6 @@ inline double dot(const double *a, const double *b, int n) {
     double s = 0;
     for (int i = 0; i < n; i++) s += a[i] * b[i];
     return s;
-}
-// TooN::Cholesky<N>(M).get_inverse(): LDL^T without square roots (Cholesky.h), column by column
-template <int N>
-inline void chol_inverse(const double *M, double *inv) {
-    double a[N * N];
-    memcpy(a, M, sizeof(a));
-    for (int col = 0; col < N; col++) {
-        double inv_diag = 1;
-        for (int row = col; row < N; row++) {
-            double val = a[row * N + col];
-            for (int c2 = 0; c2 < col; c2++) val -= a[c2 * N + col] * a[row * N + c2];
-            if (row == col) {
-                a[row * N + col] = val;
-                inv_diag = 1 / val;
-            } else {
-                a[col * N + row] = val;
-                a[row * N + col] = val * inv_diag;
-            }
-        }
-    }
-    for (int c = 0; c < N; c++) {
-        double y[N], x[N];
-        for (int i = 0; i < N; i++) {
-            double val = i == c ? 1.0 : 0.0;
-            for (int j = 0; j < i; j++) val -= a[i * N + j] * y[j];
-            y[i] = val;
-        }
-        for (int i = 0; i < N; i++) y[i] *= 1 / a[i * N + i];
-        for (int i = N - 1; i >= 0; i--) {
-            double val = y[i];
-            for (int j = i + 1; j < N; j++) val -= a[j * N + i] * x[j];
-            x[i] = val;
-        }
-        for (int i = 0; i < N; i++) inv[i * N + c] = x[i];
-    }
-}
-// SVD<N>(A).backsub(b) for a symmetric A: cyclic Jacobi eigen-decomposition, pseudo-inverse with SVD.h's condition number 1e9
-// (the n <= 6 version lives in lm.cuh; the scale filter needs 7)
-template <int N>
-inline void sym_svd_backsub_n(const double *Ain, const double *b, double *x) {
-    double A[N * N], Q[N * N];
-    memcpy(A, Ain, sizeof(A));
-    for (int i = 0; i < N; i++)
-        for (int j = 0; j < N; j++) Q[i * N + j] = (i == j) ? 1.0 : 0.0;
-    for (int sweep = 0; sweep < 30; sweep++) {
-        double off = 0, diag = 0;
-        for (int i = 0; i < N; i++) {
-            diag += A[i * N + i] * A[i * N + i];
-            for (int j = i + 1; j < N; j++) off += A[i * N + j] * A[i * N + j];
-        }
-        if (off <= 1e-34 * diag || off == 0) break;
-        for (int p = 0; p < N - 1; p++)
-            for (int q = p + 1; q < N; q++) {
-                const double apq = A[p * N + q];
-                if (apq == 0) continue;
-                const double tau = (A[q * N + q] - A[p * N + p]) / (2 * apq);
-                const double t = (tau >= 0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1 + tau * tau));
-                const double c = 1 / sqrt(1 + t * t), sn = t * c;
-                for (int k = 0; k < N; k++) {
-                    const double akp = A[k * N + p], akq = A[k * N + q];
-                    A[k * N + p] = c * akp - sn * akq;
-                    A[k * N + q] = sn * akp + c * akq;
-                }
-                for (int k = 0; k < N; k++) {
-                    const double apk = A[p * N + k], aqk = A[q * N + k];
-                    A[p * N + k] = c * apk - sn * aqk;
-                    A[q * N + k] = sn * apk + c * aqk;
-                }
-                for (int k = 0; k < N; k++) {
-                    const double qkp = Q[k * N + p], qkq = Q[k * N + q];
-                    Q[k * N + p] = c * qkp - sn * qkq;
-                    Q[k * N + q] = sn * qkp + c * qkq;
-                }
-            }
-    }
-    double smax = 0;
-    for (int i = 0; i < N; i++) smax = fmax(smax, fabs(A[i * N + i]));
-    for (int i = 0; i < N; i++) x[i] = 0;
-    for (int k = 0; k < N; k++) {
-        const double lam = A[k * N + k];
-        if (fabs(lam) * 1e9 <= smax) continue;
-        double utb = 0;
-        for (int i = 0; i < N; i++) utb += Q[i * N + k] * b[i];
-        const double coef = utb / lam;
-        for (int i = 0; i < N; i++) x[i] += Q[i * N + k] * coef;
-    }
 }
 // TooN::SO3<>(a, b): the rotation that takes the direction of a onto the direction of b (so3.h:118-134)
 inline void so3_from_two(const double *a, const double *b, double *R) {
@@ -375,8 +290,8 @@ inline void ka_problem(double *JtJ, double *JtF, const double *x, const KaParams
     for (int i = 0; i < 9; i++) Pz[i] = sa * sa * p.Rv[i] + ca * ca * p.Rs[i];
     double P[121] = {0}, W[121] = {0}, dPda[121] = {0};
     double iPz[9], iPp[49];
-    chol_inverse<3>(Pz, iPz);
-    chol_inverse<7>(p.Pp, iPp);
+    ldlt_inverse<3, false>(Pz, iPz);
+    ldlt_inverse<7, false>(p.Pp, iPp);
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) {
             P[i * 11 + j] = Pz[i * 3 + j];
@@ -472,13 +387,13 @@ inline double est_ka_gmek_bias(const double *s_acel, const double *f_acel, doubl
         ka_problem(JtJ, JtF, X, prm);
         double rhs[7], h[7];
         for (int i = 0; i < 7; i++) rhs[i] = -JtF[i];
-        sym_svd_backsub_n<7>(JtJ, rhs, h);
+        sym_svd_backsub<7>(JtJ, rhs, h);
         for (int i = 0; i < 7; i++) X[i] += h[i];
         X[0] = atan2(sin(X[0]), cos(X[0]));   // FunT_KaGMEKBias (:205-209)
         for (int i = 4; i < 7; i++) X[i] = saturate(X[i], 5e-1 / 25);
     }
     ka_problem(JtJ, JtF, X, prm);
-    chol_inverse<7>(JtJ, P);
+    ldlt_inverse<7, false>(JtJ, *(double (*)[49])P);
     double k = tan(X[0]);
     if (k < 0 || isnan(k) || isinf(k)) k = 0;
     for (int i = 0; i < 3; i++) {
@@ -499,7 +414,7 @@ inline double est_ka_gmek_bias(const double *s_acel, const double *f_acel, doubl
     for (int i = 0; i < 3; i++) WXc[3 + i] = w3[i];
     matvec(Wvw, Xvw, rhs6, 6, 6);
     for (int i = 0; i < 6; i++) rhs6[i] += WXc[i];
-    chol_inverse<6>(Wsum, iW);
+    ldlt_inverse<6, false>(Wsum, iW);
     matvec(iW, rhs6, Xc, 6, 6);
     memcpy(Xvw, Xc, sizeof(Xc));
     return k;

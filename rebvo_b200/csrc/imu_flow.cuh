@@ -174,7 +174,7 @@ static int imu_track_frame(rb_pipeline *pl, ImuFlow &f, rb_map *neu, rb_map *old
     for (int i = 0; i < 3; i++) Vgv[i] += dVgv[i];
     memcpy(f.V, Vgv, sizeof(Vgv));
     double R_Xgv[36];
-    rbimu::chol_inverse<6>(W_Xgv, R_Xgv);                    // R_Xgv=Cholesky<6>(W_Xgv).get_inverse()
+    ldlt_inverse<6, false>(W_Xgv, R_Xgv);                    // R_Xgv=Cholesky<6>(W_Xgv).get_inverse(), no zero-pivot stop
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) {
             f.P_V[i * 3 + j] = R_Xgv[i * 6 + j];

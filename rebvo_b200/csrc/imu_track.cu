@@ -286,11 +286,13 @@ extern "C" int rb_ext_rot_vel(rb_map *m, const double vel[3], double Wx[36], dou
         }
     for (int a = 0; a < 6; a++) JtF[a] = s[21 + a];
     // SVD<> SVDpTp(JtJ); X=backsub(JtF); Rx=get_pinv(); Wx=JtJ  -- symmetric input: Jacobi eigen-decomposition
-    sym_svd_backsub(JtJ, 6, JtF, X);
+    double x6[6];
+    sym_svd_backsub<6>(JtJ, JtF, x6);
+    for (int i = 0; i < 6; i++) X[i] = x6[i];
     for (int col = 0; col < 6; col++) {
         double e[6] = {0, 0, 0, 0, 0, 0}, x[6];
         e[col] = 1;
-        sym_svd_backsub(JtJ, 6, e, x);
+        sym_svd_backsub<6>(JtJ, e, x);
         for (int row = 0; row < 6; row++) Rx[row * 6 + col] = x[row];
     }
     for (int i = 0; i < 36; i++) Wx[i] = JtJ[i];
@@ -329,10 +331,8 @@ extern "C" int rb_bias_correct(double X[6], double Wx[36], double Gb[3], double 
     mat3_mul(t, Wb, t2);
     mat3_vec(t2, Gb, v3);
     for (int i = 0; i < 3; i++) X1[3 + i] += v3[i];
-    Chol6 ch;                                           // X = Cholesky<6>(Wxb).get_inverse()*X1
-    chol6_compute(Wxb, &ch);
-    double inv[36];
-    chol6_inverse(&ch, inv);
+    double inv[36];                                     // X = Cholesky<6>(Wxb).get_inverse()*X1
+    ldlt_inverse<6, true>(Wxb, inv);                    // stops at a zero pivot, as TooN does
     for (int r = 0; r < 6; r++) {
         double s = 0;
         for (int k = 0; k < 6; k++) s += inv[r * 6 + k] * X1[k];

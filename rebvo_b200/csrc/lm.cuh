@@ -1,11 +1,12 @@
-// lm.cuh -- small dense float64 algebra used by the device-resident Levenberg-Marquardt driver and the
-// per-frame scalar logic.  __host__ __device__ so that the same code is unit-tested on the CPU
-// (tests/test_host_math.py through librebvo_b200's rb_hostmath_* exports) and runs in 1-thread kernels.
+// lm.cuh -- small dense float64 algebra used by the device-resident Levenberg-Marquardt driver, the IMU stages, the
+// IMU filter and the per-frame scalar logic.  __host__ __device__ so that the same code is unit-tested on the CPU
+// (tests/test_cpu_host.py through librebvo_b200's rb_hostmath_* exports) and runs on the device.
 //
 // Restated from the published algorithms of TooN 2.2 (third-party dependency of the reference, vendored
-// there as TooN-2.2.zip): SO3::exp / ln / coerce (so3.h), Cholesky<6> = LDL^T without square roots
-// (Cholesky.h), SVD<>::backsub / get_pinv with condition number 1e9 (SVD.h; LAPACK dgesvd_ replaced by
-// a cyclic Jacobi eigen-decomposition, valid because every matrix decomposed on this path is symmetric).
+// there as TooN-2.2.zip): SO3::exp / ln / coerce (so3.h), Cholesky<N> = LDL^T without square roots
+// (Cholesky.h; ldlt_factor / ldlt_backsub / ldlt_inverse, the only LDL^T here), SVD<>::backsub / get_pinv with
+// condition number 1e9 (SVD.h; sym_svd_backsub, the only pseudo-inverse here: LAPACK dgesvd_ replaced by a cyclic
+// Jacobi eigen-decomposition, valid because every matrix decomposed on these paths is symmetric).
 #pragma once
 #include <math.h>
 
@@ -202,161 +203,147 @@ RB_HD void odom_rel_pose(const double Rrel[9], const double V[3], const double R
         }
 }
 
-// ---- Cholesky<6> (Cholesky.h do_compute / backsub / get_inverse): L D L^T, no square roots --------------
-struct Chol6 {
-    double c[36];
-    int rank;
-};
-RB_HD void chol6_compute(const double *M, Chol6 *ch) {
-    for (int i = 0; i < 36; i++) ch->c[i] = M[i];
-    double *a = ch->c;
-    const int n = 6;
+// ---- Cholesky<N> (Cholesky.h do_compute / backsub / get_inverse): L D L^T, no square roots -------------------
+// The one LDL^T of the project: the minimiser's solve and covariance, the IMU stages and the IMU filter all run these.
+// Every index is a compile-time constant and every loop is unrolled, so that on the device the factor stays in registers.
+//
+// Known deviation: TooN's do_compute stops at the first zero pivot (rank = row) and leaves the rest of the matrix as it
+// stands.  STOP_AT_ZERO = true does the same (rb_bias_correct); the minimiser (mc_solve, lm_finalize_cov), the IMU flow's
+// R_Xgv and the IMU filter (est_ka_gmek_bias, ka_problem) run STOP_AT_ZERO = false, which keeps factoring past a zero pivot
+// with 1/0 = inf.  The two agree bit for bit wherever no pivot is zero.
+//
+// a = the factor of M (L below the diagonal, D on it, L*D above it); dmin / dmax = the smallest / largest pivot of a
+// (fmin / fmax: NaN pivots are skipped unless every pivot is NaN).
+template <int N, bool STOP_AT_ZERO>
+RB_HD void ldlt_factor(const double (&M)[N * N], double (&a)[N * N], double &dmin, double &dmax) {
 #pragma unroll
-    for (int col = 0; col < n; col++) {
+    for (int i = 0; i < N * N; i++) a[i] = M[i];
+    bool full = true;
+#pragma unroll
+    for (int col = 0; col < N && full; col++) {
         double inv_diag = 1;
 #pragma unroll
-        for (int row = col; row < n; row++) {
-            double val = a[row * 6 + col];
+        for (int row = col; row < N; row++) {
+            double val = a[row * N + col];
 #pragma unroll
-            for (int col2 = 0; col2 < col; col2++) val -= a[col2 * 6 + col] * a[row * 6 + col2];
+            for (int col2 = 0; col2 < col; col2++) val -= a[col2 * N + col] * a[row * N + col2];
             if (row == col) {
-                a[row * 6 + col] = val;
-                if (val == 0) {
-                    ch->rank = row;
-                    return;
+                a[row * N + col] = val;
+                if (STOP_AT_ZERO && val == 0) {
+                    full = false;
+                    break;
                 }
                 inv_diag = 1 / val;
             } else {
-                a[col * 6 + row] = val;
-                a[row * 6 + col] = val * inv_diag;
+                a[col * N + row] = val;
+                a[row * N + col] = val * inv_diag;
             }
         }
     }
-    ch->rank = n;
-}
-RB_HD void chol6_backsub(const Chol6 *ch, const double *v, double *x) {
-    const double *a = ch->c;
-    double y[6];
+    dmin = a[0];
+    dmax = a[0];
 #pragma unroll
-    for (int i = 0; i < 6; i++) {
+    for (int i = 1; i < N; i++) {
+        dmin = fmin(dmin, a[i * N + i]);
+        dmax = fmax(dmax, a[i * N + i]);
+    }
+}
+// x = M^-1 v from the factor a.  RECIP = false: y /= diag (TooN's vector backsub); true: y *= 1/diag (the matrix overload,
+// which get_inverse uses).
+template <int N, bool RECIP = false>
+RB_HD void ldlt_backsub(const double (&a)[N * N], const double (&v)[N], double (&x)[N]) {
+    double y[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) {
         double val = v[i];
 #pragma unroll
-        for (int j = 0; j < i; j++) val -= a[i * 6 + j] * y[j];
+        for (int j = 0; j < i; j++) val -= a[i * N + j] * y[j];
         y[i] = val;
     }
 #pragma unroll
-    for (int i = 0; i < 6; i++) y[i] /= a[i * 6 + i];
+    for (int i = 0; i < N; i++) {
+        if (RECIP) y[i] *= 1 / a[i * N + i];
+        else y[i] /= a[i * N + i];
+    }
 #pragma unroll
-    for (int i = 5; i >= 0; i--) {
+    for (int i = N - 1; i >= 0; i--) {
         double val = y[i];
 #pragma unroll
-        for (int j = i + 1; j < 6; j++) val -= a[j * 6 + i] * x[j];
+        for (int j = i + 1; j < N; j++) val -= a[j * N + i] * x[j];
         x[i] = val;
     }
 }
-// get_inverse = backsub(Identity) with the matrix overload (y[i]*=(1/diag))
-RB_HD void chol6_inverse(const Chol6 *ch, double *inv) {
-    const double *a = ch->c;
-    double y[36];
-    for (int i = 0; i < 6; i++) {
-        double val[6];
-        for (int c = 0; c < 6; c++) val[c] = (i == c) ? 1.0 : 0.0;
-        for (int j = 0; j < i; j++)
-            for (int c = 0; c < 6; c++) val[c] -= a[i * 6 + j] * y[j * 6 + c];
-        for (int c = 0; c < 6; c++) y[i * 6 + c] = val[c];
-    }
-    for (int i = 0; i < 6; i++) {
-        const double s = 1 / a[i * 6 + i];
-        for (int c = 0; c < 6; c++) y[i * 6 + c] *= s;
-    }
-    for (int i = 5; i >= 0; i--) {
-        double val[6];
-        for (int c = 0; c < 6; c++) val[c] = y[i * 6 + c];
-        for (int j = i + 1; j < 6; j++)
-            for (int c = 0; c < 6; c++) val[c] -= a[j * 6 + i] * inv[j * 6 + c];
-        for (int c = 0; c < 6; c++) inv[i * 6 + c] = val[c];
+// Cholesky<N>(M).get_inverse() = backsub(Identity): each column of the matrix overload is the backsub of a unit column
+template <int N, bool STOP_AT_ZERO>
+RB_HD void ldlt_inverse(const double (&M)[N * N], double (&inv)[N * N]) {
+    double a[N * N], dmin, dmax;
+    ldlt_factor<N, STOP_AT_ZERO>(M, a, dmin, dmax);
+#pragma unroll
+    for (int c = 0; c < N; c++) {
+        double e[N], x[N];
+#pragma unroll
+        for (int i = 0; i < N; i++) e[i] = (i == c) ? 1.0 : 0.0;
+        ldlt_backsub<N, true>(a, e, x);
+#pragma unroll
+        for (int i = 0; i < N; i++) inv[i * N + c] = x[i];
     }
 }
 
-// ---- symmetric eigen-decomposition (cyclic Jacobi) standing in for SVD<> of a symmetric matrix ----------
-// A (n x n, n <= 6, symmetric) = Q diag(lam) Q^T ; Q row-major, columns are eigenvectors
-RB_HD void sym_jacobi(const double *Ain, int n, double *lam, double *Q) {
-    double A[36];
-    for (int i = 0; i < n * n; i++) A[i] = Ain[i];
-    for (int i = 0; i < n; i++)
-        for (int j = 0; j < n; j++) Q[i * n + j] = (i == j) ? 1.0 : 0.0;
+// Whether the pivots of ldlt_factor let the LDL^T solve stand in for SVD<>::backsub: every pivot positive and the spread
+// well inside SVD.h's condition cut of 1e9.  Otherwise the Jacobi pseudo-inverse (sym_svd_backsub) solves.
+RB_HD bool ldlt_solves_like_svd(double dmin, double dmax) { return dmin > 0 && dmin * 1e7 > dmax; }
+
+// ---- SVD<>(A).backsub(b) for a symmetric A (SVD.h backsub + get_inv_diag, condition_no = 1e9) ---------------------------
+// LAPACK's dgesvd_ is replaced by a cyclic Jacobi eigen-decomposition A = Q diag(lam) Q^T (Q row-major, columns are the
+// eigenvectors): x = V diag(1/s_i or 0) U^T b with s_i = |lam_i|, u_i = sign(lam_i) q_i, v_i = q_i.
+template <int N>
+RB_HD void sym_svd_backsub(const double (&Ain)[N * N], const double (&b)[N], double (&x)[N]) {
+    double A[N * N], Q[N * N];
+    for (int i = 0; i < N * N; i++) A[i] = Ain[i];
+    for (int i = 0; i < N; i++)
+        for (int j = 0; j < N; j++) Q[i * N + j] = (i == j) ? 1.0 : 0.0;
     for (int sweep = 0; sweep < 30; sweep++) {
         double off = 0, diag = 0;
-        for (int i = 0; i < n; i++) {
-            diag += A[i * n + i] * A[i * n + i];
-            for (int j = i + 1; j < n; j++) off += A[i * n + j] * A[i * n + j];
+        for (int i = 0; i < N; i++) {
+            diag += A[i * N + i] * A[i * N + i];
+            for (int j = i + 1; j < N; j++) off += A[i * N + j] * A[i * N + j];
         }
         if (off <= 1e-34 * diag || off == 0) break;
-        for (int p = 0; p < n - 1; p++)
-            for (int q = p + 1; q < n; q++) {
-                const double apq = A[p * n + q];
+        for (int p = 0; p < N - 1; p++)
+            for (int q = p + 1; q < N; q++) {
+                const double apq = A[p * N + q];
                 if (apq == 0) continue;
-                const double app = A[p * n + p], aqq = A[q * n + q];
+                const double app = A[p * N + p], aqq = A[q * N + q];
                 const double tau = (aqq - app) / (2 * apq);
                 const double t = (tau >= 0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1 + tau * tau));
                 const double c = 1 / sqrt(1 + t * t), s = t * c;
-                for (int k = 0; k < n; k++) {  // A <- A J
-                    const double akp = A[k * n + p], akq = A[k * n + q];
-                    A[k * n + p] = c * akp - s * akq;
-                    A[k * n + q] = s * akp + c * akq;
+                for (int k = 0; k < N; k++) {  // A <- A J
+                    const double akp = A[k * N + p], akq = A[k * N + q];
+                    A[k * N + p] = c * akp - s * akq;
+                    A[k * N + q] = s * akp + c * akq;
                 }
-                for (int k = 0; k < n; k++) {  // A <- J^T A
-                    const double apk = A[p * n + k], aqk = A[q * n + k];
-                    A[p * n + k] = c * apk - s * aqk;
-                    A[q * n + k] = s * apk + c * aqk;
+                for (int k = 0; k < N; k++) {  // A <- J^T A
+                    const double apk = A[p * N + k], aqk = A[q * N + k];
+                    A[p * N + k] = c * apk - s * aqk;
+                    A[q * N + k] = s * apk + c * aqk;
                 }
-                for (int k = 0; k < n; k++) {
-                    const double qkp = Q[k * n + p], qkq = Q[k * n + q];
-                    Q[k * n + p] = c * qkp - s * qkq;
-                    Q[k * n + q] = s * qkp + c * qkq;
+                for (int k = 0; k < N; k++) {
+                    const double qkp = Q[k * N + p], qkq = Q[k * N + q];
+                    Q[k * N + p] = c * qkp - s * qkq;
+                    Q[k * N + q] = s * qkp + c * qkq;
                 }
             }
     }
-    for (int i = 0; i < n; i++) lam[i] = A[i * n + i];
-}
-
-// SVD<>(A).backsub(b) for symmetric A (SVD.h backsub + get_inv_diag, condition_no = 1e9):
-// x = V diag(1/s_i or 0) U^T b with s_i = |lam_i|, u_i = sign(lam_i) q_i, v_i = q_i
-RB_HD void sym_svd_backsub(const double *A, int n, const double *b, double *x) {
-    double lam[6], Q[36];
-    sym_jacobi(A, n, lam, Q);
     double smax = 0;
-    for (int i = 0; i < n; i++) smax = fmax(smax, fabs(lam[i]));
-    for (int i = 0; i < n; i++) x[i] = 0;
-    for (int k = 0; k < n; k++) {
-        const double s = fabs(lam[k]);
-        if (s * 1e9 <= smax) continue;  // get_inv_diag: inv_diag = 0
+    for (int i = 0; i < N; i++) smax = fmax(smax, fabs(A[i * N + i]));
+    for (int i = 0; i < N; i++) x[i] = 0;
+    for (int k = 0; k < N; k++) {
+        const double lam = A[k * N + k];
+        if (fabs(lam) * 1e9 <= smax) continue;  // get_inv_diag: inv_diag = 0
         double utb = 0;
-        for (int i = 0; i < n; i++) utb += Q[i * n + k] * b[i];
-        const double coef = utb / lam[k];  // sign(lam) * (1/s)
-        for (int i = 0; i < n; i++) x[i] += Q[i * n + k] * coef;
-    }
-}
-
-// Solve (JtJ + u I) h = rhs the way the init iterations do (SVD<> svdApI(ApI); h = backsub(-JtF),
-// global_tracker.cpp:659-661).  ApI is symmetric positive definite here (u = 1e-3 * max(JtJ) bounds the
-// condition number far below SVD.h's 1e9 cut), so the pseudo-inverse equals the inverse and the cheap
-// LDL^T solve returns the same vector up to rounding; the Jacobi path is kept for rank-deficient input.
-RB_HD void solve_sym6_like_svd(const double *ApI, const double *rhs, double *h) {
-    Chol6 ch;
-    chol6_compute(ApI, &ch);
-    bool ok = ch.rank == 6;
-    double dmax = 0, dmin = 1e300;
-    for (int i = 0; i < 6 && ok; i++) {
-        const double d = ch.c[i * 6 + i];
-        if (!(d > 0)) ok = false;
-        dmax = fmax(dmax, d);
-        dmin = fmin(dmin, d);
-    }
-    if (ok && dmin * 1e7 > dmax) {
-        chol6_backsub(&ch, rhs, h);
-    } else {
-        sym_svd_backsub(ApI, 6, rhs, h);
+        for (int i = 0; i < N; i++) utb += Q[i * N + k] * b[i];
+        const double coef = utb / lam;  // sign(lam) * (1/s)
+        for (int i = 0; i < N; i++) x[i] += Q[i * N + k] * coef;
     }
 }
 

@@ -247,13 +247,13 @@ __device__ __forceinline__ bool mc_update(McChain &c, LMState &L, double last, b
     c.v *= 2;
     return false;
 }
-// h = (JtJ + u I)^-1 (-JtF), Xnew = X + h.  Every lane gathers ApI and factors it (chol6_solve_reg, the same operations in
-// the same order), so h and Xnew need no broadcast.  The main loop solves with Cholesky<6> (:766-767), the init tries with
-// SVD<> (:659-661): ApI is SPD with a condition number far below SVD.h's 1e9 cut, so the pseudo-inverse is the inverse and
-// the LDL^T solve returns the same vector up to rounding; the Jacobi pseudo-inverse (lm_solve_fallback) is kept for
-// rank-deficient input, serial and cold.
+// h = (JtJ + u I)^-1 (-JtF), Xnew = X + h.  Every lane gathers ApI and factors it (lm.cuh's ldlt_factor / ldlt_backsub,
+// without the zero-pivot stop; the same operations in the same order), so h and Xnew need no broadcast.  The main loop
+// solves with Cholesky<6> (:766-767), the init tries with SVD<> (:659-661): where ldlt_solves_like_svd accepts the pivots,
+// ApI is SPD with a condition number far below SVD.h's 1e9 cut, so the pseudo-inverse is the inverse and the LDL^T solve
+// returns the same vector up to rounding; otherwise the Jacobi pseudo-inverse (lm_solve_fallback) solves, serial and cold.
 __device__ __forceinline__ void mc_solve(McChain &c, LMState &L, bool use_svd, int lane, double (&xn)[6]) {
-    double A[36], rhs[6], hh[6], xg[6], dmin, dmax;
+    double A[36], a[36], rhs[6], hh[6], xg[6], dmin, dmax;
     mc_gather6(c.x, xg);
 #pragma unroll
     for (int a = 0; a < 6; a++)
@@ -268,8 +268,9 @@ __device__ __forceinline__ void mc_solve(McChain &c, LMState &L, bool use_svd, i
         A[i * 6 + i] = A[i * 6 + i] + c.u;  // ApI = JtJ + Identity*u
         rhs[i] = -__shfl_sync(MC_FULL, c.acc, 21 + i);
     }
-    chol6_solve_reg(A, rhs, hh, dmin, dmax);
-    if (use_svd && !(dmin > 0 && dmin * 1e7 > dmax)) {   // (uniform) rank-deficient ApI: SVD<> pseudo-inverse semantics
+    ldlt_factor<6, false>(A, a, dmin, dmax);
+    ldlt_backsub<6>(a, rhs, hh);
+    if (use_svd && !ldlt_solves_like_svd(dmin, dmax)) {   // (uniform) rank-deficient ApI: SVD<> pseudo-inverse semantics
         if (lane < 21) {
             const int a = mc_up_row(lane), b = mc_up_col(lane, a);
             L.JtJ[a * 6 + b] = c.acc;

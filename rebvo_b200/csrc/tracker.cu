@@ -224,65 +224,10 @@ __device__ void lm_build_api(const LMState &s, double *A, double *rhs) {
         rhs[i] = -s.JtF[i];
     }
 }
-// Cholesky<6>(ApI).backsub(rhs) with every index known at compile time, so that the factor lives in registers (the
-// generic chol6_* of lm.cuh share their arrays with the Jacobi fallback and end up in local memory, which made this
-// serial step the longest part of an evaluation).  Same operations in the same order as TooN's do_compute/backsub;
-// returns the smallest / largest pivot for the conditioning test of the SVD-replacement path.
-template <bool RECIP_SCALE = false>   // true: y *= 1/diag (TooN's matrix backsub, used by get_inverse); false: y /= diag
-__device__ __forceinline__ void chol6_solve_reg(const double (&M)[36], const double (&v)[6], double (&x)[6],
-                                                double &dmin, double &dmax) {
-    double a[36];
-#pragma unroll
-    for (int i = 0; i < 36; i++) a[i] = M[i];
-#pragma unroll
-    for (int col = 0; col < 6; col++) {
-        double inv_diag = 1;
-#pragma unroll
-        for (int row = col; row < 6; row++) {
-            double val = a[row * 6 + col];
-#pragma unroll
-            for (int col2 = 0; col2 < col; col2++) val -= a[col2 * 6 + col] * a[row * 6 + col2];
-            if (row == col) {
-                a[row * 6 + col] = val;
-                inv_diag = 1 / val;
-            } else {
-                a[col * 6 + row] = val;
-                a[row * 6 + col] = val * inv_diag;
-            }
-        }
-    }
-    dmin = a[0];
-    dmax = a[0];
-#pragma unroll
-    for (int i = 1; i < 6; i++) {
-        dmin = fmin(dmin, a[i * 6 + i]);
-        dmax = fmax(dmax, a[i * 6 + i]);
-    }
-    double y[6];
-#pragma unroll
-    for (int i = 0; i < 6; i++) {
-        double val = v[i];
-#pragma unroll
-        for (int j = 0; j < i; j++) val -= a[i * 6 + j] * y[j];
-        y[i] = val;
-    }
-#pragma unroll
-    for (int i = 0; i < 6; i++) {
-        if (RECIP_SCALE) y[i] *= 1 / a[i * 6 + i];
-        else y[i] /= a[i * 6 + i];
-    }
-#pragma unroll
-    for (int i = 5; i >= 0; i--) {
-        double val = y[i];
-#pragma unroll
-        for (int j = i + 1; j < 6; j++) val -= a[j * 6 + i] * x[j];
-        x[i] = val;
-    }
-}
 __device__ __noinline__ void lm_solve_fallback(LMState &s) {   // rank-deficient ApI: SVD<> pseudo-inverse semantics
     double A[36], rhs[6], h[6];
     lm_build_api(s, A, rhs);
-    sym_svd_backsub(A, 6, rhs, h);
+    sym_svd_backsub<6>(A, rhs, h);
     for (int i = 0; i < 6; i++) s.h[i] = h[i];
 }
 __device__ void lm_request(LMState &s, const double *X, int res_in, int res_out) {
@@ -291,15 +236,17 @@ __device__ void lm_request(LMState &s, const double *X, int res_in, int res_out)
     s.res_out = res_out;
 }
 // RRV = Cholesky<6>(JtJ).get_inverse() (:795-801): column c = backsub(e_c) with the matrix overload's y *= 1/diag.
-// Threads 0..5 of the calling block each factorise (registers) and solve one column.
+// Threads 0..5 of the calling block each factorise (registers) and solve one column; like the minimiser's solve, the
+// factor does not stop at a zero pivot (lm.cuh).
 __device__ __forceinline__ void lm_finalize_cov(LMState &s, int tid) {
     if (tid < 6) {
-        double A[36], ec[6], x[6], dmin, dmax;
+        double A[36], a[36], ec[6], x[6], dmin, dmax;
 #pragma unroll
         for (int i = 0; i < 36; i++) A[i] = s.JtJ[i];
 #pragma unroll
         for (int i = 0; i < 6; i++) ec[i] = (i == tid) ? 1.0 : 0.0;
-        chol6_solve_reg<true>(A, ec, x, dmin, dmax);
+        ldlt_factor<6, false>(A, a, dmin, dmax);
+        ldlt_backsub<6, true>(a, ec, x);
         if (tid < 3) {
 #pragma unroll
             for (int i = 0; i < 3; i++) s.RVel[i * 3 + tid] = x[i];

@@ -68,33 +68,103 @@ def test_so3_against_reference_toon(built):
             assert np.allclose(refapi.so3_ln(Rr), back, atol=1e-13)
 
 
+def _ldlt(L, A, b):
+    """The minimiser's LDL^T solve (no zero-pivot stop): x, (smallest, largest pivot)."""
+    x, piv = np.zeros(6), np.zeros(2)
+    L.rb_hostmath_ldlt6_solve(_p(np.ascontiguousarray(A)), _p(np.ascontiguousarray(b)), _p(x), _p(piv))
+    return x, piv
+
+
+def _inverse(L, A, stop=False):
+    """get_inverse of the LDL^T: without the zero-pivot stop at N = 3, 6, 7, with it at N = 6."""
+    A = np.ascontiguousarray(A, np.float64)
+    inv = np.zeros_like(A)
+    getattr(L, "rb_hostmath_ldlt6_inverse_stop" if stop else "rb_hostmath_ldlt%d_inverse" % len(A))(_p(A), _p(inv))
+    return inv
+
+
+def _pinv_solve(L, A, b):
+    x = np.zeros(len(b))
+    getattr(L, "rb_hostmath_sym_svd_backsub%d" % len(b))(_p(np.ascontiguousarray(A)), _p(np.ascontiguousarray(b)), _p(x))
+    return x
+
+
+def _solves_like_svd(L, dmin, dmax):
+    return bool(L.rb_hostmath_ldlt_solves_like_svd(C.c_double(dmin), C.c_double(dmax)))
+
+
+def _ldl_product(rng, n, zero_at):
+    """L D L^T with small-integer unit-lower L and D[zero_at] = 0: exact in float64, so the factor meets an exact zero pivot."""
+    Lm = np.tril(rng.integers(-2, 3, size=(n, n)), -1) + np.eye(n)
+    d = rng.integers(1, 5, size=n).astype(np.float64)
+    d[zero_at] = 0
+    return (Lm * d) @ Lm.T
+
+
 def test_ldlt_and_pinv_solvers(built):
+    """The solver instances the minimiser, the IMU stages and the IMU filter run (lm.cuh): against numpy, and bit for bit
+    against the reference's own TooN::Cholesky<N> where oracle/_ref is built."""
     from rebvo_b200 import capi
+    from oracle import refapi
     L = capi.lib()
+    toon = refapi.available()
     rng = np.random.default_rng(1)
     for _ in range(20):
         J = rng.normal(size=(40, 6)) * rng.uniform(0.1, 100, 6)
         A = J.T @ J
         A = A + np.eye(6) * 1e-3 * A.max()
         b = rng.normal(size=6)
-        x = np.zeros(6)
-        L.rb_hostmath_chol6_solve(_p(A), _p(b), _p(x))
+        x, piv = _ldlt(L, A, b)
         assert np.allclose(x, np.linalg.solve(A, b), rtol=1e-9)
-        L.rb_hostmath_solve_sym6_like_svd(_p(A), _p(b), _p(x))
-        assert np.allclose(x, np.linalg.solve(A, b), rtol=1e-9)
-        L.rb_hostmath_sym_svd_backsub(_p(A), 6, _p(b), _p(x))
+        assert _solves_like_svd(L, *piv)   # the init tries take the LDL^T solve on an SPD ApI
+        x = _pinv_solve(L, A, b)
         assert np.allclose(x, np.linalg.pinv(A, rcond=1e-9) @ b, rtol=1e-8)
-        inv = np.zeros((6, 6))
-        L.rb_hostmath_chol6_inverse(_p(A), _p(inv))
-        assert np.allclose(inv, np.linalg.inv(A), rtol=1e-8)
-    # rank deficient: pseudo-inverse semantics of SVD<>::backsub (condition 1e9)
-    J = rng.normal(size=(40, 6))
-    J[:, 5] = J[:, 0]
-    A = J.T @ J
-    b = A @ rng.normal(size=6)
-    x = np.zeros(6)
-    L.rb_hostmath_sym_svd_backsub(_p(A), 6, _p(b), _p(x))
-    assert np.allclose(x, np.linalg.pinv(A, rcond=1e-9) @ b, rtol=1e-6, atol=1e-9)
+        assert np.allclose(_inverse(L, A), np.linalg.inv(A), rtol=1e-8)
+    # SPD at every size the product factors, condition numbers 1 .. 1e12: both variants equal TooN bit for bit
+    for n in (3, 6, 7):
+        for cond in (1.0, 1e3, 1e6, 1e9, 1e12):
+            Q = np.linalg.qr(rng.normal(size=(n, n)))[0]
+            A = (Q * np.logspace(0, -np.log10(cond), n)) @ Q.T
+            A = np.ascontiguousarray((A + A.T) / 2)
+            b = rng.normal(size=n)
+            inv = _inverse(L, A)
+            if n == 6:
+                assert np.array_equal(_inverse(L, A, stop=True), inv)
+            if toon:
+                xt, invt = refapi.cholesky(A, b)
+                assert np.array_equal(inv, invt), (n, cond)
+                if n == 6:
+                    assert np.array_equal(_ldlt(L, A, b)[0], xt), cond
+    # zero pivots: the stopping variant (rb_bias_correct) is TooN's; the minimiser's rule sends the factor to Jacobi
+    b = rng.normal(size=6)
+    zero_lead = np.zeros((6, 6))   # a BiasCorrect without matches: only the gyro prior's 3x3 block is non-zero
+    zero_lead[3:, 3:] = np.eye(3) * 1e4 + 1e2
+    zero_pivots = [np.zeros((6, 6)), zero_lead] + [_ldl_product(rng, 6, p) for p in range(1, 6)]
+    for A in zero_pivots:
+        with np.errstate(all="ignore"):
+            _, piv = _ldlt(L, A, b)
+        assert not _solves_like_svd(L, *piv)
+        if toon:
+            assert np.array_equal(_inverse(L, A, stop=True), refapi.cholesky(A, b)[1], equal_nan=True)
+    # the rule itself, on pivots: NaN and zero are refused; fmin / fmax skip NaN pivots unless every pivot is NaN
+    assert not _solves_like_svd(L, np.nan, 1.0) and not _solves_like_svd(L, 1.0, np.nan)
+    assert not _solves_like_svd(L, 0.0, 1.0) and not _solves_like_svd(L, 1e-8, 1.0)
+    assert _solves_like_svd(L, 1e-6, 1.0)
+    A = np.eye(6)
+    A[5, 5] = np.nan
+    assert _solves_like_svd(L, *_ldlt(L, A, b)[1])
+    A[0, 0] = np.nan
+    assert np.isnan(_ldlt(L, A, b)[1][0]) and not _solves_like_svd(L, *_ldlt(L, A, b)[1])
+    # rank deficient: pseudo-inverse semantics of SVD<>::backsub (condition 1e9), at both sizes the product solves
+    for n in (6, 7):
+        J = rng.normal(size=(40, n))
+        A = J.T @ J
+        b = rng.normal(size=n)
+        assert np.allclose(_pinv_solve(L, A, b), np.linalg.pinv(A, rcond=1e-9) @ b, rtol=1e-8)
+        J[:, n - 1] = J[:, 0]
+        A = J.T @ J
+        b = A @ rng.normal(size=n)
+        assert np.allclose(_pinv_solve(L, A, b), np.linalg.pinv(A, rcond=1e-9) @ b, rtol=1e-6, atol=1e-9)
     M = rng.normal(size=(3, 3)) + 3 * np.eye(3)
     Mi = np.zeros((3, 3))
     L.rb_hostmath_mat3_inv(_p(M), _p(Mi))
