@@ -19,11 +19,13 @@ void rb_hostmath_ldlt6_solve(const double *A, const double *b, double *x, double
     ldlt_factor<6, false>(arr<36>(A), a, piv[0], piv[1]);
     ldlt_backsub<6>(a, arr<6>(b), arr<6>(x));
 }
-// get_inverse without the zero-pivot stop (N = 3, 6, 7: the IMU filter, the IMU flow's R_Xgv) and with it (rb_bias_correct)
+// get_inverse without the zero-pivot stop and with it (TooN's: every get_inverse site of the product), N = 3, 6, 7
 void rb_hostmath_ldlt3_inverse(const double *A, double *inv) { ldlt_inverse<3, false>(arr<9>(A), arr<9>(inv)); }
 void rb_hostmath_ldlt6_inverse(const double *A, double *inv) { ldlt_inverse<6, false>(arr<36>(A), arr<36>(inv)); }
 void rb_hostmath_ldlt7_inverse(const double *A, double *inv) { ldlt_inverse<7, false>(arr<49>(A), arr<49>(inv)); }
+void rb_hostmath_ldlt3_inverse_stop(const double *A, double *inv) { ldlt_inverse<3, true>(arr<9>(A), arr<9>(inv)); }
 void rb_hostmath_ldlt6_inverse_stop(const double *A, double *inv) { ldlt_inverse<6, true>(arr<36>(A), arr<36>(inv)); }
+void rb_hostmath_ldlt7_inverse_stop(const double *A, double *inv) { ldlt_inverse<7, true>(arr<49>(A), arr<49>(inv)); }
 int rb_hostmath_ldlt_solves_like_svd(double dmin, double dmax) { return ldlt_solves_like_svd(dmin, dmax) ? 1 : 0; }
 void rb_hostmath_sym_svd_backsub6(const double *A, const double *b, double *x) {
     sym_svd_backsub<6>(arr<36>(A), arr<6>(b), arr<6>(x));

@@ -7,7 +7,8 @@
 // the device stages through the stage-level entry points.  The reference's function-static histories (EstAcelLsq4's
 // V..V3 / T / Dt, MeanAcel4's A..A2) live in ImuFilterHist, one per pipeline.  TooN's LAPACK-backed SVD<7> of the
 // Gauss-Newton step is replaced by a Jacobi pseudo-inverse (sym_svd_backsub<7>, lm.cuh): the matrix is symmetric.  Its
-// Cholesky<3/6/7>::get_inverse calls are lm.cuh's ldlt_inverse without TooN's stop at a zero pivot (lm.cuh lists the sites).
+// Cholesky<3/6/7>::get_inverse calls are lm.cuh's ldlt_inverse; the bias-corrected Xvw's stops at a zero pivot as TooN's
+// does (lm.cuh says why the others need not).
 // Agreement with the reference: rounding level (tests/test_cpu_imu_filter.py, rel 1e-9 on the filter state).
 #pragma once
 #include <math.h>
@@ -290,7 +291,7 @@ inline void ka_problem(double *JtJ, double *JtF, const double *x, const KaParams
     for (int i = 0; i < 9; i++) Pz[i] = sa * sa * p.Rv[i] + ca * ca * p.Rs[i];
     double P[121] = {0}, W[121] = {0}, dPda[121] = {0};
     double iPz[9], iPp[49];
-    ldlt_inverse<3, false>(Pz, iPz);
+    ldlt_inverse<3, false>(Pz, iPz);   // a zero pivot here makes W, and so JtJ, NaN either way
     ldlt_inverse<7, false>(p.Pp, iPp);
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) {
@@ -393,7 +394,7 @@ inline double est_ka_gmek_bias(const double *s_acel, const double *f_acel, doubl
         for (int i = 4; i < 7; i++) X[i] = saturate(X[i], 5e-1 / 25);
     }
     ka_problem(JtJ, JtF, X, prm);
-    ldlt_inverse<7, false>(JtJ, *(double (*)[49])P);
+    ldlt_inverse<7, false>(JtJ, *(double (*)[49])P);   // J^T W J, J of full rank: no zero pivot
     double k = tan(X[0]);
     if (k < 0 || isnan(k) || isinf(k)) k = 0;
     for (int i = 0; i < 3; i++) {
@@ -414,7 +415,7 @@ inline double est_ka_gmek_bias(const double *s_acel, const double *f_acel, doubl
     for (int i = 0; i < 3; i++) WXc[3 + i] = w3[i];
     matvec(Wvw, Xvw, rhs6, 6, 6);
     for (int i = 0; i < 6; i++) rhs6[i] += WXc[i];
-    ldlt_inverse<6, false>(Wsum, iW);
+    ldlt_inverse<6, true>(Wsum, iW);   // a frame without forward matches: zero velocity block
     matvec(iW, rhs6, Xc, 6, 6);
     memcpy(Xvw, Xc, sizeof(Xc));
     return k;

@@ -207,10 +207,14 @@ RB_HD void odom_rel_pose(const double Rrel[9], const double V[3], const double R
 // The one LDL^T of the project: the minimiser's solve and covariance, the IMU stages and the IMU filter all run these.
 // Every index is a compile-time constant and every loop is unrolled, so that on the device the factor stays in registers.
 //
-// Known deviation: TooN's do_compute stops at the first zero pivot (rank = row) and leaves the rest of the matrix as it
-// stands.  STOP_AT_ZERO = true does the same (rb_bias_correct); the minimiser (mc_solve, lm_finalize_cov), the IMU flow's
-// R_Xgv and the IMU filter (est_ka_gmek_bias, ka_problem) run STOP_AT_ZERO = false, which keeps factoring past a zero pivot
-// with 1/0 = inf.  The two agree bit for bit wherever no pivot is zero.
+// TooN's do_compute stops at the first zero pivot (rank = row) and leaves the rest of the matrix as it stands, and
+// get_inverse back-substitutes through that partial factor: the rows after the pivot keep finite entries.
+// STOP_AT_ZERO = true does the same; rb_bias_correct, lm_finalize_cov, the IMU flow's R_Xgv and est_ka_gmek_bias's
+// bias-corrected Xvw run it (tests/test_cpu_zero_pivot.py, tests/test_gpu_zero_pivot.py).  STOP_AT_ZERO = false keeps
+// factoring with 1/0 = inf, which turns those entries into NaN.  It runs where the difference cannot reach an output:
+// the minimiser's solve (mc_solve: LM steps add u > 0, the init tries send a zero pivot to the Jacobi pseudo-inverse),
+// ka_problem's iPz / iPp (a zero pivot there leaves the filter all NaN in the reference too) and est_ka_gmek_bias's P
+// (J^T W J with J of full rank).  The two agree bit for bit wherever no pivot is zero.
 //
 // a = the factor of M (L below the diagonal, D on it, L*D above it); dmin / dmax = the smallest / largest pivot of a
 // (fmin / fmax: NaN pivots are skipped unless every pivot is NaN).

@@ -236,8 +236,9 @@ __device__ void lm_request(LMState &s, const double *X, int res_in, int res_out)
     s.res_out = res_out;
 }
 // RRV = Cholesky<6>(JtJ).get_inverse() (:795-801): column c = backsub(e_c) with the matrix overload's y *= 1/diag.
-// Threads 0..5 of the calling block each factorise (registers) and solve one column; like the minimiser's solve, the
-// factor does not stop at a zero pivot (lm.cuh).
+// Threads 0..5 of the calling block each factorise (registers) and solve one column.  Unlike the minimiser's solve, the
+// factor stops at a zero pivot as TooN's does: a map whose keylines leave a Jacobian column exactly zero (all gated, or
+// every edge vertical or horizontal) reaches one, and the reference's RRV keeps finite entries there.
 __device__ __forceinline__ void lm_finalize_cov(LMState &s, int tid) {
     if (tid < 6) {
         double A[36], a[36], ec[6], x[6], dmin, dmax;
@@ -245,7 +246,7 @@ __device__ __forceinline__ void lm_finalize_cov(LMState &s, int tid) {
         for (int i = 0; i < 36; i++) A[i] = s.JtJ[i];
 #pragma unroll
         for (int i = 0; i < 6; i++) ec[i] = (i == tid) ? 1.0 : 0.0;
-        ldlt_factor<6, false>(A, a, dmin, dmax);
+        ldlt_factor<6, true>(A, a, dmin, dmax);
         ldlt_backsub<6, true>(a, ec, x);
         if (tid < 3) {
 #pragma unroll
@@ -699,7 +700,10 @@ static bool mc_prepare(K kern, int threads, int clusters, size_t dyn, int dev_ma
     if (cudaFuncGetAttributes(&fa, kern) != cudaSuccess) return false;
     if (dyn + fa.sharedSizeBytes > (size_t)dev_max) return false;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) return false;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess) return false;
+    // the limit is the kernel's, shared by every context of the process: set it to the most any context can ask for, so
+    // that a context created later with a smaller slice (capacity, REBVO_B200_MIN_KPC) does not lower it under this one's
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dev_max - (int)fa.sharedSizeBytes) != cudaSuccess)
+        return false;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(MC_C * clusters);
     cfg.blockDim = dim3(threads);
