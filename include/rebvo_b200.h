@@ -218,6 +218,34 @@ int rb_minimizer_rv(rb_map *fmap, rb_map *old, double V[3], double W[3], double 
                     double match_thresh, int iter_max, int init_type, double reweight_distance,
                     double *rel_error, double *rel_error_score, double max_s_rho,
                     uint32_t match_num_thresh, int init_iter, double W_X[36], double *score);
+/* rb_minimizer_rv as the per-frame pipeline runs it, followed by FordwardMatch of old into fmap: fmap's arg-max scratch
+ * cleared, the minimiser with a scratch frame state (so that its last evaluation offers every old keyline to the
+ * arg-max), then FordwardMatch's apply.  On return fmap is what Minimizer_RV followed by FordwardMatch leaves; the other
+ * outputs are rb_minimizer_rv's.  *fwd_nmatch counts distinct matched new keylines, as rb_forward_match's. */
+int rb_minimizer_rv_forward(rb_map *fmap, rb_map *old, double V[3], double W[3], double RVel[9], double RW0[9],
+                            double match_thresh, int iter_max, int init_type, double reweight_distance,
+                            double *rel_error, double *rel_error_score, double max_s_rho,
+                            uint32_t match_num_thresh, int init_iter, double W_X[36], double *score,
+                            int *fwd_nmatch);
+/* What the per-frame map chain leaves besides the two maps (rb_map_match_update) */
+typedef struct rb_match_update_out {
+    int32_t nmatch;     /* directed_matching hits */
+    int32_t fwd_match;  /* distinct new keylines with a FordwardMatch winner */
+    int32_t reg_num;    /* keylines Regularize_1_iter smoothed */
+    int32_t do_map, est_ok, klm_num;   /* the match-count gate (rebvo_second_t.cpp:410-423) */
+    double V[3], Kp, P_Kp, P_V[9];      /* after the gate; Kp and P_Kp enter as 0 */
+    double Pose[9], Pos[3];             /* Pose = Pose*BackRot, Pos += -Pose*V*K (:545-551) */
+    double RotLie[3], PoseLie[3];       /* SO3(BackRot).ln(), SO3(Pose).ln() */
+} rb_match_update_out;
+/* The per-frame map chain of the pipeline on loaded maps: FordwardMatch of old's m_id_f into neu, directed_matching
+ * (edge_tracker.cpp:302-374) of neu against old rotated by R0 (rotate_keylines), the match-count gate
+ * (do_match && nmatch >= match_threshold), Regularize_1_iter and the EKF when the gate is open, old rotated by R0 in
+ * place, and the frame's pose integration.  V / P_V are the minimiser's outputs before directed_matching's
+ * back-rotation by BackRot.  Pose_io / Pos_io are updated in place; neu's counters start at 0. */
+int rb_map_match_update(rb_map *neu, rb_map *old, const double V[3], const double P_V[9], const double BackRot[9],
+                        const double R0[9], int do_match, double min_thr_mod, double min_thr_ang, double max_radius,
+                        double loc_uncertainty_match, int match_threshold, double reg_thresh, double reshape_q_abs,
+                        double loc_uncertainty, double Pose_io[9], double Pos_io[3], double K, rb_match_update_out *out);
 /* edge_tracker::FordwardMatch (edge_tracker.cpp:380-436): old -> new along m_id_f.  The keyline contents follow the
  * reference's sequential rule (arg-max rho, ties -> largest index) bit for bit.  *nmatch counts DISTINCT matched new
  * keylines; the reference's return value also counts the writes that a later old keyline overwrites (its nmatch++ runs

@@ -70,6 +70,11 @@ ODOM = np.dtype([("relPosPose", "f8", 6), ("WrelPosPose", "f8", (6, 6)), ("AcelM
 # one record of the pose graph file (pose_graph::saveToFile): ODOM without `tracked`, unpadded
 PS_REC = np.dtype([(n, ODOM.fields[n][0]) for n in ODOM.names if n != "tracked"])
 
+# rb_match_update_out: what the per-frame map chain leaves besides the two maps (rb_map_match_update)
+MATCH_UPDATE_OUT = np.dtype([("nmatch", "i4"), ("fwd_match", "i4"), ("reg_num", "i4"), ("do_map", "i4"), ("est_ok", "i4"),
+                             ("klm_num", "i4"), ("V", "f8", 3), ("Kp", "f8"), ("P_Kp", "f8"), ("P_V", "f8", (3, 3)),
+                             ("Pose", "f8", (3, 3)), ("Pos", "f8", 3), ("RotLie", "f8", 3), ("PoseLie", "f8", 3)])
+
 # rb_depth_cell: one cell of the viewer's depth grid (depth_filler's df_point rho, s_rho, dist, fixed)
 DEPTH_CELL = np.dtype([("rho", "f8"), ("s_rho", "f8"), ("dist", "f8"), ("fixed", "i4"), ("_pad", "i4")])
 
@@ -105,9 +110,9 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_map_dog_build", "rb_map_get_plane", "rb_map_detect", "rb_map_detect_ss", "rb_map_reestimate_thresh", "rb_map_knum",
            "rb_map_counters",
            "rb_map_sync_host_keylines", "rb_map_load_keylines", "rb_map_get_mask", "rb_map_quantile",
-           "rb_map_build_field", "rb_map_get_field", "rb_try_vel_rot", "rb_minimizer_rv", "rb_forward_match",
+           "rb_map_build_field", "rb_map_get_field", "rb_try_vel_rot", "rb_minimizer_rv", "rb_minimizer_rv_forward", "rb_forward_match",
            "rb_map_rotate_keylines", "rb_directed_matching", "rb_map_regularize", "rb_map_ekf_update",
-           "rb_map_rescale_opt", "rb_map_set_frame_count", "rb_pipeline_create", "rb_pipeline_destroy",
+           "rb_map_rescale_opt", "rb_map_set_frame_count", "rb_map_match_update", "rb_pipeline_create", "rb_pipeline_destroy",
            "rb_pipeline_last_error", "rb_pipeline_push", "rb_pipeline_push_dev", "rb_pipeline_push_mono",
            "rb_pipeline_push_mono_dev", "rb_pipeline_reset",
            "rb_pipeline_map", "rb_pipeline_launch_count", "rb_pipeline_stage_ms", "rb_pipeline_stream",
@@ -540,6 +545,37 @@ class Map:
                                               C.byref(e1), C.byref(e2), C.c_double(max_s_rho),
                                               C.c_uint32(match_num_thresh), int(init_iter), _p(WX), C.byref(sc)))
         return dict(F=sc.value, V=V, W=W, RVel=RV, RW0=RW, W_X=WX, rel_err=e1.value, rel_err_score=e2.value)
+
+    def minimizer_rv_forward(self, old, V, W, match_thresh, iter_max, init_type, reweight, max_s_rho, match_num_thresh,
+                             init_iter):
+        """minimizer_rv as the per-frame pipeline runs it, then FordwardMatch of old into this map; the result also
+        holds fwd_match, the distinct new keylines matched"""
+        V, W = np.array(V, np.float64), np.array(W, np.float64)
+        RV, RW, WX = np.zeros((3, 3)), np.zeros((3, 3)), np.zeros((6, 6))
+        e1, e2, sc, n = C.c_double(0), C.c_double(0), C.c_double(0), C.c_int(0)
+        self.ctx.check(self.L.rb_minimizer_rv_forward(self.h_, old.h_, _p(V), _p(W), _p(RV), _p(RW),
+                                                      C.c_double(match_thresh), iter_max, init_type, C.c_double(reweight),
+                                                      C.byref(e1), C.byref(e2), C.c_double(max_s_rho),
+                                                      C.c_uint32(match_num_thresh), int(init_iter), _p(WX), C.byref(sc),
+                                                      C.byref(n)))
+        return dict(F=sc.value, V=V, W=W, RVel=RV, RW0=RW, W_X=WX, rel_err=e1.value, rel_err_score=e2.value,
+                    fwd_match=n.value)
+
+    def match_update(self, old, V, P_V, BackRot, R0, do_match, thr_mod, thr_ang, max_radius, loc_unc_match,
+                     match_threshold, reg_thresh, q_abs, loc_unc, Pose, Pos, K):
+        """The pipeline's map chain on this map (new) and old: FordwardMatch along old's m_id_f, directed_matching
+        against old rotated by R0, the match-count gate, Regularize_1_iter, the EKF, old rotated in place, and the pose
+        integration from (Pose, Pos).  Returns one MATCH_UPDATE_OUT record."""
+        a = [np.ascontiguousarray(v, np.float64) for v in (V, P_V, BackRot, R0)]
+        Pose = np.array(Pose, np.float64)
+        Pos = np.array(Pos, np.float64)
+        out = np.zeros(1, MATCH_UPDATE_OUT)
+        self.ctx.check(self.L.rb_map_match_update(self.h_, old.h_, *[_p(v) for v in a], int(do_match),
+                                                  C.c_double(thr_mod), C.c_double(thr_ang), C.c_double(max_radius),
+                                                  C.c_double(loc_unc_match), int(match_threshold), C.c_double(reg_thresh),
+                                                  C.c_double(q_abs), C.c_double(loc_unc), _p(Pose), _p(Pos),
+                                                  C.c_double(K), _p(out)))
+        return out[0]
 
     def try_vel(self, old, V, match_thresh, s_rho_min, match_num_thresh, residuals, rw_dist, min_mod):
         V = np.array(V, np.float64)

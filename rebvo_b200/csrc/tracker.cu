@@ -977,7 +977,7 @@ int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu) {
     RB_LAUNCH_CHECK();
     return RB_OK;
 }
-static int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
+int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu) {
     RB_KLAUNCH(k_fm_argmax, rb_div_up(c->kcap, 256), 256, 0, old->kl, (const MapState *)old->st,
                (const MapState *)neu->st, neu->ts_host.fm_best);
     return RB_OK;

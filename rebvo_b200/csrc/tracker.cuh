@@ -58,6 +58,7 @@ int rb_build_field_enqueue(rb_ctx *c, rb_map *m, int radius, float min_mod, bool
 // FordwardMatch = init (clears neu's arg-max scratch) -> arg-max (m_id_f of old) -> apply (copies each winner into neu);
 // rb_forward_match_enqueue is the whole stage.
 int rb_forward_match_init_enqueue(rb_ctx *c, rb_map *neu);
+int rb_forward_match_argmax_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_forward_match_apply_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_forward_match_enqueue(rb_ctx *c, rb_map *old, rb_map *neu);
 int rb_rotate_enqueue(rb_ctx *c, rb_map *m, const double *R_dev);

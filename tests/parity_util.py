@@ -125,14 +125,14 @@ def _bits(a):
 
 def _diff(tag, ref, got):
     """'' if ref and got are equal bit for bit (NaN == NaN), else a short description of the first mismatches."""
-    ref, got = np.asarray(ref), np.asarray(got)
+    ref, got = np.atleast_1d(ref), np.atleast_1d(got)
     if ref.shape != got.shape:
         return "%s: shape %s vs %s" % (tag, ref.shape, got.shape)
     same = _bits(ref) == _bits(got)
     if ref.dtype.kind == "f":
         same |= np.isnan(ref) & np.isnan(got)
     if same.ndim > 1:
-        same = same.reshape(len(same), -1).all(1)
+        same = same.reshape(len(same), -1).all(1) if len(same) else np.ones(0, bool)
     bad = np.nonzero(~same)[0]
     if not len(bad):
         return ""
@@ -268,3 +268,187 @@ def tracker_parity(rep, cfg, refs, gm, rt):
     rep.close("Minimizer_RV rel_err_score", m_r["rel_err_score"], m_g["rel_err_score"], 1e-8)
     rep.exact("Minimizer_RV m_id_f", old_r.keylines()["m_id_f"], old_g.keylines()["m_id_f"])
     return m_r
+
+
+# ---- rotations for SO3<>(M).ln(): every branch of so3.h:288-334 -------------------------------------------------------
+def rot(axis, deg):
+    """the rotation by deg degrees about coordinate axis 0, 1 or 2"""
+    a = np.deg2rad(deg)
+    c, s = np.cos(a), np.sin(a)
+    i, j = [(1, 2), (2, 0), (0, 1)][axis]
+    R = np.eye(3)
+    R[i, i], R[i, j], R[j, i], R[j, j] = c, -s, s, c
+    return R
+
+
+def rodrigues(w):
+    w = np.asarray(w, np.float64)
+    t = np.linalg.norm(w)
+    if t == 0:
+        return np.eye(3)
+    k = w / t
+    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(t) * Kx + (1 - np.cos(t)) * Kx @ Kx
+
+
+def so3_ln_cases():
+    """name -> matrix: cos(angle) above sqrt(1/2), between +-sqrt(1/2), below -sqrt(1/2) with the largest diagonal
+    term d0, d1 or d2 (the three sub-branches) and with the axis against r2 (the sign flip), the identity, and matrices
+    that are not orthonormal (coerce)."""
+    rng = np.random.default_rng(12)
+    out = {"identity": np.eye(3), "small": rodrigues([0.02, -0.01, 0.03]), "cos_above": rodrigues([0.3, -0.4, 0.2]),
+           "cos_between": rodrigues([0.9, 1.1, -0.6]), "cos_between_90": rot(0, 90.0)}
+    for ax in range(3):
+        w = np.full(3, 0.15)
+        w[ax] = 2.8
+        out["cos_below_d%d" % ax] = rodrigues(w)
+        out["cos_below_d%d_flip" % ax] = rodrigues(-w)
+    out["cos_below_179.9"] = rodrigues(np.deg2rad(179.9) * np.array([0.6, -0.64, 0.48]))
+    for k, name in enumerate(("above", "between", "below")):
+        w = rng.normal(0, 1, 3)
+        w *= [0.4, 1.5, 2.9][k] / np.linalg.norm(w)
+        out["coerce_" + name] = rodrigues(w) + rng.normal(0, 2e-3, (3, 3))
+    return out
+
+
+
+def so3_ln_branch(R):
+    """(branch, sub-branch, flip) of SO3<>(M).ln() for M = R, from the lines of so3.h:288-334 on the coerced matrix"""
+    m = R.copy()
+    for i in range(3):   # Gram-Schmidt on the rows, as coerce
+        for j in range(i):
+            m[i] -= m[j] * (m[j] @ m[i])
+        m[i] /= np.sqrt(m[i] @ m[i])
+    c = (np.trace(m) - 1) / 2
+    if c > np.sqrt(0.5):
+        return "above", None, False
+    if c > -np.sqrt(0.5):
+        return "between", None, False
+    d = (np.diag(m) - c) ** 2
+    sub = 0 if d[0] > d[1] and d[0] > d[2] else 1 if d[1] > d[2] else 2
+    out = np.array([m[2, 1] - m[1, 2], m[0, 2] - m[2, 0], m[1, 0] - m[0, 1]]) / 2
+    r2 = np.array([[np.diag(m)[0] - c, (m[1, 0] + m[0, 1]) / 2, (m[0, 2] + m[2, 0]) / 2],
+                   [(m[1, 0] + m[0, 1]) / 2, np.diag(m)[1] - c, (m[2, 1] + m[1, 2]) / 2],
+                   [(m[0, 2] + m[2, 0]) / 2, (m[2, 1] + m[1, 2]) / 2, np.diag(m)[2] - c]])[sub]
+    return "below", sub, bool(r2 @ out < 0)
+
+
+# ---- the mapper stages' seeded cases (tests/test_gpu_mapper_states.py, tests/test_gpu_map_chain_states.py) ------------
+MIN_HITS = 50          # keylines (or tie groups, bins ...) a case must put on its target branch
+
+
+def _compare(kl_r, kl_g, fields, matched_fields=()):
+    """Bitwise comparison of keyline fields; matched_fields only where the reference has m_id >= 0."""
+    out = []
+    if len(kl_r) != len(kl_g):
+        return ["kn %d vs %d" % (len(kl_r), len(kl_g))]
+    for f in fields:
+        out.append(_diff(f, kl_r[f], kl_g[f]))
+    mk = kl_r["m_id"] >= 0
+    for f in matched_fields:
+        out.append(_diff(f + " (matched)", kl_r[f][mk], kl_g[f][mk]))
+    return [o for o in out if o]
+
+
+def _cut(kl, mask, k):
+    """The first k keylines of a detected map and its mask without the others (a map cut at kl_max = k)."""
+    m = mask.copy()
+    m[m >= k] = -1
+    return kl[:k].copy(), m
+
+
+def _search_setup(bench, kl_new, V, BackRot, max_radius, loc_unc):
+    """NumPy restatement of search_match's set-up lines (edge_tracker.cpp:179-229): branch, search window and t_steps of
+    every new keyline.  float64 like the reference, the projected point rounded to float as Point2DF does."""
+    zf = bench.zfm
+    Vb = BackRot @ np.asarray(V, np.float64)
+    pm = kl_new["p_m"].astype(np.float64)
+    p3 = np.stack([pm[:, 0], pm[:, 1], np.full(len(pm), zf)], 1) @ BackRot.T
+    pmx = (p3[:, 0] * zf / p3[:, 2]).astype(np.float32).astype(np.float64)
+    pmy = (p3[:, 1] * zf / p3[:, 2]).astype(np.float32).astype(np.float64)
+    k_rho = kl_new["rho"] * zf / p3[:, 2]
+    ks = kl_new["s_rho"]
+    t_x = -(Vb[0] * zf - Vb[2] * pmx)
+    t_y = -(Vb[1] * zf - Vb[2] * pmy)
+    norm_t = np.sqrt(t_x * t_x + t_y * t_y)
+    perp = ~(norm_t > 1e-6)
+    with np.errstate(all="ignore"):
+        dq_rho = norm_t * k_rho
+        dq_min = np.maximum(0.0, norm_t * (k_rho - ks)) - loc_unc
+        dq_max_raw = norm_t * (k_rho + ks)
+        dq_max = np.minimum(max_radius, dq_max_raw) + loc_unc
+        mid = ~perp & (dq_rho > dq_max)
+        dq_c = np.where(mid, (dq_max + dq_min) / 2, dq_rho)
+        span = np.where(mid, dq_c, np.maximum(dq_max - dq_rho, dq_rho - dq_min))
+        t_steps = np.floor(span + 0.5).astype(np.int64)
+        t_steps[perp] = int(max_radius + loc_unc)
+        # direction of the probes (perpendicular search: the gradient)
+        ux = np.where(perp, kl_new["m_m"][:, 0] / kl_new["n_m"], t_x / np.where(perp, 1.0, norm_t))
+        uy = np.where(perp, kl_new["m_m"][:, 1] / kl_new["n_m"], t_y / np.where(perp, 1.0, norm_t))
+        lo = np.where(perp, -(max_radius + loc_unc), dq_min)
+        hi = np.where(perp, max_radius + loc_unc, dq_max)
+    x0, y0 = pmx + bench.cam["ppx"], pmy + bench.cam["ppy"]
+    ends = [(x0 + ux * lo, y0 + uy * lo), (x0 + ux * hi, y0 + uy * hi)]
+    w, h = bench.cam["w"], bench.cam["h"]
+    edges = np.zeros((len(pm), 4), bool)   # a probe of the window lies left / right / above / below the image
+    for ex, ey in ends:
+        edges |= np.stack([ex < -0.5, ex >= w - 0.5, ey < -0.5, ey >= h - 0.5], 1)
+    edges &= (t_steps > 0)[:, None]
+    return dict(perp=perp, mid=mid, normal=~perp & ~mid, t_steps=t_steps,
+                cut=~perp & (dq_max_raw > max_radius), edges=edges)
+
+
+V_TYP = np.array([0.004, -0.003, 0.0005])
+RV_SPD = np.array([[2e-4, 5e-5, -3e-5], [5e-5, 1e-4, 2e-5], [-3e-5, 2e-5, 4e-4]])
+DM_BASE = dict(V=V_TYP, RVel=np.eye(3) * 1e-4, BackRot=np.eye(3), thr_mod=1.0, thr_ang=45.0, radius=40.0, loc_unc=2.0)
+# name -> (overrides of DM_BASE, {branch: least keyline count})
+DM_CASES = {
+    "V0": (dict(V=np.zeros(3), RVel=np.zeros((3, 3))), {"perp": -1}),
+    "V1e-9": (dict(V=np.array([1e-9, 0, 0])), {"perp": -1}),
+    "V0_loc0.5": (dict(V=np.zeros(3), loc_unc=0.5), {"perp": -1}),
+    "V0_radius12.5_loc0": (dict(V=np.zeros(3), radius=12.5, loc_unc=0.0), {"perp": -1}),
+    "Vz": (dict(V=np.array([0, 0, 0.02])), {"mid": MIN_HITS, "normal": MIN_HITS}),
+    "fast": (dict(V=np.array([0.06, -0.05, 0.03]), RVel=RV_SPD), {"mid": MIN_HITS, "cut": MIN_HITS}),
+    "fast_radius12.5": (dict(V=np.array([-0.04, 0.07, -0.02]), radius=12.5, loc_unc=0.5), {"mid": MIN_HITS, "cut": MIN_HITS}),
+    "typ_radius12.5_loc0": (dict(radius=12.5, loc_unc=0.0), {"normal": MIN_HITS, "cut": MIN_HITS}),
+    "loc0": (dict(loc_unc=0.0), {"normal": MIN_HITS}),
+    "loc0.5": (dict(loc_unc=0.5), {"normal": MIN_HITS}),
+    "loc5": (dict(loc_unc=5.0), {"normal": MIN_HITS}),
+    "RVel0": (dict(RVel=np.zeros((3, 3))), {"normal": MIN_HITS}),
+    "RVel_spd": (dict(RVel=RV_SPD), {"normal": MIN_HITS}),
+    "rot_x3": (dict(BackRot=rot(0, 3.0)), {"normal": MIN_HITS}),
+    "rot_y3": (dict(BackRot=rot(1, -3.0)), {"normal": MIN_HITS}),
+    "rot_z3": (dict(BackRot=rot(2, 3.0)), {"normal": MIN_HITS}),
+    "rot_y25": (dict(BackRot=rot(1, 25.0)), {"normal": MIN_HITS}),
+    "rot_y-25": (dict(BackRot=rot(1, -25.0), V=V_TYP[[1, 0, 2]]), {"normal": MIN_HITS}),
+    "ang10_mod0.1": (dict(thr_ang=10.0, thr_mod=0.1), {"normal": MIN_HITS}),
+    "ang90_mod10": (dict(thr_ang=90.0, thr_mod=10.0), {"normal": MIN_HITS}),
+    "ang45_mod10": (dict(thr_mod=10.0, V=np.zeros(3)), {"perp": -1}),
+    "tsteps0to8": (dict(V=np.array([0.0015, 0.001, 0.0]), loc_unc=0.0), {"tsteps": MIN_HITS}),
+}
+
+
+def _reg_gates(kl, thresh):
+    """NumPy restatement of Regularize_1_iter's two gates (edge_tracker.cpp:98-118) for keylines with both neighbours."""
+    ni, pi = kl["n_id"], kl["p_id"]
+    nb = (ni >= 0) & (pi >= 0)
+    n, p = ni[nb], pi[nb]
+    d = kl["rho"][n] - kl["rho"][p]
+    g1 = ~(d * d > kl["s_rho"][n] ** 2 + kl["s_rho"][p] ** 2)
+    mm = kl["m_m"]
+    alpha = ((mm[n, 0] * mm[p, 0] + mm[n, 1] * mm[p, 1]) / (kl["n_m"][n] * kl["n_m"][p])).astype(np.float64)
+    g2 = ~(alpha - thresh < 0)
+    return nb.sum(), g1, g2
+
+
+
+EKF_CASES = {   # name -> (vel, q_abs, loc_unc, fraction of matched keylines set to rho = 1)
+    "vel0": (np.zeros(3), 1e-4, 1.0, 0.0),                       # H = 0
+    "vel0_loc0": (np.zeros(3), 1e-4, 0.0, 0.0),                  # H = 0 and S = 0: K = NaN
+    "typical": (np.array([0.004, -0.003, 0.0005]), 1e-4, 1.0, 0.0),
+    "typical_q0_loc0": (np.array([0.004, -0.003, 0.0005]), 0.0, 0.0, 0.0),
+    "vz-1": (np.array([0.003, 0.002, -1.0]), 1e-4, 1.0, 0.3),     # rho = 1: rho_p = inf
+    "vz+0.5": (np.array([0.01, -0.004, 0.5]), 1e-4, 1.0, 0.0),
+    "vz+0.5_q0": (np.array([0.01, -0.004, 0.5]), 0.0, 1.0, 0.0),
+    "vz-0.06": (np.array([0.002, 0.001, -0.06]), 1e-4, 1.0, 0.0),   # rho > ~9: rho_p beyond RHO_MAX or negative
+}

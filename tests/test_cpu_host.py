@@ -68,6 +68,30 @@ def test_so3_against_reference_toon(built):
             assert np.allclose(refapi.so3_ln(Rr), back, atol=1e-13)
 
 
+def test_so3_ln_bitwise_against_reference_toon(built):
+    """rb_hostmath_so3_ln (the device's so3_ln_of_matrix, compiled for the host) is TooN's SO3<>(M).ln() bit for bit
+    on matrices in every branch: cos(angle) above sqrt(1/2), between, below with each of the three diagonal
+    sub-branches and the sign flip, and matrices that coerce must re-orthonormalise"""
+    from rebvo_b200 import capi
+    from oracle import refapi
+    from parity_util import so3_ln_branch, so3_ln_cases
+    if not refapi.available():
+        pytest.skip("the compiled reference is not available")
+    L = capi.lib()
+    seen, bad = set(), []
+    for name, R in so3_ln_cases().items():
+        R = np.ascontiguousarray(R)
+        w = np.zeros(3)
+        L.rb_hostmath_so3_ln(_p(R), _p(w))
+        w_ref = refapi.so3_ln(R)
+        if not np.array_equal(w.view(np.uint64), w_ref.view(np.uint64)):
+            bad.append("%s: %r vs TooN %r" % (name, w.tolist(), w_ref.tolist()))
+        seen.add(so3_ln_branch(R))
+    assert not bad, "\n".join(bad)
+    want = {("above", None, False), ("between", None, False)} | {("below", s, f) for s in range(3) for f in (False, True)}
+    assert want <= seen, want - seen
+
+
 def _ldlt(L, A, b):
     """The minimiser's LDL^T solve (no zero-pivot stop): x, (smallest, largest pivot)."""
     x, piv = np.zeros(6), np.zeros(2)

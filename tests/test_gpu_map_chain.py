@@ -3,7 +3,12 @@ old map) and k_reg_ekf (gate + Regularize_1_iter + EKF + rotate_keylines of the 
 (REBVO_B200_MAP_CHAIN=0): the stage kernels in the reference's order, k_fm_apply -> k_rotate -> k_directed_match -> gate ->
 k_regularize_a / k_regularize_b -> k_ekf, the kernels that test_gpu_parity.py and test_gpu_mapper_states.py pin to the
 reference bit for bit.  Both must give the same bits: raw nav records, the keylines and masks of the two newest maps, and
-per frame the FordwardMatch winners, directed hits and regularised keylines."""
+per frame the FordwardMatch winners, directed hits and regularised keylines.
+
+This stream makes few decisions near a threshold.  The same kernels are pinned to the reference bit for bit on seeded
+states that reach every branch by test_gpu_map_chain_states.py (k_match and k_reg_ekf, through rb_map_match_update) and
+test_gpu_minimiser_forms.py (FordwardMatch's arg-max folded into the minimiser's last round, through
+rb_minimizer_rv_forward)."""
 import numpy as np
 import pytest
 

@@ -13,7 +13,10 @@ sub-pixel jitter up to any K0 <= KEYLINE_MAX, with the depth, gate and gradient 
 are empty, partial, full and one past full, the s_rho and m_num gates (m_num beyond the kernel's 8-bit flag), runs of
 misses whose stale residual (DResidualNew[ikl] = fi of the last match, global_tracker.cpp:341,406) crosses every
 virtual-warp, slice, cluster, column and block boundary, projections on the image border, every LM schedule, degenerate
-maps, two minimisations on one new map, and schedules of more than 32 rounds.  Every case also runs a NumPy restatement of the LM driver
+maps, two minimisations on one new map, and schedules of more than 32 rounds.  Its last call also runs as the per-frame
+pipeline runs it (rb_minimizer_rv_forward: FordwardMatch's arg-max folded into the last round, then the apply), and the new
+map must be the reference's Minimizer_RV + FordwardMatch and rb_minimizer_rv + rb_forward_match bit for bit; fold_ties
+puts tie groups across slices, clusters and the spilled range, and slice ends on every step shape of the fold's loop.  Every case also runs a NumPy restatement of the LM driver
 (global_tracker.cpp:598-817) on the reference's own TryVelRot: it must agree with the reference, and its trace proves that
 the case reached its target (a vacuous case fails) and that no LM decision sits on a knife edge.
 
@@ -23,7 +26,9 @@ before it."""
 import numpy as np
 import pytest
 
-from parity_util import DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG, Bench, Report, parity_frames, tracker_parity
+from parity_util import (DOG_THRESH, EUROC_CFG, PLANE_FIT, POS_NEG, Bench, Report, _diff, parity_frames,
+                         tracker_parity)
+from parity_util import _compare as _compare_kl
 
 pytestmark = pytest.mark.gpu
 
@@ -250,6 +255,8 @@ def _state_old(name, sp, kl10, ppxy, wh):
             kl["p_m"][sel[4 + a], 1] = np.float32(tgt[a] + 0.2 * rng.choice([-1, 1], n) - ppxy[1])
             kl["rho"][sel[4 + a]] = 1.0
         ev["border"] = n
+    elif kind == "ties":
+        kl["rho"] = kl["rho"][np.arange(K0) % len(kl10)]
     elif kind == "all_skipped":
         kl["s_rho"] = 10.0 * sp["q"]
     elif kind == "five":
@@ -298,6 +305,9 @@ STATES["ns33"] = dict(K0=8000, init_iter=2, iter_max=26, prior="near", fc=0, wan
 STATES["ns49"] = dict(K0=8000, init_iter=0, iter_max=46, prior="near", fc=0, calls=["main", "main"], want=["ns49"])
 STATES["K0_then_gate"] = dict(K0=8000, fc=2, mnt=3, m_num=_mn2, calls=["empty", "main"], want=["empty"])
 STATES["back_to_back"] = dict(K0=8000, fc=2, mnt=3, m_num=_mn2, calls=["main", "main"], want=["gate_change"])
+# FordwardMatch's arg-max folded into the last round: every tile copy of a keyline has its rho, so that copies that land on
+# one new keyline tie, with their offers in different slices, clusters and spilled ranges
+STATES["fold_ties"] = dict(K0=50000, kind="ties", fc=0, init_iter=1, iter_max=3, want=["ties"])
 STATES["all_skipped"] = dict(K0=3000, kind="all_skipped", fc=0, want=["degenerate"])
 STATES["five_usable"] = dict(K0=3000, kind="five", fc=0, want=["degenerate"])
 
@@ -472,6 +482,12 @@ class Base:
             m = new.minimizer_rv(o, V, W, sp["mt"], sp["iter_max"], sp["init_type"], sp["k_huber"], sp["q"], sp["mnt"],
                                  sp["init_iter"])
             runs.append(dict(old=c, ref=m, drv=drv, tr=tr, m_id_f=o.keylines()["m_id_f"].copy() if c != "empty" else None))
+        # the last call followed by FordwardMatch, into a map of frame 11's keylines as detected
+        fwd = self.refmap()
+        fwd.set_keylines(self.kl11)
+        fwd.set_mask(self.mask11, len(self.kl11))
+        (empty_old if runs[-1]["old"] == "empty" else old).forward_match(fwd)
+        runs[-1]["fwd"] = fwd.keylines()
         st = dict(sp=sp, kl=kl, ev=ev, V=V, W=W, runs=runs)
         self.cache[name] = st
         return st
@@ -582,12 +598,54 @@ def _evidence(st, form):
                 msgs.append("gate change touches %d keylines" % n2)
             if w == "empty" and runs[0]["tr"]["evals"]:
                 msgs.append("the empty map was evaluated")
+        elif w == "ties":
+            msgs += _fold_reach(st, form, info)
         elif w == "degenerate":
             usable = int((st["kl"]["s_rho"] <= sp["q"]).sum())
             info["usable"] = usable
             if usable >= 6:
                 msgs.append("%d usable keylines" % usable)
     return msgs, info
+
+
+def _fold_reach(st, form, info):
+    """FordwardMatch's arg-max in the last round: each thread offers the keylines li and li + T - 96 of its slice per step
+    (li = tid - 96, tid - 96 + 2 (T - 96), ...).  The slices of the forms together must be empty, end in a step without a
+    second keyline and in one with it, and hold a full step; every form must have MIN_HITS tie groups (equal largest rho
+    on one new keyline) with offers in different slices, and in different clusters and in the spilled range where it has
+    them."""
+    K0 = st["sp"]["K0"]
+    ends = set()
+    for f in FORMS:
+        g = _geometry(f, K0)
+        stp = g["T"] - 96
+        for s in range(16 * g["G"]):
+            cnt = min(max(K0 - s * g["kpc"], 0), g["kpc"])
+            r = cnt % (2 * stp)
+            ends |= {"empty"} if cnt == 0 else set()
+            ends |= {"second -1" if 0 < r <= stp else "second" if r else "whole"}
+            ends |= {"full step"} if cnt >= 2 * stp else set()
+    msgs = [] if {"empty", "second -1", "second", "full step"} <= ends else ["slice ends %s" % sorted(ends)]
+    geo = _geometry(form, K0)
+    kl, f = st["kl"], st["runs"][-1]["m_id_f"]
+    idx = np.nonzero(f >= 0)[0]
+    key = np.lexsort((-kl["rho"][idx], f[idx]))   # by target, the largest rho first
+    idx = idx[key]
+    tgt, rho = f[idx], kl["rho"][idx]
+    first = np.r_[True, tgt[1:] != tgt[:-1]]
+    top = rho == np.maximum.reduceat(rho, np.nonzero(first)[0])[np.cumsum(first) - 1]
+    cnt = dict(slices=0, clusters=0, spill=0)
+    for t in np.unique(tgt[top]):
+        o = idx[top & (tgt == t)]
+        if len(o) < 2:
+            continue
+        sl = o // geo["kpc"]
+        cnt["slices"] += len(set(sl)) > 1
+        cnt["clusters"] += len(set(sl % geo["G"])) > 1
+        cnt["spill"] += bool(((o - sl * geo["kpc"]) >= geo["S"]).any())
+    need = ["slices"] + (["clusters"] if geo["G"] > 1 else []) + (["spill"] if geo["kpc"] > geo["S"] else [])
+    info.update(tie_groups=cnt, slice_ends=sorted(ends))
+    return msgs + ["%d tie groups across %s" % (cnt[k], k) for k in need if cnt[k] < MIN_HITS]
 
 
 def _carried(geo, evals, K0, k_huber):
@@ -655,13 +713,17 @@ def test_minimiser_state(base, monkeypatch, state, form):
 
     ctx = _ctx(base, form)
     assert ctx.minimizer_clusters() == CLUSTERS[form]
-    new, old, empty = ctx.new_map(), ctx.new_map(), ctx.new_map()
+    # newf repeats the calls on new, the last one as the per-frame pipeline runs it: FordwardMatch's arg-max folded into
+    # its last round, then the apply (rb_minimizer_rv_forward); fwd gets rb_forward_match after the last call on new
+    new, old, empty, newf, fwd = [ctx.new_map() for _ in range(5)]
     try:
-        new.load_keylines(base.kl11, base.mask11)
-        new.build_field(CFG["radius"], base.rt)
+        for m in (new, newf, fwd):
+            m.load_keylines(base.kl11, base.mask11)
+        for m in (new, newf):
+            m.build_field(CFG["radius"], base.rt)
+            m.set_frame_count(sp["fc"])
         old.load_keylines(st["kl"], base.empty)
         empty.load_keylines(st["kl"][:0], base.empty)
-        new.set_frame_count(sp["fc"])
         for k, run in enumerate(st["runs"]):
             o = empty if run["old"] == "empty" else old
             n0 = ctx.launches()
@@ -682,8 +744,25 @@ def test_minimiser_state(base, monkeypatch, state, form):
                 msgs.append("call %d: m_id_f differs at %d keylines" % (k, int((run["m_id_f"] != mf).sum())))
             if launches > 2:
                 msgs.append("%d launches for %d evaluations" % (launches, len(run["tr"]["evals"])))
+        o = empty if st["runs"][-1]["old"] == "empty" else old
+        args = (st["V"], st["W"], sp["mt"], sp["iter_max"], sp["init_type"], sp["k_huber"], sp["q"], sp["mnt"], sp["init_iter"])
+        for run in st["runs"][:-1]:
+            newf.minimizer_rv(empty if run["old"] == "empty" else old, *args)
+        m_f = newf.minimizer_rv_forward(o, *args)
+        n_s = o.forward_match(fwd)
+        for f in ("V", "W", "F", "RVel", "RW0", "W_X"):
+            if _diff(f, m_g[f], m_f[f]):
+                msgs.append("with the fold: " + _diff(f, m_g[f], m_f[f]))
+        r, g, s_ = st["runs"][-1]["fwd"], newf.keylines(), fwd.keylines()
+        fields, matched = ["rho", "s_rho", "m_id", "m_num", "p_m_0"], ["m_m0", "n_m0"]
+        msgs += ["FordwardMatch vs the reference: " + e for e in _compare_kl(r, g, fields, matched)]
+        msgs += ["fold vs rb_forward_match: " + e for e in _compare_kl(s_, g, fields, matched)]
+        n_r = int((r["m_id"] >= 0).sum())
+        if not m_f["fwd_match"] == n_s == n_r:
+            msgs.append("FordwardMatch count: fold %d, stage %d, reference keylines %d" % (m_f["fwd_match"], n_s, n_r))
+        print("%s / %s: FordwardMatch matched %d new keylines" % (state, form, n_r))
     finally:
-        for m in (new, old, empty):
+        for m in (new, old, empty, newf, fwd):
             m.close()
     assert not msgs, "\n".join(msgs)
 
