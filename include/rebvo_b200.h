@@ -348,6 +348,48 @@ enum { RB_FRAME_RGB24 = 0, RB_FRAME_MONO8 = 1 };
 int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out);
 int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                 rb_nav *nav_out);
+/* Asynchronous pushes: a live caller (a camera driver thread, a ROS image callback) hands over frames without waiting for
+ * them to be tracked, and keeps up to `depth` pushes in flight, as the reference's FirstThr detects frame i+1 while its
+ * SecondThread tracks frame i.  Each enqueued push (a ticket) has the records and outputs the synchronous push of the same
+ * frames would have given, byte for byte; only when they are ready differs.  See DESIGN.md §5 for how a ticket runs.
+ *
+ * rb_pipeline_set_async(pl, depth): how many tickets may be outstanding, 1..8, or 0 (off, the default).  It allocates, at
+ *   this call and never in an enqueue, an output ring of `depth` slots (nav, odometry, mirror, depth grid and depth image of
+ *   max_batch frames each, in host or device memory as rb_pipeline_set_output_memory says; the set_* calls that switch an
+ *   output on or enlarge it grow the slots too) and a second scale-space workspace of max_batch frames.  depth = 0 frees the
+ *   ring; the synchronous pushes never use it and launch what they launched before.  RB_ERR_ARG in IMU mode and for a depth
+ *   outside 0..8; RB_ERR_STATE while tickets are outstanding.
+ * rb_pipeline_enqueue(pl, format, on_device, data, ts, n, &ticket): n packed frames of RB_FRAME_RGB24 or RB_FRAME_MONO8, in
+ *   host (on_device = 0) or device memory, with the checks of rb_pipeline_push / push_mono / push_dev / push_mono_dev.
+ *   rb_pipeline_enqueue_frames: n strided frames, with the checks of rb_pipeline_push_frames(_dev).  Both return once the
+ *   work is enqueued; *ticket receives its number (0, 1, 2, ... for the pipeline's lifetime).  The frames (and the data the
+ *   rb_frame entries point to) must stay valid and unchanged until that ticket is waited.  Device frames must be complete
+ *   when the call is made: the copy and the scale space run on a stream of their own, ordered after nothing the caller
+ *   enqueued.  Host frames in pageable memory may make the call wait for the copy; pinned memory does not.  RB_ERR_STATE,
+ *   changing nothing, when `depth` tickets are outstanding; RB_ERR_ARG when asynchronous pushes are off or in IMU mode.
+ * rb_pipeline_wait(pl, ticket, nav_out): blocks until the ticket is complete and retires it with every earlier ticket, in
+ *   order, doing for each what a synchronous push does on the host after its work (odometry QK, the first frame's record, the
+ *   minimiser abort check).  nav_out (may be NULL) receives the ticket's n records.  From then until the next wait or push,
+ *   rb_pipeline_odometry, rb_pipeline_mirror(_dev), rb_pipeline_depth(_dev) and rb_pipeline_depth_image(_dev) return the
+ *   ticket's outputs; they stay valid until the enqueue that reuses the ticket's slot (ticket + depth), or the next push or
+ *   set_* call.  RB_ERR_CUDA when a minimiser of a ticket it retired aborted (as a push reports it); RB_ERR_ARG for a
+ *   ticket never issued or already retired.
+ * rb_pipeline_poll(pl, &newest): without blocking, the newest ticket whose work is complete, retired or not (-1 if none).
+ *
+ * While tickets are outstanding the synchronous pushes, rb_pipeline_reset, rb_pipeline_save_state / load_state, every set_*
+ * call (rb_pipeline_set_async, set_consumer_stream and set_imu among them), rb_pipeline_batch_plane, rb_pipeline_stage_ms
+ * and rb_pipeline_bench_pass return RB_ERR_STATE and change nothing; with none outstanding they behave as before.
+ * rb_pipeline_batch_plane has no planes to show after an enqueue, and rb_pipeline_stage_ms describes the last synchronous
+ * push.  In device output mode, each enqueue first makes the tracker stream wait for the work enqueued so far on the
+ * consumer stream (rb_pipeline_set_consumer_stream), which covers whatever still reads the slot it is about to overwrite.
+ * The calls of one pipeline are made from one thread at a time, as its pushes are. */
+int rb_pipeline_set_async(rb_pipeline *pl, int depth);
+int rb_pipeline_enqueue(rb_pipeline *pl, int format, int on_device, const uint8_t *data, const double *ts, int n,
+                        int64_t *ticket);
+int rb_pipeline_enqueue_frames(rb_pipeline *pl, int format, int on_device, const rb_frame *frames, const double *ts, int n,
+                               int64_t *ticket);
+int rb_pipeline_wait(rb_pipeline *pl, int64_t ticket, rb_nav *nav_out);
+int rb_pipeline_poll(rb_pipeline *pl, int64_t *newest_complete);
 /* REBVO::Reset (rebvo_second_t.cpp:609-620) */
 int rb_pipeline_reset(rb_pipeline *pl);
 /* newest / previous edge map of the ring (valid until the next push) */

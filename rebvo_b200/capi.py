@@ -126,7 +126,18 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_set_depth_image", "rb_pipeline_depth_image", "rb_pipeline_set_output_memory",
            "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev",
            "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev", "rb_pipeline_batch_plane", "rb_pipeline_save_state",
-           "rb_pipeline_load_state", "rb_state_info"]
+           "rb_pipeline_load_state", "rb_state_info", "rb_pipeline_set_async", "rb_pipeline_enqueue",
+           "rb_pipeline_enqueue_frames", "rb_pipeline_wait", "rb_pipeline_poll"]
+
+# ctypes prototypes of the asynchronous pushes (their tickets are int64_t, which ctypes' default conversion would cut to int)
+PROTOTYPES = {
+    "rb_pipeline_set_async": (C.c_int, [C.c_void_p, C.c_int]),
+    "rb_pipeline_enqueue": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64)]),
+    "rb_pipeline_enqueue_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                             C.POINTER(C.c_int64)]),
+    "rb_pipeline_wait": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "rb_pipeline_poll": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
+}
 
 _lib = None
 
@@ -286,6 +297,9 @@ def lib():
         L.rb_pipeline_launch_count.restype = C.c_int64
         L.rb_pipeline_map.restype = C.c_void_p
         L.rb_pipeline_stream.restype = C.c_void_p
+        for name, (res, args) in PROTOTYPES.items():
+            getattr(L, name).restype = res
+            getattr(L, name).argtypes = args
         _lib = L
     return _lib
 
@@ -774,6 +788,83 @@ class Pipeline:
         self.check(self.L.rb_pipeline_push_dev(self.h_, C.c_void_p(int(dev_ptr)), _p(ts), len(ts), _p(nav)))
         return nav
 
+    def set_async(self, depth):
+        """Asynchronous pushes (enqueue, wait, poll): up to `depth` (1..8) tickets in flight, 0 = off (the default).  Between
+        pushes, with no ticket outstanding; allocates the output ring and a second scale-space workspace."""
+        self.check(self.L.rb_pipeline_set_async(self.h_, int(depth)))
+
+    def _enqueue_args(self, frames, ts, fmt):
+        """(C function, argument tuple, objects to keep alive) of an enqueue; ValueError for anything the library would
+        refuse for its format or shape."""
+        if fmt not in ("rgb", "mono"):
+            raise ValueError("enqueue: fmt 'rgb' or 'mono', not %r" % (fmt,))
+        n = len(ts)
+        if not 1 <= n <= self.max_batch:
+            raise ValueError("enqueue: %d timestamps, the pipeline takes 1..%d frames" % (n, self.max_batch))
+        want = FRAME_MONO8 if fmt == "mono" else FRAME_RGB24
+        if isinstance(frames, (list, tuple)):
+            f, on_dev, table = frame_table(frames, self.w, self.h)
+            if f != want:
+                raise ValueError("enqueue: %s frames with fmt=%r" % ("mono8" if f == FRAME_MONO8 else "RGB24", fmt))
+            if len(table) != n:
+                raise ValueError("enqueue: %d frames, %d timestamps" % (len(table), n))
+            fr = np.array(table, FRAME)
+            return self.L.rb_pipeline_enqueue_frames, (want, int(on_dev), _p(fr)), (frames, fr), on_dev
+        shape = (n, self.h, self.w) + (() if fmt == "mono" else (3,))
+        on_dev, got, strides, u8, base = _array_layout(frames)
+        if not u8 or tuple(got) != shape:
+            raise ValueError("enqueue: packed %s frames are uint8 %s, not %s %s"
+                             % (fmt, shape, getattr(frames, "dtype", "?"), tuple(got)))
+        packed = tuple(int(np.prod(shape[k + 1:], dtype=np.int64)) for k in range(len(shape)))
+        if tuple(strides) != packed:
+            if on_dev:
+                raise ValueError("enqueue: device frames must be packed (contiguous); pass a list of frames for strided ones")
+            frames = np.ascontiguousarray(frames)
+            base = frames.__array_interface__["data"][0]
+        return self.L.rb_pipeline_enqueue, (want, int(on_dev), C.c_void_p(base)), (frames,), on_dev
+
+    def enqueue(self, frames, ts, fmt="rgb"):
+        """Hand over n frames without waiting for them (rb_pipeline_enqueue / enqueue_frames); returns the ticket to wait.
+        frames: a uint8 host array or torch CUDA tensor of packed frames, (n, h, w, 3) for fmt="rgb" or (n, h, w) for
+        fmt="mono", or a list of strided frames as push_frames takes them.  The frames are kept alive until the ticket is
+        waited.  Device frames: the call first waits (on the host) for the work torch enqueued so far on its current stream,
+        so that they are complete.  Device output mode: the enqueue's writes wait for torch's current stream, as a push's.
+        RbError when `depth` tickets are outstanding (nothing changes) or asynchronous pushes are off."""
+        fn, args, keep, on_dev = self._enqueue_args(frames, ts, fmt)
+        ts = np.ascontiguousarray(ts, np.float64)
+        if on_dev or self._out_dev:
+            import torch
+            cur = torch.cuda.current_stream(self.device)
+            if on_dev:
+                cur.synchronize()
+            if self._out_dev and getattr(self, "_consumer", None) != cur.cuda_stream:
+                self.set_consumer_stream(cur.cuda_stream)
+        ticket = C.c_int64(-1)
+        self.check(fn(self.h_, *args, _p(ts), len(ts), C.byref(ticket)))
+        if not hasattr(self, "_inflight"):
+            self._inflight = {}
+        self._inflight[ticket.value] = (len(ts), keep)
+        return ticket.value
+
+    def wait(self, ticket):
+        """Block until `ticket` is complete and retire it with every earlier one; returns its NAV records.  Until the next
+        wait or push, odometry(), mirror(), depth(), depth_image() and their _dev forms give the ticket's outputs."""
+        inflight = getattr(self, "_inflight", {})
+        n = inflight.get(int(ticket), (0, None))[0]
+        nav = np.zeros(n, NAV)
+        r = self.L.rb_pipeline_wait(self.h_, C.c_int64(int(ticket)), _p(nav) if n else None)
+        if n:
+            for t in [t for t in inflight if t <= int(ticket)]:
+                del inflight[t]
+        self.check(r)
+        return nav
+
+    def poll(self):
+        """The newest ticket whose work is complete (-1 if none), without blocking."""
+        t = C.c_int64(-1)
+        self.check(self.L.rb_pipeline_poll(self.h_, C.byref(t)))
+        return t.value
+
     def reset(self):
         self.check(self.L.rb_pipeline_reset(self.h_))
 
@@ -923,6 +1014,7 @@ class Pipeline:
         legacy default stream) when it is called.  The push wrappers set torch.cuda.current_stream() before each push in
         device mode; this call is for pushes made through the C functions.  self.stream() waits for nothing."""
         self.check(self.L.rb_pipeline_set_consumer_stream(self.h_, C.c_void_p(int(stream))))
+        self._consumer = int(stream)
 
     def _consumer_fence(self):
         """Device mode: the push overwrites no output before the work torch enqueued so far on its current stream (which

@@ -52,6 +52,36 @@ struct SubBatchPtrs {
                                 // pinned host memory, or device memory with rb_pipeline_set_output_memory(pl, 1))
 };
 
+// Asynchronous pushes (rb_pipeline_set_async / rb_pipeline_enqueue / rb_pipeline_wait).  Ticket k runs its front (staging,
+// gray, scale space) on the front stream into workspace k % 2 and its back (detect ... depth image) on the tracker stream,
+// writing its outputs into slot k % depth of the output ring; see DESIGN.md §5.
+struct AsyncSlot {
+    long long first;                  // frame number of the ticket's first frame
+    int n;                            // its frames
+    rb_nav *nav;                      // pinned [max_batch]: the nav records, copied from nav_dev after the back
+    rb_odometry *odom;                // pinned [max_batch] (odometry on)
+    int *abort;                       // pinned [RB_NMAPS]: the ring maps' minimiser abort flags after the back
+    struct FrameArgs *fa;             // pinned [max_batch]: per-frame scalars, the source of the back's fa_dev copy
+    SubBatchPtrs *tbl;                // pinned [2]: the front's table (src) and the back's (mirror and depth destinations)
+    rb_frame *frames;                 // pinned [max_batch]: strided device input, the source of the front's frame table
+    unsigned char *mirror_host, *mirror_dev, *depth_host, *depth_dev, *dimg_host, *dimg_dev;   // the slot's outputs
+    size_t mirror_host_bytes, mirror_dev_bytes, depth_host_bytes, depth_dev_bytes, dimg_host_bytes, dimg_dev_bytes;
+    cudaEvent_t done;                 // recorded on the tracker stream after the ticket's last copy
+};
+struct AsyncRing {
+    int depth;                        // 1..8 tickets in flight, one output slot each
+    AsyncSlot slot[8];
+    DogWS ws1;                        // workspace of odd tickets (even tickets use rb_pipeline::ws)
+    SubBatchPtrs *front_dev[2];       // device, per workspace: the table the front's gray pass reads
+    rb_frame *frames_dev[2];          // device, per workspace: strided device input's {data, step} table
+    cudaStream_t front;
+    cudaEvent_t ev_front[2];          // per workspace: its front is complete (the back waits for it)
+    cudaEvent_t ev_free[2];           // per workspace: the back that read it last is complete (the next front waits for it)
+    // captured halves: the front per (input format, workspace, batch size), the back per (workspace, ring phase, batch size)
+    cudaGraphExec_t *gfront, *gback;
+    int *lfront, *lback;              // kernel launches inside each graph
+};
+
 struct ImuFlow;
 struct rb_pipeline {
     rb_ctx *c;
@@ -178,6 +208,12 @@ struct rb_pipeline {
         size_t dev_bytes;
         int n;                         // frames of the last push
     } dimg;
+    // asynchronous pushes (nullptr: off).  Tickets count up from 0 for the pipeline's lifetime; [tk_retired, tk_next) are
+    // outstanding.  view: the slot of the ticket the last wait retired, which the output accessors read until the next wait
+    // or push (nullptr: the synchronous buffers)
+    AsyncRing *ar;
+    long long tk_next, tk_retired;
+    const AsyncSlot *view;
 };
 
 // input layouts of a push: packed RGB24 (3 bytes per pixel) or mono8, which stands for the RGB24 frame (m, m, m), at
@@ -191,13 +227,29 @@ static inline int graph_slots(const rb_pipeline *pl) { return RB_NFMT * RB_NMAPS
 static inline int graph_slot(const rb_pipeline *pl, int fmt, int phase, int n) {
     return (fmt * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
 }
+// the asynchronous pushes' halves (AsyncRing::gfront / gback)
+static inline int afront_slots(const rb_pipeline *pl) { return RB_NFMT * 2 * (pl->max_batch + 1); }
+static inline int afront_slot(const rb_pipeline *pl, int fmt, int par, int n) {
+    return (fmt * 2 + par) * (pl->max_batch + 1) + n;
+}
+static inline int aback_slots(const rb_pipeline *pl) { return 2 * RB_NMAPS * (pl->max_batch + 1); }
+static inline int aback_slot(const rb_pipeline *pl, int par, int phase, int n) {
+    return (par * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
+}
+static void drop_execs(cudaGraphExec_t *g, int n) {
+    for (int i = 0; g && i < n; i++)
+        if (g[i]) {
+            cudaGraphExecDestroy(g[i]);
+            g[i] = nullptr;
+        }
+}
 // captured batches contain the gray kernel, the undistortion and the mirror's pack kernels: drop them all
 static void drop_graphs(rb_pipeline *pl) {
-    for (int i = 0; i < graph_slots(pl); i++)
-        if (pl->gexec[i]) {
-            cudaGraphExecDestroy(pl->gexec[i]);
-            pl->gexec[i] = nullptr;
-        }
+    drop_execs(pl->gexec, graph_slots(pl));
+    if (pl->ar) {
+        drop_execs(pl->ar->gfront, afront_slots(pl));
+        drop_execs(pl->ar->gback, aback_slots(pl));
+    }
 }
 // `to` waits for the work enqueued on `from` so far.  One event serves every such hand-over: a wait (eager or captured)
 // takes the event's most recent record at the time of the call.
@@ -232,13 +284,21 @@ static int grow_out(rb_pipeline *pl, unsigned char **host, size_t *host_have, un
                     size_t bytes) {
     return pl->out_dev ? grow_dev(pl->c, dev, dev_have, bytes) : grow_mapped(pl->c, host, host_have, bytes);
 }
-// host frames of a push into the packed staging, frames [i0, i0 + count) of `frames` (strided, one 2D copy each) or of the
-// packed buffer `rgb`, on stream s
+// true, with the reason in the pipeline's error, while asynchronous tickets are outstanding: `what` would change or read
+// what they use
+static bool refuse_busy(rb_pipeline *pl, const char *what) {
+    if (pl->tk_next == pl->tk_retired) return false;
+    snprintf(pl->c->err, sizeof(pl->c->err), "%s: %lld asynchronous tickets are outstanding (rb_pipeline_wait them first)",
+             what, pl->tk_next - pl->tk_retired);
+    return true;
+}
+// host frames of a push into the packed staging (ws's, by default the pipeline's), frames [i0, i0 + count) of `frames`
+// (strided, one 2D copy each) or of the packed buffer `rgb`, on stream s
 static int stage_host_frames(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, int i0, int count,
-                             cudaStream_t s) {
+                             cudaStream_t s, DogWS *ws = nullptr) {
     rb_ctx *c = pl->c;
     const size_t fbytes = frame_bytes(c, fmt), row = fbytes / c->h;
-    uint8_t *dst = pl->ws.rgb + (size_t)i0 * fbytes;
+    uint8_t *dst = (ws ? ws : &pl->ws)->rgb + (size_t)i0 * fbytes;
     if (!frames) {
         RB_CUDA(cudaMemcpyAsync(dst, rgb + (size_t)i0 * fbytes, (size_t)count * fbytes, cudaMemcpyHostToDevice, s));
         return RB_OK;
@@ -256,6 +316,7 @@ static int write_frame_table(rb_pipeline *pl, const rb_frame *frames, int n) {
     return RB_OK;
 }
 #include "imu_flow.cuh"
+static void async_free(rb_pipeline *pl);
 
 enum { ST_H2D = 0, ST_GRAY, ST_DOG, ST_DETECT, ST_REEST, ST_FIELD, ST_MINIM, ST_FWD_ROT, ST_DMATCH, ST_REG_EKF, ST_RESCALE,
        ST_FINISH, ST_NAV };
@@ -437,6 +498,7 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
 
 extern "C" int rb_pipeline_set_imu(rb_pipeline *pl, const rb_imu_params *ip, const double *samples, int n) {
     if (!pl || !ip || !samples || n < 2) return RB_ERR_ARG;
+    if (refuse_busy(pl, "set_imu")) return RB_ERR_STATE;
     if (!pl->imu) pl->imu = new (std::nothrow) ImuFlow();
     if (!pl->imu) return RB_ERR_ARG;
     ImuFlow &f = *pl->imu;
@@ -451,6 +513,7 @@ extern "C" int rb_pipeline_set_imu(rb_pipeline *pl, const rb_imu_params *ip, con
 
 extern "C" int rb_pipeline_set_imu_live(rb_pipeline *pl, const rb_imu_params *ip, double sample_time, int buffer_size) {
     if (!pl || !ip || !(sample_time > 0) || buffer_size < 1 || buffer_size == INT_MAX) return RB_ERR_ARG;
+    if (refuse_busy(pl, "set_imu_live")) return RB_ERR_STATE;
     std::vector<rbimu::ImuSample> slots;
     try {
         slots.resize((size_t)buffer_size + 1);
@@ -516,6 +579,7 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
         if (s) cudaStreamSynchronize(s);
     for (cudaStream_t s : own)
         if (s) cudaStreamDestroy(s);
+    async_free(pl);
     cudaEvent_t events[] = {pl->ev_hop, pl->ev_trk[0], pl->ev_trk[1], pl->ev_rjoin, pl->ev_copy[0], pl->ev_copy[1],
                             pl->ev[0], pl->ev[1], pl->ev[2], pl->ev[3]};
     for (cudaEvent_t e : events)
@@ -553,12 +617,14 @@ extern "C" rb_map *rb_pipeline_map(rb_pipeline *pl, int age) {
     return pl->maps[(pl->n_pushed - 1 - age) % RB_NMAPS];
 }
 extern "C" int rb_pipeline_stage_ms(const rb_pipeline *pl, float out[6]) {
+    if (refuse_busy(const_cast<rb_pipeline *>(pl), "stage_ms")) return RB_ERR_STATE;
     memcpy(out, pl->stage_ms, sizeof(float) * 6);
     return RB_OK;
 }
 
 extern "C" int rb_pipeline_reset(rb_pipeline *pl) {
     rb_ctx *c = pl->c;
+    if (refuse_busy(pl, "reset")) return RB_ERR_STATE;
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return pl_reset_state(pl);
 }
@@ -682,23 +748,28 @@ static int track_frame(rb_pipeline *pl, rb_map *neu, rb_map *old, const FrameArg
     return RB_OK;
 }
 
-// everything of a batch after the H2D copy: gray, batched scale space, then per frame detect + track + map
-static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame, bool with_events) {
+// the front of a batch, after the H2D copy: its gray plane (rebvo_first_t.cpp:231 undistortion + RGB -> BW) from the
+// frames at tbl->src, or through frames_dev for the strided layouts, then the batched scale space, into ws
+static int enqueue_front(rb_pipeline *pl, DogWS *ws, SubBatchPtrs *tbl, const rb_frame *frames_dev, int fmt, int n,
+                         bool with_events) {
+    rb_ctx *c = pl->c;
+    int r;
+    prof_mark(pl, ST_H2D);
+    if ((r = rb_gray_enqueue(c, ws, pl->und, in_mono(fmt), &tbl->src, in_strided(fmt) ? frames_dev : nullptr, n))) return r;
+    prof_mark(pl, ST_GRAY);
+    if (with_events) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
+    if ((r = rb_dog_build_batch(c, ws, n))) return r;
+    prof_mark(pl, ST_DOG);
+    if (with_events) RB_CUDA(cudaEventRecord(pl->ev[2], c->stream));
+    return RB_OK;
+}
+
+// the back of a batch: per frame detect + track + map on the scale space in ws, and the per-frame outputs
+static int enqueue_back(rb_pipeline *pl, const DogWS *ws, int n, long long first_frame) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
     pl->resc_open = false;   // (a batch joins its last rescaling at its end; a failed enqueue must not leave a join behind)
-    prof_mark(pl, ST_H2D);
-    // the batch's gray plane (rebvo_first_t.cpp:231 undistortion + RGB -> BW) from the frames at sb_dev->src, or through
-    // frames_dev for the strided layouts
-    if ((r = rb_gray_enqueue(c, &pl->ws, pl->und, in_mono(fmt), &pl->sb_dev->src, in_strided(fmt) ? pl->frames_dev : nullptr,
-                             n)))
-        return r;
-    prof_mark(pl, ST_GRAY);
-    if (with_events) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
-    if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
-    prof_mark(pl, ST_DOG);
-    if (with_events) RB_CUDA(cudaEventRecord(pl->ev[2], c->stream));
     // Two streams, like the reference's first and second thread: the detector of frame f+1 only needs the scale space
     // and the previous detector state (threshold chain), so it runs on det_stream while the main stream tracks
     // frame f.  detect(f) overwrites the map of frame f-3, which track(f-2) was the last to read.
@@ -709,7 +780,7 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     for (int i = 0; i < n; i++) {
         const long long fr = first_frame + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
-        const float *img0 = pl->ws.img0 + (size_t)i * c->NP, *dog = pl->ws.dog + (size_t)i * c->NP;
+        const float *img0 = ws->img0 + (size_t)i * c->NP, *dog = ws->dog + (size_t)i * c->NP;
         // FirstThr: detect + reEstimateThresh (rebvo_first_t.cpp:266-272)
         if (ov) {
             if (i >= 2) RB_CUDA(cudaStreamWaitEvent(pl->det_stream, pl->ev_trk[i % 2], 0));   // track(i-2)
@@ -780,6 +851,42 @@ static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame,
     return RB_OK;
 }
 
+// everything of a batch after the H2D copy, on the tracker stream in the pipeline's workspace: front, then back
+static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame, bool with_events) {
+    int r = enqueue_front(pl, &pl->ws, pl->sb_dev, pl->frames_dev, fmt, n, with_events);
+    return r ? r : enqueue_back(pl, &pl->ws, n, first_frame);
+}
+
+// Capture the work body() enqueues on stream s (and the streams it forks) as one graph, instantiated into *exec; *launches
+// receives the kernels it launches, which are counted at each replay and not at the capture.
+template <class F>
+static int capture_graph(rb_pipeline *pl, cudaStream_t s, F &&body, cudaGraphExec_t *exec, int *launches) {
+    rb_ctx *c = pl->c;
+    cudaGraph_t g = nullptr;
+    const int64_t l0 = c->launches;
+    RB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    int r = body();
+    cudaError_t e = cudaStreamEndCapture(s, &g);
+    if (r) {
+        if (g) cudaGraphDestroy(g);
+        return r;
+    }
+    if (e != cudaSuccess) {
+        snprintf(c->err, sizeof(c->err), "graph capture: %s", cudaGetErrorString(e));
+        return RB_ERR_CUDA;
+    }
+    *launches = (int)(c->launches - l0);
+    c->launches = l0;
+    e = cudaGraphInstantiate(exec, g, 0);
+    cudaGraphDestroy(g);
+    if (e != cudaSuccess) {
+        *exec = nullptr;
+        snprintf(c->err, sizeof(c->err), "graph instantiate: %s", cudaGetErrorString(e));
+        return RB_ERR_CUDA;
+    }
+    return RB_OK;
+}
+
 // rgb: n packed frames of frame_bytes(fmt) each, host or device memory; or (rgb == nullptr) frames: n strided frames, checked
 // by push_frames, whose layout is fmt (device memory) or whose packed format is fmt (host memory)
 static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
@@ -787,6 +894,8 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts) return RB_ERR_ARG;
+    if (refuse_busy(pl, "push")) return RB_ERR_STATE;
+    pl->view = nullptr;
     // (the packed mono kernels read a device buffer as aligned 32-bit words; the RGB kernels test the alignment of the source
     // on the device -- k_gray<false, GRAY_ALIGNED> and ug_pixel take a path for unaligned sources -- and the any-width kernels
     // read every source through aligned words around it)
@@ -873,28 +982,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
             for (int ph = 0; ph < RB_NMAPS && build; ph++) {
                 const int k = graph_slot(pl, fmt, ph, nj);
                 if (pl->gexec[k]) continue;
-                cudaGraph_t g = nullptr;
-                const int64_t l0 = c->launches;
-                RB_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-                r = enqueue_batch(pl, fmt, nj, ph == 0 ? RB_NMAPS : ph, false);   // any first frame > 0 of that phase
-                cudaError_t e = cudaStreamEndCapture(c->stream, &g);
-                if (r) {
-                    if (g) cudaGraphDestroy(g);
-                    return r;
-                }
-                if (e != cudaSuccess) {
-                    snprintf(c->err, sizeof(c->err), "graph capture: %s", cudaGetErrorString(e));
-                    return RB_ERR_CUDA;
-                }
-                pl->glaunches[k] = (int)(c->launches - l0);
-                c->launches = l0;
-                e = cudaGraphInstantiate(&pl->gexec[k], g, 0);
-                cudaGraphDestroy(g);
-                if (e != cudaSuccess) {
-                    pl->gexec[k] = nullptr;
-                    snprintf(c->err, sizeof(c->err), "graph instantiate: %s", cudaGetErrorString(e));
-                    return RB_ERR_CUDA;
-                }
+                // (any first frame > 0 of that phase)
+                auto body = [&]() { return enqueue_batch(pl, fmt, nj, ph == 0 ? RB_NMAPS : ph, false); };
+                if ((r = capture_graph(pl, c->stream, body, &pl->gexec[k], &pl->glaunches[k]))) return r;
             }
             if (j == 0) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
             RB_CUDA(cudaGraphLaunch(pl->gexec[key], c->stream));
@@ -966,6 +1056,7 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
 static int set_begin(rb_pipeline *pl, const char *imu_refused) {
     rb_ctx *c = pl->c;
     RB_CUDA(cudaSetDevice(c->device));
+    if (refuse_busy(pl, "set_* call")) return RB_ERR_STATE;
     if (imu_refused && pl->imu) {
         snprintf(c->err, sizeof(c->err), "%s: not available in IMU mode", imu_refused);
         return RB_ERR_ARG;
@@ -973,6 +1064,103 @@ static int set_begin(rb_pipeline *pl, const char *imu_refused) {
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return RB_OK;
 }
+// every output slot of the asynchronous ring holds the outputs that are on now, where rb_pipeline_set_output_memory puts
+// them: made by rb_pipeline_set_async and by the set_* calls that switch an output on or enlarge it, never by an enqueue
+static int async_grow(rb_pipeline *pl) {
+    AsyncRing *ar = pl->ar;
+    if (!ar) return RB_OK;
+    rb_ctx *c = pl->c;
+    const size_t mb = (size_t)pl->max_batch;
+    int r = RB_OK;
+    for (int k = 0; k < ar->depth && !r; k++) {
+        AsyncSlot &s = ar->slot[k];
+        if (pl->odom.on && !s.odom) RB_CUDA(cudaMallocHost(&s.odom, sizeof(rb_odometry) * mb));
+        if (pl->mirror.on)   // (host mode: the frames are packed into the pipeline's staging, then copied into the slot)
+            r = pl->out_dev ? grow_dev(c, &s.mirror_dev, &s.mirror_dev_bytes, mb * pl->mirror.stride)
+                            : grow_mapped(c, &s.mirror_host, &s.mirror_host_bytes, mb * pl->mirror.stride);
+        if (!r && pl->depth.on)
+            r = grow_out(pl, &s.depth_host, &s.depth_host_bytes, &s.depth_dev, &s.depth_dev_bytes,
+                         mb * pl->depth.plan.cells_bytes);
+        if (!r && pl->dimg.mode)
+            r = grow_out(pl, &s.dimg_host, &s.dimg_host_bytes, &s.dimg_dev, &s.dimg_dev_bytes, mb * pl->dimg.stride);
+    }
+    return r;
+}
+// the ring and everything it owns (no ticket outstanding, or the pipeline is being destroyed); the outputs of a ticket it
+// held are gone with it
+static void async_free(rb_pipeline *pl) {
+    AsyncRing *ar = pl->ar;
+    if (!ar) return;
+    if (ar->front) {
+        cudaStreamSynchronize(ar->front);
+        cudaStreamDestroy(ar->front);
+    }
+    drop_execs(ar->gfront, afront_slots(pl));
+    drop_execs(ar->gback, aback_slots(pl));
+    delete[] ar->gfront;
+    delete[] ar->gback;
+    delete[] ar->lfront;
+    delete[] ar->lback;
+    cudaEvent_t events[] = {ar->ev_front[0], ar->ev_front[1], ar->ev_free[0], ar->ev_free[1]};
+    for (cudaEvent_t e : events)
+        if (e) cudaEventDestroy(e);
+    for (AsyncSlot &s : ar->slot) {
+        if (s.done) cudaEventDestroy(s.done);
+        void *host[] = {s.nav, s.odom, s.abort, s.fa, s.tbl, s.frames, s.mirror_host, s.depth_host, s.dimg_host};
+        for (void *p : host)
+            if (p) cudaFreeHost(p);
+        void *dev[] = {s.mirror_dev, s.depth_dev, s.dimg_dev};
+        for (void *p : dev) cudaFree(p);
+    }
+    for (int k = 0; k < 2; k++) {
+        cudaFree(ar->front_dev[k]);
+        cudaFree(ar->frames_dev[k]);
+    }
+    rb_dogws_free(&ar->ws1);
+    if (pl->view) {
+        pl->view = nullptr;
+        pl->mirror.n = pl->depth.n = pl->dimg.n = pl->odom.n = 0;
+    }
+    delete ar;
+    pl->ar = nullptr;
+}
+static int async_alloc(rb_pipeline *pl, int depth) {
+    rb_ctx *c = pl->c;
+    AsyncRing *ar = new (std::nothrow) AsyncRing();
+    if (!ar) return RB_ERR_ARG;
+    memset(ar, 0, sizeof(*ar));
+    pl->ar = ar;
+    ar->depth = depth;
+    const size_t mb = (size_t)pl->max_batch;
+    int r;
+    if ((r = rb_dogws_alloc(c, &ar->ws1, pl->max_batch))) return r;
+    // lowest priority: the back of the ticket before is the critical path, and a front has the whole of it to finish in
+    int lo = 0, hi = 0;
+    RB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    RB_CUDA(cudaStreamCreateWithPriority(&ar->front, cudaStreamNonBlocking, lo));
+    for (int k = 0; k < 2; k++) {
+        RB_CUDA(cudaEventCreateWithFlags(&ar->ev_front[k], cudaEventDisableTiming));
+        RB_CUDA(cudaEventCreateWithFlags(&ar->ev_free[k], cudaEventDisableTiming));
+        RB_CUDA(cudaMalloc(&ar->front_dev[k], sizeof(SubBatchPtrs)));
+        RB_CUDA(cudaMalloc(&ar->frames_dev[k], sizeof(rb_frame) * mb));
+    }
+    ar->gfront = new (std::nothrow) cudaGraphExec_t[afront_slots(pl)]();
+    ar->gback = new (std::nothrow) cudaGraphExec_t[aback_slots(pl)]();
+    ar->lfront = new (std::nothrow) int[afront_slots(pl)]();
+    ar->lback = new (std::nothrow) int[aback_slots(pl)]();
+    if (!ar->gfront || !ar->gback || !ar->lfront || !ar->lback) return RB_ERR_ARG;
+    for (int k = 0; k < depth; k++) {
+        AsyncSlot &s = ar->slot[k];
+        RB_CUDA(cudaMallocHost(&s.nav, sizeof(rb_nav) * mb));
+        RB_CUDA(cudaMallocHost(&s.abort, sizeof(int) * RB_NMAPS));
+        RB_CUDA(cudaMallocHost(&s.fa, sizeof(FrameArgs) * mb));
+        RB_CUDA(cudaMallocHost(&s.tbl, 2 * sizeof(SubBatchPtrs)));
+        RB_CUDA(cudaMallocHost(&s.frames, sizeof(rb_frame) * mb));
+        RB_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+    }
+    return async_grow(pl);
+}
+
 extern "C" int rb_pipeline_set_undistort(rb_pipeline *pl, const double kc[5]) {
     if (!pl) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
@@ -1012,7 +1200,7 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     pl->mirror.rec = on == 2 ? 15 : sizeof(rb_keyline);
     pl->mirror.stride = stride;
     pl->mirror.n = 0;
-    return RB_OK;
+    return async_grow(pl);
 }
 extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) {
     if (!pl) return RB_ERR_ARG;
@@ -1060,14 +1248,14 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
     pl->depth.on = 1;
     pl->depth.n = 0;
     pl->dimg.n = 0;
-    return RB_OK;
+    return async_grow(pl);
 }
 extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
     if (!pl || !cells) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
     const DepthGeom &g = pl->depth.plan.g;
-    const unsigned char *slot = pl->depth.host + (size_t)i * pl->depth.plan.cells_bytes;
+    const unsigned char *slot = (pl->view ? pl->view->depth_host : pl->depth.host) + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
     if (gw) *gw = g.gw;
     if (gh) *gh = g.gh;
@@ -1092,13 +1280,14 @@ extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
     if (mode != pl->dimg.mode) drop_graphs(pl);   // the captured batches contain (or not) the image pass
     pl->dimg.mode = mode;
     pl->dimg.n = 0;
-    return RB_OK;
+    return async_grow(pl);
 }
 extern "C" int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
     if (!pl || !rho) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
-    const float *p = reinterpret_cast<const float *>(pl->dimg.host + (size_t)i * pl->dimg.stride);
+    const unsigned char *planes = pl->view ? pl->view->dimg_host : pl->dimg.host;
+    const float *p = reinterpret_cast<const float *>(planes + (size_t)i * pl->dimg.stride);
     *rho = p;
     if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
@@ -1116,12 +1305,12 @@ extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
     if (on != pl->odom.on) drop_graphs(pl);   // the captured batches pass (or not) the record slots to their kernels
     pl->odom.on = on;
     pl->odom.n = 0;
-    return RB_OK;
+    return async_grow(pl);
 }
 extern "C" int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, int *n) {
     if (!pl || !recs || !n) return RB_ERR_ARG;
     if (!pl->odom.n) return RB_ERR_STATE;
-    *recs = pl->odom.pin;
+    *recs = pl->view ? pl->view->odom : pl->odom.pin;
     *n = pl->odom.n;
     return RB_OK;
 }
@@ -1129,8 +1318,8 @@ extern "C" int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, 
     if (!pl || !records || !n) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
-    *records = pl->mirror.host + (size_t)i * pl->mirror.stride;
-    *n = pl->nav_pin[i].kn;
+    *records = (pl->view ? pl->view->mirror_host : pl->mirror.host) + (size_t)i * pl->mirror.stride;
+    *n = (pl->view ? pl->view->nav : pl->nav_pin)[i].kn;
     return RB_OK;
 }
 
@@ -1158,11 +1347,12 @@ extern "C" int rb_pipeline_set_output_memory(rb_pipeline *pl, int where) {
     }
     drop_graphs(pl);   // the captured batches contain (or not) k_mirror_to_host and its join
     pl->mirror.n = pl->depth.n = pl->dimg.n = 0;
-    return RB_OK;
+    return async_grow(pl);
 }
 extern "C" int rb_pipeline_set_consumer_stream(rb_pipeline *pl, void *stream) {
     if (!pl) return RB_ERR_ARG;
     RB_ENTER(pl->c);
+    if (refuse_busy(pl, "set_consumer_stream")) return RB_ERR_STATE;
     pl->consumer = (cudaStream_t)stream;
     return RB_OK;
 }
@@ -1170,8 +1360,8 @@ extern "C" int rb_pipeline_mirror_dev(rb_pipeline *pl, int i, const void **recor
     if (!pl || !records || !n) return RB_ERR_ARG;
     if (!pl->out_dev) return RB_ERR_STATE;
     if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
-    *records = pl->mirror.dev + (size_t)i * pl->mirror.stride;
-    *n = pl->nav_pin[i].kn;
+    *records = (pl->view ? pl->view->mirror_dev : pl->mirror.dev) + (size_t)i * pl->mirror.stride;
+    *n = (pl->view ? pl->view->nav : pl->nav_pin)[i].kn;
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh,
@@ -1180,7 +1370,7 @@ extern "C" int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell
     if (!pl->out_dev) return RB_ERR_STATE;
     if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
     const DepthGeom &g = pl->depth.plan.g;
-    const unsigned char *slot = pl->depth.dev + (size_t)i * pl->depth.plan.cells_bytes;
+    const unsigned char *slot = (pl->view ? pl->view->depth_dev : pl->depth.dev) + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
     if (gw) *gw = g.gw;
     if (gh) *gh = g.gh;
@@ -1191,7 +1381,8 @@ extern "C" int rb_pipeline_depth_image_dev(rb_pipeline *pl, int i, const float *
     if (!pl || !rho) return RB_ERR_ARG;
     if (!pl->out_dev) return RB_ERR_STATE;
     if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
-    const float *p = reinterpret_cast<const float *>(pl->dimg.dev + (size_t)i * pl->dimg.stride);
+    const unsigned char *planes = pl->view ? pl->view->dimg_dev : pl->dimg.dev;
+    const float *p = reinterpret_cast<const float *>(planes + (size_t)i * pl->dimg.stride);
     *rho = p;
     if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
@@ -1213,28 +1404,34 @@ extern "C" int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_de
 }
 // strided frames: every argument is checked before anything is enqueued; host frames then run the packed format's batches,
 // device frames the strided layout's
-static int push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out,
-                       bool on_device) {
-    if (!pl) return RB_ERR_ARG;
+static int check_frames(rb_pipeline *pl, const char *what, int format, const rb_frame *frames, const double *ts, int n,
+                        bool on_device, int *fmt) {
     rb_ctx *c = pl->c;
     if (format != RB_FRAME_RGB24 && format != RB_FRAME_MONO8) {
-        snprintf(c->err, sizeof(c->err), "push_frames: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", format);
+        snprintf(c->err, sizeof(c->err), "%s: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", what, format);
         return RB_ERR_ARG;
     }
     if (n < 1 || n > pl->max_batch || !frames || !ts) return RB_ERR_ARG;
     const int64_t row = (int64_t)(format == RB_FRAME_MONO8 ? 1 : 3) * c->w;
     for (int i = 0; i < n; i++)
         if (!frames[i].data || frames[i].step < row) {
-            snprintf(c->err, sizeof(c->err), "push_frames: frame %d has %s (rows need %lld bytes)", i,
+            snprintf(c->err, sizeof(c->err), "%s: frame %d has %s (rows need %lld bytes)", what, i,
                      frames[i].data ? "a step shorter than a row" : "no data", (long long)row);
             return RB_ERR_ARG;
         }
     if (on_device && pl->und && (c->w > 65535 || c->h > 65535)) {   // (the strided undistortion's 16-bit tap coordinates)
-        snprintf(c->err, sizeof(c->err), "push_frames_dev: undistorted frames wider or higher than 65535 pixels");
+        snprintf(c->err, sizeof(c->err), "%s_dev: undistorted frames wider or higher than 65535 pixels", what);
         return RB_ERR_ARG;
     }
-    const int fmt = format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB;
-    return push_impl(pl, nullptr, frames, on_device ? fmt + RB_IN_RGB_STRIDED : fmt, on_device, ts, n, nav_out);
+    const int f = format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB;
+    *fmt = on_device ? f + RB_IN_RGB_STRIDED : f;
+    return RB_OK;
+}
+static int push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out,
+                       bool on_device) {
+    if (!pl) return RB_ERR_ARG;
+    int fmt = 0, r = check_frames(pl, "push_frames", format, frames, ts, n, on_device, &fmt);
+    return r ? r : push_impl(pl, nullptr, frames, fmt, on_device, ts, n, nav_out);
 }
 extern "C" int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                        rb_nav *nav_out) {
@@ -1243,6 +1440,214 @@ extern "C" int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_fra
 extern "C" int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                            rb_nav *nav_out) {
     return push_frames(pl, format, frames, ts, n, nav_out, true);
+}
+
+// ---- asynchronous pushes (DESIGN.md §5) ----------------------------------------------------------------------------------
+extern "C" int rb_pipeline_set_async(rb_pipeline *pl, int depth) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    if (depth < 0 || depth > 8) {
+        snprintf(c->err, sizeof(c->err), "set_async: depth %d is outside 0..8", depth);
+        return RB_ERR_ARG;
+    }
+    int r = set_begin(pl, "set_async");
+    if (r) return r;
+    async_free(pl);
+    if (depth && (r = async_alloc(pl, depth))) async_free(pl);
+    return r;
+}
+
+// one ticket: the front on the front stream into workspace k % 2, the back on the tracker stream into output slot
+// k % depth.  Arguments as push_impl's.
+static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
+                        int n, int64_t *ticket) {
+    rb_ctx *c = pl->c;
+    const rb_params &p = pl->p;
+    AsyncRing *ar = pl->ar;
+    if (!ar || pl->imu) {
+        snprintf(c->err, sizeof(c->err), "enqueue: %s", pl->imu ? "not available in IMU mode"
+                                                                  : "asynchronous pushes are off (rb_pipeline_set_async)");
+        return RB_ERR_ARG;
+    }
+    if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts || !ticket) return RB_ERR_ARG;
+    if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
+    if (pl->tk_next - pl->tk_retired >= ar->depth) {
+        snprintf(c->err, sizeof(c->err), "enqueue: %d tickets are outstanding, the depth of rb_pipeline_set_async: wait first",
+                 ar->depth);
+        return RB_ERR_STATE;
+    }
+    RB_CUDA(cudaSetDevice(c->device));
+    const long long k = pl->tk_next, first = pl->n_pushed;
+    AsyncSlot &s = ar->slot[k % ar->depth];
+    const int par = (int)(k & 1);
+    DogWS *ws = par ? &ar->ws1 : &pl->ws;
+    int r;
+    for (int i = 0; i < n; i++) {   // (as push_impl)
+        const long long fr = first + i;
+        double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
+        if (dt < 0.001) dt = 1 / p.config_fps;
+        s.fa[i].t = ts[i];
+        s.fa[i].dt = dt;
+        s.fa[i].frame_count = fr > 0 ? (unsigned int)((fr - 1) / 8) : 0;
+    }
+    // front: once the back of ticket k - 2 (the last to read this workspace) is done, the frames into its staging (host
+    // input) or its frame table (strided device input), then gray and scale space
+    cudaStream_t fs = ar->front, main_stream = c->stream;
+    RB_CUDA(cudaStreamWaitEvent(fs, ar->ev_free[par], 0));
+    if (!on_device && (r = stage_host_frames(pl, rgb, frames, fmt, 0, n, fs, ws))) return r;
+    s.tbl[0].src = on_device ? (const void *)rgb : (const void *)ws->rgb;   // (strided: unused)
+    RB_CUDA(cudaMemcpyAsync(ar->front_dev[par], &s.tbl[0], sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, fs));
+    if (in_strided(fmt)) {
+        memcpy(s.frames, frames, sizeof(rb_frame) * n);
+        RB_CUDA(cudaMemcpyAsync(ar->frames_dev[par], s.frames, sizeof(rb_frame) * n, cudaMemcpyHostToDevice, fs));
+    }
+    auto front = [&]() {
+        c->stream = fs;
+        const int e = enqueue_front(pl, ws, ar->front_dev[par], ar->frames_dev[par], fmt, n, false);
+        c->stream = main_stream;
+        return e;
+    };
+    if (!pl->use_graph) {
+        if ((r = front())) return r;
+    } else {
+        const int key = afront_slot(pl, fmt, par, n);
+        if (!ar->gfront[key] && (r = capture_graph(pl, fs, front, &ar->gfront[key], &ar->lfront[key]))) return r;
+        RB_CUDA(cudaGraphLaunch(ar->gfront[key], fs));
+        c->launches += ar->lfront[key];
+    }
+    RB_CUDA(cudaEventRecord(ar->ev_front[par], fs));
+    // back: after the consumer's reads of the outputs this slot held (device mode) and this ticket's front, behind the back
+    // of ticket k - 1 on the tracker stream
+    if (pl->out_dev && pl->consumer != c->stream && (r = stream_wait(pl, pl->consumer, c->stream))) return r;
+    RB_CUDA(cudaStreamWaitEvent(c->stream, ar->ev_front[par], 0));
+    RB_CUDA(cudaMemcpyAsync(pl->fa_dev, s.fa, sizeof(FrameArgs) * n, cudaMemcpyHostToDevice, c->stream));
+    SubBatchPtrs &t = s.tbl[1];
+    memset(&t, 0, sizeof(t));
+    if (pl->mirror.on) {   // (host mode: the pipeline's staging, then the slot's mapped memory; device mode: the slot)
+        t.mirror[0] = pl->out_dev ? s.mirror_dev : pl->mirror.dev;
+        t.mirror[1] = pl->out_dev ? nullptr : s.mirror_host;
+    }
+    if (pl->depth.on) {
+        t.depth[0] = pl->depth.stage;
+        t.depth[1] = pl->out_dev ? s.depth_dev : s.depth_host;
+        t.depth[2] = pl->dimg.mode ? (pl->out_dev ? s.dimg_dev : s.dimg_host) : nullptr;
+    }
+    RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
+    if (!pl->use_graph || first == 0) {
+        if ((r = enqueue_back(pl, ws, n, first))) return r;
+    } else {
+        const int key = aback_slot(pl, par, (int)(first % RB_NMAPS), n);
+        // (every workspace and ring phase of this size at once, as the synchronous batches)
+        const bool build = !ar->gback[key];
+        for (int pa = 0; pa < 2 && build; pa++)
+            for (int ph = 0; ph < RB_NMAPS; ph++) {
+                const int kk = aback_slot(pl, pa, ph, n);
+                if (ar->gback[kk]) continue;
+                const DogWS *w = pa ? &ar->ws1 : &pl->ws;
+                auto body = [&]() { return enqueue_back(pl, w, n, ph == 0 ? RB_NMAPS : ph); };
+                if ((r = capture_graph(pl, c->stream, body, &ar->gback[kk], &ar->lback[kk]))) return r;
+            }
+        RB_CUDA(cudaGraphLaunch(ar->gback[key], c->stream));
+        c->launches += ar->lback[key];
+    }
+    RB_CUDA(cudaEventRecord(ar->ev_free[par], c->stream));
+    RB_CUDA(cudaMemcpyAsync(s.nav, pl->nav_dev, sizeof(rb_nav) * n, cudaMemcpyDeviceToHost, c->stream));
+    if (pl->odom.on)
+        RB_CUDA(cudaMemcpyAsync(s.odom, pl->odom.dev, sizeof(rb_odometry) * n, cudaMemcpyDeviceToHost, c->stream));
+    // the abort flags of this ticket alone: read, then cleared for the next ticket (a push clears them when it finds one set)
+    for (int m = 0; m < RB_NMAPS; m++) {
+        int *flag = &pl->maps[m]->ts_host.ctl->abort;
+        RB_CUDA(cudaMemcpyAsync(&s.abort[m], flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        RB_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), c->stream));
+    }
+    RB_CUDA(cudaEventRecord(s.done, c->stream));
+    s.first = first;
+    s.n = n;
+    pl->tk_next = k + 1;
+    pl->n_pushed += n;
+    pl->t_prev = ts[n - 1];
+    pl->restored = false;
+    pl->last_sub = 0;   // (the workspaces are the tickets': rb_pipeline_batch_plane has nothing to show)
+    *ticket = k;
+    return RB_OK;
+}
+extern "C" int rb_pipeline_enqueue(rb_pipeline *pl, int format, int on_device, const uint8_t *data, const double *ts, int n,
+                                   int64_t *ticket) {
+    if (!pl) return RB_ERR_ARG;
+    if (format != RB_FRAME_RGB24 && format != RB_FRAME_MONO8) {
+        snprintf(pl->c->err, sizeof(pl->c->err), "enqueue: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", format);
+        return RB_ERR_ARG;
+    }
+    return enqueue_impl(pl, data, nullptr, format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB, on_device != 0, ts, n, ticket);
+}
+extern "C" int rb_pipeline_enqueue_frames(rb_pipeline *pl, int format, int on_device, const rb_frame *frames, const double *ts,
+                                          int n, int64_t *ticket) {
+    if (!pl) return RB_ERR_ARG;
+    int fmt = 0, r = check_frames(pl, "enqueue_frames", format, frames, ts, n, on_device != 0, &fmt);
+    return r ? r : enqueue_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, ticket);
+}
+
+// the host side of push_impl after its synchronisation, for one completed ticket, in ticket order
+static bool async_retire(rb_pipeline *pl, AsyncSlot &s) {
+    for (int i = 0; i < s.n && pl->odom.on; i++) {
+        if (s.first + i == 0) {   // the first frame of a sequence only initialises the ring (:109-121)
+            memset(&s.odom[i], 0, sizeof(rb_odometry));
+            continue;
+        }
+        s.odom[i].QK = i == 0 ? pl->odom.rkp_last : s.nav[i - 1].RKp;
+    }
+    pl->odom.rkp_last = s.nav[s.n - 1].RKp;
+    bool aborted = false;
+    for (int m = 0; m < RB_NMAPS; m++) aborted = aborted || s.abort[m] != 0;
+    return aborted;
+}
+extern "C" int rb_pipeline_wait(rb_pipeline *pl, int64_t ticket, rb_nav *nav_out) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    if (ticket < pl->tk_retired || ticket >= pl->tk_next) {
+        snprintf(c->err, sizeof(c->err), "wait: ticket %lld is %s", (long long)ticket,
+                 ticket >= pl->tk_next ? "not issued" : "already retired");
+        return RB_ERR_ARG;
+    }
+    RB_CUDA(cudaSetDevice(c->device));
+    AsyncRing *ar = pl->ar;
+    long long aborted = -1;
+    while (pl->tk_retired <= ticket) {
+        AsyncSlot &s = ar->slot[pl->tk_retired % ar->depth];
+        RB_CUDA(cudaEventSynchronize(s.done));
+        if (async_retire(pl, s) && aborted < 0) aborted = pl->tk_retired;
+        pl->tk_retired++;
+    }
+    const AsyncSlot &s = ar->slot[ticket % ar->depth];
+    pl->view = &s;
+    pl->odom.n = pl->odom.on ? s.n : 0;
+    pl->mirror.n = pl->mirror.on ? s.n : 0;
+    pl->depth.n = pl->depth.on ? s.n : 0;
+    pl->dimg.n = pl->depth.on && pl->dimg.mode ? s.n : 0;
+    if (nav_out) memcpy(nav_out, s.nav, sizeof(rb_nav) * s.n);
+    if (aborted >= 0) {
+        snprintf(c->err, sizeof(c->err),
+                 "Minimizer_RV: an exchange between the kernel's CTAs timed out in ticket %lld (poses are NaN)", aborted);
+        return RB_ERR_CUDA;
+    }
+    return RB_OK;
+}
+extern "C" int rb_pipeline_poll(rb_pipeline *pl, int64_t *newest_complete) {
+    if (!pl || !newest_complete) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    long long t = pl->tk_retired - 1;   // (retired tickets are complete; the tracker stream completes them in order)
+    while (t + 1 < pl->tk_next) {
+        const cudaError_t e = cudaEventQuery(pl->ar->slot[(t + 1) % pl->ar->depth].done);
+        if (e == cudaErrorNotReady) {
+            if (cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();   // (not an error of a later launch)
+            break;
+        }
+        RB_CUDA(e);
+        t++;
+    }
+    *newest_complete = t;
+    return RB_OK;
 }
 
 extern "C" int rb_pipeline_event_record(rb_pipeline *pl, int slot) {
@@ -1272,6 +1677,7 @@ extern "C" int rb_pipeline_batch_plane(rb_pipeline *pl, int slot, int which, flo
     if (!pl || !out) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
+    if (refuse_busy(pl, "batch_plane")) return RB_ERR_STATE;
     if (slot < 0 || slot >= pl->last_sub || (which != 0 && which != 2 && which != 5)) return RB_ERR_ARG;
     const float *src = (which == 0 ? pl->ws.img0 : which == 2 ? pl->ws.dog : pl->ws.gray) + (size_t)slot * c->NP;
     // the pitched plane without its padding columns: w * h floats (as rb_map_get_plane)
@@ -1285,6 +1691,7 @@ extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, in
                                       double *bytes_per_launch) {
     rb_ctx *c = pl->c;
     if (nimg < 1 || nimg > pl->max_batch || iters < 1) return RB_ERR_ARG;
+    if (refuse_busy(pl, "bench_pass")) return RB_ERR_STATE;
     int r;
     double bytes = 0;
     // passes 4-7: the gray pass on the workspace's frames, 4 and 5 from RGB24, 6 and 7 from mono8; 5 and 7 with the
@@ -1345,6 +1752,7 @@ extern "C" int rb_pipeline_save_state(rb_pipeline *pl, void *buf, size_t cap, si
     if (!pl || !written || (cap && !buf)) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
+    if (refuse_busy(pl, "save_state")) return RB_ERR_STATE;
     RB_CUDA(cudaStreamSynchronize(c->stream));
     rb_map *m = pl->n_pushed > 0 ? pl->maps[(pl->n_pushed - 1) % RB_NMAPS] : nullptr;
     MapState ms;
@@ -1414,6 +1822,7 @@ extern "C" int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n
     if (!pl) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
     RB_ENTER(c);
+    if (refuse_busy(pl, "load_state")) return RB_ERR_STATE;
     int r = rb_state_check(buf, n, c->err, sizeof(c->err));
     if (r) return r;
     const unsigned char *b = static_cast<const unsigned char *>(buf);
@@ -1492,6 +1901,7 @@ extern "C" int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n
         }
     }
     // the outputs of the last push are not this session's
+    pl->view = nullptr;
     pl->mirror.n = pl->depth.n = pl->dimg.n = pl->odom.n = 0;
     pl->last_sub = 0;
     return RB_OK;
