@@ -188,6 +188,11 @@ int rb_map_detect(rb_map *m, const rb_detect_params *p, double *tresh, int *l_kl
 /* same, reading the scale space of another ring object (the reference passes `sspace *ss` to detect()) */
 int rb_map_detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p, double *tresh, int *l_kl_num,
                      int *kn_out);
+/* rb_map_detect_ss with a detection mask: w x h bytes of host memory with a row step (step >= w); a zero byte at (x, y)
+ * keeps pixel (x, y) from being a keyline candidate, as rb_pipeline_set_detect_mask does in the pipeline.  The mask is
+ * copied to the device for this call.  RB_ERR_ARG for a NULL mask or a step < w. */
+int rb_map_detect_masked(rb_map *m, rb_map *ss, const rb_detect_params *p, const uint8_t *mask, int64_t step,
+                         double *tresh, int *l_kl_num, int *kn_out);
 /* edge_finder::reEstimateThresh (edge_finder.cpp:373-405) */
 int rb_map_reestimate_thresh(rb_map *m, int knum, int nbins, float *out_thresh);
 int rb_map_knum(rb_map *m, int *kn);
@@ -348,6 +353,36 @@ enum { RB_FRAME_RGB24 = 0, RB_FRAME_MONO8 = 1 };
 int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out);
 int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                 rb_nav *nav_out);
+/* Detection masks: keep keylines off pixels that must not be tracked (the robot's own body, the camera housing, burned-in
+ * overlays, objects that move on their own).  A mask is w x h bytes with a row step (>= w).  A zero byte at (x, y) means
+ * no keyline is detected at the detector's pixel (x, y), the one that becomes the keyline's p_inx = y * w + x (c_p is that
+ * pixel plus the sub-pixel offset); any other value allows detection there.  With undistortion on, (x, y) is a pixel of
+ * the undistorted image: the caller draws the mask in that frame (masks are not undistorted).  A masked pixel is simply
+ * not a candidate; everything after the candidate test is unchanged: the raster-order compaction, the kl_max cut (which
+ * counts unmasked candidates only), join_edges, the threshold feedback (l_kl_num = the masked count) and the rest of the
+ * flow.  A pixel is kept only when no mask that is set zeroes it.
+ *
+ * rb_pipeline_set_detect_mask(pl, mask, step, on_device): copies the mask (host or device memory) into device memory the
+ *   pipeline owns.  It applies to every later push and enqueue, in every input layout, with and without undistortion, and
+ *   in IMU dataset and live mode.  mask = NULL clears it.  Setting or clearing it re-captures no batch: pipelines with no
+ *   mask set launch the kernels, with the arguments, of a pipeline that never had one.  The fixed mask is configuration,
+ *   not session state: rb_pipeline_reset and rb_pipeline_load_state keep it, and session blobs do not carry it.
+ *   RB_ERR_ARG for a step < w; RB_ERR_STATE while asynchronous tickets are outstanding (as every set_* call).
+ * rb_pipeline_push_masked(pl, format, on_device, frames, masks, ts, n, nav_out) and
+ * rb_pipeline_masked_enqueue(pl, format, on_device, frames, masks, ts, n, &ticket): frames exactly as
+ *   rb_pipeline_push_frames(_dev) and rb_pipeline_enqueue_frames take them, plus one rb_frame {data, step} per frame for
+ *   its mask, in device memory on the pipeline's device (masks[] itself is host memory).  The masks are read in place
+ *   through a per-frame device table written before the batch, so one captured batch serves every mask buffer; masked
+ *   pushes have captured batches of their own.  The masks must be complete when the call is made and stay unchanged until
+ *   the push returns or the ticket is waited, as device frames.  A fixed mask applies as well.  Argument checks are those
+ *   of the strided calls, plus RB_ERR_ARG for a NULL masks, a NULL mask data or a mask step < w, before anything is
+ *   enqueued and with the state unchanged.  rb_pipeline_masked_enqueue is refused in IMU mode, as rb_pipeline_enqueue;
+ *   rb_pipeline_push_masked works there. */
+int rb_pipeline_set_detect_mask(rb_pipeline *pl, const uint8_t *mask, int64_t step, int on_device);
+int rb_pipeline_push_masked(rb_pipeline *pl, int format, int on_device, const rb_frame *frames, const rb_frame *masks,
+                            const double *ts, int n, rb_nav *nav_out);
+int rb_pipeline_masked_enqueue(rb_pipeline *pl, int format, int on_device, const rb_frame *frames,
+                               const rb_frame *masks, const double *ts, int n, int64_t *ticket);
 /* Asynchronous pushes: a live caller (a camera driver thread, a ROS image callback) hands over frames without waiting for
  * them to be tracked, and keeps up to `depth` pushes in flight, as the reference's FirstThr detects frame i+1 while its
  * SecondThread tracks frame i.  Each enqueued push (a ticket) has the records and outputs the synchronous push of the same
@@ -593,8 +628,8 @@ int rb_pipeline_push_imu(rb_pipeline *pl, const double *samples, int n);
  * load), pose, velocity and their covariances, K / Kp / P_Kp, the detector's threshold feedback, the frame count, the last
  * timestamp, and in IMU mode the filter, the scale estimator's history and the sample ring's read position (live mode: also
  * the samples it has not released).  It does not hold the configuration, which stays with the pipeline object: mirror, depth
- * grid and image, odometry records, undistortion, output memory, consumer stream, and the rb_params fields other than the
- * geometry.  About 120 bytes per keyline (2 MB at 15 k keylines).  Layout: DESIGN.md §5.
+ * grid and image, odometry records, undistortion, the fixed detection mask, output memory, consumer stream, and the
+ * rb_params fields other than the geometry.  About 120 bytes per keyline (2 MB at 15 k keylines).  Layout: DESIGN.md §5.
  *
  * rb_pipeline_save_state writes the blob into buf and its size into *written.  When cap is too small it writes nothing,
  * still reports the size needed and returns RB_ERR_ARG (buf = NULL, cap = 0 asks for the size).  Between pushes;

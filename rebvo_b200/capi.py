@@ -127,7 +127,8 @@ SYMBOLS = ["rb_ctx_create", "rb_ctx_destroy", "rb_last_error", "rb_ctx_sync", "r
            "rb_pipeline_set_consumer_stream", "rb_pipeline_mirror_dev", "rb_pipeline_depth_dev", "rb_pipeline_depth_image_dev",
            "rb_pipeline_push_frames", "rb_pipeline_push_frames_dev", "rb_pipeline_batch_plane", "rb_pipeline_save_state",
            "rb_pipeline_load_state", "rb_state_info", "rb_pipeline_set_async", "rb_pipeline_enqueue",
-           "rb_pipeline_enqueue_frames", "rb_pipeline_wait", "rb_pipeline_poll"]
+           "rb_pipeline_enqueue_frames", "rb_pipeline_wait", "rb_pipeline_poll", "rb_map_detect_masked",
+           "rb_pipeline_set_detect_mask", "rb_pipeline_push_masked", "rb_pipeline_masked_enqueue"]
 
 # ctypes prototypes of the asynchronous pushes (their tickets are int64_t, which ctypes' default conversion would cut to int)
 PROTOTYPES = {
@@ -210,6 +211,40 @@ def frame_table(frames, w, h):
     if not table:
         raise ValueError("frames: no frames")
     return fmt, dev, table
+
+
+def _mask_layout(a, h, w, what):
+    """(on_device, [(address, row stride)] per mask) of one (h, w) mask or one (n, h, w) array of masks, bool or uint8 with a
+    pixel stride of 1 byte and any row stride: the bytes the library reads in place.  ValueError otherwise."""
+    on_dev, shape, strides, u8, base = _array_layout(a)
+    dt = str(getattr(a, "dtype", ""))
+    if not (u8 or dt in ("bool", "torch.bool") or
+            (hasattr(a, "__cuda_array_interface__") and a.__cuda_array_interface__["typestr"] == "|b1")):
+        raise ValueError("%s: dtype %s, not bool or uint8" % (what, dt or "?"))
+    if len(shape) not in (2, 3) or tuple(shape[-2:]) != (h, w):
+        raise ValueError("%s: shape %s, not (%d, %d) or (n, %d, %d)" % (what, tuple(shape), h, w, h, w))
+    if strides[-1] != 1 or strides[-2] < w:
+        raise ValueError("%s: strides %s bytes; masks need a pixel stride of 1 and a row stride of at least %d"
+                         % (what, tuple(strides), w))
+    if len(shape) == 2:
+        return on_dev, [(base, int(strides[0]))]
+    return on_dev, [(base + i * int(strides[0]), int(strides[1])) for i in range(shape[0])]
+
+
+def mask_table(masks, w, h):
+    """How push_masked / enqueue pass per-frame detection masks, without copying anything: the FRAME table of a list of
+    CUDA (h, w) arrays or one CUDA (n, h, w) array, bool or uint8, any row stride.  ValueError for host arrays or anything
+    that cannot be read in place."""
+    items = list(masks) if isinstance(masks, (list, tuple)) else [masks]
+    table = []
+    for a in items:
+        on_dev, t = _mask_layout(a, h, w, "masks")
+        if not on_dev:
+            raise ValueError("masks: per-frame masks are device arrays (CUDA tensors); use set_detect_mask for a host mask")
+        table += t
+    if not table:
+        raise ValueError("masks: no masks")
+    return np.array(table, FRAME)
 
 
 def _format_nav(fn, nav, *args):
@@ -479,6 +514,19 @@ class Map:
         self.ctx.check(self.L.rb_map_detect(self.h_, C.byref(det), C.byref(t), C.byref(l), C.byref(kn)))
         return kn.value, t.value, l.value
 
+    def detect_masked(self, det, mask, tresh, l_kl_num, ss=None):
+        """detect() with a host detection mask, (h, w) bool or uint8 with any row stride: no keyline where it is zero
+        (rb_map_detect_masked).  ss: the map whose scale space is read (default this one)."""
+        mask = np.asarray(mask)
+        if mask.dtype == np.bool_:
+            mask = mask.view(np.uint8)
+        if mask.dtype != np.uint8 or mask.shape != (self.h, self.w) or mask.strides[1] != 1:
+            mask = np.ascontiguousarray(mask, np.uint8)
+        t, l, kn = C.c_double(tresh), C.c_int(l_kl_num), C.c_int(0)
+        self.ctx.check(self.L.rb_map_detect_masked(self.h_, (ss or self).h_, C.byref(det), _p(mask),
+                                                   C.c_int64(mask.strides[0]), C.byref(t), C.byref(l), C.byref(kn)))
+        return kn.value, t.value, l.value
+
     def reestimate(self, knum, nbins):
         o = C.c_float(0)
         self.ctx.check(self.L.rb_map_reestimate_thresh(self.h_, knum, nbins, C.byref(o)))
@@ -743,6 +791,44 @@ class Pipeline:
         self.check(fn(self.h_, fmt, _p(fr), _p(ts), n, _p(nav)))
         return nav
 
+    def set_detect_mask(self, mask):
+        """A fixed detection mask for every later push and enqueue (rb_pipeline_set_detect_mask): (h, w) bool or uint8, a
+        NumPy array or a CUDA array, any row stride; no keyline is detected where it is zero.  None clears it.  A CUDA mask is
+        copied after the work torch enqueued so far on its current stream."""
+        if mask is None:
+            self.check(self.L.rb_pipeline_set_detect_mask(self.h_, None, C.c_int64(0), 0))
+            return
+        if isinstance(mask, np.ndarray):
+            if mask.dtype == np.bool_:
+                mask = mask.view(np.uint8)
+            if mask.ndim == 2 and mask.strides[1] != 1:
+                mask = np.ascontiguousarray(mask)
+        on_dev, table = _mask_layout(mask, self.h, self.w, "set_detect_mask")
+        if len(table) != 1:
+            raise ValueError("set_detect_mask: one (%d, %d) mask" % (self.h, self.w))
+        if on_dev:
+            self._after_torch_stream()
+        ptr, step = table[0]
+        self.check(self.L.rb_pipeline_set_detect_mask(self.h_, C.c_void_p(ptr), C.c_int64(step), int(on_dev)))
+
+    def push_masked(self, frames, masks, ts):
+        """push_frames with per-frame detection masks (rb_pipeline_push_masked): masks is a list of CUDA (h, w) arrays or one
+        CUDA (n, h, w) array, bool or uint8, any row stride, read in place (see mask_table); no keyline is detected where a
+        frame's mask is zero.  Frames as push_frames takes them, host or device.  Frames and masks are ordered after the work
+        torch enqueued so far on its current stream.  A fixed mask (set_detect_mask) applies as well."""
+        fmt, on_dev, table = frame_table(frames, self.w, self.h)
+        mt = mask_table(masks, self.w, self.h)
+        ts = np.ascontiguousarray(ts, np.float64)
+        n = len(ts)
+        if len(table) != n or len(mt) != n:
+            raise ValueError("push_masked: %d frames, %d masks, %d timestamps" % (len(table), len(mt), n))
+        self._after_torch_stream()
+        fr = np.array(table, FRAME)
+        nav = np.zeros(n, NAV)
+        self._consumer_fence()
+        self.check(self.L.rb_pipeline_push_masked(self.h_, fmt, int(on_dev), _p(fr), _p(mt), _p(ts), n, _p(nav)))
+        return nav
+
     def _after_torch_stream(self):
         """The pipeline's stream waits for the work torch enqueued so far on its current stream of this device: an event
         recorded there (one event, reused: a wait takes the record made just before it)."""
@@ -823,14 +909,24 @@ class Pipeline:
             base = frames.__array_interface__["data"][0]
         return self.L.rb_pipeline_enqueue, (want, int(on_dev), C.c_void_p(base)), (frames,), on_dev
 
-    def enqueue(self, frames, ts, fmt="rgb"):
+    def enqueue(self, frames, ts, fmt="rgb", masks=None):
         """Hand over n frames without waiting for them (rb_pipeline_enqueue / enqueue_frames); returns the ticket to wait.
         frames: a uint8 host array or torch CUDA tensor of packed frames, (n, h, w, 3) for fmt="rgb" or (n, h, w) for
         fmt="mono", or a list of strided frames as push_frames takes them.  The frames are kept alive until the ticket is
         waited.  Device frames: the call first waits (on the host) for the work torch enqueued so far on its current stream,
         so that they are complete.  Device output mode: the enqueue's writes wait for torch's current stream, as a push's.
-        RbError when `depth` tickets are outstanding (nothing changes) or asynchronous pushes are off."""
+        masks: per-frame detection masks as push_masked takes them (rb_pipeline_masked_enqueue), kept alive with the frames
+        and read after the work torch enqueued so far on its current stream.  RbError when `depth` tickets are outstanding
+        (nothing changes) or asynchronous pushes are off."""
         fn, args, keep, on_dev = self._enqueue_args(frames, ts, fmt)
+        if masks is not None:
+            f, on_dev, table = frame_table(frames, self.w, self.h)
+            mt = mask_table(masks, self.w, self.h)
+            if len(mt) != len(ts):
+                raise ValueError("enqueue: %d masks, %d timestamps" % (len(mt), len(ts)))
+            fr = np.array(table, FRAME)
+            fn, args, keep = self.L.rb_pipeline_masked_enqueue, (f, int(on_dev), _p(fr), _p(mt)), (frames, fr, masks, mt)
+            self._after_torch_stream()
         ts = np.ascontiguousarray(ts, np.float64)
         if on_dev or self._out_dev:
             import torch

@@ -510,20 +510,17 @@ extern "C" int rb_map_detect(rb_map *m, const rb_detect_params *p, double *tresh
     RB_ENTER(m->c);
     return rb_map_detect_ss(m, m, p, tresh, l_kl_num, kn_out);
 }
-extern "C" int rb_map_detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p, double *tresh, int *l_kl_num,
-                                int *kn_out) {
-    if (!m) return RB_ERR_ARG;
-    RB_ENTER(m->c);
-    if (!m || !ss) return RB_ERR_ARG;
+// rb_map_detect_ss with the detection masks at mask_dev (nullptr: the unmasked detector)
+static int detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p, double *tresh, int *l_kl_num, int *kn_out,
+                     const DetMask *mask_dev) {
     rb_ctx *c = m->c;
-    if (!ss->img0 || ss->c != c || !p || !tresh || !l_kl_num) return RB_ERR_ARG;
     DetChain *ch_dev = (DetChain *)((char *)c->dev_small + RB_DS_CHAIN);
     DetChain *ch_host = (DetChain *)((char *)c->pinned + RB_DS_CHAIN);
     ch_host->tresh = *tresh;
     ch_host->l_kl_num = *l_kl_num;
     ch_host->pad = 0;
     RB_CUDA(cudaMemcpyAsync(ch_dev, ch_host, sizeof(DetChain), cudaMemcpyHostToDevice, c->stream));
-    int r = rb_detect_enqueue(c, m, ss->img0, ss->dog, p, ch_dev);
+    int r = rb_detect_enqueue(c, m, ss->img0, ss->dog, p, ch_dev, mask_dev);
     if (r) return r;
     RB_CUDA(cudaMemcpyAsync(ch_host, ch_dev, sizeof(DetChain), cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
@@ -531,6 +528,46 @@ extern "C" int rb_map_detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p
     *l_kl_num = ch_host->l_kl_num;
     if (kn_out) *kn_out = ch_host->l_kl_num;
     return RB_OK;
+}
+extern "C" int rb_map_detect_ss(rb_map *m, rb_map *ss, const rb_detect_params *p, double *tresh, int *l_kl_num,
+                                int *kn_out) {
+    if (!m) return RB_ERR_ARG;
+    RB_ENTER(m->c);
+    if (!m || !ss) return RB_ERR_ARG;
+    rb_ctx *c = m->c;
+    if (!ss->img0 || ss->c != c || !p || !tresh || !l_kl_num) return RB_ERR_ARG;
+    return detect_ss(m, ss, p, tresh, l_kl_num, kn_out, nullptr);
+}
+// the host mask is copied into a device buffer of this call (a stage-level entry point: tests and tools)
+extern "C" int rb_map_detect_masked(rb_map *m, rb_map *ss, const rb_detect_params *p, const uint8_t *mask, int64_t step,
+                                    double *tresh, int *l_kl_num, int *kn_out) {
+    if (!m) return RB_ERR_ARG;
+    RB_ENTER(m->c);
+    if (!ss) return RB_ERR_ARG;
+    rb_ctx *c = m->c;
+    if (!ss->img0 || ss->c != c || !p || !tresh || !l_kl_num || !mask || step < c->w) return RB_ERR_ARG;
+    unsigned char *buf = nullptr;
+    const size_t off = ((size_t)c->N + 255) & ~(size_t)255;
+    RB_CUDA(cudaMalloc(&buf, off + sizeof(DetMask)));
+    DetMask dm;
+    dm.fixed = nullptr;
+    dm.fixed_step = 0;
+    dm.frame = buf;
+    dm.frame_step = c->w;
+    cudaError_t e = cudaMemcpy2DAsync(buf, (size_t)c->w, mask, (size_t)step, (size_t)c->w, c->h, cudaMemcpyHostToDevice,
+                                      c->stream);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(buf + off, &dm, sizeof(dm), cudaMemcpyHostToDevice, c->stream);
+    int r = RB_OK;
+    if (e != cudaSuccess) {
+        snprintf(c->err, sizeof(c->err), "detect_masked: %s", cudaGetErrorString(e));
+        r = RB_ERR_CUDA;
+    } else {
+        r = detect_ss(m, ss, p, tresh, l_kl_num, kn_out, reinterpret_cast<const DetMask *>(buf + off));
+    }
+    cudaStreamSynchronize(c->stream);
+    cudaFree(buf);
+    return r;
 }
 
 extern "C" int rb_map_reestimate_thresh(rb_map *m, int knum, int nbins, float *out_thresh) {

@@ -62,6 +62,15 @@ struct DetChain {
     int pad;
 };
 
+// detection masks of one frame (rb_pipeline_set_detect_mask, rb_pipeline_push_masked): w x h bytes each with a row step,
+// nullptr when not set.  A pixel is a candidate only where no mask that is set holds a zero byte.
+struct DetMask {
+    const uint8_t *fixed;
+    int64_t fixed_step;
+    const uint8_t *frame;
+    int64_t frame_step;
+};
+
 struct BoxPlan {
     int d[2][3];         // box widths per filter (iigauss.cpp:43-81)
     double sigma_r[2];
@@ -265,6 +274,7 @@ int rb_dog_make_tmaps(rb_ctx *c, DogWS *ws);
 int rb_gray_enqueue(rb_ctx *c, DogWS *ws, const rb_undistort *und, bool mono, const void *const *src_pp,
                     const rb_frame *frames_dev, int nimg);
 // detect.cu
+// mask_dev: the frame's masks (device memory), or nullptr for the unmasked detector
 int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
-                      const rb_detect_params *p, DetChain *chain_dev);
+                      const rb_detect_params *p, DetChain *chain_dev, const DetMask *mask_dev = nullptr);
 int rb_reestimate_enqueue(rb_ctx *c, rb_map *m, int knum, int nbins);

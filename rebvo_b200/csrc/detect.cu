@@ -5,7 +5,8 @@
 //   k_update_thresh : the P-controller on the device-resident feedback state (no host round trip)
 //   k_detect_a<R>   : all per-pixel tests in the (2R+1)^2 window of DetectorPlaneFitSize R = 1..4; candidates get
 //                     mask=-2 and a float4 payload {m.x,m.y,xs,ys}; one warp owns a (row, 32-pixel) segment and writes
-//                     its candidate count
+//                     its candidate count.  k_detect_a_masked<R>: the same with the frame's detection masks gating the
+//                     candidate test (a masked pixel is simply not a candidate; nothing after the test changes)
 //   k_seg_scan      : exclusive scan of the segment counts in raster order -> keyline ids, kn=min(total,kl_max)
 //   k_detect_b      : ordered scatter of the keyline records (SoA) and of the id mask, cut at kl_max
 //   k_join          : NextPoint/join_edges; "last writer wins" on p_id == atomicMax of the writer id
@@ -37,14 +38,13 @@ __global__ void k_update_thresh(DetChain *ch, MapState *st, double gain, int kl_
 // grid: (ceil(w/32), ceil(h/DET_BY)), block (32, DET_BY).  R = DetectorPlaneFitSize (build_mask's win_s): a (2R+1)^2
 // window, interior R <= x < w-R, R <= y < h-R (edge_finder.cpp:108-109).  img0 / dog are scale-space planes with rows of
 // `pitch` floats; mask and cand are w-indexed.
-template <int R>
-__global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restrict__ img0,
-                                                          const float *__restrict__ dog,
-                                                          int *__restrict__ mask,
-                                                          float4 *__restrict__ cand,
-                                                          int *__restrict__ seg_cnt,
-                                                          const MapState *__restrict__ st, int w, int h, int pitch,
-                                                          int nchunk, float per_hist, float dog_thesh_f) {
+// MASKED: the instance for frames with detection masks (dm, DetMask): a pixel whose byte is zero in a mask that is set is
+// not a candidate.  Each interior pixel reads one byte of each mask, coalesced along the warp's row segment.
+template <int R, bool MASKED>
+__device__ __forceinline__ void detect_a(const float *__restrict__ img0, const float *__restrict__ dog,
+                                         int *__restrict__ mask, float4 *__restrict__ cand, int *__restrict__ seg_cnt,
+                                         const MapState *__restrict__ st, int w, int h, int pitch, int nchunk,
+                                         float per_hist, float dog_thesh_f, const DetMask *__restrict__ dm) {
     constexpr int NW = 2 * R + 1;                  // window width
     constexpr int TW = 32 + 2 * R, TH = DET_BY + 2 * R;
     constexpr int P0 = rb_pinv_offset(R), P1 = P0 + NW * NW, P2 = P1 + NW * NW;   // rows of PInv in c_pinv
@@ -66,11 +66,18 @@ __global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restric
     if (interior) {
         const size_t idx = (size_t)y * w + x, ip = (size_t)y * pitch + x;
         const float grad_thesh = st->thresh_used;
-        const float gx = img0[ip + 1] - img0[ip - 1];     // sspace::calc_gradient
-        const float gy = img0[ip + pitch] - img0[ip - pitch];
-        const float n2gI = gx * gx + gy * gy;             // util::norm2
         const float t1 = grad_thesh * (float)RB_MAX_IMG_VALUE;
-        bool ok = !(n2gI < t1 * t1);                      // edge_finder.cpp:117-120
+        bool ok = true;
+        if (MASKED) {
+            const uint8_t *fixed = dm->fixed, *frame = dm->frame;
+            ok = !(fixed && fixed[(size_t)y * dm->fixed_step + x] == 0) && !(frame && frame[(size_t)y * dm->frame_step + x] == 0);
+        }
+        if (ok) {
+            const float gx = img0[ip + 1] - img0[ip - 1];     // sspace::calc_gradient
+            const float gy = img0[ip + pitch] - img0[ip - pitch];
+            const float n2gI = gx * gx + gy * gy;             // util::norm2
+            ok = !(n2gI < t1 * t1);                           // edge_finder.cpp:117-120
+        }
         if (ok) {
             int pn = 0;
 #pragma unroll
@@ -112,6 +119,27 @@ __global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restric
     }
     const unsigned bal = __ballot_sync(0xffffffffu, is_cand);
     if (lane == 0) seg_cnt[y * nchunk + blockIdx.x] = __popc(bal);
+}
+template <int R>
+__global__ void __launch_bounds__(32 * DET_BY) k_detect_a(const float *__restrict__ img0,
+                                                          const float *__restrict__ dog,
+                                                          int *__restrict__ mask,
+                                                          float4 *__restrict__ cand,
+                                                          int *__restrict__ seg_cnt,
+                                                          const MapState *__restrict__ st, int w, int h, int pitch,
+                                                          int nchunk, float per_hist, float dog_thesh_f) {
+    detect_a<R, false>(img0, dog, mask, cand, seg_cnt, st, w, h, pitch, nchunk, per_hist, dog_thesh_f, nullptr);
+}
+template <int R>
+__global__ void __launch_bounds__(32 * DET_BY) k_detect_a_masked(const float *__restrict__ img0,
+                                                                 const float *__restrict__ dog,
+                                                                 int *__restrict__ mask,
+                                                                 float4 *__restrict__ cand,
+                                                                 int *__restrict__ seg_cnt,
+                                                                 const MapState *__restrict__ st, int w, int h,
+                                                                 int pitch, int nchunk, float per_hist,
+                                                                 float dog_thesh_f, const DetMask *__restrict__ dm) {
+    detect_a<R, true>(img0, dog, mask, cand, seg_cnt, st, w, h, pitch, nchunk, per_hist, dog_thesh_f, dm);
 }
 
 // A detect with a wider window than the map's previous one: the pixels between the two margins leave the interior, and
@@ -342,7 +370,7 @@ __global__ void __launch_bounds__(256) k_nm_histo(const float *__restrict__ n_m,
 
 // ---------------------------------------------------------------------------------------------------
 int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
-                      const rb_detect_params *p, DetChain *chain_dev) {
+                      const rb_detect_params *p, DetChain *chain_dev, const DetMask *mask_dev) {
     const int R = p->plane_fit_size;
     if (R < 1 || R > RB_PLANE_FIT_MAX) {   // (0: Phi^T Phi is singular)
         snprintf(c->err, sizeof(c->err), "DetectorPlaneFitSize must be 1..%d", RB_PLANE_FIT_MAX);
@@ -367,8 +395,15 @@ int rb_detect_enqueue(rb_ctx *c, rb_map *m, const float *img0, const float *dog,
     void (*const detect_a[RB_PLANE_FIT_MAX])(const float *, const float *, int *, float4 *, int *, const MapState *, int,
                                              int, int, int, float, float) = {k_detect_a<1>, k_detect_a<2>, k_detect_a<3>,
                                                                               k_detect_a<4>};
-    detect_a[R - 1]<<<ga, ba, 0, c->stream>>>(img0, dog, m->mask, c->cand, c->seg_cnt, m->st, w, h, c->pitch, nchunk,
-                                              (float)p->pos_neg_thresh, (float)p->dog_thresh);
+    void (*const detect_a_masked[RB_PLANE_FIT_MAX])(const float *, const float *, int *, float4 *, int *, const MapState *,
+                                                    int, int, int, int, float, float, const DetMask *) = {
+        k_detect_a_masked<1>, k_detect_a_masked<2>, k_detect_a_masked<3>, k_detect_a_masked<4>};
+    if (mask_dev)
+        detect_a_masked[R - 1]<<<ga, ba, 0, c->stream>>>(img0, dog, m->mask, c->cand, c->seg_cnt, m->st, w, h, c->pitch,
+                                                         nchunk, (float)p->pos_neg_thresh, (float)p->dog_thresh, mask_dev);
+    else
+        detect_a[R - 1]<<<ga, ba, 0, c->stream>>>(img0, dog, m->mask, c->cand, c->seg_cnt, m->st, w, h, c->pitch, nchunk,
+                                                  (float)p->pos_neg_thresh, (float)p->dog_thresh);
     RB_LAUNCH_CHECK();
     const int nseg = h * nchunk;
     k_seg_scan<<<1, 1024, 0, c->stream>>>(c->seg_cnt, nseg, m->st, chain_dev, kl_max);

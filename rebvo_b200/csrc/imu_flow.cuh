@@ -327,14 +327,16 @@ static int imu_live_check(rb_pipeline *pl, const ImuFlow &f, const double *ts, i
 }
 
 // a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking
-// (rgb, frames, fmt as push_impl's)
+// (rgb, frames, fmt as push_impl's; masked: det_mask_pin holds the frames' detection masks)
 static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device,
-                    const double *ts, int n, rb_nav *nav_out, rb_odometry *odom_out) {
+                    const double *ts, int n, rb_nav *nav_out, rb_odometry *odom_out, bool masked) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
     if (!on_device && (r = stage_host_frames(pl, rgb, frames, fmt, 0, n, c->stream))) return r;
     if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;
+    if (masked)
+        RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, pl->det_mask_pin, sizeof(DetMask) * n, cudaMemcpyHostToDevice, c->stream));
     pl->sb_pin[0].src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
     RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
     if ((r = rb_gray_enqueue(c, &pl->ws, pl->und, in_mono(fmt), &pl->sb_dev->src, in_strided(fmt) ? pl->frames_dev : nullptr,
@@ -345,7 +347,7 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_fr
         const long long fr = pl->n_pushed + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
         const float *img0 = pl->ws.img0 + (size_t)i * c->NP, *dog = pl->ws.dog + (size_t)i * c->NP;
-        if ((r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain))) return r;
+        if ((r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain, masked ? pl->det_mask_dev + i : nullptr))) return r;
         if ((r = rb_reestimate_enqueue(c, neu, p.TrackPoints, p.QCutOffNumBins))) return r;
         // FirstThr :296: the gyro / accelerometer samples between the previous frame and this one
         const rbimu::ImuIntegral imu = f.buf.grab(f.t_prev_grab + f.ip.TimeDesinc, ts[i] + f.ip.TimeDesinc);

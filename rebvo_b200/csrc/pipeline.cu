@@ -64,6 +64,8 @@ struct AsyncSlot {
     struct FrameArgs *fa;             // pinned [max_batch]: per-frame scalars, the source of the back's fa_dev copy
     SubBatchPtrs *tbl;                // pinned [2]: the front's table (src) and the back's (mirror and depth destinations)
     rb_frame *frames;                 // pinned [max_batch]: strided device input, the source of the front's frame table
+    DetMask *masks;                   // pinned [max_batch]: the detection masks of a masked ticket, the source of the back's
+                                      // det_mask_dev copy (detection runs in the back)
     unsigned char *mirror_host, *mirror_dev, *depth_host, *depth_dev, *dimg_host, *dimg_dev;   // the slot's outputs
     size_t mirror_host_bytes, mirror_dev_bytes, depth_host_bytes, depth_dev_bytes, dimg_host_bytes, dimg_dev_bytes;
     cudaEvent_t done;                 // recorded on the tracker stream after the ticket's last copy
@@ -77,7 +79,8 @@ struct AsyncRing {
     cudaStream_t front;
     cudaEvent_t ev_front[2];          // per workspace: its front is complete (the back waits for it)
     cudaEvent_t ev_free[2];           // per workspace: the back that read it last is complete (the next front waits for it)
-    // captured halves: the front per (input format, workspace, batch size), the back per (workspace, ring phase, batch size)
+    // captured halves: the front per (input format, workspace, batch size), the back per (masked, workspace, ring phase, batch
+    // size)
     cudaGraphExec_t *gfront, *gback;
     int *lfront, *lback;              // kernel launches inside each graph
 };
@@ -118,6 +121,13 @@ struct rb_pipeline {
     // packed pushes' per-sub-batch copy does not grow.
     rb_frame *frames_dev;         // device [max_batch]
     rb_frame *frames_pin;         // pinned [max_batch]
+    // detection masks (rb_pipeline_set_detect_mask, rb_pipeline_push_masked): a masked push writes frame i's DetMask into
+    // det_mask_dev[i] before its batch, as frames_dev, so that one captured batch serves every mask buffer.  Unmasked pushes
+    // neither write nor read the table.  det_fixed: the fixed mask, packed w x h (kept when cleared, for the next set).
+    DetMask *det_mask_dev;        // device [max_batch]
+    DetMask *det_mask_pin;        // pinned [max_batch]
+    unsigned char *det_fixed;     // device [w * h]
+    bool det_fixed_on;
     int sub;                      // head sub-batch of a host-input push (env REBVO_B200_SUB, default 8 frames)
     int last_sub;                 // frames of the last scale-space batch (the rest of a head / rest push): ws slots in use
     DetChain *chain;      // device
@@ -135,9 +145,9 @@ struct rb_pipeline {
     cudaEvent_t user_ev[8];
     float stage_ms[6];
     struct FrameArgs *fa_dev, *fa_pin;
-    // one instantiated CUDA graph per (input format, ring phase of the first frame, batch size): the kernel sequence of a
-    // batch is static once the per-frame scalars live in fa_dev
-    cudaGraphExec_t *gexec;       // [RB_NFMT * RB_NMAPS * (max_batch + 1)], see graph_slot
+    // one instantiated CUDA graph per (masked, input format, ring phase of the first frame, batch size): the kernel sequence
+    // of a batch is static once the per-frame scalars live in fa_dev
+    cudaGraphExec_t *gexec;       // [2 * RB_NFMT * RB_NMAPS * (max_batch + 1)], see graph_slot
     int *glaunches;               // kernel launches inside each graph
     bool use_graph;
     // optional in-situ stage profile (REBVO_B200_STAGE_PROF=1, forces eager launches): CUDA events between stages
@@ -223,18 +233,19 @@ enum { RB_IN_RGB = 0, RB_IN_MONO = 1, RB_IN_RGB_STRIDED = 2, RB_IN_MONO_STRIDED 
 static inline bool in_mono(int fmt) { return fmt == RB_IN_MONO || fmt == RB_IN_MONO_STRIDED; }
 static inline bool in_strided(int fmt) { return fmt == RB_IN_RGB_STRIDED || fmt == RB_IN_MONO_STRIDED; }
 static inline size_t frame_bytes(const rb_ctx *c, int fmt) { return (in_mono(fmt) ? (size_t)1 : (size_t)3) * c->N; }
-static inline int graph_slots(const rb_pipeline *pl) { return RB_NFMT * RB_NMAPS * (pl->max_batch + 1); }
-static inline int graph_slot(const rb_pipeline *pl, int fmt, int phase, int n) {
-    return (fmt * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
+// (masked: the batch detects through k_detect_a_masked, with the frames' detection masks in det_mask_dev)
+static inline int graph_slots(const rb_pipeline *pl) { return 2 * RB_NFMT * RB_NMAPS * (pl->max_batch + 1); }
+static inline int graph_slot(const rb_pipeline *pl, bool masked, int fmt, int phase, int n) {
+    return (((masked ? RB_NFMT : 0) + fmt) * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
 }
 // the asynchronous pushes' halves (AsyncRing::gfront / gback)
 static inline int afront_slots(const rb_pipeline *pl) { return RB_NFMT * 2 * (pl->max_batch + 1); }
 static inline int afront_slot(const rb_pipeline *pl, int fmt, int par, int n) {
     return (fmt * 2 + par) * (pl->max_batch + 1) + n;
 }
-static inline int aback_slots(const rb_pipeline *pl) { return 2 * RB_NMAPS * (pl->max_batch + 1); }
-static inline int aback_slot(const rb_pipeline *pl, int par, int phase, int n) {
-    return (par * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
+static inline int aback_slots(const rb_pipeline *pl) { return 2 * 2 * RB_NMAPS * (pl->max_batch + 1); }
+static inline int aback_slot(const rb_pipeline *pl, bool masked, int par, int phase, int n) {
+    return (((masked ? 2 : 0) + par) * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
 }
 static void drop_execs(cudaGraphExec_t *g, int n) {
     for (int i = 0; g && i < n; i++)
@@ -314,6 +325,18 @@ static int write_frame_table(rb_pipeline *pl, const rb_frame *frames, int n) {
     memcpy(pl->frames_pin, frames, sizeof(rb_frame) * n);
     RB_CUDA(cudaMemcpyAsync(pl->frames_dev, pl->frames_pin, sizeof(rb_frame) * n, cudaMemcpyHostToDevice, c->stream));
     return RB_OK;
+}
+// the detection masks of the n frames of a push into dst (pinned): the fixed mask and masks[i] (device rb_frame entries, or
+// nullptr).  False, writing nothing, when no mask applies: the push runs the unmasked batches.
+static bool fill_masks(const rb_pipeline *pl, const rb_frame *masks, int n, DetMask *dst) {
+    if (!masks && !pl->det_fixed_on) return false;
+    for (int i = 0; i < n; i++) {
+        dst[i].fixed = pl->det_fixed_on ? pl->det_fixed : nullptr;
+        dst[i].fixed_step = pl->c->w;
+        dst[i].frame = masks ? masks[i].data : nullptr;
+        dst[i].frame_step = masks ? masks[i].step : 0;
+    }
+    return true;
 }
 #include "imu_flow.cuh"
 static void async_free(rb_pipeline *pl);
@@ -475,6 +498,8 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
         RB_CUDA(cudaMallocHost(&pl->sb_pin, 2 * sizeof(SubBatchPtrs)));
         RB_CUDA(cudaMalloc(&pl->frames_dev, sizeof(rb_frame) * max_batch));
         RB_CUDA(cudaMallocHost(&pl->frames_pin, sizeof(rb_frame) * max_batch));
+        RB_CUDA(cudaMalloc(&pl->det_mask_dev, sizeof(DetMask) * max_batch));
+        RB_CUDA(cudaMallocHost(&pl->det_mask_pin, sizeof(DetMask) * max_batch));
         RB_CUDA(cudaEventCreateWithFlags(&pl->ev_hop, cudaEventDisableTiming));
         for (int i = 0; i < 2; i++) {
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
@@ -599,10 +624,10 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
     if (pl->und) rb_undistort_destroy(pl->und);
     rb_dogws_free(&pl->ws);
     void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->frames_dev, pl->mirror.dev, pl->odom.dev,
-                   pl->depth.stage, pl->depth.ws, pl->depth.dev, pl->dimg.dev};
+                   pl->depth.stage, pl->depth.ws, pl->depth.dev, pl->dimg.dev, pl->det_mask_dev, pl->det_fixed};
     for (void *p : dev) cudaFree(p);
     void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->frames_pin, pl->mirror.host, pl->odom.pin,
-                    pl->depth.host, pl->dimg.host, pl->state_host};
+                    pl->depth.host, pl->dimg.host, pl->state_host, pl->det_mask_pin};
     for (void *p : host)
         if (p) cudaFreeHost(p);
     rb_ctx_destroy(c);
@@ -764,8 +789,9 @@ static int enqueue_front(rb_pipeline *pl, DogWS *ws, SubBatchPtrs *tbl, const rb
     return RB_OK;
 }
 
-// the back of a batch: per frame detect + track + map on the scale space in ws, and the per-frame outputs
-static int enqueue_back(rb_pipeline *pl, const DogWS *ws, int n, long long first_frame) {
+// the back of a batch: per frame detect + track + map on the scale space in ws, and the per-frame outputs.  masked: frame i
+// detects through the detection masks of det_mask_dev[i].
+static int enqueue_back(rb_pipeline *pl, const DogWS *ws, int n, long long first_frame, bool masked) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     int r;
@@ -787,7 +813,7 @@ static int enqueue_back(rb_pipeline *pl, const DogWS *ws, int n, long long first
             c->stream = pl->det_stream;
         }
         RB_TRACE(c->stream, 6);
-        r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain);
+        r = rb_detect_enqueue(c, neu, img0, dog, &p.det, pl->chain, masked ? pl->det_mask_dev + i : nullptr);
         prof_mark(pl, ST_DETECT);
         if (!r) r = rb_reestimate_enqueue(c, neu, p.TrackPoints, p.QCutOffNumBins);
         prof_mark(pl, ST_REEST);
@@ -852,9 +878,9 @@ static int enqueue_back(rb_pipeline *pl, const DogWS *ws, int n, long long first
 }
 
 // everything of a batch after the H2D copy, on the tracker stream in the pipeline's workspace: front, then back
-static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame, bool with_events) {
+static int enqueue_batch(rb_pipeline *pl, int fmt, int n, long long first_frame, bool with_events, bool masked) {
     int r = enqueue_front(pl, &pl->ws, pl->sb_dev, pl->frames_dev, fmt, n, with_events);
-    return r ? r : enqueue_back(pl, &pl->ws, n, first_frame);
+    return r ? r : enqueue_back(pl, &pl->ws, n, first_frame, masked);
 }
 
 // Capture the work body() enqueues on stream s (and the streams it forks) as one graph, instantiated into *exec; *launches
@@ -888,9 +914,10 @@ static int capture_graph(rb_pipeline *pl, cudaStream_t s, F &&body, cudaGraphExe
 }
 
 // rgb: n packed frames of frame_bytes(fmt) each, host or device memory; or (rgb == nullptr) frames: n strided frames, checked
-// by push_frames, whose layout is fmt (device memory) or whose packed format is fmt (host memory)
+// by push_frames, whose layout is fmt (device memory) or whose packed format is fmt (host memory).  masks: n per-frame
+// detection masks in device memory, checked by check_masks, or nullptr.
 static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
-                     int n, rb_nav *nav_out) {
+                     int n, rb_nav *nav_out, const rb_frame *masks = nullptr) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts) return RB_ERR_ARG;
@@ -907,9 +934,10 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
     pl->depth.n = 0;
     pl->dimg.n = 0;
     pl->last_sub = 0;
+    const bool masked = fill_masks(pl, masks, n, pl->det_mask_pin);
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
         if ((r = imu_push(pl, *pl->imu, rgb, frames, fmt, on_device, ts, n, pl->nav_pin,
-                          pl->odom.on ? pl->odom.pin : nullptr)))
+                          pl->odom.on ? pl->odom.pin : nullptr, masked)))
             return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
         pl->last_sub = n;   // (one scale-space batch)
@@ -956,6 +984,9 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
         const long long first_j = first + (long long)off;
         if (!on_device && nsub > 1) RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_copy[j], 0));
         RB_CUDA(cudaMemcpyAsync(pl->fa_dev, pl->fa_pin + off, sizeof(FrameArgs) * nj, cudaMemcpyHostToDevice, c->stream));
+        if (masked)
+            RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, pl->det_mask_pin + off, sizeof(DetMask) * nj, cudaMemcpyHostToDevice,
+                                    c->stream));
         SubBatchPtrs &t = pl->sb_pin[j];
         t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);   // (strided: unused)
         if (pl->mirror.on) {
@@ -972,18 +1003,18 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
         RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
         const bool graph_ok = pl->use_graph && first_j > 0;
         if (!graph_ok) {
-            if ((r = enqueue_batch(pl, fmt, nj, first_j, j == 0))) return r;
+            if ((r = enqueue_batch(pl, fmt, nj, first_j, j == 0, masked))) return r;
         } else {
-            const int key = graph_slot(pl, fmt, (int)(first_j % RB_NMAPS), nj);
+            const int key = graph_slot(pl, masked, fmt, (int)(first_j % RB_NMAPS), nj);
             // capture the batch once per ring phase; replays only differ through fa_dev / sb_dev contents.  All
             // phases of this format and batch size are instantiated together, so that no later push pays for a capture.
             // The other format's graphs are left as they are: a stream may alternate formats.
             const bool build = !pl->gexec[key];
             for (int ph = 0; ph < RB_NMAPS && build; ph++) {
-                const int k = graph_slot(pl, fmt, ph, nj);
+                const int k = graph_slot(pl, masked, fmt, ph, nj);
                 if (pl->gexec[k]) continue;
                 // (any first frame > 0 of that phase)
-                auto body = [&]() { return enqueue_batch(pl, fmt, nj, ph == 0 ? RB_NMAPS : ph, false); };
+                auto body = [&]() { return enqueue_batch(pl, fmt, nj, ph == 0 ? RB_NMAPS : ph, false, masked); };
                 if ((r = capture_graph(pl, c->stream, body, &pl->gexec[k], &pl->glaunches[k]))) return r;
             }
             if (j == 0) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
@@ -1106,7 +1137,7 @@ static void async_free(rb_pipeline *pl) {
         if (e) cudaEventDestroy(e);
     for (AsyncSlot &s : ar->slot) {
         if (s.done) cudaEventDestroy(s.done);
-        void *host[] = {s.nav, s.odom, s.abort, s.fa, s.tbl, s.frames, s.mirror_host, s.depth_host, s.dimg_host};
+        void *host[] = {s.nav, s.odom, s.abort, s.fa, s.tbl, s.frames, s.masks, s.mirror_host, s.depth_host, s.dimg_host};
         for (void *p : host)
             if (p) cudaFreeHost(p);
         void *dev[] = {s.mirror_dev, s.depth_dev, s.dimg_dev};
@@ -1156,6 +1187,7 @@ static int async_alloc(rb_pipeline *pl, int depth) {
         RB_CUDA(cudaMallocHost(&s.fa, sizeof(FrameArgs) * mb));
         RB_CUDA(cudaMallocHost(&s.tbl, 2 * sizeof(SubBatchPtrs)));
         RB_CUDA(cudaMallocHost(&s.frames, sizeof(rb_frame) * mb));
+        RB_CUDA(cudaMallocHost(&s.masks, sizeof(DetMask) * mb));
         RB_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     }
     return async_grow(pl);
@@ -1442,6 +1474,50 @@ extern "C" int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb
     return push_frames(pl, format, frames, ts, n, nav_out, true);
 }
 
+// ---- detection masks (DESIGN.md §5) --------------------------------------------------------------------------------------
+extern "C" int rb_pipeline_set_detect_mask(rb_pipeline *pl, const uint8_t *mask, int64_t step, int on_device) {
+    if (!pl) return RB_ERR_ARG;
+    rb_ctx *c = pl->c;
+    RB_ENTER(c);
+    if (mask && step < c->w) {
+        snprintf(c->err, sizeof(c->err), "set_detect_mask: step %lld is shorter than a row (%d bytes)", (long long)step, c->w);
+        return RB_ERR_ARG;
+    }
+    int r = set_begin(pl, nullptr);
+    if (r) return r;
+    // (no captured batch changes: masked pushes read the fixed mask through det_mask_dev, unmasked ones never see it)
+    pl->det_fixed_on = false;
+    if (!mask) return RB_OK;
+    if (!pl->det_fixed) RB_CUDA(cudaMalloc(&pl->det_fixed, (size_t)c->N));
+    RB_CUDA(cudaMemcpy2DAsync(pl->det_fixed, (size_t)c->w, mask, (size_t)step, (size_t)c->w, c->h,
+                              on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    pl->det_fixed_on = true;
+    return RB_OK;
+}
+// per-frame detection masks: n device {data, step} entries, each step at least a row of w bytes
+static int check_masks(rb_pipeline *pl, const char *what, const rb_frame *masks, int n) {
+    rb_ctx *c = pl->c;
+    if (!masks) {
+        snprintf(c->err, sizeof(c->err), "%s: no masks", what);
+        return RB_ERR_ARG;
+    }
+    for (int i = 0; i < n; i++)
+        if (!masks[i].data || masks[i].step < c->w) {
+            snprintf(c->err, sizeof(c->err), "%s: mask %d has %s (rows need %d bytes)", what, i,
+                     masks[i].data ? "a step shorter than a row" : "no data", c->w);
+            return RB_ERR_ARG;
+        }
+    return RB_OK;
+}
+extern "C" int rb_pipeline_push_masked(rb_pipeline *pl, int format, int on_device, const rb_frame *frames,
+                                       const rb_frame *masks, const double *ts, int n, rb_nav *nav_out) {
+    if (!pl) return RB_ERR_ARG;
+    int fmt = 0, r = check_frames(pl, "push_masked", format, frames, ts, n, on_device != 0, &fmt);
+    if (!r) r = check_masks(pl, "push_masked", masks, n);
+    return r ? r : push_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, nav_out, masks);
+}
+
 // ---- asynchronous pushes (DESIGN.md §5) ----------------------------------------------------------------------------------
 extern "C" int rb_pipeline_set_async(rb_pipeline *pl, int depth) {
     if (!pl) return RB_ERR_ARG;
@@ -1461,7 +1537,7 @@ extern "C" int rb_pipeline_set_async(rb_pipeline *pl, int depth) {
 // one ticket: the front on the front stream into workspace k % 2, the back on the tracker stream into output slot
 // k % depth.  Arguments as push_impl's.
 static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
-                        int n, int64_t *ticket) {
+                        int n, int64_t *ticket, const rb_frame *masks = nullptr) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
     AsyncRing *ar = pl->ar;
@@ -1522,6 +1598,10 @@ static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *fra
     if (pl->out_dev && pl->consumer != c->stream && (r = stream_wait(pl, pl->consumer, c->stream))) return r;
     RB_CUDA(cudaStreamWaitEvent(c->stream, ar->ev_front[par], 0));
     RB_CUDA(cudaMemcpyAsync(pl->fa_dev, s.fa, sizeof(FrameArgs) * n, cudaMemcpyHostToDevice, c->stream));
+    // (the slot's table: its previous ticket, the last reader of s.masks, has been waited)
+    const bool masked = fill_masks(pl, masks, n, s.masks);
+    if (masked)
+        RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, s.masks, sizeof(DetMask) * n, cudaMemcpyHostToDevice, c->stream));
     SubBatchPtrs &t = s.tbl[1];
     memset(&t, 0, sizeof(t));
     if (pl->mirror.on) {   // (host mode: the pipeline's staging, then the slot's mapped memory; device mode: the slot)
@@ -1535,17 +1615,17 @@ static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *fra
     }
     RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
     if (!pl->use_graph || first == 0) {
-        if ((r = enqueue_back(pl, ws, n, first))) return r;
+        if ((r = enqueue_back(pl, ws, n, first, masked))) return r;
     } else {
-        const int key = aback_slot(pl, par, (int)(first % RB_NMAPS), n);
+        const int key = aback_slot(pl, masked, par, (int)(first % RB_NMAPS), n);
         // (every workspace and ring phase of this size at once, as the synchronous batches)
         const bool build = !ar->gback[key];
         for (int pa = 0; pa < 2 && build; pa++)
             for (int ph = 0; ph < RB_NMAPS; ph++) {
-                const int kk = aback_slot(pl, pa, ph, n);
+                const int kk = aback_slot(pl, masked, pa, ph, n);
                 if (ar->gback[kk]) continue;
                 const DogWS *w = pa ? &ar->ws1 : &pl->ws;
-                auto body = [&]() { return enqueue_back(pl, w, n, ph == 0 ? RB_NMAPS : ph); };
+                auto body = [&]() { return enqueue_back(pl, w, n, ph == 0 ? RB_NMAPS : ph, masked); };
                 if ((r = capture_graph(pl, c->stream, body, &ar->gback[kk], &ar->lback[kk]))) return r;
             }
         RB_CUDA(cudaGraphLaunch(ar->gback[key], c->stream));
@@ -1586,6 +1666,13 @@ extern "C" int rb_pipeline_enqueue_frames(rb_pipeline *pl, int format, int on_de
     if (!pl) return RB_ERR_ARG;
     int fmt = 0, r = check_frames(pl, "enqueue_frames", format, frames, ts, n, on_device != 0, &fmt);
     return r ? r : enqueue_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, ticket);
+}
+extern "C" int rb_pipeline_masked_enqueue(rb_pipeline *pl, int format, int on_device, const rb_frame *frames,
+                                          const rb_frame *masks, const double *ts, int n, int64_t *ticket) {
+    if (!pl) return RB_ERR_ARG;
+    int fmt = 0, r = check_frames(pl, "masked_enqueue", format, frames, ts, n, on_device != 0, &fmt);
+    if (!r) r = check_masks(pl, "masked_enqueue", masks, n);
+    return r ? r : enqueue_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, ticket, masks);
 }
 
 // the host side of push_impl after its synchronisation, for one completed ticket, in ticket order
