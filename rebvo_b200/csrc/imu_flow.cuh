@@ -326,23 +326,19 @@ static int imu_live_check(rb_pipeline *pl, const ImuFlow &f, const double *ts, i
     return RB_OK;
 }
 
-// a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking
-// (rgb, frames, fmt as push_impl's; masked: det_mask_pin holds the frames' detection masks)
-static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device,
-                    const double *ts, int n, rb_nav *nav_out, rb_odometry *odom_out, bool masked) {
+// a push in IMU mode: batched scale space, then frame by frame detect (device chain) + host-driven IMU tracking, into the
+// pipeline's slot, whose FrameArgs push_impl has written (masked: it holds the frames' detection masks too)
+static int imu_push(rb_pipeline *pl, ImuFlow &f, const PushIn &in, bool masked) {
     rb_ctx *c = pl->c;
     const rb_params &p = pl->p;
+    OutSlot &s = pl->out;
+    rb_odometry *odom = pl->odom.on ? s.odom : nullptr;
+    const double *ts = in.ts;
+    const int n = in.n, soff[2] = {0, n};
     int r;
-    if (!on_device && (r = stage_host_frames(pl, rgb, frames, fmt, 0, n, c->stream))) return r;
-    if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;
-    if (masked)
-        RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, pl->det_mask_pin, sizeof(DetMask) * n, cudaMemcpyHostToDevice, c->stream));
-    pl->sb_pin[0].src = on_device ? (const void *)rgb : (const void *)pl->ws.rgb;
-    RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
-    if ((r = rb_gray_enqueue(c, &pl->ws, pl->und, in_mono(fmt), &pl->sb_dev->src, in_strided(fmt) ? pl->frames_dev : nullptr,
-                             n)))
-        return r;
-    if ((r = rb_dog_build_batch(c, &pl->ws, n))) return r;
+    if ((r = stage_push(pl, in, soff, 1))) return r;
+    if ((r = write_tables(pl, s, 0, in.on_device ? (const void *)in.data : (const void *)pl->ws.rgb, 0, n, masked))) return r;
+    if ((r = enqueue_front(pl, &pl->ws, pl->sb_dev, pl->frames_dev, in.fmt, n, false))) return r;
     for (int i = 0; i < n; i++) {
         const long long fr = pl->n_pushed + i;
         rb_map *neu = pl->maps[fr % RB_NMAPS], *old = pl->maps[(fr + RB_NMAPS - 1) % RB_NMAPS];
@@ -356,7 +352,7 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_fr
             return RB_ERR_STATE;
         }
         f.t_prev_grab = ts[i];
-        rb_nav *no = nav_out ? nav_out + i : pl->nav_pin + i;
+        rb_nav *no = s.nav + i;
         if (fr == 0) {
             MapState ns;
             if ((r = rb_read_map_state(neu, &ns))) return r;
@@ -369,11 +365,9 @@ static int imu_push(rb_pipeline *pl, ImuFlow &f, const uint8_t *rgb, const rb_fr
             no->kn = ns.kn;
             no->thresh = ns.thresh_used;
             no->retuned_thresh = ns.retuned;
-            if (odom_out) memset(odom_out + i, 0, sizeof(rb_odometry));   // tracked = 0
-        } else {
-            double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
-            if (dt < 0.001) dt = 1 / p.config_fps;
-            if ((r = imu_track_frame(pl, f, neu, old, ts[i], dt, imu, no, odom_out ? odom_out + i : nullptr))) return r;
+            if (odom) memset(odom + i, 0, sizeof(rb_odometry));   // tracked = 0
+        } else if ((r = imu_track_frame(pl, f, neu, old, ts[i], s.fa[i].dt, imu, no, odom ? odom + i : nullptr))) {
+            return r;
         }
     }
     pl->t_prev = ts[n - 1];

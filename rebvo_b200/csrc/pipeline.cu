@@ -52,27 +52,38 @@ struct SubBatchPtrs {
                                 // pinned host memory, or device memory with rb_pipeline_set_output_memory(pl, 1))
 };
 
-// Asynchronous pushes (rb_pipeline_set_async / rb_pipeline_enqueue / rb_pipeline_wait).  Ticket k runs its front (staging,
-// gray, scale space) on the front stream into workspace k % 2 and its back (detect ... depth image) on the tracker stream,
-// writing its outputs into slot k % depth of the output ring; see DESIGN.md §5.
-struct AsyncSlot {
-    long long first;                  // frame number of the ticket's first frame
+// The per-push sources and outputs of one push: rb_pipeline::out for the synchronous pushes, AsyncRing::slot[k % depth] for
+// ticket k of the asynchronous ones (rb_pipeline_set_async / rb_pipeline_enqueue / rb_pipeline_wait).  The output accessors
+// read the slot rb_pipeline::view points at.
+struct OutSlot {
+    long long first;                  // frame number of the push's first frame
     int n;                            // its frames
-    rb_nav *nav;                      // pinned [max_batch]: the nav records, copied from nav_dev after the back
+    rb_nav *nav;                      // pinned [max_batch]: the nav records, copied from nav_dev after each batch
     rb_odometry *odom;                // pinned [max_batch] (odometry on)
-    int *abort;                       // pinned [RB_NMAPS]: the ring maps' minimiser abort flags after the back
-    struct FrameArgs *fa;             // pinned [max_batch]: per-frame scalars, the source of the back's fa_dev copy
-    SubBatchPtrs *tbl;                // pinned [2]: the front's table (src) and the back's (mirror and depth destinations)
-    rb_frame *frames;                 // pinned [max_batch]: strided device input, the source of the front's frame table
-    DetMask *masks;                   // pinned [max_batch]: the detection masks of a masked ticket, the source of the back's
-                                      // det_mask_dev copy (detection runs in the back)
-    unsigned char *mirror_host, *mirror_dev, *depth_host, *depth_dev, *dimg_host, *dimg_dev;   // the slot's outputs
+    int *abort;                       // pinned [RB_NMAPS]: the ring maps' minimiser abort flags after the push
+    struct FrameArgs *fa;             // pinned [max_batch]: per-frame scalars, the source of the fa_dev copies
+    SubBatchPtrs *tbl;                // pinned [2]: per sub-batch the table copied into sb_dev (a ticket: the front's table
+                                      // in [0], the back's in [1])
+    rb_frame *frames;                 // pinned [max_batch]: strided device input, the source of the frame table
+    DetMask *masks;                   // pinned [max_batch]: the detection masks of a masked push, the source of the
+                                      // det_mask_dev copies
+    // the mirror, depth grid and depth image: host buffers in host output mode, device ones in device mode.  The
+    // synchronous slot's mirror_dev is the mirror's staging in either mode; the ring slots pack into it in host mode too
+    unsigned char *mirror_host, *mirror_dev, *depth_host, *depth_dev, *dimg_host, *dimg_dev;
     size_t mirror_host_bytes, mirror_dev_bytes, depth_host_bytes, depth_dev_bytes, dimg_host_bytes, dimg_dev_bytes;
-    cudaEvent_t done;                 // recorded on the tracker stream after the ticket's last copy
+    cudaEvent_t done;                 // a ticket's: recorded on the tracker stream after its last copy
 };
+// captured graphs by key: exec[k] (nullptr: not captured yet) launches launches[k] kernels
+struct GraphCache {
+    cudaGraphExec_t *exec;
+    int *launches;
+    int size;
+};
+// Asynchronous pushes.  Ticket k runs its front (staging, gray, scale space) on the front stream into workspace k % 2 and its
+// back (detect ... depth image) on the tracker stream, writing its outputs into slot k % depth; see DESIGN.md §5.
 struct AsyncRing {
     int depth;                        // 1..8 tickets in flight, one output slot each
-    AsyncSlot slot[8];
+    OutSlot slot[8];
     DogWS ws1;                        // workspace of odd tickets (even tickets use rb_pipeline::ws)
     SubBatchPtrs *front_dev[2];       // device, per workspace: the table the front's gray pass reads
     rb_frame *frames_dev[2];          // device, per workspace: strided device input's {data, step} table
@@ -81,8 +92,7 @@ struct AsyncRing {
     cudaEvent_t ev_free[2];           // per workspace: the back that read it last is complete (the next front waits for it)
     // captured halves: the front per (input format, workspace, batch size), the back per (masked, workspace, ring phase, batch
     // size)
-    cudaGraphExec_t *gfront, *gback;
-    int *lfront, *lback;              // kernel launches inside each graph
+    GraphCache front_graphs, back_graphs;
 };
 
 struct ImuFlow;
@@ -114,18 +124,15 @@ struct rb_pipeline {
     // kernels of the head
     cudaStream_t copy_stream;
     cudaEvent_t ev_copy[2];       // per sub-batch: its frames are on the device
-    SubBatchPtrs *sb_dev;         // device: the table of the sub-batch being processed
-    SubBatchPtrs *sb_pin;         // pinned: one entry per sub-batch of the current push (at most two)
-    // strided device input (rb_pipeline_push_frames_dev): frame i of the push is frames_dev[i], written from frames_pin
-    // before the batch runs, so that one captured batch serves every push of that layout.  Apart from SubBatchPtrs: the
-    // packed pushes' per-sub-batch copy does not grow.
+    SubBatchPtrs *sb_dev;         // device: the table of the sub-batch being processed, from its slot's tbl entry
+    // strided device input (rb_pipeline_push_frames_dev): frame i of the push is frames_dev[i], written from the slot's
+    // frames before the batch runs, so that one captured batch serves every push of that layout.  Apart from SubBatchPtrs:
+    // the packed pushes' per-sub-batch copy does not grow.
     rb_frame *frames_dev;         // device [max_batch]
-    rb_frame *frames_pin;         // pinned [max_batch]
     // detection masks (rb_pipeline_set_detect_mask, rb_pipeline_push_masked): a masked push writes frame i's DetMask into
     // det_mask_dev[i] before its batch, as frames_dev, so that one captured batch serves every mask buffer.  Unmasked pushes
     // neither write nor read the table.  det_fixed: the fixed mask, packed w x h (kept when cleared, for the next set).
     DetMask *det_mask_dev;        // device [max_batch]
-    DetMask *det_mask_pin;        // pinned [max_batch]
     unsigned char *det_fixed;     // device [w * h]
     bool det_fixed_on;
     int sub;                      // head sub-batch of a host-input push (env REBVO_B200_SUB, default 8 frames)
@@ -133,9 +140,6 @@ struct rb_pipeline {
     DetChain *chain;      // device
     FrameState *fs;       // device
     rb_nav *nav_dev;
-    rb_nav *nav_pin;
-    int *abort_pin;       // pinned: abort flags of the three maps' minimisers, read back with every push
-    uint8_t *rgb_pin;     // optional pinned staging (unused when the caller's buffer is pinned)
     long long n_pushed;   // frames pushed so far
     bool restored;        // rb_pipeline_load_state since the last push: the ring holds the newest map alone
     unsigned char *state_host;    // mapped pinned staging of a state blob's device section (rb_pipeline_save_state)
@@ -144,11 +148,10 @@ struct rb_pipeline {
     cudaEvent_t ev[4];
     cudaEvent_t user_ev[8];
     float stage_ms[6];
-    struct FrameArgs *fa_dev, *fa_pin;
+    struct FrameArgs *fa_dev;
     // one instantiated CUDA graph per (masked, input format, ring phase of the first frame, batch size): the kernel sequence
     // of a batch is static once the per-frame scalars live in fa_dev
-    cudaGraphExec_t *gexec;       // [2 * RB_NFMT * RB_NMAPS * (max_batch + 1)], see graph_slot
-    int *glaunches;               // kernel launches inside each graph
+    GraphCache graphs;            // [2 * RB_NFMT * RB_NMAPS * (max_batch + 1)], see graph_slot
     bool use_graph;
     // optional in-situ stage profile (REBVO_B200_STAGE_PROF=1, forces eager launches): CUDA events between stages
     bool prof_on;
@@ -160,30 +163,28 @@ struct rb_pipeline {
     rb_undistort *und;    // UseUndistort=1 (rb_pipeline_set_undistort): fused into the gray pass
     // where the mirror, the depth grid and the depth image go (rb_pipeline_set_output_memory): 0 mapped pinned host memory,
     // 1 device memory.  In device mode the mirror's staging slots are its output (no k_mirror_to_host), and the fill and
-    // the image pass write into depth.dev / dimg.dev instead of depth.host / dimg.host; no kernel changes.  Each mode's
-    // buffers are made by the set_* call that needs them and kept (grown, never shrunk) across switches.
+    // the image pass write into a slot's depth_dev / dimg_dev instead of depth_host / dimg_host; no kernel changes.  Each
+    // mode's buffers are made by the set_* call that needs them and kept (grown, never shrunk) across switches.
     int out_dev;
     // device mode: each push first waits for the work enqueued on this stream so far (rb_pipeline_set_consumer_stream), so
     // that it overwrites no output a consumer of the last push still reads; the pipeline's own stream = nothing to wait for
     cudaStream_t consumer;
-    // The optional per-frame outputs.  Each keeps its own frame count of the last push, which its set_* call clears (and
-    // set_depth the image's too: the images are of the grid).
+    // The optional per-frame outputs, whose buffers are in the OutSlots.  Each keeps its own frame count of the shown push,
+    // which its set_* call clears (and set_depth the image's too: the images are of the grid).
     // Keyline mirror (rb_pipeline_set_mirror): every frame's keylines are packed into a device staging slot right after its
     // map update (tracker stream), then (host mode) a small kernel on the mirror's stream writes exactly kn records into
     // mapped pinned host memory while the next frames are tracked; both are part of the captured batch
     struct {
         int on;                        // 0 off, 1 = 168-byte KeyLine records, 2 = 15-byte net_keyline records
         size_t rec, stride;            // bytes per record / per frame slot (multiple of 256)
-        unsigned char *dev, *host;     // [max_batch * stride]: device staging, mapped pinned host memory
-        size_t host_bytes;
         cudaStream_t stream;
-        int n;                         // frames of the last push
+        int n;                         // frames of the shown push
     } mirror;
     // odometry records (rb_pipeline_set_odometry): written beside the nav records, copied with them
     struct {
         int on;
-        rb_odometry *dev, *pin;        // [max_batch]
-        int n;                         // records of the last push
+        rb_odometry *dev;              // [max_batch]
+        int n;                         // records of the shown push
         double rkp_last;               // RKp of the last frame pushed: QK of the next push's first record
     } odom;
     // depth grid (rb_pipeline_set_depth): right after its map update each frame's net_keyline records are packed into a
@@ -195,14 +196,11 @@ struct rb_pipeline {
         int on;
         DepthPlan plan;
         size_t rec_stride;             // bytes per frame staging slot (kcap records, multiple of 256)
-        unsigned char *stage, *host;   // [max_batch * stride]: device staging, mapped pinned host cells
-        size_t host_bytes;
-        unsigned char *dev;            // [max_batch * cells_bytes]: the cells in device mode
-        size_t dev_bytes;
+        unsigned char *stage;          // [max_batch * rec_stride]: device staging
         void *ws;                      // per stream: bucketing scratch (and the grid when it does not fit in smem)
         size_t ws_bytes;               // (per stream)
         cudaStream_t stream[RB_DEPTH_STREAMS];
-        int n;                         // frames of the last push
+        int n;                         // frames of the shown push
     } depth;
     // dense image of the grid (rb_pipeline_set_depth_image): right after each frame's fill, on the same side stream,
     // k_depth_image reads the fill's final cells from that stream's workspace and writes 1 (rho) or 2 (rho, s_rho) w x h
@@ -212,18 +210,15 @@ struct rb_pipeline {
         int mode;                      // 0 off, 1 rho, 2 rho and s_rho
         DepthImgPlan plan;             // (of depth.plan's grid, when both are on)
         size_t plane, stride;          // floats per plane (a multiple of 64); bytes per frame slot
-        unsigned char *host;           // [max_batch * stride] mapped pinned host memory
-        size_t host_bytes;
-        unsigned char *dev;            // [max_batch * stride]: the planes in device mode
-        size_t dev_bytes;
-        int n;                         // frames of the last push
+        int n;                         // frames of the shown push
     } dimg;
+    OutSlot out;                  // the synchronous pushes'
     // asynchronous pushes (nullptr: off).  Tickets count up from 0 for the pipeline's lifetime; [tk_retired, tk_next) are
-    // outstanding.  view: the slot of the ticket the last wait retired, which the output accessors read until the next wait
-    // or push (nullptr: the synchronous buffers)
+    // outstanding
     AsyncRing *ar;
     long long tk_next, tk_retired;
-    const AsyncSlot *view;
+    // the slot the output accessors read: &out, or after a wait the retired ticket's until the next wait or push (show)
+    const OutSlot *view;
 };
 
 // input layouts of a push: packed RGB24 (3 bytes per pixel) or mono8, which stands for the RGB24 frame (m, m, m), at
@@ -238,7 +233,7 @@ static inline int graph_slots(const rb_pipeline *pl) { return 2 * RB_NFMT * RB_N
 static inline int graph_slot(const rb_pipeline *pl, bool masked, int fmt, int phase, int n) {
     return (((masked ? RB_NFMT : 0) + fmt) * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
 }
-// the asynchronous pushes' halves (AsyncRing::gfront / gback)
+// the asynchronous pushes' halves (AsyncRing::front_graphs / back_graphs)
 static inline int afront_slots(const rb_pipeline *pl) { return RB_NFMT * 2 * (pl->max_batch + 1); }
 static inline int afront_slot(const rb_pipeline *pl, int fmt, int par, int n) {
     return (fmt * 2 + par) * (pl->max_batch + 1) + n;
@@ -247,19 +242,31 @@ static inline int aback_slots(const rb_pipeline *pl) { return 2 * 2 * RB_NMAPS *
 static inline int aback_slot(const rb_pipeline *pl, bool masked, int par, int phase, int n) {
     return (((masked ? 2 : 0) + par) * RB_NMAPS + phase) * (pl->max_batch + 1) + n;
 }
-static void drop_execs(cudaGraphExec_t *g, int n) {
-    for (int i = 0; g && i < n; i++)
-        if (g[i]) {
-            cudaGraphExecDestroy(g[i]);
-            g[i] = nullptr;
+static int graphs_alloc(GraphCache &g, int size) {
+    g.exec = new (std::nothrow) cudaGraphExec_t[size]();
+    g.launches = new (std::nothrow) int[size]();
+    g.size = size;
+    return g.exec && g.launches ? RB_OK : RB_ERR_ARG;
+}
+static void graphs_drop(GraphCache &g) {
+    for (int i = 0; g.exec && i < g.size; i++)
+        if (g.exec[i]) {
+            cudaGraphExecDestroy(g.exec[i]);
+            g.exec[i] = nullptr;
         }
+}
+static void graphs_free(GraphCache &g) {
+    graphs_drop(g);
+    delete[] g.exec;
+    delete[] g.launches;
+    g = GraphCache();
 }
 // captured batches contain the gray kernel, the undistortion and the mirror's pack kernels: drop them all
 static void drop_graphs(rb_pipeline *pl) {
-    drop_execs(pl->gexec, graph_slots(pl));
+    graphs_drop(pl->graphs);
     if (pl->ar) {
-        drop_execs(pl->ar->gfront, afront_slots(pl));
-        drop_execs(pl->ar->gback, aback_slots(pl));
+        graphs_drop(pl->ar->front_graphs);
+        graphs_drop(pl->ar->back_graphs);
     }
 }
 // `to` waits for the work enqueued on `from` so far.  One event serves every such hand-over: a wait (eager or captured)
@@ -295,6 +302,83 @@ static int grow_out(rb_pipeline *pl, unsigned char **host, size_t *host_have, un
                     size_t bytes) {
     return pl->out_dev ? grow_dev(pl->c, dev, dev_have, bytes) : grow_mapped(pl->c, host, host_have, bytes);
 }
+
+// ---- output slots ----------------------------------------------------------------------------------------------------------
+// a slot's pinned sources and records; its outputs are slot_grow's
+static int slot_alloc(rb_pipeline *pl, OutSlot &s) {
+    rb_ctx *c = pl->c;
+    const size_t mb = (size_t)pl->max_batch;
+    RB_CUDA(cudaMallocHost(&s.nav, sizeof(rb_nav) * mb));
+    RB_CUDA(cudaMallocHost(&s.abort, sizeof(int) * RB_NMAPS));
+    memset(s.abort, 0, sizeof(int) * RB_NMAPS);
+    RB_CUDA(cudaMallocHost(&s.fa, sizeof(FrameArgs) * mb));
+    RB_CUDA(cudaMallocHost(&s.tbl, 2 * sizeof(SubBatchPtrs)));
+    RB_CUDA(cudaMallocHost(&s.frames, sizeof(rb_frame) * mb));
+    RB_CUDA(cudaMallocHost(&s.masks, sizeof(DetMask) * mb));
+    return RB_OK;
+}
+// slot s's outputs as large as the outputs that are on now need, where rb_pipeline_set_output_memory puts them.  The
+// synchronous slot's mirror_dev is the mirror's staging, so it is there in both modes; a ring slot's is its device output.
+static int slot_grow(rb_pipeline *pl, OutSlot &s) {
+    rb_ctx *c = pl->c;
+    const size_t mb = (size_t)pl->max_batch;
+    int r = RB_OK;
+    if (pl->odom.on && !s.odom) RB_CUDA(cudaMallocHost(&s.odom, sizeof(rb_odometry) * mb));
+    if (pl->mirror.on && (pl->out_dev || &s == &pl->out))
+        r = grow_dev(c, &s.mirror_dev, &s.mirror_dev_bytes, mb * pl->mirror.stride);
+    if (!r && pl->mirror.on && !pl->out_dev)
+        r = grow_mapped(c, &s.mirror_host, &s.mirror_host_bytes, mb * pl->mirror.stride);
+    if (!r && pl->depth.on)
+        r = grow_out(pl, &s.depth_host, &s.depth_host_bytes, &s.depth_dev, &s.depth_dev_bytes, mb * pl->depth.plan.cells_bytes);
+    if (!r && pl->dimg.mode)
+        r = grow_out(pl, &s.dimg_host, &s.dimg_host_bytes, &s.dimg_dev, &s.dimg_dev_bytes, mb * pl->dimg.stride);
+    return r;
+}
+// slot_grow for every slot: by the set_* calls that switch an output on, enlarge it or move it, and by rb_pipeline_set_async,
+// never by a push
+static int grow_outputs(rb_pipeline *pl) {
+    int r = slot_grow(pl, pl->out);
+    for (int k = 0; pl->ar && k < pl->ar->depth && !r; k++) r = slot_grow(pl, pl->ar->slot[k]);
+    return r;
+}
+static void slot_free(OutSlot &s) {
+    if (s.done) cudaEventDestroy(s.done);
+    void *host[] = {s.nav, s.odom, s.abort, s.fa, s.tbl, s.frames, s.masks, s.mirror_host, s.depth_host, s.dimg_host};
+    for (void *p : host)
+        if (p) cudaFreeHost(p);
+    void *dev[] = {s.mirror_dev, s.depth_dev, s.dimg_dev};
+    for (void *p : dev) cudaFree(p);
+}
+// the output accessors show n frames of slot s (n = 0: none)
+static void show(rb_pipeline *pl, const OutSlot &s, int n) {
+    pl->view = &s;
+    pl->odom.n = pl->odom.on ? n : 0;
+    pl->mirror.n = pl->mirror.on ? n : 0;
+    pl->depth.n = pl->depth.on ? n : 0;
+    pl->dimg.n = pl->depth.on && pl->dimg.mode ? n : 0;
+}
+// the host side of a push or ticket whose records in s are complete, in push order: odometry QK, the P_Kp a frame found =
+// RKp of the previous frame's record, which holds the value after that frame's rescaling also when the rescaling ran on the
+// side stream (:382, :480-487); the zero record of a sequence's first frame, which only initialises the ring (:109-121);
+// and the minimisers' abort flags (an exchange between a minimiser's CTAs timed out)
+static int retire(rb_pipeline *pl, OutSlot &s) {
+    for (int i = 0; i < s.n && pl->odom.on; i++) {
+        if (s.first + i == 0) {
+            memset(&s.odom[i], 0, sizeof(rb_odometry));
+            continue;
+        }
+        s.odom[i].QK = i == 0 ? pl->odom.rkp_last : s.nav[i - 1].RKp;
+    }
+    pl->odom.rkp_last = s.nav[s.n - 1].RKp;
+    for (int m = 0; m < RB_NMAPS; m++)
+        if (s.abort[m]) {
+            snprintf(pl->c->err, sizeof(pl->c->err), "Minimizer_RV: an exchange between the kernel's CTAs timed out in frames "
+                     "%lld to %lld (poses are NaN)", s.first, s.first + s.n - 1);
+            return RB_ERR_CUDA;
+        }
+    return RB_OK;
+}
+
 // true, with the reason in the pipeline's error, while asynchronous tickets are outstanding: `what` would change or read
 // what they use
 static bool refuse_busy(rb_pipeline *pl, const char *what) {
@@ -303,41 +387,140 @@ static bool refuse_busy(rb_pipeline *pl, const char *what) {
              what, pl->tk_next - pl->tk_retired);
     return true;
 }
-// host frames of a push into the packed staging (ws's, by default the pipeline's), frames [i0, i0 + count) of `frames`
-// (strided, one 2D copy each) or of the packed buffer `rgb`, on stream s
-static int stage_host_frames(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, int i0, int count,
-                             cudaStream_t s, DogWS *ws = nullptr) {
+
+// ---- a push's input --------------------------------------------------------------------------------------------------------
+// as the C entry point received it; push_in checks it and sets fmt
+struct PushIn {
+    const uint8_t *data;          // n packed frames (host or device memory), or nullptr for
+    const rb_frame *frames;       // n strided frames
+    int format;                   // RB_FRAME_RGB24 or RB_FRAME_MONO8
+    bool on_device;
+    bool with_masks;              // the call takes per-frame detection masks:
+    const rb_frame *masks;        // n device {data, step} entries
+    const double *ts;
+    int n;
+    int fmt;                      // the input layout (RB_IN_*): host strided frames run the packed format's batches
+};
+// every argument check of a push, before anything is enqueued
+static int push_in(rb_pipeline *pl, const char *what, PushIn &in) {
     rb_ctx *c = pl->c;
-    const size_t fbytes = frame_bytes(c, fmt), row = fbytes / c->h;
+    if (in.format != RB_FRAME_RGB24 && in.format != RB_FRAME_MONO8) {
+        snprintf(c->err, sizeof(c->err), "%s: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", what, in.format);
+        return RB_ERR_ARG;
+    }
+    if (in.n < 1 || in.n > pl->max_batch || !(in.data || in.frames) || !in.ts) return RB_ERR_ARG;
+    const bool mono = in.format == RB_FRAME_MONO8;
+    const int64_t row = (int64_t)(mono ? 1 : 3) * c->w;
+    for (int i = 0; in.frames && i < in.n; i++)
+        if (!in.frames[i].data || in.frames[i].step < row) {
+            snprintf(c->err, sizeof(c->err), "%s: frame %d has %s (rows need %lld bytes)", what, i,
+                     in.frames[i].data ? "a step shorter than a row" : "no data", (long long)row);
+            return RB_ERR_ARG;
+        }
+    const bool strided = in.frames && in.on_device;
+    if (strided && pl->und && (c->w > 65535 || c->h > 65535)) {   // (the strided undistortion's 16-bit tap coordinates)
+        snprintf(c->err, sizeof(c->err), "%s_dev: undistorted frames wider or higher than 65535 pixels", what);
+        return RB_ERR_ARG;
+    }
+    if (in.with_masks && !in.masks) {
+        snprintf(c->err, sizeof(c->err), "%s: no masks", what);
+        return RB_ERR_ARG;
+    }
+    for (int i = 0; in.with_masks && i < in.n; i++)   // (each step at least a row of w bytes)
+        if (!in.masks[i].data || in.masks[i].step < c->w) {
+            snprintf(c->err, sizeof(c->err), "%s: mask %d has %s (rows need %d bytes)", what, i,
+                     in.masks[i].data ? "a step shorter than a row" : "no data", c->w);
+            return RB_ERR_ARG;
+        }
+    in.fmt = (mono ? RB_IN_MONO : RB_IN_RGB) + (strided ? RB_IN_RGB_STRIDED : 0);
+    // (the packed mono kernels read a device buffer as aligned 32-bit words; the RGB kernels test the alignment of the source
+    // on the device -- k_gray<false, GRAY_ALIGNED> and ug_pixel take a path for unaligned sources -- and the any-width kernels
+    // read every source through aligned words around it)
+    if (in.fmt == RB_IN_MONO && in.on_device && (reinterpret_cast<uintptr_t>(in.data) & 3)) return RB_ERR_ARG;
+    return RB_OK;
+}
+// host frames [i0, i0 + count) of a push into the packed staging (ws's, by default the pipeline's), one 2D copy each when
+// strided, on stream s
+static int stage_host_frames(rb_pipeline *pl, const PushIn &in, int i0, int count, cudaStream_t s, DogWS *ws = nullptr) {
+    rb_ctx *c = pl->c;
+    const size_t fbytes = frame_bytes(c, in.fmt), row = fbytes / c->h;
     uint8_t *dst = (ws ? ws : &pl->ws)->rgb + (size_t)i0 * fbytes;
-    if (!frames) {
-        RB_CUDA(cudaMemcpyAsync(dst, rgb + (size_t)i0 * fbytes, (size_t)count * fbytes, cudaMemcpyHostToDevice, s));
+    if (!in.frames) {
+        RB_CUDA(cudaMemcpyAsync(dst, in.data + (size_t)i0 * fbytes, (size_t)count * fbytes, cudaMemcpyHostToDevice, s));
         return RB_OK;
     }
     for (int i = 0; i < count; i++)
-        RB_CUDA(cudaMemcpy2DAsync(dst + (size_t)i * fbytes, row, frames[i0 + i].data, (size_t)frames[i0 + i].step, row, c->h,
-                                  cudaMemcpyHostToDevice, s));
+        RB_CUDA(cudaMemcpy2DAsync(dst + (size_t)i * fbytes, row, in.frames[i0 + i].data, (size_t)in.frames[i0 + i].step, row,
+                                  c->h, cudaMemcpyHostToDevice, s));
     return RB_OK;
 }
-// strided device frames: the push's {data, step} table into frames_dev, on the tracker stream before the batch
-static int write_frame_table(rb_pipeline *pl, const rb_frame *frames, int n) {
+// a synchronous push's frames onto the device, before its batches: host frames into the pipeline's staging, sub-batch j
+// (frames [soff[j], soff[j + 1])) on the copy stream, recording ev_copy[j], when there are two, else on the tracker stream;
+// strided device frames as their {data, step} table in frames_dev, on the tracker stream
+static int stage_push(rb_pipeline *pl, const PushIn &in, const int *soff, int nsub) {
     rb_ctx *c = pl->c;
-    memcpy(pl->frames_pin, frames, sizeof(rb_frame) * n);
-    RB_CUDA(cudaMemcpyAsync(pl->frames_dev, pl->frames_pin, sizeof(rb_frame) * n, cudaMemcpyHostToDevice, c->stream));
+    int r;
+    for (int j = 0; j < nsub && !in.on_device; j++) {
+        cudaStream_t cs = nsub > 1 ? pl->copy_stream : c->stream;
+        if ((r = stage_host_frames(pl, in, soff[j], soff[j + 1] - soff[j], cs))) return r;
+        if (nsub > 1) RB_CUDA(cudaEventRecord(pl->ev_copy[j], cs));
+    }
+    if (in_strided(in.fmt)) {
+        memcpy(pl->out.frames, in.frames, sizeof(rb_frame) * in.n);
+        RB_CUDA(cudaMemcpyAsync(pl->frames_dev, pl->out.frames, sizeof(rb_frame) * in.n, cudaMemcpyHostToDevice, c->stream));
+    }
     return RB_OK;
 }
-// the detection masks of the n frames of a push into dst (pinned): the fixed mask and masks[i] (device rb_frame entries, or
-// nullptr).  False, writing nothing, when no mask applies: the push runs the unmasked batches.
-static bool fill_masks(const rb_pipeline *pl, const rb_frame *masks, int n, DetMask *dst) {
+// the per-frame scalars of a push of n frames, the next frames of the stream, into s (SecondThread :146-149 for dt;
+// FrameCount of the reference's 8-slot ring: frame fr is served by slot (fr+1)%8, whose global_tracker has run (fr-1)/8
+// minimisations before)
+static void write_args(rb_pipeline *pl, OutSlot &s, const double *ts, int n) {
+    s.first = pl->n_pushed;
+    s.n = n;
+    for (int i = 0; i < n; i++) {
+        const long long fr = s.first + i;
+        double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
+        if (dt < 0.001) dt = 1 / pl->p.config_fps;
+        s.fa[i].t = ts[i];
+        s.fa[i].dt = dt;
+        s.fa[i].frame_count = fr > 0 ? (unsigned int)((fr - 1) / 8) : 0;
+    }
+}
+// the detection masks of the n frames of a push into s: the fixed mask and masks[i] (device rb_frame entries, or nullptr).
+// False, writing nothing, when no mask applies: the push runs the unmasked batches.
+static bool fill_masks(const rb_pipeline *pl, const rb_frame *masks, int n, OutSlot &s) {
     if (!masks && !pl->det_fixed_on) return false;
     for (int i = 0; i < n; i++) {
-        dst[i].fixed = pl->det_fixed_on ? pl->det_fixed : nullptr;
-        dst[i].fixed_step = pl->c->w;
-        dst[i].frame = masks ? masks[i].data : nullptr;
-        dst[i].frame_step = masks ? masks[i].step : 0;
+        s.masks[i].fixed = pl->det_fixed_on ? pl->det_fixed : nullptr;
+        s.masks[i].fixed_step = pl->c->w;
+        s.masks[i].frame = masks ? masks[i].data : nullptr;
+        s.masks[i].frame_step = masks ? masks[i].step : 0;
     }
     return true;
 }
+// on the tracker stream before a batch of frames [off, off + nj) of slot s: their detection masks into det_mask_dev
+// (masked), and the batch's pointer table -- its frames at src, its outputs in s -- from s.tbl[j] into sb_dev
+static int write_tables(rb_pipeline *pl, OutSlot &s, int j, const void *src, int off, int nj, bool masked) {
+    rb_ctx *c = pl->c;
+    if (masked)
+        RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, s.masks + off, sizeof(DetMask) * nj, cudaMemcpyHostToDevice, c->stream));
+    SubBatchPtrs &t = s.tbl[j];
+    memset(&t, 0, sizeof(t));
+    t.src = src;
+    if (pl->mirror.on) {   // (host mode: packed into the synchronous slot's staging, then copied into s's mapped memory)
+        t.mirror[0] = (pl->out_dev ? s.mirror_dev : pl->out.mirror_dev) + (size_t)off * pl->mirror.stride;
+        t.mirror[1] = pl->out_dev ? nullptr : s.mirror_host + (size_t)off * pl->mirror.stride;
+    }
+    if (pl->depth.on) {
+        t.depth[0] = pl->depth.stage + (size_t)off * pl->depth.rec_stride;
+        t.depth[1] = (pl->out_dev ? s.depth_dev : s.depth_host) + (size_t)off * pl->depth.plan.cells_bytes;
+        t.depth[2] = pl->dimg.mode ? (pl->out_dev ? s.dimg_dev : s.dimg_host) + (size_t)off * pl->dimg.stride : nullptr;
+    }
+    RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
+    return RB_OK;
+}
+static int enqueue_front(rb_pipeline *pl, DogWS *ws, SubBatchPtrs *tbl, const rb_frame *frames_dev, int fmt, int n,
+                         bool with_events);
 #include "imu_flow.cuh"
 static void async_free(rb_pipeline *pl);
 
@@ -460,18 +643,10 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
     RB_CUDA(cudaMalloc(&pl->chain, sizeof(DetChain)));
     RB_CUDA(cudaMalloc(&pl->fs, sizeof(FrameState)));
     RB_CUDA(cudaMalloc(&pl->nav_dev, sizeof(rb_nav) * max_batch));
-    RB_CUDA(cudaMallocHost(&pl->nav_pin, sizeof(rb_nav) * max_batch));
-    RB_CUDA(cudaMallocHost(&pl->abort_pin, sizeof(int) * RB_NMAPS));
-    memset(pl->abort_pin, 0, sizeof(int) * RB_NMAPS);
     RB_CUDA(cudaMalloc(&pl->fa_dev, sizeof(FrameArgs) * max_batch));
-    RB_CUDA(cudaMallocHost(&pl->fa_pin, sizeof(FrameArgs) * max_batch));
-    pl->gexec = new (std::nothrow) cudaGraphExec_t[graph_slots(pl)];
-    pl->glaunches = new (std::nothrow) int[graph_slots(pl)];
-    if (!pl->gexec || !pl->glaunches) return RB_ERR_ARG;
-    for (int i = 0; i < graph_slots(pl); i++) {
-        pl->gexec[i] = nullptr;
-        pl->glaunches[i] = 0;
-    }
+    if ((r = slot_alloc(pl, pl->out))) return r;
+    pl->view = &pl->out;
+    if ((r = graphs_alloc(pl->graphs, graph_slots(pl)))) return r;
     const char *ng = getenv("REBVO_B200_NO_GRAPH");
     pl->use_graph = !(ng && ng[0] == '1');
     const char *sp = getenv("REBVO_B200_STAGE_PROF");
@@ -495,11 +670,8 @@ extern "C" int rb_pipeline_create(rb_pipeline **out, int device, const rb_params
         pl->sub = sb ? atoi(sb) : 8;
         if (pl->sub < 1) pl->sub = max_batch;
         RB_CUDA(cudaMalloc(&pl->sb_dev, sizeof(SubBatchPtrs)));
-        RB_CUDA(cudaMallocHost(&pl->sb_pin, 2 * sizeof(SubBatchPtrs)));
         RB_CUDA(cudaMalloc(&pl->frames_dev, sizeof(rb_frame) * max_batch));
-        RB_CUDA(cudaMallocHost(&pl->frames_pin, sizeof(rb_frame) * max_batch));
         RB_CUDA(cudaMalloc(&pl->det_mask_dev, sizeof(DetMask) * max_batch));
-        RB_CUDA(cudaMallocHost(&pl->det_mask_pin, sizeof(DetMask) * max_batch));
         RB_CUDA(cudaEventCreateWithFlags(&pl->ev_hop, cudaEventDisableTiming));
         for (int i = 0; i < 2; i++) {
             RB_CUDA(cudaEventCreateWithFlags(&pl->ev_trk[i], cudaEventDisableTiming));
@@ -615,21 +787,16 @@ extern "C" void rb_pipeline_destroy(rb_pipeline *pl) {
         if (pl->pev[i]) cudaEventDestroy(pl->pev[i]);
     delete[] pl->pev;
     delete[] pl->ptag;
-    for (int i = 0; pl->gexec && i < graph_slots(pl); i++)
-        if (pl->gexec[i]) cudaGraphExecDestroy(pl->gexec[i]);
-    delete[] pl->gexec;
-    delete[] pl->glaunches;
+    graphs_free(pl->graphs);
     for (int i = 0; i < RB_NMAPS; i++)
         if (pl->maps[i]) rb_map_destroy(pl->maps[i]);
     if (pl->und) rb_undistort_destroy(pl->und);
     rb_dogws_free(&pl->ws);
-    void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->frames_dev, pl->mirror.dev, pl->odom.dev,
-                   pl->depth.stage, pl->depth.ws, pl->depth.dev, pl->dimg.dev, pl->det_mask_dev, pl->det_fixed};
+    slot_free(pl->out);
+    void *dev[] = {pl->chain, pl->fs, pl->nav_dev, pl->fa_dev, pl->sb_dev, pl->frames_dev, pl->odom.dev, pl->depth.stage,
+                   pl->depth.ws, pl->det_mask_dev, pl->det_fixed};
     for (void *p : dev) cudaFree(p);
-    void *host[] = {pl->nav_pin, pl->abort_pin, pl->fa_pin, pl->sb_pin, pl->frames_pin, pl->mirror.host, pl->odom.pin,
-                    pl->depth.host, pl->dimg.host, pl->state_host, pl->det_mask_pin};
-    for (void *p : host)
-        if (p) cudaFreeHost(p);
+    if (pl->state_host) cudaFreeHost(pl->state_host);
     rb_ctx_destroy(c);
     delete pl;
 }
@@ -913,52 +1080,48 @@ static int capture_graph(rb_pipeline *pl, cudaStream_t s, F &&body, cudaGraphExe
     return RB_OK;
 }
 
-// rgb: n packed frames of frame_bytes(fmt) each, host or device memory; or (rgb == nullptr) frames: n strided frames, checked
-// by push_frames, whose layout is fmt (device memory) or whose packed format is fmt (host memory).  masks: n per-frame
-// detection masks in device memory, checked by check_masks, or nullptr.
-static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
-                     int n, rb_nav *nav_out, const rb_frame *masks = nullptr) {
+// Launch graph `key` of g on stream s.  One that is not captured yet is captured first, together with those of its nsib
+// siblings that are missing: sibling i is graph sib_key(i) with the body sib_body(i), and the key is one of them.
+template <class K, class B>
+static int graph_launch(rb_pipeline *pl, GraphCache &g, cudaStream_t s, int key, int nsib, K &&sib_key, B &&sib_body) {
     rb_ctx *c = pl->c;
-    const rb_params &p = pl->p;
-    if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts) return RB_ERR_ARG;
-    if (refuse_busy(pl, "push")) return RB_ERR_STATE;
-    pl->view = nullptr;
-    // (the packed mono kernels read a device buffer as aligned 32-bit words; the RGB kernels test the alignment of the source
-    // on the device -- k_gray<false, GRAY_ALIGNED> and ug_pixel take a path for unaligned sources -- and the any-width kernels
-    // read every source through aligned words around it)
-    if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
     int r;
-    if (pl->imu && pl->imu->live && (r = imu_live_check(pl, *pl->imu, ts, n))) return r;
+    if (!g.exec[key])
+        for (int i = 0; i < nsib; i++) {
+            const int k = sib_key(i);
+            if (g.exec[k]) continue;
+            auto body = [&]() { return sib_body(i); };
+            if ((r = capture_graph(pl, s, body, &g.exec[k], &g.launches[k]))) return r;
+        }
+    RB_CUDA(cudaGraphLaunch(g.exec[key], s));
+    c->launches += g.launches[key];
+    return RB_OK;
+}
+
+// a synchronous push of input that push_in has checked, into the pipeline's slot
+static int push_impl(rb_pipeline *pl, const PushIn &in, rb_nav *nav_out) {
+    rb_ctx *c = pl->c;
+    if (refuse_busy(pl, "push")) return RB_ERR_STATE;
+    const int n = in.n;
+    int r;
+    if (pl->imu && pl->imu->live && (r = imu_live_check(pl, *pl->imu, in.ts, n))) return r;
     RB_CUDA(cudaSetDevice(c->device));
-    pl->odom.n = 0;
-    pl->depth.n = 0;
-    pl->dimg.n = 0;
+    OutSlot &s = pl->out;
+    show(pl, s, 0);
     pl->last_sub = 0;
-    const bool masked = fill_masks(pl, masks, n, pl->det_mask_pin);
+    write_args(pl, s, in.ts, n);
+    const bool masked = fill_masks(pl, in.masks, n, s);
     if (pl->imu) {   // IMU mode: host-driven frame loop (imu_flow.cuh)
-        if ((r = imu_push(pl, *pl->imu, rgb, frames, fmt, on_device, ts, n, pl->nav_pin,
-                          pl->odom.on ? pl->odom.pin : nullptr, masked)))
-            return r;
+        if ((r = imu_push(pl, *pl->imu, in, masked))) return r;
         RB_CUDA(cudaStreamSynchronize(c->stream));
         pl->last_sub = n;   // (one scale-space batch)
-        if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
+        if (nav_out) memcpy(nav_out, s.nav, sizeof(rb_nav) * n);
         pl->odom.n = pl->odom.on ? n : 0;
         return RB_OK;
     }
     // device outputs: nothing of this push may overwrite them before the consumer's reads of the last push's are done.  The
     // side streams that write them fork from the tracker stream, so one wait at its head covers them (outside any graph).
     if (pl->out_dev && pl->consumer != c->stream && (r = stream_wait(pl, pl->consumer, c->stream))) return r;
-    const long long first = pl->n_pushed;
-    // per-frame scalars -> device (SecondThread :146-149 for dt; FrameCount of the reference's 8-slot ring:
-    // frame fr is served by slot (fr+1)%8, whose global_tracker has run (fr-1)/8 minimisations before)
-    for (int i = 0; i < n; i++) {
-        const long long fr = first + i;
-        double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
-        if (dt < 0.001) dt = 1 / p.config_fps;
-        pl->fa_pin[i].t = ts[i];
-        pl->fa_pin[i].dt = dt;
-        pl->fa_pin[i].frame_count = fr > 0 ? (unsigned int)((fr - 1) / 8) : 0;
-    }
     pl->pn = 0;
     prof_mark(pl, ST_NAV);   // origin of this push
     RB_CUDA(cudaEventRecord(pl->ev[0], c->stream));
@@ -967,70 +1130,40 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
     // their own staging region while the head computes (a frame costs ~8x more to track than to copy), and the scale
     // space of the rest still runs as one large batch.
     int soff[3] = {0, n, n}, nsub = 1;
-    if (!(on_device || pl->prof_on || n < 3 * pl->sub)) {
+    if (!(in.on_device || pl->prof_on || n < 3 * pl->sub)) {
         soff[1] = pl->sub;
         nsub = 2;
     }
-    const size_t fbytes = frame_bytes(c, fmt);   // (ws.rgb holds max_batch frames of either format)
-    for (int j = 0; j < nsub && !on_device; j++) {
-        const int off = soff[j], nj = soff[j + 1] - soff[j];
-        cudaStream_t cs = nsub > 1 ? pl->copy_stream : c->stream;
-        if ((r = stage_host_frames(pl, rgb, frames, fmt, off, nj, cs))) return r;
-        if (nsub > 1) RB_CUDA(cudaEventRecord(pl->ev_copy[j], cs));
-    }
-    if (in_strided(fmt) && (r = write_frame_table(pl, frames, n))) return r;   // (device input: one sub-batch)
+    if ((r = stage_push(pl, in, soff, nsub))) return r;
+    const size_t fbytes = frame_bytes(c, in.fmt);   // (ws.rgb holds max_batch frames of either format)
     for (int j = 0; j < nsub; j++) {
         const int off = soff[j], nj = soff[j + 1] - soff[j];
-        const long long first_j = first + (long long)off;
-        if (!on_device && nsub > 1) RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_copy[j], 0));
-        RB_CUDA(cudaMemcpyAsync(pl->fa_dev, pl->fa_pin + off, sizeof(FrameArgs) * nj, cudaMemcpyHostToDevice, c->stream));
-        if (masked)
-            RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, pl->det_mask_pin + off, sizeof(DetMask) * nj, cudaMemcpyHostToDevice,
-                                    c->stream));
-        SubBatchPtrs &t = pl->sb_pin[j];
-        t.src = on_device ? (const void *)rgb : (const void *)(pl->ws.rgb + (size_t)off * fbytes);   // (strided: unused)
-        if (pl->mirror.on) {
-            t.mirror[0] = pl->mirror.dev + (size_t)off * pl->mirror.stride;
-            t.mirror[1] = pl->out_dev ? nullptr : pl->mirror.host + (size_t)off * pl->mirror.stride;
-        }
-        if (pl->depth.on) {
-            unsigned char *cells = pl->out_dev ? pl->depth.dev : pl->depth.host;
-            unsigned char *img = pl->out_dev ? pl->dimg.dev : pl->dimg.host;
-            t.depth[0] = pl->depth.stage + (size_t)off * pl->depth.rec_stride;
-            t.depth[1] = cells + (size_t)off * pl->depth.plan.cells_bytes;
-            t.depth[2] = pl->dimg.mode ? img + (size_t)off * pl->dimg.stride : nullptr;
-        }
-        RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
-        const bool graph_ok = pl->use_graph && first_j > 0;
-        if (!graph_ok) {
-            if ((r = enqueue_batch(pl, fmt, nj, first_j, j == 0, masked))) return r;
+        const long long first_j = s.first + off;
+        if (!in.on_device && nsub > 1) RB_CUDA(cudaStreamWaitEvent(c->stream, pl->ev_copy[j], 0));
+        RB_CUDA(cudaMemcpyAsync(pl->fa_dev, s.fa + off, sizeof(FrameArgs) * nj, cudaMemcpyHostToDevice, c->stream));
+        const void *src = in.on_device ? (const void *)in.data : (const void *)(pl->ws.rgb + (size_t)off * fbytes);
+        if ((r = write_tables(pl, s, j, src, off, nj, masked))) return r;   // (strided: src unused)
+        if (!pl->use_graph || first_j == 0) {
+            if ((r = enqueue_batch(pl, in.fmt, nj, first_j, j == 0, masked))) return r;
         } else {
-            const int key = graph_slot(pl, masked, fmt, (int)(first_j % RB_NMAPS), nj);
-            // capture the batch once per ring phase; replays only differ through fa_dev / sb_dev contents.  All
-            // phases of this format and batch size are instantiated together, so that no later push pays for a capture.
-            // The other format's graphs are left as they are: a stream may alternate formats.
-            const bool build = !pl->gexec[key];
-            for (int ph = 0; ph < RB_NMAPS && build; ph++) {
-                const int k = graph_slot(pl, masked, fmt, ph, nj);
-                if (pl->gexec[k]) continue;
-                // (any first frame > 0 of that phase)
-                auto body = [&]() { return enqueue_batch(pl, fmt, nj, ph == 0 ? RB_NMAPS : ph, false, masked); };
-                if ((r = capture_graph(pl, c->stream, body, &pl->gexec[k], &pl->glaunches[k]))) return r;
-            }
+            // capture the batch once per ring phase (from any first frame > 0 of that phase); replays only differ through
+            // fa_dev / sb_dev contents.  All phases of this format and batch size are instantiated together, so that no later
+            // push pays for a capture.  The other format's graphs are left as they are: a stream may alternate formats.
             if (j == 0) RB_CUDA(cudaEventRecord(pl->ev[1], c->stream));
-            RB_CUDA(cudaGraphLaunch(pl->gexec[key], c->stream));
+            auto sib_key = [&](int ph) { return graph_slot(pl, masked, in.fmt, ph, nj); };
+            auto sib_body = [&](int ph) { return enqueue_batch(pl, in.fmt, nj, ph == 0 ? RB_NMAPS : ph, false, masked); };
+            if ((r = graph_launch(pl, pl->graphs, c->stream, sib_key((int)(first_j % RB_NMAPS)), RB_NMAPS, sib_key, sib_body)))
+                return r;
             if (j == 0) RB_CUDA(cudaEventRecord(pl->ev[2], c->stream));
-            c->launches += pl->glaunches[key];
         }
-        RB_CUDA(cudaMemcpyAsync(pl->nav_pin + off, pl->nav_dev, sizeof(rb_nav) * nj, cudaMemcpyDeviceToHost, c->stream));
+        RB_CUDA(cudaMemcpyAsync(s.nav + off, pl->nav_dev, sizeof(rb_nav) * nj, cudaMemcpyDeviceToHost, c->stream));
         if (pl->odom.on)
-            RB_CUDA(cudaMemcpyAsync(pl->odom.pin + off, pl->odom.dev, sizeof(rb_odometry) * nj, cudaMemcpyDeviceToHost,
-                                    c->stream));
+            RB_CUDA(cudaMemcpyAsync(s.odom + off, pl->odom.dev, sizeof(rb_odometry) * nj, cudaMemcpyDeviceToHost, c->stream));
     }
     for (int k = 0; k < RB_NMAPS; k++)
-        RB_CUDA(cudaMemcpyAsync(&pl->abort_pin[k], &pl->maps[k]->ts_host.ctl->abort, sizeof(int), cudaMemcpyDeviceToHost,
+        RB_CUDA(cudaMemcpyAsync(&s.abort[k], &pl->maps[k]->ts_host.ctl->abort, sizeof(int), cudaMemcpyDeviceToHost,
                                 c->stream));
-    pl->t_prev = ts[n - 1];
+    pl->t_prev = in.ts[n - 1];
     pl->n_pushed += n;
     pl->restored = false;
     prof_mark(pl, ST_NAV);
@@ -1044,30 +1177,12 @@ static int push_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames
         }
         pl->pframes += n;
     }
-    if (nav_out) memcpy(nav_out, pl->nav_pin, sizeof(rb_nav) * n);
+    if (nav_out) memcpy(nav_out, s.nav, sizeof(rb_nav) * n);
     pl->last_sub = soff[nsub] - soff[nsub - 1];
-    pl->mirror.n = pl->mirror.on ? n : 0;
-    pl->depth.n = pl->depth.on ? n : 0;
-    pl->dimg.n = pl->depth.on && pl->dimg.mode ? n : 0;
-    // QK of a record: P_Kp as the frame found it = RKp of the previous frame's record, which holds the value after that frame's
-    // rescaling also when the rescaling ran on the side stream (:382, :480-487)
-    for (int i = 0; i < n && pl->odom.on; i++) {
-        if (first + i == 0) {   // the first frame of a sequence only initialises the ring (:109-121)
-            memset(&pl->odom.pin[i], 0, sizeof(rb_odometry));
-            continue;
-        }
-        pl->odom.pin[i].QK = i == 0 ? pl->odom.rkp_last : pl->nav_pin[i - 1].RKp;
-    }
-    pl->odom.n = pl->odom.on ? n : 0;
-    pl->odom.rkp_last = pl->nav_pin[n - 1].RKp;
-    {   // did a minimiser of this push abort (an exchange between its CTAs timed out)?  Checked on every push.
-        bool aborted = false;
-        for (int k = 0; k < RB_NMAPS; k++) aborted = aborted || pl->abort_pin[k] != 0;
-        if (aborted) {
-            for (int k = 0; k < RB_NMAPS; k++) cudaMemset(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int));
-            snprintf(c->err, sizeof(c->err), "Minimizer_RV: an exchange between the kernel's CTAs timed out (poses are NaN)");
-            return RB_ERR_CUDA;
-        }
+    show(pl, s, n);
+    if ((r = retire(pl, s))) {   // (checked on every push; the flags are cleared for the next one)
+        for (int k = 0; k < RB_NMAPS; k++) cudaMemset(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int));
+        return r;
     }
     float ms;
     cudaEventElapsedTime(&ms, pl->ev[0], pl->ev[1]);
@@ -1095,28 +1210,6 @@ static int set_begin(rb_pipeline *pl, const char *imu_refused) {
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return RB_OK;
 }
-// every output slot of the asynchronous ring holds the outputs that are on now, where rb_pipeline_set_output_memory puts
-// them: made by rb_pipeline_set_async and by the set_* calls that switch an output on or enlarge it, never by an enqueue
-static int async_grow(rb_pipeline *pl) {
-    AsyncRing *ar = pl->ar;
-    if (!ar) return RB_OK;
-    rb_ctx *c = pl->c;
-    const size_t mb = (size_t)pl->max_batch;
-    int r = RB_OK;
-    for (int k = 0; k < ar->depth && !r; k++) {
-        AsyncSlot &s = ar->slot[k];
-        if (pl->odom.on && !s.odom) RB_CUDA(cudaMallocHost(&s.odom, sizeof(rb_odometry) * mb));
-        if (pl->mirror.on)   // (host mode: the frames are packed into the pipeline's staging, then copied into the slot)
-            r = pl->out_dev ? grow_dev(c, &s.mirror_dev, &s.mirror_dev_bytes, mb * pl->mirror.stride)
-                            : grow_mapped(c, &s.mirror_host, &s.mirror_host_bytes, mb * pl->mirror.stride);
-        if (!r && pl->depth.on)
-            r = grow_out(pl, &s.depth_host, &s.depth_host_bytes, &s.depth_dev, &s.depth_dev_bytes,
-                         mb * pl->depth.plan.cells_bytes);
-        if (!r && pl->dimg.mode)
-            r = grow_out(pl, &s.dimg_host, &s.dimg_host_bytes, &s.dimg_dev, &s.dimg_dev_bytes, mb * pl->dimg.stride);
-    }
-    return r;
-}
 // the ring and everything it owns (no ticket outstanding, or the pipeline is being destroyed); the outputs of a ticket it
 // held are gone with it
 static void async_free(rb_pipeline *pl) {
@@ -1126,32 +1219,18 @@ static void async_free(rb_pipeline *pl) {
         cudaStreamSynchronize(ar->front);
         cudaStreamDestroy(ar->front);
     }
-    drop_execs(ar->gfront, afront_slots(pl));
-    drop_execs(ar->gback, aback_slots(pl));
-    delete[] ar->gfront;
-    delete[] ar->gback;
-    delete[] ar->lfront;
-    delete[] ar->lback;
+    graphs_free(ar->front_graphs);
+    graphs_free(ar->back_graphs);
     cudaEvent_t events[] = {ar->ev_front[0], ar->ev_front[1], ar->ev_free[0], ar->ev_free[1]};
     for (cudaEvent_t e : events)
         if (e) cudaEventDestroy(e);
-    for (AsyncSlot &s : ar->slot) {
-        if (s.done) cudaEventDestroy(s.done);
-        void *host[] = {s.nav, s.odom, s.abort, s.fa, s.tbl, s.frames, s.masks, s.mirror_host, s.depth_host, s.dimg_host};
-        for (void *p : host)
-            if (p) cudaFreeHost(p);
-        void *dev[] = {s.mirror_dev, s.depth_dev, s.dimg_dev};
-        for (void *p : dev) cudaFree(p);
-    }
+    for (OutSlot &s : ar->slot) slot_free(s);
     for (int k = 0; k < 2; k++) {
         cudaFree(ar->front_dev[k]);
         cudaFree(ar->frames_dev[k]);
     }
     rb_dogws_free(&ar->ws1);
-    if (pl->view) {
-        pl->view = nullptr;
-        pl->mirror.n = pl->depth.n = pl->dimg.n = pl->odom.n = 0;
-    }
+    if (pl->view != &pl->out) show(pl, pl->out, 0);
     delete ar;
     pl->ar = nullptr;
 }
@@ -1162,7 +1241,6 @@ static int async_alloc(rb_pipeline *pl, int depth) {
     memset(ar, 0, sizeof(*ar));
     pl->ar = ar;
     ar->depth = depth;
-    const size_t mb = (size_t)pl->max_batch;
     int r;
     if ((r = rb_dogws_alloc(c, &ar->ws1, pl->max_batch))) return r;
     // lowest priority: the back of the ticket before is the critical path, and a front has the whole of it to finish in
@@ -1173,24 +1251,15 @@ static int async_alloc(rb_pipeline *pl, int depth) {
         RB_CUDA(cudaEventCreateWithFlags(&ar->ev_front[k], cudaEventDisableTiming));
         RB_CUDA(cudaEventCreateWithFlags(&ar->ev_free[k], cudaEventDisableTiming));
         RB_CUDA(cudaMalloc(&ar->front_dev[k], sizeof(SubBatchPtrs)));
-        RB_CUDA(cudaMalloc(&ar->frames_dev[k], sizeof(rb_frame) * mb));
+        RB_CUDA(cudaMalloc(&ar->frames_dev[k], sizeof(rb_frame) * pl->max_batch));
     }
-    ar->gfront = new (std::nothrow) cudaGraphExec_t[afront_slots(pl)]();
-    ar->gback = new (std::nothrow) cudaGraphExec_t[aback_slots(pl)]();
-    ar->lfront = new (std::nothrow) int[afront_slots(pl)]();
-    ar->lback = new (std::nothrow) int[aback_slots(pl)]();
-    if (!ar->gfront || !ar->gback || !ar->lfront || !ar->lback) return RB_ERR_ARG;
+    if ((r = graphs_alloc(ar->front_graphs, afront_slots(pl))) || (r = graphs_alloc(ar->back_graphs, aback_slots(pl))))
+        return r;
     for (int k = 0; k < depth; k++) {
-        AsyncSlot &s = ar->slot[k];
-        RB_CUDA(cudaMallocHost(&s.nav, sizeof(rb_nav) * mb));
-        RB_CUDA(cudaMallocHost(&s.abort, sizeof(int) * RB_NMAPS));
-        RB_CUDA(cudaMallocHost(&s.fa, sizeof(FrameArgs) * mb));
-        RB_CUDA(cudaMallocHost(&s.tbl, 2 * sizeof(SubBatchPtrs)));
-        RB_CUDA(cudaMallocHost(&s.frames, sizeof(rb_frame) * mb));
-        RB_CUDA(cudaMallocHost(&s.masks, sizeof(DetMask) * mb));
-        RB_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+        if ((r = slot_alloc(pl, ar->slot[k]))) return r;
+        RB_CUDA(cudaEventCreateWithFlags(&ar->slot[k].done, cudaEventDisableTiming));
     }
-    return async_grow(pl);
+    return grow_outputs(pl);
 }
 
 extern "C" int rb_pipeline_set_undistort(rb_pipeline *pl, const double kc[5]) {
@@ -1220,19 +1289,13 @@ extern "C" int rb_pipeline_set_mirror(rb_pipeline *pl, int on) {
     int r = set_begin(pl, "set_mirror");
     if (r) return r;
     const size_t stride = ((size_t)c->kcap * sizeof(rb_keyline) + 255) & ~(size_t)255;   // (sized for the larger record)
-    if (on) {
-        if (!pl->mirror.dev) RB_CUDA(cudaMalloc(&pl->mirror.dev, (size_t)pl->max_batch * stride));
-        // (device mode: the staging slots are the output)
-        if (!pl->out_dev && (r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, (size_t)pl->max_batch * stride)))
-            return r;
-        if (!pl->mirror.stream) RB_CUDA(cudaStreamCreateWithFlags(&pl->mirror.stream, cudaStreamNonBlocking));
-    }
+    if (on && !pl->mirror.stream) RB_CUDA(cudaStreamCreateWithFlags(&pl->mirror.stream, cudaStreamNonBlocking));
     if (on != pl->mirror.on) drop_graphs(pl);   // the captured batches contain (or not) the pack kernels
     pl->mirror.on = on;
     pl->mirror.rec = on == 2 ? 15 : sizeof(rb_keyline);
     pl->mirror.stride = stride;
     pl->mirror.n = 0;
-    return async_grow(pl);
+    return grow_outputs(pl);
 }
 extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) {
     if (!pl) return RB_ERR_ARG;
@@ -1263,9 +1326,6 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
         for (int k = 0; k < RB_DEPTH_STREAMS; k++)
             RB_CUDA(cudaStreamCreateWithPriority(&pl->depth.stream[k], cudaStreamNonBlocking, (dp && atoi(dp) == 1) ? hi : lo));
     }
-    if ((r = grow_out(pl, &pl->depth.host, &pl->depth.host_bytes, &pl->depth.dev, &pl->depth.dev_bytes,
-                      (size_t)pl->max_batch * plan.cells_bytes)))
-        return r;
     const size_t ws_bytes = rb_depth_ws_bytes(plan, c->kcap);
     if (ws_bytes > pl->depth.ws_bytes) {
         cudaFree(pl->depth.ws);
@@ -1280,14 +1340,14 @@ extern "C" int rb_pipeline_set_depth(rb_pipeline *pl, const rb_depth_params *p) 
     pl->depth.on = 1;
     pl->depth.n = 0;
     pl->dimg.n = 0;
-    return async_grow(pl);
+    return grow_outputs(pl);
 }
 extern "C" int rb_pipeline_depth(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh, double *min_dist) {
     if (!pl || !cells) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
     const DepthGeom &g = pl->depth.plan.g;
-    const unsigned char *slot = (pl->view ? pl->view->depth_host : pl->depth.host) + (size_t)i * pl->depth.plan.cells_bytes;
+    const unsigned char *slot = pl->view->depth_host + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
     if (gw) *gw = g.gw;
     if (gh) *gh = g.gh;
@@ -1302,9 +1362,6 @@ extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
     if (r) return r;
     if (mode) {
         const size_t plane = ((size_t)c->N + 63) & ~(size_t)63, stride = (size_t)mode * plane * sizeof(float);
-        if ((r = grow_out(pl, &pl->dimg.host, &pl->dimg.host_bytes, &pl->dimg.dev, &pl->dimg.dev_bytes,
-                          (size_t)pl->max_batch * stride)))
-            return r;
         if (pl->depth.on && (r = rb_depth_image_plan(c, pl->depth.plan.g, mode, &pl->dimg.plan))) return r;
         pl->dimg.plane = plane;
         pl->dimg.stride = stride;
@@ -1312,14 +1369,13 @@ extern "C" int rb_pipeline_set_depth_image(rb_pipeline *pl, int mode) {
     if (mode != pl->dimg.mode) drop_graphs(pl);   // the captured batches contain (or not) the image pass
     pl->dimg.mode = mode;
     pl->dimg.n = 0;
-    return async_grow(pl);
+    return grow_outputs(pl);
 }
 extern "C" int rb_pipeline_depth_image(rb_pipeline *pl, int i, const float **rho, const float **s_rho) {
     if (!pl || !rho) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
-    const unsigned char *planes = pl->view ? pl->view->dimg_host : pl->dimg.host;
-    const float *p = reinterpret_cast<const float *>(planes + (size_t)i * pl->dimg.stride);
+    const float *p = reinterpret_cast<const float *>(pl->view->dimg_host + (size_t)i * pl->dimg.stride);
     *rho = p;
     if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
@@ -1330,19 +1386,16 @@ extern "C" int rb_pipeline_set_odometry(rb_pipeline *pl, int on) {
     RB_ENTER(c);
     int r = set_begin(pl, nullptr);
     if (r) return r;
-    if (on && !pl->odom.dev) {
-        RB_CUDA(cudaMalloc(&pl->odom.dev, sizeof(rb_odometry) * pl->max_batch));
-        RB_CUDA(cudaMallocHost(&pl->odom.pin, sizeof(rb_odometry) * pl->max_batch));
-    }
+    if (on && !pl->odom.dev) RB_CUDA(cudaMalloc(&pl->odom.dev, sizeof(rb_odometry) * pl->max_batch));
     if (on != pl->odom.on) drop_graphs(pl);   // the captured batches pass (or not) the record slots to their kernels
     pl->odom.on = on;
     pl->odom.n = 0;
-    return async_grow(pl);
+    return grow_outputs(pl);
 }
 extern "C" int rb_pipeline_odometry(rb_pipeline *pl, const rb_odometry **recs, int *n) {
     if (!pl || !recs || !n) return RB_ERR_ARG;
     if (!pl->odom.n) return RB_ERR_STATE;
-    *recs = pl->view ? pl->view->odom : pl->odom.pin;
+    *recs = pl->view->odom;
     *n = pl->odom.n;
     return RB_OK;
 }
@@ -1350,8 +1403,8 @@ extern "C" int rb_pipeline_mirror(rb_pipeline *pl, int i, const void **records, 
     if (!pl || !records || !n) return RB_ERR_ARG;
     if (pl->out_dev) return RB_ERR_STATE;
     if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
-    *records = (pl->view ? pl->view->mirror_host : pl->mirror.host) + (size_t)i * pl->mirror.stride;
-    *n = (pl->view ? pl->view->nav : pl->nav_pin)[i].kn;
+    *records = pl->view->mirror_host + (size_t)i * pl->mirror.stride;
+    *n = pl->view->nav[i].kn;
     return RB_OK;
 }
 
@@ -1365,21 +1418,13 @@ extern "C" int rb_pipeline_set_output_memory(rb_pipeline *pl, int where) {
     // the buffers of the products that are on, in the new place; the other place's stay for a switch back
     const int was = pl->out_dev;
     pl->out_dev = where;
-    const size_t mb = (size_t)pl->max_batch;
-    if (pl->mirror.on && !where)
-        r = grow_mapped(c, &pl->mirror.host, &pl->mirror.host_bytes, mb * pl->mirror.stride);
-    if (!r && pl->depth.on)
-        r = grow_out(pl, &pl->depth.host, &pl->depth.host_bytes, &pl->depth.dev, &pl->depth.dev_bytes,
-                     mb * pl->depth.plan.cells_bytes);
-    if (!r && pl->dimg.mode)
-        r = grow_out(pl, &pl->dimg.host, &pl->dimg.host_bytes, &pl->dimg.dev, &pl->dimg.dev_bytes, mb * pl->dimg.stride);
-    if (r) {
+    if ((r = grow_outputs(pl))) {
         pl->out_dev = was;
         return r;
     }
     drop_graphs(pl);   // the captured batches contain (or not) k_mirror_to_host and its join
     pl->mirror.n = pl->depth.n = pl->dimg.n = 0;
-    return async_grow(pl);
+    return RB_OK;
 }
 extern "C" int rb_pipeline_set_consumer_stream(rb_pipeline *pl, void *stream) {
     if (!pl) return RB_ERR_ARG;
@@ -1392,8 +1437,8 @@ extern "C" int rb_pipeline_mirror_dev(rb_pipeline *pl, int i, const void **recor
     if (!pl || !records || !n) return RB_ERR_ARG;
     if (!pl->out_dev) return RB_ERR_STATE;
     if (!pl->mirror.on || i < 0 || i >= pl->mirror.n) return RB_ERR_ARG;
-    *records = (pl->view ? pl->view->mirror_dev : pl->mirror.dev) + (size_t)i * pl->mirror.stride;
-    *n = (pl->view ? pl->view->nav : pl->nav_pin)[i].kn;
+    *records = pl->view->mirror_dev + (size_t)i * pl->mirror.stride;
+    *n = pl->view->nav[i].kn;
     return RB_OK;
 }
 extern "C" int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell **cells, int *gw, int *gh,
@@ -1402,7 +1447,7 @@ extern "C" int rb_pipeline_depth_dev(rb_pipeline *pl, int i, const rb_depth_cell
     if (!pl->out_dev) return RB_ERR_STATE;
     if (!pl->depth.on || i < 0 || i >= pl->depth.n) return RB_ERR_ARG;
     const DepthGeom &g = pl->depth.plan.g;
-    const unsigned char *slot = (pl->view ? pl->view->depth_dev : pl->depth.dev) + (size_t)i * pl->depth.plan.cells_bytes;
+    const unsigned char *slot = pl->view->depth_dev + (size_t)i * pl->depth.plan.cells_bytes;
     *cells = reinterpret_cast<const rb_depth_cell *>(slot);
     if (gw) *gw = g.gw;
     if (gh) *gh = g.gh;
@@ -1413,65 +1458,39 @@ extern "C" int rb_pipeline_depth_image_dev(rb_pipeline *pl, int i, const float *
     if (!pl || !rho) return RB_ERR_ARG;
     if (!pl->out_dev) return RB_ERR_STATE;
     if (i < 0 || i >= pl->dimg.n) return RB_ERR_ARG;
-    const unsigned char *planes = pl->view ? pl->view->dimg_dev : pl->dimg.dev;
-    const float *p = reinterpret_cast<const float *>(planes + (size_t)i * pl->dimg.stride);
+    const float *p = reinterpret_cast<const float *>(pl->view->dimg_dev + (size_t)i * pl->dimg.stride);
     *rho = p;
     if (s_rho) *s_rho = pl->dimg.mode == 2 ? p + pl->dimg.plane : nullptr;
     return RB_OK;
 }
 
+// the synchronous pushes' C entry points: push_in's checks, then push_impl
+static int push(rb_pipeline *pl, const char *what, PushIn in, rb_nav *nav_out) {
+    if (!pl) return RB_ERR_ARG;
+    const int r = push_in(pl, what, in);
+    return r ? r : push_impl(pl, in, nav_out);
+}
 extern "C" int rb_pipeline_push(rb_pipeline *pl, const uint8_t *rgb, const double *ts, int n, rb_nav *nav_out) {
-    return push_impl(pl, rgb, nullptr, RB_IN_RGB, false, ts, n, nav_out);
+    return push(pl, "push", {rgb, nullptr, RB_FRAME_RGB24, false, false, nullptr, ts, n}, nav_out);
 }
 extern "C" int rb_pipeline_push_dev(rb_pipeline *pl, const uint8_t *rgb_dev, const double *ts, int n,
                                     rb_nav *nav_out) {
-    return push_impl(pl, rgb_dev, nullptr, RB_IN_RGB, true, ts, n, nav_out);
+    return push(pl, "push_dev", {rgb_dev, nullptr, RB_FRAME_RGB24, true, false, nullptr, ts, n}, nav_out);
 }
 extern "C" int rb_pipeline_push_mono(rb_pipeline *pl, const uint8_t *mono, const double *ts, int n, rb_nav *nav_out) {
-    return push_impl(pl, mono, nullptr, RB_IN_MONO, false, ts, n, nav_out);
+    return push(pl, "push_mono", {mono, nullptr, RB_FRAME_MONO8, false, false, nullptr, ts, n}, nav_out);
 }
 extern "C" int rb_pipeline_push_mono_dev(rb_pipeline *pl, const uint8_t *mono_dev, const double *ts, int n,
                                          rb_nav *nav_out) {
-    return push_impl(pl, mono_dev, nullptr, RB_IN_MONO, true, ts, n, nav_out);
-}
-// strided frames: every argument is checked before anything is enqueued; host frames then run the packed format's batches,
-// device frames the strided layout's
-static int check_frames(rb_pipeline *pl, const char *what, int format, const rb_frame *frames, const double *ts, int n,
-                        bool on_device, int *fmt) {
-    rb_ctx *c = pl->c;
-    if (format != RB_FRAME_RGB24 && format != RB_FRAME_MONO8) {
-        snprintf(c->err, sizeof(c->err), "%s: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", what, format);
-        return RB_ERR_ARG;
-    }
-    if (n < 1 || n > pl->max_batch || !frames || !ts) return RB_ERR_ARG;
-    const int64_t row = (int64_t)(format == RB_FRAME_MONO8 ? 1 : 3) * c->w;
-    for (int i = 0; i < n; i++)
-        if (!frames[i].data || frames[i].step < row) {
-            snprintf(c->err, sizeof(c->err), "%s: frame %d has %s (rows need %lld bytes)", what, i,
-                     frames[i].data ? "a step shorter than a row" : "no data", (long long)row);
-            return RB_ERR_ARG;
-        }
-    if (on_device && pl->und && (c->w > 65535 || c->h > 65535)) {   // (the strided undistortion's 16-bit tap coordinates)
-        snprintf(c->err, sizeof(c->err), "%s_dev: undistorted frames wider or higher than 65535 pixels", what);
-        return RB_ERR_ARG;
-    }
-    const int f = format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB;
-    *fmt = on_device ? f + RB_IN_RGB_STRIDED : f;
-    return RB_OK;
-}
-static int push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n, rb_nav *nav_out,
-                       bool on_device) {
-    if (!pl) return RB_ERR_ARG;
-    int fmt = 0, r = check_frames(pl, "push_frames", format, frames, ts, n, on_device, &fmt);
-    return r ? r : push_impl(pl, nullptr, frames, fmt, on_device, ts, n, nav_out);
+    return push(pl, "push_mono_dev", {mono_dev, nullptr, RB_FRAME_MONO8, true, false, nullptr, ts, n}, nav_out);
 }
 extern "C" int rb_pipeline_push_frames(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                        rb_nav *nav_out) {
-    return push_frames(pl, format, frames, ts, n, nav_out, false);
+    return push(pl, "push_frames", {nullptr, frames, format, false, false, nullptr, ts, n}, nav_out);
 }
 extern "C" int rb_pipeline_push_frames_dev(rb_pipeline *pl, int format, const rb_frame *frames, const double *ts, int n,
                                            rb_nav *nav_out) {
-    return push_frames(pl, format, frames, ts, n, nav_out, true);
+    return push(pl, "push_frames", {nullptr, frames, format, true, false, nullptr, ts, n}, nav_out);
 }
 
 // ---- detection masks (DESIGN.md §5) --------------------------------------------------------------------------------------
@@ -1495,27 +1514,9 @@ extern "C" int rb_pipeline_set_detect_mask(rb_pipeline *pl, const uint8_t *mask,
     pl->det_fixed_on = true;
     return RB_OK;
 }
-// per-frame detection masks: n device {data, step} entries, each step at least a row of w bytes
-static int check_masks(rb_pipeline *pl, const char *what, const rb_frame *masks, int n) {
-    rb_ctx *c = pl->c;
-    if (!masks) {
-        snprintf(c->err, sizeof(c->err), "%s: no masks", what);
-        return RB_ERR_ARG;
-    }
-    for (int i = 0; i < n; i++)
-        if (!masks[i].data || masks[i].step < c->w) {
-            snprintf(c->err, sizeof(c->err), "%s: mask %d has %s (rows need %d bytes)", what, i,
-                     masks[i].data ? "a step shorter than a row" : "no data", c->w);
-            return RB_ERR_ARG;
-        }
-    return RB_OK;
-}
 extern "C" int rb_pipeline_push_masked(rb_pipeline *pl, int format, int on_device, const rb_frame *frames,
                                        const rb_frame *masks, const double *ts, int n, rb_nav *nav_out) {
-    if (!pl) return RB_ERR_ARG;
-    int fmt = 0, r = check_frames(pl, "push_masked", format, frames, ts, n, on_device != 0, &fmt);
-    if (!r) r = check_masks(pl, "push_masked", masks, n);
-    return r ? r : push_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, nav_out, masks);
+    return push(pl, "push_masked", {nullptr, frames, format, on_device != 0, true, masks, ts, n}, nav_out);
 }
 
 // ---- asynchronous pushes (DESIGN.md §5) ----------------------------------------------------------------------------------
@@ -1534,48 +1535,39 @@ extern "C" int rb_pipeline_set_async(rb_pipeline *pl, int depth) {
     return r;
 }
 
-// one ticket: the front on the front stream into workspace k % 2, the back on the tracker stream into output slot
-// k % depth.  Arguments as push_impl's.
-static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *frames, int fmt, bool on_device, const double *ts,
-                        int n, int64_t *ticket, const rb_frame *masks = nullptr) {
+// one ticket of input that push_in has checked: the front on the front stream into workspace k % 2, the back on the tracker
+// stream into output slot k % depth
+static int enqueue_impl(rb_pipeline *pl, const PushIn &in, int64_t *ticket) {
     rb_ctx *c = pl->c;
-    const rb_params &p = pl->p;
     AsyncRing *ar = pl->ar;
     if (!ar || pl->imu) {
         snprintf(c->err, sizeof(c->err), "enqueue: %s", pl->imu ? "not available in IMU mode"
                                                                   : "asynchronous pushes are off (rb_pipeline_set_async)");
         return RB_ERR_ARG;
     }
-    if (n < 1 || n > pl->max_batch || !(rgb || frames) || !ts || !ticket) return RB_ERR_ARG;
-    if (fmt == RB_IN_MONO && on_device && (reinterpret_cast<uintptr_t>(rgb) & 3)) return RB_ERR_ARG;
+    if (!ticket) return RB_ERR_ARG;
     if (pl->tk_next - pl->tk_retired >= ar->depth) {
         snprintf(c->err, sizeof(c->err), "enqueue: %d tickets are outstanding, the depth of rb_pipeline_set_async: wait first",
                  ar->depth);
         return RB_ERR_STATE;
     }
     RB_CUDA(cudaSetDevice(c->device));
-    const long long k = pl->tk_next, first = pl->n_pushed;
-    AsyncSlot &s = ar->slot[k % ar->depth];
+    const int n = in.n, fmt = in.fmt;
+    const long long k = pl->tk_next;
+    OutSlot &s = ar->slot[k % ar->depth];
     const int par = (int)(k & 1);
     DogWS *ws = par ? &ar->ws1 : &pl->ws;
     int r;
-    for (int i = 0; i < n; i++) {   // (as push_impl)
-        const long long fr = first + i;
-        double dt = ts[i] - (i == 0 ? pl->t_prev : ts[i - 1]);
-        if (dt < 0.001) dt = 1 / p.config_fps;
-        s.fa[i].t = ts[i];
-        s.fa[i].dt = dt;
-        s.fa[i].frame_count = fr > 0 ? (unsigned int)((fr - 1) / 8) : 0;
-    }
+    write_args(pl, s, in.ts, n);
     // front: once the back of ticket k - 2 (the last to read this workspace) is done, the frames into its staging (host
     // input) or its frame table (strided device input), then gray and scale space
     cudaStream_t fs = ar->front, main_stream = c->stream;
     RB_CUDA(cudaStreamWaitEvent(fs, ar->ev_free[par], 0));
-    if (!on_device && (r = stage_host_frames(pl, rgb, frames, fmt, 0, n, fs, ws))) return r;
-    s.tbl[0].src = on_device ? (const void *)rgb : (const void *)ws->rgb;   // (strided: unused)
+    if (!in.on_device && (r = stage_host_frames(pl, in, 0, n, fs, ws))) return r;
+    s.tbl[0].src = in.on_device ? (const void *)in.data : (const void *)ws->rgb;   // (strided: unused)
     RB_CUDA(cudaMemcpyAsync(ar->front_dev[par], &s.tbl[0], sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, fs));
     if (in_strided(fmt)) {
-        memcpy(s.frames, frames, sizeof(rb_frame) * n);
+        memcpy(s.frames, in.frames, sizeof(rb_frame) * n);
         RB_CUDA(cudaMemcpyAsync(ar->frames_dev[par], s.frames, sizeof(rb_frame) * n, cudaMemcpyHostToDevice, fs));
     }
     auto front = [&]() {
@@ -1584,13 +1576,11 @@ static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *fra
         c->stream = main_stream;
         return e;
     };
+    const int fkey = afront_slot(pl, fmt, par, n);
     if (!pl->use_graph) {
         if ((r = front())) return r;
-    } else {
-        const int key = afront_slot(pl, fmt, par, n);
-        if (!ar->gfront[key] && (r = capture_graph(pl, fs, front, &ar->gfront[key], &ar->lfront[key]))) return r;
-        RB_CUDA(cudaGraphLaunch(ar->gfront[key], fs));
-        c->launches += ar->lfront[key];
+    } else if ((r = graph_launch(pl, ar->front_graphs, fs, fkey, 1, [&](int) { return fkey; }, [&](int) { return front(); }))) {
+        return r;
     }
     RB_CUDA(cudaEventRecord(ar->ev_front[par], fs));
     // back: after the consumer's reads of the outputs this slot held (device mode) and this ticket's front, behind the back
@@ -1598,38 +1588,20 @@ static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *fra
     if (pl->out_dev && pl->consumer != c->stream && (r = stream_wait(pl, pl->consumer, c->stream))) return r;
     RB_CUDA(cudaStreamWaitEvent(c->stream, ar->ev_front[par], 0));
     RB_CUDA(cudaMemcpyAsync(pl->fa_dev, s.fa, sizeof(FrameArgs) * n, cudaMemcpyHostToDevice, c->stream));
-    // (the slot's table: its previous ticket, the last reader of s.masks, has been waited)
-    const bool masked = fill_masks(pl, masks, n, s.masks);
-    if (masked)
-        RB_CUDA(cudaMemcpyAsync(pl->det_mask_dev, s.masks, sizeof(DetMask) * n, cudaMemcpyHostToDevice, c->stream));
-    SubBatchPtrs &t = s.tbl[1];
-    memset(&t, 0, sizeof(t));
-    if (pl->mirror.on) {   // (host mode: the pipeline's staging, then the slot's mapped memory; device mode: the slot)
-        t.mirror[0] = pl->out_dev ? s.mirror_dev : pl->mirror.dev;
-        t.mirror[1] = pl->out_dev ? nullptr : s.mirror_host;
-    }
-    if (pl->depth.on) {
-        t.depth[0] = pl->depth.stage;
-        t.depth[1] = pl->out_dev ? s.depth_dev : s.depth_host;
-        t.depth[2] = pl->dimg.mode ? (pl->out_dev ? s.dimg_dev : s.dimg_host) : nullptr;
-    }
-    RB_CUDA(cudaMemcpyAsync(pl->sb_dev, &t, sizeof(t), cudaMemcpyHostToDevice, c->stream));
-    if (!pl->use_graph || first == 0) {
-        if ((r = enqueue_back(pl, ws, n, first, masked))) return r;
-    } else {
-        const int key = aback_slot(pl, masked, par, (int)(first % RB_NMAPS), n);
-        // (every workspace and ring phase of this size at once, as the synchronous batches)
-        const bool build = !ar->gback[key];
-        for (int pa = 0; pa < 2 && build; pa++)
-            for (int ph = 0; ph < RB_NMAPS; ph++) {
-                const int kk = aback_slot(pl, masked, pa, ph, n);
-                if (ar->gback[kk]) continue;
-                const DogWS *w = pa ? &ar->ws1 : &pl->ws;
-                auto body = [&]() { return enqueue_back(pl, w, n, ph == 0 ? RB_NMAPS : ph, masked); };
-                if ((r = capture_graph(pl, c->stream, body, &ar->gback[kk], &ar->lback[kk]))) return r;
-            }
-        RB_CUDA(cudaGraphLaunch(ar->gback[key], c->stream));
-        c->launches += ar->lback[key];
+    // (the slot's sources: its previous ticket, their last reader, has been waited)
+    const bool masked = fill_masks(pl, in.masks, n, s);
+    if ((r = write_tables(pl, s, 1, nullptr, 0, n, masked))) return r;
+    if (!pl->use_graph || s.first == 0) {
+        if ((r = enqueue_back(pl, ws, n, s.first, masked))) return r;
+    } else {   // (every workspace and ring phase of this size at once, as the synchronous batches)
+        auto sib_key = [&](int i) { return aback_slot(pl, masked, i / RB_NMAPS, i % RB_NMAPS, n); };
+        auto sib_body = [&](int i) {
+            const int ph = i % RB_NMAPS;
+            return enqueue_back(pl, i / RB_NMAPS ? &ar->ws1 : &pl->ws, n, ph == 0 ? RB_NMAPS : ph, masked);
+        };
+        if ((r = graph_launch(pl, ar->back_graphs, c->stream, sib_key(par * RB_NMAPS + (int)(s.first % RB_NMAPS)),
+                              2 * RB_NMAPS, sib_key, sib_body)))
+            return r;
     }
     RB_CUDA(cudaEventRecord(ar->ev_free[par], c->stream));
     RB_CUDA(cudaMemcpyAsync(s.nav, pl->nav_dev, sizeof(rb_nav) * n, cudaMemcpyDeviceToHost, c->stream));
@@ -1642,53 +1614,33 @@ static int enqueue_impl(rb_pipeline *pl, const uint8_t *rgb, const rb_frame *fra
         RB_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), c->stream));
     }
     RB_CUDA(cudaEventRecord(s.done, c->stream));
-    s.first = first;
-    s.n = n;
     pl->tk_next = k + 1;
     pl->n_pushed += n;
-    pl->t_prev = ts[n - 1];
+    pl->t_prev = in.ts[n - 1];
     pl->restored = false;
     pl->last_sub = 0;   // (the workspaces are the tickets': rb_pipeline_batch_plane has nothing to show)
     *ticket = k;
     return RB_OK;
 }
+// the asynchronous pushes' C entry points: push_in's checks, then enqueue_impl
+static int enqueue(rb_pipeline *pl, const char *what, PushIn in, int64_t *ticket) {
+    if (!pl) return RB_ERR_ARG;
+    const int r = push_in(pl, what, in);
+    return r ? r : enqueue_impl(pl, in, ticket);
+}
 extern "C" int rb_pipeline_enqueue(rb_pipeline *pl, int format, int on_device, const uint8_t *data, const double *ts, int n,
                                    int64_t *ticket) {
-    if (!pl) return RB_ERR_ARG;
-    if (format != RB_FRAME_RGB24 && format != RB_FRAME_MONO8) {
-        snprintf(pl->c->err, sizeof(pl->c->err), "enqueue: format %d is neither RB_FRAME_RGB24 nor RB_FRAME_MONO8", format);
-        return RB_ERR_ARG;
-    }
-    return enqueue_impl(pl, data, nullptr, format == RB_FRAME_MONO8 ? RB_IN_MONO : RB_IN_RGB, on_device != 0, ts, n, ticket);
+    return enqueue(pl, "enqueue", {data, nullptr, format, on_device != 0, false, nullptr, ts, n}, ticket);
 }
 extern "C" int rb_pipeline_enqueue_frames(rb_pipeline *pl, int format, int on_device, const rb_frame *frames, const double *ts,
                                           int n, int64_t *ticket) {
-    if (!pl) return RB_ERR_ARG;
-    int fmt = 0, r = check_frames(pl, "enqueue_frames", format, frames, ts, n, on_device != 0, &fmt);
-    return r ? r : enqueue_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, ticket);
+    return enqueue(pl, "enqueue_frames", {nullptr, frames, format, on_device != 0, false, nullptr, ts, n}, ticket);
 }
 extern "C" int rb_pipeline_masked_enqueue(rb_pipeline *pl, int format, int on_device, const rb_frame *frames,
                                           const rb_frame *masks, const double *ts, int n, int64_t *ticket) {
-    if (!pl) return RB_ERR_ARG;
-    int fmt = 0, r = check_frames(pl, "masked_enqueue", format, frames, ts, n, on_device != 0, &fmt);
-    if (!r) r = check_masks(pl, "masked_enqueue", masks, n);
-    return r ? r : enqueue_impl(pl, nullptr, frames, fmt, on_device != 0, ts, n, ticket, masks);
+    return enqueue(pl, "masked_enqueue", {nullptr, frames, format, on_device != 0, true, masks, ts, n}, ticket);
 }
 
-// the host side of push_impl after its synchronisation, for one completed ticket, in ticket order
-static bool async_retire(rb_pipeline *pl, AsyncSlot &s) {
-    for (int i = 0; i < s.n && pl->odom.on; i++) {
-        if (s.first + i == 0) {   // the first frame of a sequence only initialises the ring (:109-121)
-            memset(&s.odom[i], 0, sizeof(rb_odometry));
-            continue;
-        }
-        s.odom[i].QK = i == 0 ? pl->odom.rkp_last : s.nav[i - 1].RKp;
-    }
-    pl->odom.rkp_last = s.nav[s.n - 1].RKp;
-    bool aborted = false;
-    for (int m = 0; m < RB_NMAPS; m++) aborted = aborted || s.abort[m] != 0;
-    return aborted;
-}
 extern "C" int rb_pipeline_wait(rb_pipeline *pl, int64_t ticket, rb_nav *nav_out) {
     if (!pl) return RB_ERR_ARG;
     rb_ctx *c = pl->c;
@@ -1699,26 +1651,18 @@ extern "C" int rb_pipeline_wait(rb_pipeline *pl, int64_t ticket, rb_nav *nav_out
     }
     RB_CUDA(cudaSetDevice(c->device));
     AsyncRing *ar = pl->ar;
-    long long aborted = -1;
-    while (pl->tk_retired <= ticket) {
-        AsyncSlot &s = ar->slot[pl->tk_retired % ar->depth];
+    int r = RB_OK;
+    while (pl->tk_retired <= ticket) {   // (in ticket order)
+        OutSlot &s = ar->slot[pl->tk_retired % ar->depth];
         RB_CUDA(cudaEventSynchronize(s.done));
-        if (async_retire(pl, s) && aborted < 0) aborted = pl->tk_retired;
+        const int e = retire(pl, s);
+        if (!r) r = e;
         pl->tk_retired++;
     }
-    const AsyncSlot &s = ar->slot[ticket % ar->depth];
-    pl->view = &s;
-    pl->odom.n = pl->odom.on ? s.n : 0;
-    pl->mirror.n = pl->mirror.on ? s.n : 0;
-    pl->depth.n = pl->depth.on ? s.n : 0;
-    pl->dimg.n = pl->depth.on && pl->dimg.mode ? s.n : 0;
+    const OutSlot &s = ar->slot[ticket % ar->depth];
+    show(pl, s, s.n);
     if (nav_out) memcpy(nav_out, s.nav, sizeof(rb_nav) * s.n);
-    if (aborted >= 0) {
-        snprintf(c->err, sizeof(c->err),
-                 "Minimizer_RV: an exchange between the kernel's CTAs timed out in ticket %lld (poses are NaN)", aborted);
-        return RB_ERR_CUDA;
-    }
-    return RB_OK;
+    return r;
 }
 extern "C" int rb_pipeline_poll(rb_pipeline *pl, int64_t *newest_complete) {
     if (!pl || !newest_complete) return RB_ERR_ARG;
@@ -1794,8 +1738,8 @@ extern "C" int rb_pipeline_bench_pass(rb_pipeline *pl, int pass_id, int nimg, in
                                nimg);
     };
     if (und_pass) {
-        pl->sb_pin[0].src = pl->ws.rgb;
-        RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->sb_pin, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
+        pl->out.tbl[0].src = pl->ws.rgb;
+        RB_CUDA(cudaMemcpyAsync(pl->sb_dev, pl->out.tbl, sizeof(SubBatchPtrs), cudaMemcpyHostToDevice, c->stream));
     }
     for (int i = 0; i < 3; i++)
         if ((r = one())) return r;
@@ -1964,7 +1908,7 @@ extern "C" int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n
     for (int k = 0; k < RB_NMAPS; k++) {
         RB_CUDA(cudaMemsetAsync(&pl->maps[k]->ts_host.ctl->abort, 0, sizeof(int), c->stream));
         if (pl->maps[k] != m) RB_CUDA(cudaMemsetAsync(&pl->maps[k]->st->frame_count, 0, sizeof(unsigned int), c->stream));
-        pl->abort_pin[k] = 0;
+        pl->out.abort[k] = 0;
     }
     if ((r = rb_state_unpack_enqueue(c, m, pl->fs, pl->chain, pl->state_host, h.kn))) return r;
     RB_CUDA(cudaStreamSynchronize(c->stream));
@@ -1988,8 +1932,7 @@ extern "C" int rb_pipeline_load_state(rb_pipeline *pl, const void *buf, size_t n
         }
     }
     // the outputs of the last push are not this session's
-    pl->view = nullptr;
-    pl->mirror.n = pl->depth.n = pl->dimg.n = pl->odom.n = 0;
+    show(pl, pl->out, 0);
     pl->last_sub = 0;
     return RB_OK;
 }
